@@ -2,6 +2,7 @@
 """Benchmark of the rollout hot path (BASELINE.json metric).
 
     python bench.py --gpus 1 --steps 20 --warmup 3            # our arm, 1 GPU
+    python bench.py --gpus 1 --steps 4 --dump-outputs out/    # ... and write what the last timed step computed
     torchrun --nproc-per-node N ... bench.py --gpus N ...     # one rank per GPU, weak scaling
     python bench.py --impl reference --steps 5 --warmup 1     # CPU reference arm
 
@@ -16,7 +17,12 @@ The same invocation also measures (sub-records under ``configs``, skipped with `
   config 4  GraphCast 6-h step on (2 x 83, 721, 1440), refinement-6 multimesh       -> configs.graphcast
   config 5  Pangu ensemble with 4 members per GPU (32 members on 8 GPUs)      -> configs.ensemble_m4
 each with ms/step, member-steps/s, per-family roofline fractions, fixture verification, and (N = 1) its e2e figure.
-One JSON line on rank 0.
+One JSON line on rank 0, with the GPU's name and power limit (the numbers depend on both).
+
+``--dump-outputs DIR`` writes, after the timed steps of the headline workload, the state its last timed step returned as
+DIR/<model>_state.npy (float32): all of it when it is at most 64 MB, else the values at a fixed seeded set of flat indices
+(numpy default_rng(0), sorted) of 15 M elements.  Inputs are seeded, so two builds run with the same arguments can be
+compared output for output.
 """
 from __future__ import annotations
 
@@ -44,11 +50,38 @@ def _peaks():
         d = json.load(open(p))
         return dict(hbm=d["hbm_gbs"], tensor_burst=d["bf16_tflops"],
                     tensor_sustained=d.get("bf16_tflops_sustained", d["bf16_tflops"]), source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm=6650.0, tensor_burst=1590.0, tensor_sustained=1400.0, source="fallback (B200_PROFILING.md)")
+    # NVIDIA H100 SXM data sheet (700 W card): 3.35 TB/s HBM3, 989 TFLOP/s dense FP16 / BF16 — upper bounds, not reached figures
+    return dict(hbm=3350.0, tensor_burst=989.0, tensor_sustained=989.0, source="H100 SXM data sheet (700 W)")
+
+
+def gpu_identity(index: int) -> dict:
+    """Name and power limit of the card the numbers were measured on (read-only nvidia-smi query)."""
+    out = {"name": None, "power_limit_w": None, "sm_max_mhz": None}
+    try:
+        import torch
+        out["name"] = torch.cuda.get_device_name(index)
+        r = subprocess.run(["nvidia-smi", f"--id={index}", "--query-gpu=power.limit,clocks.max.sm", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True, timeout=20)
+        f = [t.strip() for t in r.stdout.strip().split(",")]
+        out["power_limit_w"], out["sm_max_mhz"] = float(f[0]), float(f[1])
+    except Exception:
+        pass
+    return out
+
+
+def dump_state(state, path: str, limit_bytes: int = 64 << 20, n_sample: int = 15 << 20):
+    """float32 copy of `state` (any shape) -> path; larger than limit_bytes: the values at a seeded sorted index sample."""
+    import numpy as np
+    import torch
+    flat = state.detach().reshape(-1).float()
+    if flat.numel() * 4 > limit_bytes:
+        idx = np.sort(np.random.default_rng(0).choice(flat.numel(), size=n_sample, replace=False))
+        flat = flat[torch.from_numpy(idx).to(flat.device)]
+    np.save(path, flat.cpu().numpy().astype(np.float32, copy=False))
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -74,6 +107,11 @@ class ClockSampler:
             return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
         time.sleep(0.15)
         self.proc.terminate()
+        try:
+            self.proc.wait(timeout=5)
+        except Exception:
+            self.proc.kill()
+            self.proc.wait()
         sm, mx, reasons = [], None, set()
         for ln in self.lines:
             f = [t.strip() for t in ln.split(",")]
@@ -298,7 +336,7 @@ def family_roofline(model, cfg, M, fam_ms, peaks):
     return out, fl, by
 
 
-def bench_model(model: str, M: int, steps: int, warmup: int, d: Dist, e2e: bool = True):
+def bench_model(model: str, M: int, steps: int, warmup: int, d: Dist, e2e: bool = True, dump_dir: str | None = None):
     import torch
     from skyrim_b200.engine import launch_count, perturb_ic
     from skyrim_b200.verify import compare_fullsize, load_fixture, summarise
@@ -369,6 +407,9 @@ def bench_model(model: str, M: int, steps: int, warmup: int, d: Dist, e2e: bool 
     launches = launch_count() - launches0
     finite = bool(torch.isfinite(src).all())
     z_first = z[0].clone()
+    if dump_dir and d.rank == 0:   # what the last timed step returned, before the profiled pass reuses the buffers
+        os.makedirs(dump_dir, exist_ok=True)
+        dump_state(src, os.path.join(dump_dir, f"{model}_state.npy"))
 
     # ---- the same K steps once more with CUDA events around every launch of the dominant family (plain launches: the
     # per-launch events cannot live inside a replayed graph) -> roofline.achieved; its wall time is reported beside it ----
@@ -461,26 +502,11 @@ def bench_model(model: str, M: int, steps: int, warmup: int, d: Dist, e2e: bool 
     return rec
 
 
-def _traffic(family):
-    """DRAM bytes per launch of a kernel family from the committed `ncu --set full` capture of this round's kernels
-    (profiles/r2f_traffic.json, provenance and kernel names inside); None when no capture covers the family."""
-    for name in ("r2f_traffic.json", "r2_traffic.json", "r1_traffic.json"):
-        p = os.path.join(ROOT, "profiles", name)
-        try:
-            with open(p) as f:
-                e = json.load(f).get(family)
-            if e:
-                return e.get("bytes_per_launch"), f"profiles/{name}"
-        except (OSError, ValueError):
-            pass
-    return None, None
-
-
 def run_ours(args):
     import torch
     d = Dist(args)
     M = args.members_per_gpu
-    head = bench_model(args.model, M, args.steps, args.warmup, d)
+    head = bench_model(args.model, M, args.steps, args.warmup, d, dump_dir=args.dump_outputs)
     subs = {}
     if not args.only_headline:
         k = max(3, min(args.steps, 8))
@@ -503,7 +529,6 @@ def run_ours(args):
         work = head["_dominant_flops"] if tensor_bound else head["_dominant_bytes"]
         achieved = work / max(n_l, 1) / (avg_ms * 1e-3) / (1e12 if tensor_bound else 1e9)
         peak = peaks["tensor_sustained"] if tensor_bound else peaks["hbm"]
-        traffic, tsrc = _traffic(dom)
         sfno = args.model == "sfno"
         for r in [head] + list(subs.values()):
             r.pop("_dominant_flops", None); r.pop("_dominant_bytes", None)
@@ -513,9 +538,9 @@ def run_ours(args):
             "metric": METRIC, "value": head["value"], "unit": UNIT, "n_gpus": d.world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": head["ms_per_step"], "higher_is_better": True, "scaling": "weak",
             "vs_baseline": None,
-            "dtype": ("f16 hi+lo split operands / f32 accumulate (tcgen05 kind::f16), f32 state" if sfno else
-                      "f16 operands / f32 accumulate (tcgen05 kind::f16), f32 state, residual streams, LayerNorm" if args.model == "graphcast" else
-                      "f16 operands / f32 accumulate (tcgen05 kind::f16), f32 state, LN, softmax"),
+            "dtype": ("f16 hi+lo split operands / f32 accumulate (wgmma), f32 state" if sfno else
+                      "f16 operands / f32 accumulate (wgmma), f32 state, residual streams, LayerNorm" if args.model == "graphcast" else
+                      "f16 operands / f32 accumulate (wgmma; attention on mma.sync), f32 state, LN, softmax"),
             "data": "synthetic",
             "config": {"workload": ("FourCastNet-v2 SFNO rollout (chained 6-h steps), synthetic (73,721,1440) IC, state resident in HBM"
                                     if sfno else
@@ -526,12 +551,12 @@ def run_ours(args):
                        "l2": "inputs larger than L2 (state 0.3 GB + >2 GB activations streamed per step)",
                        "weights": "synthetic seed 0", "verified_against_oracle_fixture": bool(head["verify"] and head["verify"]["ok"])},
             "e2e": head.get("e2e"),
+            "gpu": gpu_identity(d.local),
             "gpu_launches": head["gpu_launches"],
             "clocks": head["clocks"],
             "roofline": {"bound": "tensor" if tensor_bound else "hbm", "kernel": dom, "achieved": achieved, "peak": peak,
-                         "unit": "TFLOP/s" if tensor_bound else "GB/s", "frac": achieved / peak, "traffic": traffic,
-                         "traffic_source": tsrc, "peak_source": peaks["source"] + (", bf16 cuBLAS sustained (kernel timed inside a long step)"
-                                                                                   if tensor_bound else ", device copy"),
+                         "unit": "TFLOP/s" if tensor_bound else "GB/s", "frac": achieved / peak,
+                         "peak_source": peaks["source"],
                          "launches_per_step": n_l, "avg_launch_ms": avg_ms,
                          "timing": ("CUDA events around every launch of the family on the launching stream, during a repeat of the "
                                     "timed K steps with plain launches (the timed region itself replays each step as one CUDA graph)"),
@@ -565,6 +590,8 @@ def main():
                     help="headline workload: pangu (default) or sfno (FourCastNet-v2 73-channel rollout)")
     ap.add_argument("--only-headline", action="store_true", help="skip the configs.sfno / configs.ensemble_m4 sub-records")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the headline workload's last timed output as DIR/<model>_state.npy (float32, <= 64 MB)")
     ap.add_argument("--allow-unverified", action="store_true",
                     help="print the line (verify.ok = false) instead of exiting 3 when the fixture comparison fails")
     args = ap.parse_args()

@@ -1,4 +1,4 @@
-/* skyrim_b200 — C-ABI of the B200-native step operators behind the Skyrim rollout path.
+/* skyrim_b200 — C-ABI of the H100 (sm_90a) step operators behind the Skyrim rollout path.
  *
  * The reference has no FFI of its own: its seam is the Python earth2mip ``TimeLoop``
  * protocol consumed at

@@ -70,7 +70,7 @@ class PanguRef:
 
     ``emulate`` reproduces the engine's storage/operand precision so that the error budget
     can be studied on CPU: "fp16" rounds GEMM operands (activations and weights) to half,
-    accumulates in fp32 — what tcgen05 kind::f16 does.
+    accumulates in fp32 — what the engine's tensor-core GEMMs do.
     """
 
     def __init__(self, cfg: PanguConfig, weights, dtype=torch.float32, emulate: str | None = None):

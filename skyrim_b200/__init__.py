@@ -1,4 +1,4 @@
-"""skyrim_b200 — B200-native rollout engine behind the Skyrim API (see DESIGN.md)."""
+"""skyrim_b200 — H100-native rollout engine behind the Skyrim API (see DESIGN.md)."""
 __all__ = ["Skyrim"]
 
 

@@ -1,7 +1,7 @@
 """ctypes binding of the C-ABI in include/skyrim_b200.h (libskyrim_b200.so, built in-tree by
 ``__graft_entry__.build()`` / ``make -C skyrim_b200/csrc``).
 
-There is deliberately no fallback: if the shared library is missing or no sm_100 device is
+There is deliberately no fallback: if the shared library is missing or no sm_90 (H100) device is
 visible, every entry point raises.
 """
 from __future__ import annotations
@@ -11,8 +11,7 @@ import os
 from pathlib import Path
 
 LIB_PATH = Path(__file__).resolve().parent / "libskyrim_b200.so"
-# development build (-DSKY_EXPERIMENTS: CUDA-core reference GEMM, single-CTA kernel variants, timing-experiment
-# switches).  Never loaded unless a test asks for it with lib("dev") / SKYRIM_B200_LIB=dev.
+# development build (-DSKY_EXPERIMENTS: CUDA-core reference GEMM and attention, timing-experiment switches).  Never loaded unless a test asks for it with lib("dev") / SKYRIM_B200_LIB=dev.
 DEV_LIB_PATH = Path(__file__).resolve().parent / "libskyrim_b200_dev.so"
 
 SKY_MODEL_PANGU6 = 1

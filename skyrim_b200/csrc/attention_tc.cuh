@@ -1,4 +1,4 @@
-// Earth-specific 3-D window attention on tcgen05 + TMEM, fed by bulk (TMA-engine) copies.
+// Earth-specific 3-D window attention on the tensor cores (mma.sync m16n8k16, fp16 operands, fp32 accumulation).
 //
 //     O = softmax(scale * Q K^T + B[type, head] + shift_mask) V      per (window, head); 144 tokens, head_dim 32
 //
@@ -6,27 +6,14 @@
 //   qkv "window image"  [part q|k|v][member][window][head pair] -> tile of 144 rows x 128 B
 //     row j    = position in the (rolled) window, (zj, hj, wj) order
 //     128 B    = [head 2p: 32 halves | head 2p+1: 32 halves], 16-byte chunk c stored at c ^ (j & 7)
-//   i.e. byte for byte a K-major SWIZZLE_128B UMMA operand for Q and K (the two heads are k-steps {0,1} and {2,3}
-//   of the 64-wide row) and an MN-major SWIZZLE_128B B operand for V ([key][dims]); tools/umma_probe.cu verified
-//   every descriptor variant used here on the hardware (profiles/r2_umma_probe.md).  Windowing, the cyclic shift and
-//   the latitude padding were applied by the producer, so one work item is FOUR contiguous bulk copies.
+//   Windowing, the cyclic shift and the latitude padding were applied by the producer, so one work item is three
+//   contiguous 18 KB tiles.
 //
-// One persistent CTA per SM, 320 threads:
-//   warp 0     loader: cp.async.bulk global -> shared; Q+K ring (2 slots) and V ring (3 slots) are separate because Q and K
-//              die as soon as the item's three QK^T products are issued while V lives until its last PV product
-//   warp 1     MMA issuer (one elected thread): S = Q K^T (M=128, N=144, K=32) into TMEM, O = P V with P read from
-//              TMEM (A operand) and V from shared memory (MN-major B operand)
-//   warps 2..9 two softmax groups of four warps (TMEM lane quarter = warp % 4): thread = query row.  The 144 scores
-//              of the row come out of TMEM into registers and the group at once hands the S buffer back ("s_taken"), so
-//              the scores of its NEXT tile are computed while it works: bias (expanded per (window type, head) into
-//              shared memory, shift mask folded in), exp2 / row sum, P back to TMEM as fp16 in a separate P buffer, then
-//              the O row of the group's previous tile is scaled by 1/sum and stored (64 B of the projection's image).
-// 144 query rows = one M=128 tile + 16 left-over rows.  The left-over rows of the TWO heads of a pair share one
-// M=128 tile: head A's rows sit in lanes 32q..32q+15 and head B's in lanes 32q+16..32q+31 of a single accumulator
-// (two accumulating MMA pairs whose A tiles start at different rows of [Q rows | 16 zero rows | left-over rows |
-// 16 zero rows]), with q rotating over the lane quarters from item to item.  Its PV product runs over K = 288: P is
-// written in place over the scores as [P_A | 0] in head A's lanes and [0 | P_B] in head B's, against [V_A ; V_B].
-// TMEM columns: S0 | S1 (144 each) | P0 | P1 (72 each) | O0 | O1 (32 each) = 496 of 512.
+// One CTA per item (window, head pair), nine warps: warp w owns query rows 16w .. 16w+15 of both heads.  The q, k, v
+// tiles and the pair's two compact bias tables are copied to shared memory once; per head the warp computes its 16 x 144
+// score block in registers (ldmatrix + mma.sync), adds the bias gathered from the compact table (shift mask folded in,
+// in fp16), takes exp2 against the row max, and multiplies P (fp16, straight from the score registers) by V
+// (ldmatrix.trans).  1/sum is applied to the 32 outputs of each row, which go to the projection's operand image.
 #pragma once
 #include <cstdio>
 #include <cstdlib>
@@ -38,23 +25,11 @@ namespace sky {
 
 constexpr int AT_TABLE = (2 * WW - 1) * WH * WH * WZ * WZ;   // 3312 entries of the compact bias table per (type, head)
 constexpr int AT_TILE_B = WIN_TOK * 128;                     // 18432: one (window, head pair) tile of q, k or v
-constexpr int AT_BIAS_LD = 304;                              // bytes per expanded-bias row: 144 halves + 16 B pad (conflict-free LDS.128)
-constexpr int AT_BIAS_HEAD_B = WIN_TOK * AT_BIAS_LD;         // 43776
-constexpr int AT_BIAS_B = (2 * AT_BIAS_HEAD_B + 1023) / 1024 * 1024;   // 88064
-constexpr int AT_Q = 0, AT_Z0 = 128 * 128, AT_L = AT_Z0 + 2048, AT_Z1 = AT_L + 2048;   // inside one Q slot
-constexpr int AT_QSLOT_B = AT_Z1 + 2048;                     // 22528
-constexpr int AT_NQK = 2, AT_NV = 3;                         // ring depths
-constexpr int AT_OFF_Q = AT_BIAS_B, AT_OFF_K = AT_OFF_Q + AT_NQK * AT_QSLOT_B, AT_OFF_V = AT_OFF_K + AT_NQK * AT_TILE_B;
-constexpr int AT_OFF_BAR = AT_OFF_V + AT_NV * AT_TILE_B;
-constexpr int AT_QK_TX = 128 * 128 + 2048 + AT_TILE_B;       // bytes landing per item in the Q+K ring
-constexpr int AT_SMEM_BYTES = 1024 + AT_OFF_BAR + 256;
-constexpr int AT_THREADS = 384;   // warpgroup 0: loader, MMA issuer, 2 idle warps | warpgroups 1, 2: the softmax groups
-
-constexpr int AT_S_COLS = 144, AT_P_COL0 = 2 * AT_S_COLS, AT_P_COLS = 72, AT_O_COL0 = AT_P_COL0 + 2 * AT_P_COLS, AT_O_COLS = 32;
-static_assert(AT_QSLOT_B % 1024 == 0 && AT_BIAS_B % 1024 == 0 && AT_TILE_B % 1024 == 0, "swizzle atom alignment");
-static_assert(AT_SMEM_BYTES <= 232448, "smem budget");
-static_assert(AT_O_COL0 + 2 * AT_O_COLS <= 512, "TMEM budget");
-static_assert(2 * AT_TABLE * 2 <= AT_TILE_B, "compact bias tables are staged in a V slot");
+constexpr int AT_OFF_TAB = 3 * AT_TILE_B;                    // q | k | v tiles, then the two heads' compact tables (fp16)
+constexpr int AT_OFF_KEY = AT_OFF_TAB + 2 * AT_TABLE * 2;    // per key: table offset and shift-region flags (int32 each)
+constexpr int AT_SMEM_BYTES = AT_OFF_KEY + 2 * WIN_TOK * 4;
+constexpr int AT_THREADS = 32 * (WIN_TOK / 16);              // one warp per 16 query rows
+static_assert(WIN_TOK % 16 == 0 && (2 * AT_TABLE * 2) % 16 == 0, "tile shapes");
 
 struct AttnArgs {
   const uint8_t* qkv;        // window image, 3 parts
@@ -65,100 +40,26 @@ struct AttnArgs {
   float sl2;                 // head_dim^-0.5 * log2 e
   float mask_l2;             // mask value * log2 e
   long long items;           // B * nWin * pairs
-  long long* dbg = nullptr;  // dev build (SKY_ATTN_DBG): per-phase cycle accounting of the softmax warps
 };
 
-// instruction descriptors: A, B fp16, D fp32; B MN-major for the PV products
-__host__ __device__ constexpr uint32_t make_idesc_f16_bmn(int M, int N) { return make_idesc_f16(M, N) | (1u << 16); }
-
-__device__ __forceinline__ void tc_mma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
+__device__ __forceinline__ void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
 }
-__device__ __forceinline__ void tmem_ld16_nowait(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+__device__ __forceinline__ void ldsm_x4_t(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(addr));
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-      "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-      "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-      "r"(r[31])
-      : "memory");
+// c (16 x 8, fp32) += a (16 x 16, fp16, row-major fragment) * b (16 x 8, fp16, column fragment)
+__device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+  asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.f16.f16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
+               : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+               : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
+// shared address of 16-byte chunk c of row j of a window tile (swizzled: chunk c sits at c ^ (j & 7))
+__device__ __forceinline__ uint32_t at_chunk(uint32_t tile_s, int j, int c) {
+  return tile_s + (uint32_t)j * 128u + ((uint32_t)(c ^ (j & 7)) << 4);
 }
-__device__ __forceinline__ void tmem_ld8_nowait(uint32_t taddr, float* v) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr)
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st4(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(r[0]), "r"(r[1]),
-               "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ uint4 lds_b128(uint32_t a) {
-  uint4 v;
-  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a));
-  return v;
-}
-__device__ __forceinline__ float2 h2_to_f2(uint32_t u) { return __half22float2(*reinterpret_cast<const __half2*>(&u)); }
-
-// Handshake waits of the attention pipeline (softmax group <-> MMA issuer, several dependent hand-offs per tile).
-// mbar_wait() suspends the warp with a time hint, which is right for the GEMM pipelines (their waits are normally already
-// satisfied) but wakes up late; here the barrier is about to complete almost every time, so poll with plain try_wait
-// (SKY_ATTN_WAIT_SUSPEND selects the suspending wait again for A/B timing).
-__device__ __forceinline__ void mbar_wait_poll(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "SKY_POLL_%=:\n\t"
-      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
-      "@p bra SKY_POLLD_%=;\n\t"
-      "bra SKY_POLL_%=;\n\t"
-      "SKY_POLLD_%=:\n\t}\n" ::"r"(smem_u32(bar)),
-      "r"(parity)
-      : "memory");
-}
-__device__ __forceinline__ bool mbar_test(uint64_t* bar, uint32_t parity) {   // non-blocking
-  uint32_t ok;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}\n"
-      : "=r"(ok)
-      : "r"(smem_u32(bar)), "r"(parity)
-      : "memory");
-  return ok != 0;
-}
-#ifdef SKY_ATTN_WAIT_SUSPEND
-#define AT_WAIT(bar, parity) mbar_wait(bar, parity)
-#else
-#define AT_WAIT(bar, parity) mbar_wait_poll(bar, parity)
-#endif
 
 // window position (wz, wh, ww, row j) -> natural token of member b, or -1 for a latitude-padding row
 __device__ __forceinline__ long long at_row_token(const Geo& g, int roll, int b, int wz, int wh, int ww, int j) {
@@ -278,390 +179,135 @@ __global__ void __launch_bounds__(256) k_qkv_fill_pad(uint8_t* __restrict__ out,
 // ---------------------------------------------------------------------------------------------------------------
 // the attention kernel
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(AT_THREADS, 1) k_window_attention_tc(const AttnArgs a) {
-  extern __shared__ uint8_t at_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(at_raw) + 1023) & ~uintptr_t(1023));
-  uint8_t* bias_s = smem;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + AT_OFF_BAR);
-  uint64_t* qk_full = bars;          // [2] loader -> MMA
-  uint64_t* qk_empty = bars + 2;     // [2] MMA -> loader (commit after the item's last QK^T product)
-  uint64_t* v_full = bars + 4;       // [3]
-  uint64_t* v_empty = bars + 7;      // [3] (commit after the item's last PV product)
-  uint64_t* s_full = bars + 10;      // [2] MMA -> softmax group: scores of a tile are in TMEM
-  uint64_t* s_taken = bars + 12;     // [2] softmax group (4 warps) -> MMA: the scores are in registers, S may be overwritten
-  uint64_t* p_ready = bars + 14;     // [2] softmax group (4 warps) -> MMA: P is in TMEM and the group's O buffer is drained
-  uint64_t* o_full = bars + 16;      // [2] MMA -> softmax group: O of a tile is complete (and its P has been consumed)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 18);
-
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0), lane = threadIdx.x % 32;
-  const int tid = threadIdx.x;
+__global__ void __launch_bounds__(AT_THREADS) k_window_attention_tc(const AttnArgs a) {
+  extern __shared__ __align__(1024) uint8_t at_smem[];
   const Geo& g = a.g;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  // item n = ((type * pairs + pair) * B + b) * nWw + ww
+  const long long n = blockIdx.x;
+  const long long key = n / ((long long)a.B * g.nWw);
+  const int type = (int)(key / a.pairs), pair = (int)(key % a.pairs);
+  const int wz = type / g.nWh, wh = type % g.nWh;
+  const int ww = (int)(n % g.nWw), b = (int)((n / g.nWw) % a.B);
+  const uint8_t* src = a.qkv + ((size_t)(((long long)b * g.nWin + (long long)type * g.nWw + ww) * a.pairs + pair)) * AT_TILE_B;
 
-  if (tid == 0) {
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&qk_full[i], 1); mbar_init(&qk_empty[i], 1); mbar_init(&s_full[i], 1); mbar_init(&s_taken[i], 4);
-      mbar_init(&p_ready[i], 4); mbar_init(&o_full[i], 1);
-    }
-    for (int i = 0; i < AT_NV; ++i) { mbar_init(&v_full[i], 1); mbar_init(&v_empty[i], 1); }
-    mbar_fence_init();
+  // ---- q, k, v tiles and the pair's two compact bias tables -> shared memory ----
+  for (int i = tid; i < 3 * AT_TILE_B / 16; i += AT_THREADS) {
+    const int part = i / (AT_TILE_B / 16), off = i - part * (AT_TILE_B / 16);
+    reinterpret_cast<uint4*>(at_smem)[i] = __ldg(reinterpret_cast<const uint4*>(src + (size_t)part * a.part_stride) + off);
   }
-  // the two 16-row zero blocks around the left-over rows of each Q slot: written once, never overwritten
-  for (int i = tid; i < AT_NQK * 2 * 128; i += AT_THREADS) {
-    const int st = i / 256, r = i % 256;
-    *reinterpret_cast<uint4*>(smem + AT_OFF_Q + st * AT_QSLOT_B + (r < 128 ? AT_Z0 : AT_Z1 - 2048) + r * 16) = make_uint4(0, 0, 0, 0);
+  {
+    const uint4* tsrc = reinterpret_cast<const uint4*>(a.bias_tab + ((long long)type * g.heads + 2 * pair) * AT_TABLE);
+    for (int i = tid; i < 2 * AT_TABLE * 2 / 16; i += AT_THREADS) reinterpret_cast<uint4*>(at_smem + AT_OFF_TAB)[i] = __ldg(tsrc + i);
   }
-  fence_proxy_async_smem();
-  if (warp == 1) tmem_alloc<512>(tmem_ptr);
-  tc_fence_before();
+  int* kpart = reinterpret_cast<int*>(at_smem + AT_OFF_KEY);
+  int* kflag = kpart + WIN_TOK;
+  for (int j = tid; j < WIN_TOK; j += AT_THREADS) {
+    const int wj = j % WW, hj = (j / WW) % WH, zj = j / (WW * WH);
+    kpart[j] = (WZ * zj) * ((2 * WW - 1) * WH * WH) + (WH * hj) * (2 * WW - 1) - wj;
+    kflag[j] = (zj >= WZ - SZ ? 1 : 0) | (hj >= WH - SH ? 2 : 0);
+  }
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem = *tmem_ptr;
 
-  // this CTA's contiguous share of the items; item n = ((type * pairs + pair) * B + b) * nWw + ww.  The share is cut into
-  // SEGMENTS of one (window type, head pair): the expanded bias in shared memory is rebuilt at every segment start.
-  const long long n_begin = a.items * blockIdx.x / gridDim.x, n_end = a.items * (blockIdx.x + 1) / gridDim.x;
-  const int per_group = a.B * g.nWw;
-  uint32_t items_done = 0;          // items of all earlier segments (ring slot / phase bookkeeping of loader and MMA)
-  uint32_t cnt_a[2] = {0, 0};       // MMA: s_taken waits per group        | softmax warp: [0] = tiles of its group so far
-  uint32_t cnt_b[2] = {0, 0};       // MMA: p_ready waits per group
-#define AT_SEGMENT_HEAD                                                                            \
-    const long long key = seg0 / per_group;                                                        \
-    long long seg1 = (key + 1) * per_group;                                                        \
-    if (seg1 > n_end) seg1 = n_end;                                                                \
-    const int n_items = (int)(seg1 - seg0);                                                        \
-    const int type = (int)(key / a.pairs), pair = (int)(key % a.pairs);                            \
-    const int wz = type / g.nWh, wh = type % g.nWh;                                                \
-    const int T = 3 * n_items; /* tiles: per item [head A rows 0..127, head B rows 0..127, left-over rows of both] */ \
-    (void)wz; (void)wh; (void)pair; (void)type; (void)T;
+  const uint32_t q_s = smem_u32(at_smem), k_s = q_s + AT_TILE_B, v_s = q_s + 2 * AT_TILE_B;
+  const __half* tabs = reinterpret_cast<const __half*>(at_smem + AT_OFF_TAB);
+  const int fmask = a.roll ? ((wz == g.nWz - 1 ? 1 : 0) | (wh == g.nWh - 1 ? 2 : 0)) : 0;
+  const __half mask_h = __float2half_rn(a.mask_l2);
+  // this thread's two query rows (fragment rows l/4 and l/4 + 8 of the warp's 16)
+  int row[2], rpart[2], rflag[2];
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    const int i = 16 * warp + (lane >> 2) + 8 * u;
+    const int wi = i % WW, hi = (i / WW) % WH, zi = i / (WW * WH);
+    row[u] = i;
+    rpart[u] = zi * ((2 * WW - 1) * WH * WH) + hi * (2 * WW - 1) + wi + (WW - 1);
+    rflag[u] = (zi >= WZ - SZ ? 1 : 0) | (hi >= WH - SH ? 2 : 0);
+  }
+  const int c2 = 2 * (lane & 3);   // first of this thread's two columns in every 8-column fragment
 
-  // Register reallocation: the softmax threads keep a whole 144-wide score row in registers (and want many exponentials in
-  // flight); warpgroup 0 (loader, MMA issuer, two idle warps) gives registers up, the softmax warpgroups take them:
-  // 384 x 168 = 64.5 K >= 128 x 48 + 256 x 224.  The roles therefore split HERE, each with its own segment loop;
-  // one CTA barrier per segment (after the bias expansion, which borrows V slot 0 as staging) keeps them in step.
-  if (warp >= 4) {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 224;");
-    for (long long seg0 = n_begin; seg0 < n_end;) {
-      AT_SEGMENT_HEAD
-      asm volatile("bar.sync 1, 256;" ::: "memory");   // every softmax warp is done with the previous segment's bias
-    // ---- expand the bias of the pair's two heads: B[i][j] = table[idx(i, j)] (+ shift mask), fp16, log2 units.
-    //      The compact tables (2 x 3312 halves) are staged in V slot 0 (the rings are drained between segments). ----
-    {
-      uint8_t* stage = smem + AT_OFF_V;
-      const uint4* src = reinterpret_cast<const uint4*>(a.bias_tab + ((long long)type * g.heads + 2 * pair) * AT_TABLE);
-      for (int i = tid - 128; i < 2 * AT_TABLE * 2 / 16; i += 256) reinterpret_cast<uint4*>(stage)[i] = __ldg(src + i);
-      asm volatile("bar.sync 1, 256;" ::: "memory");   // the 8 softmax warps
-      const int fmask = a.roll ? ((wz == g.nWz - 1 ? 1 : 0) | (wh == g.nWh - 1 ? 2 : 0)) : 0;
-      const __half mask_h = __float2half_rn(a.mask_l2);
-      for (int u = tid - 128; u < 2 * WIN_TOK; u += 256) {      // one (head, query row) per thread
-        const int hd = u / WIN_TOK, i = u % WIN_TOK;
-        const int wi = i % WW, hi = (i / WW) % WH, zi = i / (WW * WH);
-        const int rflag = (zi >= WZ - SZ ? 1 : 0) | (hi >= WH - SH ? 2 : 0);
-        const __half* tab = reinterpret_cast<const __half*>(stage) + hd * AT_TABLE + zi * ((2 * WW - 1) * WH * WH) + hi * (2 * WW - 1) + wi + (WW - 1);
-        uint8_t* dst = bias_s + hd * AT_BIAS_HEAD_B + i * AT_BIAS_LD;
 #pragma unroll 1
-        for (int zh = 0; zh < WZ * WH; ++zh) {                   // key rows (zj, hj): 12 consecutive table entries, descending in wj
-          const int zj = zh / WH, hj = zh % WH;
-          const __half* run = tab + (WZ * zj) * ((2 * WW - 1) * WH * WH) + (WH * hj) * (2 * WW - 1);
-          const int cflag = (zj >= WZ - SZ ? 1 : 0) | (hj >= WH - SH ? 2 : 0);
-          const bool masked = ((rflag ^ cflag) & fmask) != 0;
-          uint32_t v[WW / 2];
+  for (int hd = 0; hd < 2; ++hd) {
+    // ---- S = Q K^T: 16 rows x 144 keys, K = 32 (two k16 steps = the head's four 16-byte chunks) ----
+    uint32_t qa[2][4];
 #pragma unroll
-          for (int wj = 0; wj < WW; wj += 2) {
-            __half t0 = run[-wj], t1 = run[-wj - 1];
-            if (masked) { t0 = __hadd(t0, mask_h); t1 = __hadd(t1, mask_h); }
-            const __half2 h2 = __halves2half2(t0, t1);
-            v[wj / 2] = *reinterpret_cast<const uint32_t*>(&h2);
-          }
-          uint2* d2 = reinterpret_cast<uint2*>(dst + zh * (WW * 2));   // 24 bytes per run: 8-byte aligned
-          d2[0] = make_uint2(v[0], v[1]); d2[1] = make_uint2(v[2], v[3]); d2[2] = make_uint2(v[4], v[5]);
-        }
+    for (int ks = 0; ks < 2; ++ks)
+      ldsm_x4(at_chunk(q_s, 16 * warp + (lane & 7) + 8 * ((lane >> 3) & 1), hd * 4 + 2 * ks + (lane >> 4)), qa[ks]);
+    float s[WIN_TOK / 8][4];
+#pragma unroll
+    for (int j = 0; j < WIN_TOK / 8; ++j) {
+      s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+      uint32_t kb[4];   // keys 8j .. 8j+7: dims 0-7 | 8-15 | 16-23 | 24-31
+      ldsm_x4(at_chunk(k_s, 8 * j + (lane & 7), hd * 4 + (lane >> 3)), kb);
+      mma_16816(s[j], qa[0], kb[0], kb[1]);
+      mma_16816(s[j], qa[1], kb[2], kb[3]);
+    }
+    // ---- scale + bias (+ shift mask), row max ----
+    const __half* tab = tabs + hd * AT_TABLE;
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j = 0; j < WIN_TOK / 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int u = e >> 1, col = 8 * j + c2 + (e & 1);
+        __half bh = tab[rpart[u] + kpart[col]];
+        if ((rflag[u] ^ kflag[col]) & fmask) bh = __hadd(bh, mask_h);
+        s[j][e] = fmaf(s[j][e], a.sl2, __half2float(bh));
+        mx[u] = fmaxf(mx[u], s[j][e]);
       }
     }
-      __syncthreads();
-    // ===================== softmax groups =====================
-    const int grp = (warp - 4) >> 2, q = warp & 3;
-    const uint32_t lane_base = tmem + ((uint32_t)(q * 32) << 16);
-    const uint32_t s_t = lane_base + grp * AT_S_COLS, p_t = lane_base + AT_P_COL0 + grp * AT_P_COLS;
-    const uint32_t o_t = lane_base + AT_O_COL0 + grp * AT_O_COLS;
-    bool have_prev = false, prev_active = false;
-    int prev_kind = 0; long long prev_item = 0; float prev_inv = 0.f;
-#ifdef SKY_EXPERIMENTS
-    long long tacc[8] = {0, 0, 0, 0, 0, 0, 0, 0}, tmark = 0;
-#define AT_T(i) do { if (a.dbg) { const long long _n = clock64(); tacc[i] += _n - tmark; tmark = _n; } } while (0)
-    if (a.dbg) tmark = clock64();
-#else
-#define AT_T(i) do { } while (0)
-#endif
-    // O row of the group's previous tile -> 1/sum -> fp16 -> 64 bytes of the projection's operand image
-    auto epilogue_store = [&](const float (&o)[32]) {
-      const int i = prev_kind < 2 ? q * 32 + lane : 128 + (lane & 15);
-      const int hd = prev_kind < 2 ? prev_kind : (lane >> 4);
-      const int ww = (int)(prev_item % g.nWw), b = (int)((prev_item / g.nWw) % a.B);
-      const long long tok = at_row_token(g, a.roll, b, wz, wh, ww, i);
-      if (tok >= 0) {
-        uint8_t* row = a.att_img + ((size_t)(tok >> 7) * a.att_nkb + pair) * (size_t)G2_A_BYTES + (size_t)(tok & 127) * 128;
-        const uint32_t r7 = (uint32_t)tok & 7u;
-        const uint64_t inv2 = pack_f32x2(prev_inv, prev_inv);
 #pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          uint4 pk;
-          float y[8];
-#pragma unroll
-          for (int e = 0; e < 8; e += 2) unpack_f32x2(mul_f32x2(pack_f32x2(o[8 * c + e], o[8 * c + e + 1]), inv2), y[e], y[e + 1]);
-          pk.x = pack_half2(y[0], y[1]); pk.y = pack_half2(y[2], y[3]);
-          pk.z = pack_half2(y[4], y[5]); pk.w = pack_half2(y[6], y[7]);
-          *reinterpret_cast<uint4*>(row + ((((uint32_t)(hd * 4 + c)) ^ r7) << 4)) = pk;
-        }
-      }
-    };
-    for (int t = grp; t < T; t += 2) {
-      const int it = t / 3, kind = t - 3 * it;
-      const long long item = seg0 + it;
-      const bool active = kind < 2 || q == (int)(item & 3);
-      AT_T(7);
-      AT_WAIT(&s_full[grp], cnt_a[0] & 1);
-      tc_fence_after();
-      AT_T(0);
-      float s[AT_S_COLS];
-      if (active) {
-        __syncwarp();
-        tmem_ld32_nowait(s_t, *reinterpret_cast<float(*)[32]>(s));
-        tmem_ld32_nowait(s_t + 32, *reinterpret_cast<float(*)[32]>(s + 32));
-        tmem_ld32_nowait(s_t + 64, *reinterpret_cast<float(*)[32]>(s + 64));
-        tmem_ld32_nowait(s_t + 96, *reinterpret_cast<float(*)[32]>(s + 96));
-        tmem_ld16_nowait(s_t + 128, s + 128);
-        tmem_ld_wait();
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_taken[grp]);   // the scores are in registers: the group's next tile may be computed now
-      AT_T(1);
-      float inv = 0.f;
-      float mx = -INFINITY;
-      if (active) {
-        const int i = kind < 2 ? q * 32 + lane : 128 + (lane & 15);
-        const int hd = kind < 2 ? kind : (lane >> 4);
-        const uint32_t brow = smem_u32(bias_s) + hd * AT_BIAS_HEAD_B + i * AT_BIAS_LD;
-        const uint64_t sl22 = pack_f32x2(a.sl2, a.sl2);
-#pragma unroll
-        for (int c8 = 0; c8 < 18; ++c8) {
-          const uint4 bb = lds_b128(brow + c8 * 16);
-          const float2 b0 = h2_to_f2(bb.x), b1 = h2_to_f2(bb.y), b2 = h2_to_f2(bb.z), b3 = h2_to_f2(bb.w);
-          float* sp = s + 8 * c8;
-          // packed fp32x2 (FFMA2): one instruction per two scores
-          unpack_f32x2(fma_f32x2(pack_f32x2(sp[0], sp[1]), sl22, pack_f32x2(b0.x, b0.y)), sp[0], sp[1]);
-          unpack_f32x2(fma_f32x2(pack_f32x2(sp[2], sp[3]), sl22, pack_f32x2(b1.x, b1.y)), sp[2], sp[3]);
-          unpack_f32x2(fma_f32x2(pack_f32x2(sp[4], sp[5]), sl22, pack_f32x2(b2.x, b2.y)), sp[4], sp[5]);
-          unpack_f32x2(fma_f32x2(pack_f32x2(sp[6], sp[7]), sl22, pack_f32x2(b3.x, b3.y)), sp[6], sp[7]);
-          mx = fmaxf(mx, fmaxf(fmaxf(fmaxf(sp[0], sp[1]), fmaxf(sp[2], sp[3])), fmaxf(fmaxf(sp[4], sp[5]), fmaxf(sp[6], sp[7]))));
-        }
-      }
-      AT_T(2);
-      // the previous tile's PV product has finished: its O row is complete and the group's P buffer may be rewritten
-      if (have_prev) { AT_WAIT(&o_full[grp], (cnt_a[0] - 1) & 1); tc_fence_after(); }
-      AT_T(3);
-      // fetch the previous tile's O row now: the TMEM read overlaps the exponentials below
-      float o[32];
-      const bool do_epi = have_prev && prev_active;
-      if (do_epi) { __syncwarp(); tmem_ld32_nowait(o_t, o); }
-      if (active) {
-        // P = exp2(s - max) in (0, 1]: un-normalised into the tensor core, 1/sum applied to the 32 outputs of the row
-        uint64_t sum2 = pack_f32x2(0.f, 0.f);
-        const uint64_t nmx2 = pack_f32x2(-mx, -mx);
-        const bool second = kind == 2 && lane >= 16;   // left-over tile: head B's lanes own the second K half
-#pragma unroll
-        for (int c = 0; c < 5; ++c) {
-          uint32_t p[16];
-#pragma unroll
-          for (int k = 0; k < (c < 4 ? 16 : 8); ++k) {
-            float d0, d1, e0, e1;
-            unpack_f32x2(add_f32x2(pack_f32x2(s[32 * c + 2 * k], s[32 * c + 2 * k + 1]), nmx2), d0, d1);
-            e0 = mufu_ex2(d0); e1 = mufu_ex2(d1);
-            sum2 = add_f32x2(sum2, pack_f32x2(e0, e1));
-            p[k] = pack_half2(e0, e1);
-          }
-          if (kind < 2) {
-            if (c < 4) tmem_st16(p_t + 16 * c, p); else tmem_st8(p_t + 64, p);
-          } else {
-            uint32_t pa[16], pb[16];
-#pragma unroll
-            for (int k = 0; k < 16; ++k) { pa[k] = second ? 0u : p[k]; pb[k] = second ? p[k] : 0u; }
-            if (c < 4) { tmem_st16(s_t + 16 * c, pa); tmem_st16(s_t + AT_P_COLS + 16 * c, pb); }
-            else { tmem_st8(s_t + 64, pa); tmem_st8(s_t + AT_P_COLS + 64, pb); }
-          }
-        }
-        { float u0, u1; unpack_f32x2(sum2, u0, u1); inv = 1.f / (u0 + u1); }
-      }
-      AT_T(4);
-      if (do_epi) {
-        tmem_ld_wait();
-        epilogue_store(o);
-      }
-      AT_T(5);
-      tmem_st_wait();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&p_ready[grp]);
-      AT_T(6);
-      ++cnt_a[0];
-      have_prev = true; prev_active = active; prev_kind = kind; prev_item = item; prev_inv = inv;
+    for (int u = 0; u < 2; ++u) {
+      mx[u] = fmaxf(mx[u], __shfl_xor_sync(0xffffffffu, mx[u], 1));
+      mx[u] = fmaxf(mx[u], __shfl_xor_sync(0xffffffffu, mx[u], 2));
     }
-#ifdef SKY_EXPERIMENTS
-    if (a.dbg && lane == 0 && blockIdx.x == 0)
-      for (int i = 0; i < 8; ++i) atomicAdd(reinterpret_cast<unsigned long long*>(a.dbg + (warp - 4) * 8 + i), (unsigned long long)tacc[i]);
-#endif
-    if (have_prev) {
-      AT_WAIT(&o_full[grp], (cnt_a[0] - 1) & 1);
-      tc_fence_after();
-      if (prev_active) {
-        float o[32];
-        __syncwarp();
-        tmem_ld32(o_t, o);
-        epilogue_store(o);
-      }
-    }
-      seg0 = seg1;
-    }
-  } else {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 48;");
-    for (long long seg0 = n_begin; seg0 < n_end;) {
-      AT_SEGMENT_HEAD
-      __syncthreads();                                  // the segment's bias is expanded; V slot 0 is free again
-      if (warp == 0) {
-      // ===================== loader =====================
-      for (int it = 0; it < n_items; ++it) {
-        const uint32_t n = items_done + it, sq = n & 1, sv = n % AT_NV;
-        const long long item = seg0 + it;
-        const int ww = (int)(item % g.nWw), b = (int)((item / g.nWw) % a.B);
-        const uint8_t* src = a.qkv + ((size_t)(((long long)b * g.nWin + (long long)type * g.nWw + ww) * a.pairs + pair)) * AT_TILE_B;
-        mbar_wait(&qk_empty[sq], ((n >> 1) & 1) ^ 1);
-        if (lane == 0) {
-          uint8_t* dq = smem + AT_OFF_Q + sq * AT_QSLOT_B;
-          mbar_arrive_expect_tx(&qk_full[sq], AT_QK_TX);
-          bulk_g2s(dq + AT_Q, src, 128 * 128, &qk_full[sq]);
-          bulk_g2s(dq + AT_L, src + 128 * 128, 2048, &qk_full[sq]);
-          bulk_g2s(smem + AT_OFF_K + sq * AT_TILE_B, src + a.part_stride, AT_TILE_B, &qk_full[sq]);
-        }
-        __syncwarp();
-        mbar_wait(&v_empty[sv], ((n / AT_NV) & 1) ^ 1);
-        if (lane == 0) {
-          mbar_arrive_expect_tx(&v_full[sv], AT_TILE_B);
-          bulk_g2s(smem + AT_OFF_V + sv * AT_TILE_B, src + 2 * a.part_stride, AT_TILE_B, &v_full[sv]);
-        }
-        __syncwarp();
-      }
-      } else if (warp == 1) {
-      // ===================== MMA issuer =====================
-      constexpr uint32_t idesc_s = make_idesc_f16(128, AT_S_COLS);
-      constexpr uint32_t idesc_o = make_idesc_f16_bmn(128, 32);
-      const uint32_t smem0 = smem_u32(smem);
-      int qk_issued[2] = {0, 0};   // QK^T products issued per Q+K slot: the slot is released after the third (issue order is
-                                   // 3i, 3i+2, 3i+1: tile 3i+1 waits for the PV product of the previous left-over tile)
-      auto issue_scores = [&](int t) {
-        const int it = t / 3, kind = t - 3 * it, grp = t & 1;
-        const uint32_t n = items_done + it, sq = n & 1;
-        if (kind == 0) { AT_WAIT(&qk_full[sq], (n >> 1) & 1); tc_fence_after(); }
-        const bool last_qk = ++qk_issued[sq] == 3;
-        if (last_qk) qk_issued[sq] = 0;
-        const uint32_t qb = smem0 + AT_OFF_Q + sq * AT_QSLOT_B;
-        const uint32_t d = tmem + grp * AT_S_COLS;
-        const uint64_t dk = make_desc_sw128(smem0 + AT_OFF_K + sq * AT_TILE_B);
-        if (kind < 2) {
-          const uint64_t dq = make_desc_sw128(qb + AT_Q) + 4 * kind;   // head B = k-steps 2, 3 of the 64-wide row (+64 B)
-          if (elect_one()) {
-            tc_mma_f16(d, dq, dk + 4 * kind, idesc_s, 0u);
-            tc_mma_f16(d, dq + 2, dk + 4 * kind + 2, idesc_s, 1u);
-            tc_commit(&s_full[grp]);
-            if (last_qk) tc_commit(&qk_empty[sq]);   // Q and K may be refilled once the item's QK^T products complete
-          }
-        } else {
-          // left-over rows of both heads into lanes 32q .. 32q+31:  [head A rows | zeros] x K_A  +  [zeros | head B rows] x K_B
-          const uint32_t q = (uint32_t)((seg0 + it) & 3);
-          const uint64_t dlo = make_desc_sw128(qb + AT_L - q * 4096), dhi = make_desc_sw128(qb + AT_Z0 - q * 4096);
-          if (elect_one()) {
-            tc_mma_f16(d, dlo, dk, idesc_s, 0u);
-            tc_mma_f16(d, dlo + 2, dk + 2, idesc_s, 1u);
-            tc_mma_f16(d, dhi + 4, dk + 4, idesc_s, 1u);
-            tc_mma_f16(d, dhi + 6, dk + 6, idesc_s, 1u);
-            tc_commit(&s_full[grp]);
-            if (last_qk) tc_commit(&qk_empty[sq]);
-          }
-        }
-        __syncwarp();
-      };
-      auto issue_pv = [&](int t) {
-        const int it = t / 3, kind = t - 3 * it, grp = t & 1;
-        const uint32_t n = items_done + it, sv = n % AT_NV;
-        if (kind == 0) { AT_WAIT(&v_full[sv], (n / AT_NV) & 1); tc_fence_after(); }
-        const uint32_t o = tmem + AT_O_COL0 + grp * AT_O_COLS;
-        const uint64_t dv = make_desc_sw128(smem0 + AT_OFF_V + sv * AT_TILE_B);
-        if (kind < 2) {
-          const uint32_t pa = tmem + AT_P_COL0 + grp * AT_P_COLS;
-          const uint64_t dvh = dv + (kind == 1 ? 4 : 0);            // head B's dims start 64 B into the row
-          if (elect_one()) {
+    // ---- P = exp2(s - max) in (0, 1]: fp16 into the tensor core, fp32 row sums ----
+    uint32_t p[WIN_TOK / 8][2];
+    float sum[2] = {0.f, 0.f};
 #pragma unroll
-            for (int ks = 0; ks < 9; ++ks)    // 16 keys per step: 8 TMEM columns of P, 16 rows (2048 B) of V
-              tc_mma_f16_ts(o, pa + 8 * ks, dvh + 128 * ks, idesc_o, ks != 0 ? 1u : 0u);
-            tc_commit(&o_full[grp]);
-          }
-        } else {
-          const uint32_t pa = tmem + grp * AT_S_COLS;               // [P_A | 0] / [0 | P_B] in place over the scores: K = 288
-          if (elect_one()) {
-#pragma unroll
-            for (int ks = 0; ks < 18; ++ks)
-              tc_mma_f16_ts(o, pa + 8 * ks, dv + (ks >= 9 ? 4 : 0) + 128 * (ks % 9), idesc_o, ks != 0 ? 1u : 0u);
-            tc_commit(&o_full[grp]);
-            tc_commit(&v_empty[sv]);           // the item's last PV product
-          }
-        }
-        __syncwarp();
-      };
-      issue_scores(0);
-      issue_scores(1);
-      int deferred = -1;
-      for (int t = 0; t < T; ++t) {
-        const int grp = t & 1;
-        AT_WAIT(&s_taken[grp], cnt_a[grp] & 1);
-        ++cnt_a[grp];
-        tc_fence_after();
-        if (t + 2 < T) {
-          if (t % 3 == 2) deferred = t + 2;    // a left-over tile keeps P in its S buffer until its PV product is issued
-          else issue_scores(t + 2);
-        }
-        if (t >= 1) {
-          AT_WAIT(&p_ready[grp ^ 1], cnt_b[grp ^ 1] & 1);
-          ++cnt_b[grp ^ 1];
-          tc_fence_after();
-          issue_pv(t - 1);
-          if (deferred == t + 1) { issue_scores(t + 1); deferred = -1; }
-        }
-      }
-      {
-        const int grp = (T - 1) & 1;
-        AT_WAIT(&p_ready[grp], cnt_b[grp] & 1);
-        ++cnt_b[grp];
-        tc_fence_after();
-        issue_pv(T - 1);
-      }
-      }
-      items_done += (uint32_t)n_items;
-      seg0 = seg1;
+    for (int j = 0; j < WIN_TOK / 8; ++j) {
+      const float e0 = mufu_ex2(s[j][0] - mx[0]), e1 = mufu_ex2(s[j][1] - mx[0]);
+      const float e2 = mufu_ex2(s[j][2] - mx[1]), e3 = mufu_ex2(s[j][3] - mx[1]);
+      sum[0] += e0 + e1; sum[1] += e2 + e3;
+      p[j][0] = pack_half2(e0, e1); p[j][1] = pack_half2(e2, e3);
     }
-  }
-#undef AT_SEGMENT_HEAD
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 1) {
-    __syncwarp();
-    tmem_dealloc<512>(tmem);
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      sum[u] += __shfl_xor_sync(0xffffffffu, sum[u], 1);
+      sum[u] += __shfl_xor_sync(0xffffffffu, sum[u], 2);
+    }
+    // ---- O = P V: K = 144 keys (nine k16 steps), N = 32 dims (four n8 fragments) ----
+    float o[4][4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) o[c][0] = o[c][1] = o[c][2] = o[c][3] = 0.f;
+#pragma unroll
+    for (int t = 0; t < WIN_TOK / 16; ++t) {
+      const uint32_t pa[4] = {p[2 * t][0], p[2 * t][1], p[2 * t + 1][0], p[2 * t + 1][1]};
+      uint32_t v0[4], v1[4];   // keys 16t .. 16t+7 | 16t+8 .. 16t+15, dims 8c .. 8c+7 in register c
+      ldsm_x4_t(at_chunk(v_s, 16 * t + (lane & 7), hd * 4 + (lane >> 3)), v0);
+      ldsm_x4_t(at_chunk(v_s, 16 * t + 8 + (lane & 7), hd * 4 + (lane >> 3)), v1);
+#pragma unroll
+      for (int c = 0; c < 4; ++c) mma_16816(o[c], pa, v0[c], v1[c]);
+    }
+    // ---- 1/sum -> fp16 -> 64 bytes of the projection's operand image per row ----
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const long long tok = at_row_token(g, a.roll, b, wz, wh, ww, row[u]);
+      if (tok < 0) continue;
+      const float inv = 1.f / sum[u];
+      uint8_t* dst = a.att_img + ((size_t)(tok >> 7) * a.att_nkb + pair) * (size_t)G2_A_BYTES + (size_t)(tok & 127) * 128;
+      const uint32_t r7 = (uint32_t)tok & 7u;
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        *reinterpret_cast<uint32_t*>(dst + ((((uint32_t)(hd * 4 + c)) ^ r7) << 4) + 2 * c2) =
+            pack_half2(o[c][2 * u] * inv, o[c][2 * u + 1] * inv);
+    }
   }
 }
 
 #ifdef SKY_EXPERIMENTS
 // CUDA-core reference of the same operator on the same window image (development library, SKY_ATTN=ref): one thread
-// per query row, fp32 scores, bias gathered from the compact table (independent of the expansion above).  Bisects
-// "window image / index arithmetic" from "tensor pipeline" failures; never benchmarked.
+// per query row, fp32 scores, bias gathered from the compact table.  Bisects "window image / index arithmetic" from
+// "tensor pipeline" failures; never benchmarked.
 __global__ void __launch_bounds__(WIN_TOK) k_window_attention_ref(const AttnArgs a) {
   const Geo& g = a.g;
   const long long item = blockIdx.x;
@@ -709,30 +355,13 @@ __global__ void __launch_bounds__(WIN_TOK) k_window_attention_ref(const AttnArgs
 }
 #endif
 
-inline int launch_window_attention_tc(const AttnArgs& a_in, int num_sms, cudaStream_t st) {
-  AttnArgs a = a_in;
-#ifdef SKY_EXPERIMENTS
-  static long long* dbg = nullptr;
-  static int dbg_runs = 0;
-  if (getenv("SKY_ATTN_DBG") && !dbg) cudaMallocManaged(&dbg, 8 * 8 * 8);
-  if (dbg && dbg_runs < 16) { memset(dbg, 0, 8 * 8 * 8); a.dbg = dbg; }
-#endif
+inline int launch_window_attention_tc(const AttnArgs& a, int num_sms, cudaStream_t st) {
+  (void)num_sms;
   static std::atomic<uint64_t> configured{0};
   if (int rc = smem_opt_in(configured, reinterpret_cast<const void*>(k_window_attention_tc), AT_SMEM_BYTES)) return rc;
-  const long long grid = a.items < num_sms ? a.items : num_sms;
-  k_window_attention_tc<<<(unsigned)grid, AT_THREADS, AT_SMEM_BYTES, st>>>(a);
+  if (a.items <= 0) return 0;
+  k_window_attention_tc<<<(unsigned)a.items, AT_THREADS, AT_SMEM_BYTES, st>>>(a);
   SKY_CUDA_OK(cudaGetLastError());
-#ifdef SKY_EXPERIMENTS
-  if (dbg && dbg_runs < 16) {
-    ++dbg_runs;
-    cudaDeviceSynchronize();
-    for (int w = 0; w < 8; w += 4) {   // one warp of each group (CTA 0): cycles per phase over the launch
-      const long long* t = dbg + w * 8;
-      printf("[attn C=%d grp %d cta0] wait_s %lld  ld_S %lld  bias+max %lld  wait_o %lld  exp+P %lld  epilogue %lld  st_wait+arrive %lld  loop %lld\n",
-             a.g.C, w / 4, t[0], t[1], t[2], t[3], t[4], t[5], t[6], t[7]);
-    }
-  }
-#endif
   return 0;
 }
 

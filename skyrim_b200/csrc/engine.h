@@ -31,7 +31,7 @@ struct ParamView {
 // Base class of a step operator bound to one device.
 struct Engine {
   int device = 0;
-  int num_sms = 148;
+  int num_sms = 132;
   float* arena = nullptr;  // fp32 copy of the weight arena: alive during load_arena() only (freed after repacking)
   uint64_t arena_floats = 0;
   std::map<std::string, ParamView> params;

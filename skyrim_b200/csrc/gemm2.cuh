@@ -1,4 +1,4 @@
-// TMA-fed persistent tcgen05 GEMM (v2 data flow):
+// TMA-fed persistent wgmma GEMM (v2 data flow):
 //
 //   D[M, N] = A[M, K] * W[N, K]^T -> fused epilogue
 //
@@ -7,13 +7,17 @@
 //   A image  [ceil(M/128)][K/64][128 rows x 128 B]   fp16 activations, written in this layout
 //                                                     by the epilogue of the producing kernel
 //   W image  [N/BLOCK_N][K/64][BLOCK_N rows x 128 B]  packed once at weight load
-// so no warp ever touches the operands with ld/st.  Warp roles: 0..EPI_WARPS-1 epilogue
-// (warp%4 selects the TMEM lane quarter, warp/4 the column partition), then one loader warp
-// and one MMA warp.  Epilogues re-tile their 32x32 accumulator blocks through a padded smem
-// patch so that every global access is a full 64/128-byte row segment (the v1 row-per-lane
-// epilogue was L1-wavefront and latency bound: profiles/r1_gemm_v1.md).
+// so no warp ever touches the operands with ld/st.  Warp roles: 0..7 = two consumer warpgroups,
+// 8 = loader.  Warpgroup g issues the wgmma products of rows 64g .. 64g+63 of the 128-row tile
+// over all BLOCK_N columns (fp32 accumulators in registers, BLOCK_N / 2 per thread).  At the end of
+// a tile both warpgroups stage their accumulators in shared memory — over the operand ring, which
+// is drained by then — and the same eight warps run the row-owner epilogue on the staged tile
+// (warp%4 selects the 32-row quarter, warp/4 the column partition).  Epilogues re-tile their 32x32
+// accumulator blocks through a padded smem patch so that every global access is a full
+// 64/128-byte row segment.
 #pragma once
 #include "pangu_ops.cuh"
+#include "wgmma_ops.cuh"
 
 namespace sky {
 
@@ -50,8 +54,6 @@ struct AImage {
 
 template <int BLOCK_N, int EPI_WARPS>
 struct G2Cfg {
-  static constexpr int N_INST = BLOCK_N <= 256 ? BLOCK_N : BLOCK_N / 2;
-  static constexpr int N_SPLIT = BLOCK_N / N_INST;
   static constexpr int B_BYTES = BLOCK_N * 128;
   static constexpr int STAGE_BYTES = G2_A_BYTES + B_BYTES;
   static constexpr int PATCH_BYTES = EPI_WARPS * G2_PATCH_FLOATS * 4;
@@ -59,15 +61,17 @@ struct G2Cfg {
   static constexpr int FIXED = 1024 /*align*/ + 256 /*barriers*/ + PATCH_BYTES + VEC_BYTES;
   static constexpr int MAXS = (232448 - FIXED) / STAGE_BYTES;
   static constexpr int STAGES = MAXS > 6 ? 6 : MAXS;
-  static constexpr int NBUF = 2 * BLOCK_N <= 512 ? 2 : 1;
-  static constexpr int COLS = NBUF * BLOCK_N;
-  static constexpr int TMEM_COLS = COLS <= 32 ? 32 : COLS <= 64 ? 64 : COLS <= 128 ? 128 : COLS <= 256 ? 256 : 512;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + FIXED;
-  static constexpr int THREADS = (EPI_WARPS + 2) * 32;
-  static_assert(N_INST % 16 == 0 && N_INST <= 256, "UMMA shape");
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+  // accumulator staging over the drained ring: all 128 rows when they fit, else 64 rows (one warpgroup) at a time
+  static constexpr int STG_LD = (BLOCK_N + 31) / 32 * 32 + 4;
+  static constexpr int STG_ROWS = 128 * STG_LD * 4 <= RING_BYTES ? 128 : 64;
+  static constexpr int SMEM_BYTES = RING_BYTES + FIXED;
+  static constexpr int THREADS = (EPI_WARPS + 1) * 32;
+  static_assert(BLOCK_N % 8 == 0 && BLOCK_N <= 384, "wgmma N, accumulator registers");
   static_assert(STAGE_BYTES % 1024 == 0, "stage alignment");
   static_assert(STAGES >= 2, "pipeline depth");
-  static_assert(EPI_WARPS == 4 || EPI_WARPS == 8, "epilogue warps");
+  static_assert(STG_ROWS * STG_LD * 4 <= RING_BYTES, "accumulator staging");
+  static_assert(EPI_WARPS == 8, "two consumer warpgroups");
 };
 
 struct EpiCtx {
@@ -91,53 +95,136 @@ struct EpiCtx {
   uint32_t x_parity = 0;
 };
 
-struct AccTmem2 {
-  uint32_t taddr;
-  __device__ void load32(int c, float (&v)[32]) const { tmem_ld32(taddr + (uint32_t)c, v); }
+// ---------------------------------------------------------------------------------------------------------------
+// consumer side shared by the wgmma GEMM kernels
+// ---------------------------------------------------------------------------------------------------------------
+// Accumulators of warpgroup wg: rows 64 wg .. 64 wg + 63 of the 128-row tile, all BN columns (N > 256: two products of N/2).
+template <int BN, bool kBMN = false>
+struct WgAcc {
+  static constexpr int NI = BN <= 256 ? BN : BN / 2;
+  static constexpr int NS = BN / NI;
+  float d[NS][NI / 2];
+  // zeroed at the start of every tile (rather than a scale-d = 0 first product): the registers are then dead between the
+  // staging of one tile and the main loop of the next, i.e. free for the epilogue
+  __device__ __forceinline__ void zero() {
+#pragma unroll
+    for (int ni = 0; ni < NS; ++ni)
+#pragma unroll
+      for (int i = 0; i < NI / 2; ++i) d[ni][i] = 0.f;
+  }
+  // one k-block: A = 128 rows x 64 halves at a_addr; B = BN rows x 64 halves, K-major, at b_addr, or (kBMN) 64 k-rows x BN
+  // columns in 64-column atoms 8 KB apart
+  __device__ __forceinline__ void kblock(uint32_t a_addr, uint32_t b_addr, int wg) {
+    wgmma_fence();
+    const uint64_t da = make_desc_sw128(a_addr + (uint32_t)wg * 8192u);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+#pragma unroll
+      for (int ni = 0; ni < NS; ++ni) {
+        const uint64_t db = kBMN ? make_desc_sw128_mn(b_addr, 8192) + (uint64_t)(k * (2048 >> 4))
+                                 : make_desc_sw128(b_addr + (uint32_t)(ni * NI * 128)) + (uint64_t)(2 * k);
+        Wgmma<NI, kBMN>::mma(d[ni], da + 2 * k, db);
+      }
+    }
+    wgmma_commit();
+  }
+  __device__ __forceinline__ void settle() {
+    wgmma_wait<0>();
+#pragma unroll
+    for (int ni = 0; ni < NS; ++ni) wgmma_fence_operands(d[ni]);
+  }
+  // fragment -> staging (row-major, ld floats per row); row_off = first row of this warpgroup minus the staging's first row
+  __device__ __forceinline__ void dump(uint32_t stg_s, int ld, int row_off) const {
+    const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
+    const uint32_t r = (uint32_t)(16 * w + (l >> 2) + row_off);
+    const uint32_t a0 = stg_s + (r * (uint32_t)ld + 2u * (uint32_t)(l & 3)) * 4u, a8 = a0 + 8u * (uint32_t)ld * 4u;
+#pragma unroll
+    for (int ni = 0; ni < NS; ++ni) {
+#pragma unroll
+      for (int i = 0; i < NI / 8; ++i) {
+        const uint32_t o = (uint32_t)(ni * NI + 8 * i) * 4u;
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a0 + o), "f"(d[ni][4 * i]), "f"(d[ni][4 * i + 1]) : "memory");
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a8 + o), "f"(d[ni][4 * i + 2]), "f"(d[ni][4 * i + 3]) : "memory");
+      }
+    }
+  }
 };
 
+// Main loop of one tile over the stage ring (stage = A tile | B tile).  One wgmma group stays in flight: the stage of
+// k-block kb - 1 is released once the products of kb are issued.  empty[] counts the eight consumer warps.
+template <int STAGES, int STAGE_BYTES, class Acc>
+__device__ __forceinline__ void wg_mainloop(Acc& acc, uint8_t* smem, uint64_t* full, uint64_t* empty, int& s, uint32_t& ph,
+                                            int num_kb, int wg, int lane) {
+  int prev = -1;
+  acc.zero();
+  for (int kb = 0; kb < num_kb; ++kb) {
+    mbar_wait(&full[s], ph);
+    const uint32_t a = smem_u32(smem + s * STAGE_BYTES);
+    acc.kblock(a, a + G2_A_BYTES, wg);
+    wgmma_wait<1>();
+    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
+    prev = s;
+    if (++s == STAGES) { s = 0; ph ^= 1; }
+  }
+  acc.settle();
+  if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
+}
+
+// Stage the accumulators at the base of the (drained) ring and run fn(AccSmem) in every consumer warp whose 32-row quarter
+// (warp % 4) is staged; STG_ROWS = 64 stages and finishes one warpgroup's rows at a time.  The caller signals the loader
+// afterwards (the ring is free again).
+template <int STG_ROWS, class Acc, class Fn>
+__device__ __forceinline__ void wg_epilogue(const Acc& acc, uint8_t* smem, int ld, int wg, int warp, int lane, Fn&& fn) {
+  const uint32_t stg = smem_u32(smem);
+  const int q = warp & 3;
+  named_bar_sync(1, 256);   // both warpgroups' products have completed: no wgmma still reads the ring the staging overwrites
+#pragma unroll 1
+  for (int h = 0; h < 128 / STG_ROWS; ++h) {
+    if (STG_ROWS == 128 || wg == h) acc.dump(stg, ld, 64 * wg - h * STG_ROWS);
+    named_bar_sync(1, 256);
+    if (q * 32 >= h * STG_ROWS && q * 32 < (h + 1) * STG_ROWS)
+      fn(AccSmem{stg + (uint32_t)((q * 32 + lane - h * STG_ROWS) * ld) * 4u});
+    named_bar_sync(1, 256);
+  }
+  fence_proxy_async_smem();   // the staging's generic accesses are ordered before the next bulk copies into the ring
+}
+
 template <class Epi, int BLOCK_N, int EPI_WARPS>
-__global__ void __launch_bounds__((EPI_WARPS + 2) * 32, 1)
+__global__ void __launch_bounds__((EPI_WARPS + 1) * 32, 1)
 k_gemm2(const AImage A, const Epi epi, const uint8_t* __restrict__ Wimg, long long M, int num_kb,
         int num_m_tiles, int num_n_tiles) {
   using Cfg = G2Cfg<BLOCK_N, EPI_WARPS>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* patches = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+  float* patches = reinterpret_cast<float*>(smem + Cfg::RING_BYTES);
   float* sbias = patches + EPI_WARPS * G2_PATCH_FLOATS;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sbias + 3 * 512);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::STAGES;
-  uint64_t* tmem_full = bars + 2 * Cfg::STAGES;
-  uint64_t* tmem_empty = bars + 2 * Cfg::STAGES + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::STAGES + 4);
+  uint64_t* stg_free = bars + 2 * Cfg::STAGES;   // consumers -> loader: the tile's epilogue has left the ring
 
-  // warp index through a shuffle: provably warp-uniform, so the role branches are uniform control flow and the
-  // issuer's descriptor arithmetic runs on the uniform datapath (no per-MMA R2UR/ELECT waterfall)
+  // warp index through a shuffle: provably warp-uniform, so the role branches are uniform control flow
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0), lane = threadIdx.x % 32;
   const int num_tiles = num_m_tiles * num_n_tiles;
-  constexpr int LOADER = EPI_WARPS, MMAW = EPI_WARPS + 1;
+  constexpr int LOADER = EPI_WARPS;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], EPI_WARPS); }
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], EPI_WARPS); }
+    mbar_init(stg_free, EPI_WARPS);
     mbar_fence_init();
   }
-  if (warp == MMAW) tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
   if constexpr (Epi::kNeedsBias) if (threadIdx.x < EPI_WARPS * 32)
     for (int i = threadIdx.x; i < BLOCK_N; i += EPI_WARPS * 32) {
       sbias[i] = epi.bias[i]; sbias[512 + i] = epi.gamma[i]; sbias[1024 + i] = epi.beta[i];
     }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp == LOADER) {
-    int s = 0; uint32_t ph = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int s = 0; uint32_t ph = 0; int it = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
       const int mt = tile / num_n_tiles, nt = tile % num_n_tiles;
       const uint8_t* wsrc = Wimg + (size_t)nt * num_kb * Cfg::B_BYTES;
+      if (it > 0) mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&empty[s], ph ^ 1);
         if (lane == 0) {
@@ -150,68 +237,25 @@ k_gemm2(const AImage A, const Epi epi, const uint8_t* __restrict__ Wimg, long lo
         if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == MMAW) {
-    constexpr uint32_t idesc = make_idesc_f16(G2_BLOCK_M, Cfg::N_INST);
-    int s = 0; uint32_t ph = 0; int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int buf = it % Cfg::NBUF;
-      const uint32_t use = (uint32_t)(it / Cfg::NBUF);
-      mbar_wait(&tmem_empty[buf], (use & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BLOCK_N);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        {
-          const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES);
-          const uint64_t da = make_desc_sw128(a_addr);                 // +2 in the address field = +32 B = one K=16 step
-          const uint64_t db = make_desc_sw128(a_addr + G2_A_BYTES);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-#pragma unroll
-              for (int ni = 0; ni < Cfg::N_SPLIT; ++ni)
-                tc_mma_f16(d_tmem + ni * Cfg::N_INST, da + 2 * k, db + (uint64_t)(ni * Cfg::N_INST * 8 + 2 * k), idesc,
-                           (kb | k) != 0 ? 1u : 0u);
-            }
-            tc_commit(&empty[s]);
-            if (kb == num_kb - 1) tc_commit(&tmem_full[buf]);
-          }
-        }
-        __syncwarp();
-        if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
-      }
-    }
   } else {
-    // ---------------- epilogue warps ----------------
-    const int q = warp & 3, part = warp >> 2;
+    // ---------------- consumer warpgroups: MMA, then epilogue ----------------
+    const int q = warp & 3, part = warp >> 2, wg = warp >> 2;
     EpiCtx ctx;
     ctx.M = M; ctx.lane = lane; ctx.part = part; ctx.nparts = EPI_WARPS / 4;
     ctx.patch = patches + warp * G2_PATCH_FLOATS;
     ctx.patch_s = smem_u32(ctx.patch);
     ctx.svec_s = smem_u32(sbias);
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int buf = it % Cfg::NBUF;
-      const uint32_t use = (uint32_t)(it / Cfg::NBUF);
+    WgAcc<BLOCK_N> acc;
+    int s = 0; uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       ctx.row0 = (long long)(tile / num_n_tiles) * G2_BLOCK_M + q * 32;
       ctx.n0 = (tile % num_n_tiles) * BLOCK_N;
       if constexpr (Epi::kNeedsBias) epi.template prefetch<BLOCK_N>(ctx);  // LN + residual epilogues
-      mbar_wait(&tmem_full[buf], use & 1);
-      tc_fence_after();
-      AccTmem2 acc{tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BLOCK_N)};
-      epi.template run<BLOCK_N>(acc, ctx);
-      tc_fence_before();
+      wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, num_kb, wg, lane);
+      wg_epilogue<Cfg::STG_ROWS>(acc, smem, Cfg::STG_LD, wg, warp, lane, [&](AccSmem a) { epi.template run<BLOCK_N>(a, ctx); });
       __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[buf]);
+      if (lane == 0) mbar_arrive(stg_free);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == MMAW) {
-    __syncwarp();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
   }
 }
 
@@ -290,7 +334,7 @@ struct Epi2F16 {
     const int rsub = x.lane >> 2, ch = x.lane & 3;
     const uint32_t r0 = (uint32_t)(x.row0 & 127);
     for (int c = x.part * 32; c < BN; c += 32 * x.nparts) {
-      // this lane's 8 output columns are the same for all its rows: their bias is loaded once, ahead of the TMEM read
+      // this lane's 8 output columns are the same for all its rows: their bias is loaded once, ahead of the accumulator read
       const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + x.n0 + c + ch * 8));
       const float4 b1 = __ldg(reinterpret_cast<const float4*>(bias + x.n0 + c + ch * 8 + 4));
       {
@@ -361,9 +405,7 @@ struct Epi2F32Img {
 #else
   static constexpr int exp = 0;
 #endif
-  // Pull this warp's residual rows into L2 ahead of time.  A register-destination prefetch does
-  // not work here: tcgen05.wait::ld also waits for the thread's outstanding global loads, so
-  // every TMEM read in run() would expose the full HBM latency (profiles/r1_mlp.md).
+  // Pull this warp's residual rows into L2 ahead of time, while the tile's main loop runs.
   // four residual values of row (row0 + rr) at tile column n0 + c + 4 * c4, read from the fp16 image
   __device__ __forceinline__ uint2 img_res_raw(const EpiCtx& e, int rr, int c, int c4) const {
     const int col = e.n0 + c + c4 * 4;
@@ -397,8 +439,7 @@ struct Epi2F32Img {
   // fp16 image chunks (8 columns = 16 bytes) are assembled from lane pairs by shuffle, not through
   // shared memory.  Every warp reduces the statistics of its own column groups only; the warps that
   // share a lane quarter exchange partial sums through their patches.
-  // kPrefetch: load the residual of the next column group while this one is processed (32 more registers; kernels
-  // with 16 epilogue warps hide the latency with occupancy instead)
+  // kPrefetch: load the residual of the next column group while this one is processed (32 more registers)
   template <int BN, bool kPrefetch = true, class Acc>
   __device__ void run(Acc& acc, const EpiCtx& e) const {
     constexpr int NG = BN / 32;

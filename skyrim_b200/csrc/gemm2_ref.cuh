@@ -1,6 +1,6 @@
 // CUDA-core twin of gemm2.cuh (same image operands, same epilogue functors).
 // DEVICE-SIDE TEST INFRASTRUCTURE: SKY_GEMM=ref runs the step on these to bisect a parity
-// failure between "epilogue / index arithmetic" and "TMA + tcgen05 pipeline".  Never the
+// failure between "epilogue / index arithmetic" and "TMA + wgmma pipeline".  Never the
 // benchmarked path.
 #pragma once
 #include "gemm2.cuh"

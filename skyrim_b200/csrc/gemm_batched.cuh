@@ -1,4 +1,4 @@
-// Batched, K-segmented variant of the TMA-fed tcgen05 GEMM (gemm2.cuh), used by the SFNO path:
+// Batched, K-segmented variant of the TMA-fed wgmma GEMM (gemm2.cuh), used by the SFNO path:
 //
 //   for b in batches:  D_b[M, N] = A_b[M, Ktot] * W_b[N, Ktot]^T      -> fused epilogue
 //
@@ -63,47 +63,41 @@ __device__ __forceinline__ void cta_stats_flush(const Epi& epi, const float* sbi
 }
 
 template <class Epi, int BLOCK_N, int EPI_WARPS>
-__global__ void __launch_bounds__((EPI_WARPS + 2) * 32, 1)
+__global__ void __launch_bounds__((EPI_WARPS + 1) * 32, 1)
 k_gemm_batched(const AOperand A, const Epi epi, const uint8_t* __restrict__ Wimg, long long w_batch_stride,
                long long M, int num_kb, int num_m_tiles, int num_n_tiles, int batches) {
   using Cfg = G2Cfg<BLOCK_N, EPI_WARPS>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* patches = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+  float* patches = reinterpret_cast<float*>(smem + Cfg::RING_BYTES);
   float* sbias = patches + EPI_WARPS * G2_PATCH_FLOATS;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sbias + 3 * 512);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::STAGES;
-  uint64_t* tmem_full = bars + 2 * Cfg::STAGES;
-  uint64_t* tmem_empty = bars + 2 * Cfg::STAGES + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::STAGES + 4);
+  uint64_t* stg_free = bars + 2 * Cfg::STAGES;
 
-  // warp index through a shuffle: provably warp-uniform, so the role branches are uniform control flow and the
-  // issuer's descriptor arithmetic runs on the uniform datapath (no per-MMA R2UR/ELECT waterfall)
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0), lane = threadIdx.x % 32;
   const int tiles_per_batch = num_m_tiles * num_n_tiles;
   const long long num_tiles = (long long)tiles_per_batch * batches;
-  constexpr int LOADER = EPI_WARPS, MMAW = EPI_WARPS + 1;
+  constexpr int LOADER = EPI_WARPS;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], EPI_WARPS); }
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], EPI_WARPS); }
+    mbar_init(stg_free, EPI_WARPS);
     mbar_fence_init();
   }
-  if (warp == MMAW) tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
   if constexpr (has_cta_stats<Epi>::value)
     for (int i = threadIdx.x; i < 3 * 512; i += blockDim.x) sbias[i] = 0.f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp == LOADER) {
-    int s = 0; uint32_t ph = 0;
+    int s = 0; uint32_t ph = 0; int it = 0;
     for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int b = (int)(tile / tiles_per_batch), t = (int)(tile % tiles_per_batch);
       const int mt = t / num_n_tiles, nt = t % num_n_tiles;
       if (A.tri && mt * G2_BLOCK_M > b) continue;
+      if (it > 0) mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
+      ++it;
       // W image = [hi | lo] (nkw k-blocks each), consumed as hi, hi, lo against A = hi, lo, hi
       const int nkw = num_kb / 3;
       const uint8_t* wsrc = Wimg + (size_t)b * w_batch_stride + (size_t)nt * (2 * nkw) * Cfg::B_BYTES;
@@ -119,74 +113,29 @@ k_gemm_batched(const AOperand A, const Epi epi, const uint8_t* __restrict__ Wimg
         if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == MMAW) {
-    constexpr uint32_t idesc = make_idesc_f16(G2_BLOCK_M, Cfg::N_INST);
-    int s = 0; uint32_t ph = 0; int it = 0;
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      if (A.tri && (int)((tile % tiles_per_batch) / num_n_tiles) * G2_BLOCK_M > (int)(tile / tiles_per_batch)) continue;
-      const int buf = it % Cfg::NBUF;
-      const uint32_t use = (uint32_t)(it / Cfg::NBUF);
-      ++it;
-      mbar_wait(&tmem_empty[buf], (use & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BLOCK_N);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        {
-          const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES);
-          const uint64_t da = make_desc_sw128(a_addr);                 // +2 in the address field = +32 B = one K=16 step
-          const uint64_t db = make_desc_sw128(a_addr + G2_A_BYTES);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-#pragma unroll
-              for (int ni = 0; ni < Cfg::N_SPLIT; ++ni)
-                tc_mma_f16(d_tmem + ni * Cfg::N_INST, da + 2 * k, db + (uint64_t)(ni * Cfg::N_INST * 8 + 2 * k), idesc,
-                           (kb | k) != 0 ? 1u : 0u);
-            }
-            tc_commit(&empty[s]);
-            if (kb == num_kb - 1) tc_commit(&tmem_full[buf]);
-          }
-        }
-        __syncwarp();
-        if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
-      }
-    }
   } else {
-    const int q = warp & 3, part = warp >> 2;
+    const int q = warp & 3, part = warp >> 2, wg = warp >> 2;
     EpiCtxB ctx;
     ctx.M = M; ctx.lane = lane; ctx.part = part; ctx.nparts = EPI_WARPS / 4;
     ctx.patch = patches + warp * G2_PATCH_FLOATS;
     ctx.patch_s = smem_u32(ctx.patch);
     ctx.svec_s = smem_u32(sbias);
-    int it = 0;
+    WgAcc<BLOCK_N> acc;
+    int s = 0; uint32_t ph = 0;
     for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int b = (int)(tile / tiles_per_batch), t = (int)(tile % tiles_per_batch);
       if (A.tri && (t / num_n_tiles) * G2_BLOCK_M > b) continue;
-      const int buf = it % Cfg::NBUF;
-      const uint32_t use = (uint32_t)(it / Cfg::NBUF);
-      ++it;
       ctx.batch = b;
       ctx.row0 = (long long)(t / num_n_tiles) * G2_BLOCK_M + q * 32;
       ctx.n0 = (t % num_n_tiles) * BLOCK_N;
-      mbar_wait(&tmem_full[buf], use & 1);
-      tc_fence_after();
-      AccTmem2 acc{tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BLOCK_N)};
-      epi.template run<BLOCK_N>(acc, ctx);
-      tc_fence_before();
+      wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, num_kb, wg, lane);
+      wg_epilogue<Cfg::STG_ROWS>(acc, smem, Cfg::STG_LD, wg, warp, lane, [&](AccSmem a) { epi.template run<BLOCK_N>(a, ctx); });
       __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[buf]);
+      if (lane == 0) mbar_arrive(stg_free);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   cta_stats_flush(epi, sbias);
-  if (warp == MMAW) {
-    __syncwarp();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
 }
 
 template <class Epi, int BLOCK_N, int EPI_WARPS>
@@ -224,7 +173,7 @@ struct EpiF32Batched {
     const float* ap = add ? add + (size_t)e.batch * batch_stride + e.row0 * ldo + e.n0 + c4 * 4 : nullptr;
     for (int c = e.part * 32; c < BN; c += step) {
       const int col = e.n0 + c + c4 * 4;
-      // BN need not be a multiple of 32 (16, 80, 240): the 32-column TMEM read then runs past the tile; those columns
+      // BN need not be a multiple of 32 (16, 80, 240): the 32-column accumulator read then runs past the tile; those columns
       // belong to the NEXT n-tile (another CTA's work) and must not be stored from here (round-1 bug: they were, and
       // raced with the owner's store whenever N had more than one such tile, e.g. nlon = 1440 or lmax = 240)
       const bool act = col < n_valid && c + c4 * 4 < BN;

@@ -1,4 +1,4 @@
-// Plain CUDA-core GEMM with the same producers / epilogues as the tcgen05 kernel.
+// Plain CUDA-core GEMM with the same producers / epilogues as the wgmma kernel.
 // DEVICE-SIDE TEST INFRASTRUCTURE: selected with SKY_GEMM=ref to bisect a parity failure
 // between "index arithmetic / epilogue" and "tensor-core pipeline".  Same numerics contract
 // (fp16 operands, fp32 accumulate); never the benchmarked path.

@@ -1,67 +1,58 @@
-// Column-split CTA pairs for GEMMs whose epilogue needs whole rows wider than half of TMEM (GraphCast: second MLP layer +
-// LayerNorm over 512 columns; Pangu: attention projection + LayerNorm at C = 384):
+// Column-split CTA pairs for GEMMs whose epilogue needs whole rows wider than one CTA's accumulators hold (GraphCast:
+// second MLP layer + LayerNorm over 512 columns; Pangu: attention projection + LayerNorm at C = 384):
 //
 //     D[M, 2 BLOCK_N] = A[M, K] W[2 BLOCK_N, K]^T  ->  epilogue over full rows
 //
-// k_gemm2 with BLOCK_N = 512 fills all 512 TMEM columns with ONE accumulator: the epilogue of a tile (residual read-modify-
-// write of 2 KB per row, HBM bound) and the main loop of the next one (640 KB of L2 -> SM traffic through a 2-stage ring)
-// cannot overlap, and ncu showed the kernel at 56 % of the DRAM and 15 % of the tensor roofline.  Here the two CTAs of a
-// cluster take the SAME 128-row tile and 256 output columns each: two independent cta_group::1 pipelines with
-// double-buffered 256-column accumulators (epilogue of tile i under the main loop of tile i + 1, 3-stage ring of 48 KB),
-// and the only coupling is the LayerNorm statistics: per lane quarter and tile, 32 (sum, sum of squares) pairs cross to
-// the peer through distributed shared memory (st.async completing the peer's mbarrier; gemm2.cuh EpiCtx::x_*).
-// Slots and barriers are double buffered by tile parity; a CTA can run at most one tile ahead of its peer, because its
-// next statistics wait needs the peer's sums of that tile.
+// A 128 x 512 fp32 accumulator is the whole register file of an SM.  Here the two CTAs of a cluster take the SAME 128-row
+// tile and BLOCK_N output columns each (k_gemm2's pipeline: two consumer warpgroups, accumulators staged over the drained
+// ring for the epilogue), and the only coupling is the LayerNorm statistics: per lane quarter and tile, 32 (sum, sum of
+// squares) pairs cross to the peer through distributed shared memory (st.async completing the peer's mbarrier; gemm2.cuh
+// EpiCtx::x_*).  Slots and barriers are double buffered by tile parity; a CTA can run at most one tile ahead of its peer,
+// because its next statistics wait needs the peer's sums of that tile.
 #pragma once
 #include "gemm2.cuh"
 
 namespace sky {
 
 template <class Epi, int EPI_WARPS, int BLOCK_N = 256>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__((EPI_WARPS + 2) * 32, 1)
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__((EPI_WARPS + 1) * 32, 1)
 k_gemm_split(const AImage A, const Epi epi, const uint8_t* __restrict__ Wimg, long long M, int num_kb, int num_m_tiles) {
   using Cfg = G2Cfg<BLOCK_N, EPI_WARPS>;
-  static_assert(2 * BLOCK_N <= 512, "two accumulators per CTA");
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* patches = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+  float* patches = reinterpret_cast<float*>(smem + Cfg::RING_BYTES);
   float* sbias = patches + EPI_WARPS * G2_PATCH_FLOATS;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sbias + 3 * 512);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::STAGES;
-  uint64_t* tmem_full = bars + 2 * Cfg::STAGES;
-  uint64_t* tmem_empty = bars + 2 * Cfg::STAGES + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::STAGES + 4);
-  uint64_t* xbar = bars + 2 * Cfg::STAGES + 5;                          // [2 tile parities][4 lane quarters]
+  uint64_t* stg_free = bars + 2 * Cfg::STAGES;
+  uint64_t* xbar = bars + 2 * Cfg::STAGES + 1;                          // [2 tile parities][4 lane quarters]
   float* xstat = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);   // [2][4][32 lanes][2]
-  static_assert((2 * Cfg::STAGES + 5 + 8) * 8 <= 256, "barrier block");
+  static_assert((2 * Cfg::STAGES + 1 + 8) * 8 <= 256, "barrier block");
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0), lane = threadIdx.x % 32;
   const uint32_t rank = cluster_ctarank();
   const int pair = blockIdx.x >> 1, npairs = gridDim.x >> 1;
-  constexpr int LOADER = EPI_WARPS, MMAW = EPI_WARPS + 1;
+  constexpr int LOADER = EPI_WARPS;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], EPI_WARPS); }
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], EPI_WARPS); }
+    mbar_init(stg_free, EPI_WARPS);
     for (int i = 0; i < 8; ++i) mbar_init(&xbar[i], 1);
     mbar_fence_init();
   }
-  if (warp == MMAW) tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
   if (threadIdx.x < EPI_WARPS * 32)
     for (int i = threadIdx.x; i < BLOCK_N; i += EPI_WARPS * 32) {
       sbias[i] = epi.bias[rank * BLOCK_N + i]; sbias[512 + i] = epi.gamma[rank * BLOCK_N + i]; sbias[1024 + i] = epi.beta[rank * BLOCK_N + i];
     }
-  tc_fence_before();
   __syncthreads();
   cluster_sync_all();   // the peer's exchange barriers exist before anything is posted to them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp == LOADER) {
-    int s = 0; uint32_t ph = 0;
+    int s = 0; uint32_t ph = 0; int it = 0;
     const uint8_t* wsrc = Wimg + (size_t)rank * num_kb * Cfg::B_BYTES;
-    for (int mt = pair; mt < num_m_tiles; mt += npairs) {
+    for (int mt = pair; mt < num_m_tiles; mt += npairs, ++it) {
+      if (it > 0) mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&empty[s], ph ^ 1);
         if (lane == 0) {
@@ -74,42 +65,16 @@ k_gemm_split(const AImage A, const Epi epi, const uint8_t* __restrict__ Wimg, lo
         if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == MMAW) {
-    constexpr uint32_t idesc = make_idesc_f16(G2_BLOCK_M, BLOCK_N);
-    int s = 0; uint32_t ph = 0; int it = 0;
-    for (int mt = pair; mt < num_m_tiles; mt += npairs, ++it) {
-      const int buf = it & 1;
-      const uint32_t use = (uint32_t)(it >> 1);
-      mbar_wait(&tmem_empty[buf], (use & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BLOCK_N);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        {
-          const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES);
-          const uint64_t da = make_desc_sw128(a_addr);
-          const uint64_t db = make_desc_sw128(a_addr + G2_A_BYTES);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) tc_mma_f16(d_tmem, da + 2 * k, db + 2 * k, idesc, (kb | k) != 0 ? 1u : 0u);
-            tc_commit(&empty[s]);
-            if (kb == num_kb - 1) tc_commit(&tmem_full[buf]);
-          }
-        }
-        __syncwarp();
-        if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
-      }
-    }
   } else {
-    const int q = warp & 3, part = warp >> 2;
+    const int q = warp & 3, part = warp >> 2, wg = warp >> 2;
     EpiCtx ctx;
     ctx.M = M; ctx.lane = lane; ctx.part = part; ctx.nparts = EPI_WARPS / 4;
     ctx.patch = patches + warp * G2_PATCH_FLOATS;
     ctx.patch_s = smem_u32(ctx.patch);
     ctx.svec_s = smem_u32(sbias);
     ctx.n0 = (int)rank * BLOCK_N;
-    int it = 0;
+    WgAcc<BLOCK_N> acc;
+    int s = 0; uint32_t ph = 0; int it = 0;
     for (int mt = pair; mt < num_m_tiles; mt += npairs, ++it) {
       const int buf = it & 1;
       const uint32_t use = (uint32_t)(it >> 1);
@@ -120,23 +85,14 @@ k_gemm_split(const AImage A, const Epi epi, const uint8_t* __restrict__ Wimg, lo
       ctx.x_peer_bar = mapa_u32(smem_u32(ctx.x_own_bar), rank ^ 1u);
       ctx.x_parity = use & 1;
       epi.template prefetch<BLOCK_N>(ctx);
-      mbar_wait(&tmem_full[buf], use & 1);
-      tc_fence_after();
-      AccTmem2 acc{tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BLOCK_N)};
-      epi.template run<BLOCK_N>(acc, ctx);
-      tc_fence_before();
+      wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, num_kb, wg, lane);
+      wg_epilogue<Cfg::STG_ROWS>(acc, smem, Cfg::STG_LD, wg, warp, lane, [&](AccSmem a) { epi.template run<BLOCK_N>(a, ctx); });
       __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[buf]);
+      if (lane == 0) mbar_arrive(stg_free);
     }
   }
-  tc_fence_before();
   __syncthreads();
   cluster_sync_all();   // nobody leaves while the peer may still post into this CTA's slots
-  tc_fence_after();
-  if (warp == MMAW) {
-    __syncwarp();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
 }
 
 // Wimg: [2][K/64][BLOCK_N rows x 128 B] (weight packed with BLOCK_N = half of the row width: 256 for GraphCast's 512-wide

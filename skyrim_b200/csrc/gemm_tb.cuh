@@ -1,4 +1,4 @@
-// "Table x data" variant of the batched tcgen05 GEMM (SFNO transforms):
+// "Table x data" variant of the batched wgmma GEMM (SFNO transforms):
 //
 //   for b in batches:  D_b[M, N] = T_b[M, Ktot] * X_b[Ktot, N]        -> fused epilogue
 //
@@ -6,8 +6,8 @@
 //     hi, hi, lo), 128-row tiles (a W3 image with BN = 128), optionally one table per batch.
 // B = the DATA, used where it lies: an fp16 tile image whose ROWS are the contraction index (pixels of one latitude,
 //     latitudes, degrees l, (m, re/im)) and whose 128-byte row chunks hold 64 consecutive channels.  Those bytes are a
-//     valid MN-MAJOR SWIZZLE_128B B operand (tools/umma_probe.cu cases 3 and 7: atoms of [64 k-rows][128 B] stacked along
-//     N with the atom stride in the descriptor's LBO field), so no transposing pack pass is needed between two
+//     valid MN-MAJOR SWIZZLE_128B B operand (atoms of [64 k-rows][128 B] stacked along N with the atom stride in the
+//     descriptor's LBO field, sky_common.cuh make_desc_sw128_mn), so no transposing pack pass is needed between two
 //     contractions over different indices: each GEMM's epilogue writes its fp16 hi / lo result rows straight into the
 //     next GEMM's data image (EpiSplitRemap), K-concatenated as [hi | lo | hi] by reading the hi image twice.
 //
@@ -28,7 +28,7 @@ struct BData {
 };
 
 template <class Epi, int BLOCK_N, int EPI_WARPS>
-__global__ void __launch_bounds__((EPI_WARPS + 2) * 32, 1)
+__global__ void __launch_bounds__((EPI_WARPS + 1) * 32, 1)
 k_gemm_tb(const uint8_t* __restrict__ Timg, long long t_batch_stride, const BData B, const Epi epi, long long M, int nkb,
           int num_m_tiles, int num_n_tiles, int batches) {
   using Cfg = G2Cfg<BLOCK_N, EPI_WARPS>;
@@ -36,42 +36,37 @@ k_gemm_tb(const uint8_t* __restrict__ Timg, long long t_batch_stride, const BDat
   constexpr int ATOMS = BLOCK_N / 64;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* patches = reinterpret_cast<float*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+  float* patches = reinterpret_cast<float*>(smem + Cfg::RING_BYTES);
   float* sbias = patches + EPI_WARPS * G2_PATCH_FLOATS;
   uint64_t* bars = reinterpret_cast<uint64_t*>(sbias + 3 * 512);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::STAGES;
-  uint64_t* tmem_full = bars + 2 * Cfg::STAGES;
-  uint64_t* tmem_empty = bars + 2 * Cfg::STAGES + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::STAGES + 4);
+  uint64_t* stg_free = bars + 2 * Cfg::STAGES;
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0), lane = threadIdx.x % 32;
   const int tiles_per_batch = num_m_tiles * num_n_tiles;
   const long long num_tiles = (long long)tiles_per_batch * batches;
   const int num_kb = 3 * nkb;
-  constexpr int LOADER = EPI_WARPS, MMAW = EPI_WARPS + 1;
+  constexpr int LOADER = EPI_WARPS;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&tmem_full[b], 1); mbar_init(&tmem_empty[b], EPI_WARPS); }
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], EPI_WARPS); }
+    mbar_init(stg_free, EPI_WARPS);
     mbar_fence_init();
   }
-  if (warp == MMAW) tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
   if constexpr (has_cta_stats<Epi>::value)
     for (int i = threadIdx.x; i < 3 * 512; i += blockDim.x) sbias[i] = 0.f;
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   if (warp == LOADER) {
-    int s = 0; uint32_t ph = 0;
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int s = 0; uint32_t ph = 0; int it = 0;
+    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
       const int b = (int)(tile / tiles_per_batch), t = (int)(tile % tiles_per_batch);
       const int mt = t / num_n_tiles, nt = t % num_n_tiles;
       const uint8_t* tsrc = Timg + (size_t)b * t_batch_stride + (size_t)mt * (2 * nkb) * G2_A_BYTES;   // [hi | lo] image
       const long long row_b = (long long)b * B.rows_per_batch;
       const size_t boff = (size_t)b * B.batch_bytes;
+      if (it > 0) mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&empty[s], ph ^ 1);
         uint8_t* dst = smem + s * Cfg::STAGE_BYTES;
@@ -98,68 +93,28 @@ k_gemm_tb(const uint8_t* __restrict__ Timg, long long t_batch_stride, const BDat
         if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == MMAW) {
-    constexpr uint32_t idesc = make_idesc_f16(G2_BLOCK_M, BLOCK_N) | (1u << 16);   // B is MN-major
-    int s = 0; uint32_t ph = 0; int it = 0;
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int buf = it % Cfg::NBUF;
-      const uint32_t use = (uint32_t)(it / Cfg::NBUF);
-      mbar_wait(&tmem_empty[buf], (use & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BLOCK_N);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        {
-          const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES);
-          const uint64_t da = make_desc_sw128(a_addr);                   // K-major: +32 B per K=16 step
-          // MN-major data: atoms 8 KB apart along N (LBO), 8-row groups 1 KB apart along K (SBO); +16 rows per step
-          uint64_t db = make_desc_sw128(a_addr + G2_A_BYTES);
-          db = (db & ~((uint64_t)0x3FFF << 16)) | ((uint64_t)(8192 >> 4) << 16);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              tc_mma_f16(d_tmem, da + 2 * k, db + (uint64_t)(k * (2048 >> 4)), idesc, (kb | k) != 0 ? 1u : 0u);
-            tc_commit(&empty[s]);
-            if (kb == num_kb - 1) tc_commit(&tmem_full[buf]);
-          }
-        }
-        __syncwarp();
-        if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
-      }
-    }
   } else {
-    const int q = warp & 3, part = warp >> 2;
+    const int q = warp & 3, part = warp >> 2, wg = warp >> 2;
     EpiCtxB ctx;
     ctx.M = M; ctx.lane = lane; ctx.part = part; ctx.nparts = EPI_WARPS / 4;
     ctx.patch = patches + warp * G2_PATCH_FLOATS;
     ctx.patch_s = smem_u32(ctx.patch);
     ctx.svec_s = smem_u32(sbias);
-    int it = 0;
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int buf = it % Cfg::NBUF;
-      const uint32_t use = (uint32_t)(it / Cfg::NBUF);
+    WgAcc<BLOCK_N, true> acc;   // B = the data, MN-major
+    int s = 0; uint32_t ph = 0;
+    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const int b = (int)(tile / tiles_per_batch), t = (int)(tile % tiles_per_batch);
       ctx.batch = b;
       ctx.row0 = (long long)(t / num_n_tiles) * G2_BLOCK_M + q * 32;
       ctx.n0 = (t % num_n_tiles) * BLOCK_N;
-      mbar_wait(&tmem_full[buf], use & 1);
-      tc_fence_after();
-      AccTmem2 acc{tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BLOCK_N)};
-      epi.template run<BLOCK_N>(acc, ctx);
-      tc_fence_before();
+      wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, num_kb, wg, lane);
+      wg_epilogue<Cfg::STG_ROWS>(acc, smem, Cfg::STG_LD, wg, warp, lane, [&](AccSmem a) { epi.template run<BLOCK_N>(a, ctx); });
       __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[buf]);
+      if (lane == 0) mbar_arrive(stg_free);
     }
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
   cta_stats_flush(epi, sbias);
-  if (warp == MMAW) {
-    __syncwarp();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
-  }
 }
 
 // T: W3-style image with 128-row tiles (N = padded table rows, Kp = padded K of one segment)

@@ -1,4 +1,4 @@
-// Persistent warp-specialised tcgen05 GEMM for sm_100a:
+// Persistent warp-specialised wgmma GEMM for sm_90a:
 //
 //      D[M, N] = A(prod)[M, K] * W[N, K]^T  ->  epilogue(epi)
 //
@@ -6,42 +6,32 @@
 //     straight into a SWIZZLE_128B K-major smem tile (no intermediate HBM copy of the
 //     windowed / im2col'd activations ever exists);
 //   * B operand: weights pre-packed at load time as the exact smem tile image
-//     (prep.cu::k_pack_weight_image), fetched with one 1-D bulk copy (TMA engine,
-//     cp.async.bulk + mbarrier complete_tx) per k-block;
-//   * one elected thread issues tcgen05.mma (kind::f16, M=128, fp32 accumulators in TMEM),
-//     tcgen05.commit frees smem stages and publishes the accumulator;
-//   * four epilogue warps read their TMEM lane quarter (tcgen05.ld 32x32b) and run the fused
-//     epilogue; accumulators are double buffered in TMEM when 2*BLOCK_N <= 512 columns so
-//     the epilogue of tile i overlaps the MMAs of tile i+1.
+//     (k_pack_weight), fetched with one 1-D bulk copy (TMA engine, cp.async.bulk +
+//     mbarrier complete_tx) per k-block;
+//   * two consumer warpgroups issue the wgmma products (gemm2.cuh WgAcc) and stage the
+//     accumulator in shared memory; warps 0..3 then run the row-owner epilogue on it.
 #pragma once
-#include "pangu_ops.cuh"
+#include "gemm2.cuh"
 
 namespace sky {
 
 constexpr int TC_BLOCK_M = 128;
 constexpr int TC_BLOCK_K = 64;                      // halves: one 128-byte swizzle row
 constexpr int TC_A_BYTES = TC_BLOCK_M * 128;        // 16 KB
-constexpr int TC_THREADS = 320;                     // 4 epilogue + 4 producer + MMA + B-loader warps
+constexpr int TC_THREADS = 416;                     // 8 consumer + 4 producer + B-loader warps
 constexpr int TC_NUM_PRODUCER_THREADS = 128;
 
 template <int BLOCK_N>
 struct TcCfg {
-  static constexpr int N_INST = BLOCK_N <= 256 ? BLOCK_N : BLOCK_N / 2;  // UMMA N per instruction
-  static constexpr int N_SPLIT = BLOCK_N / N_INST;
   static constexpr int B_BYTES = BLOCK_N * 128;
   static constexpr int STAGE_BYTES = TC_A_BYTES + B_BYTES;
   static constexpr int STAGES = (200 * 1024) / STAGE_BYTES >= 6 ? 6 : (200 * 1024) / STAGE_BYTES;
-  static constexpr int NBUF = 2 * BLOCK_N <= 512 ? 2 : 1;
-  static constexpr int TMEM_COLS = NBUF * BLOCK_N <= 32 ? 32 : NBUF * BLOCK_N <= 64 ? 64
-                                   : NBUF * BLOCK_N <= 128 ? 128 : NBUF * BLOCK_N <= 256 ? 256 : 512;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
-  static_assert(N_INST % 16 == 0 && N_INST <= 256, "UMMA shape");
+  static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
+  static constexpr int STG_LD = (BLOCK_N + 31) / 32 * 32 + 4;
+  static constexpr int SMEM_BYTES = RING_BYTES + 1024 /*align slack*/ + 256 /*barriers*/;
+  static_assert(BLOCK_N % 32 == 0 && BLOCK_N <= 256, "wgmma N");
   static_assert(STAGE_BYTES % 1024 == 0, "stage alignment");
-};
-
-struct AccTmem {
-  uint32_t taddr;  // lane quarter base | column base
-  __device__ void load32(int c, float (&v)[32]) const { tmem_ld32(taddr + (uint32_t)c, v); }
+  static_assert(128 * STG_LD * 4 <= RING_BYTES, "accumulator staging");
 };
 
 template <class Prod, class Epi, int BLOCK_N>
@@ -51,12 +41,10 @@ k_gemm_tc(const Prod prod, const Epi epi, const uint8_t* __restrict__ Wimg, long
   using Cfg = TcCfg<BLOCK_N>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::RING_BYTES);
   uint64_t* full = bars;                       // [STAGES]  producers(128) + B loader(1 + tx)
-  uint64_t* empty = bars + Cfg::STAGES;        // [STAGES]  tcgen05.commit
-  uint64_t* tmem_full = bars + 2 * Cfg::STAGES;       // [2]
-  uint64_t* tmem_empty = bars + 2 * Cfg::STAGES + 2;  // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 2 * Cfg::STAGES + 4);
+  uint64_t* empty = bars + Cfg::STAGES;        // [STAGES]  the 8 consumer warps
+  uint64_t* stg_free = bars + 2 * Cfg::STAGES; // consumers -> producers / B loader: the epilogue has left the ring
 
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0), lane = threadIdx.x % 32;  // provably warp-uniform
   const int num_tiles = num_m_tiles * num_n_tiles;
@@ -64,30 +52,24 @@ k_gemm_tc(const Prod prod, const Epi epi, const uint8_t* __restrict__ Wimg, long
   if (threadIdx.x == 0) {
     for (int s = 0; s < Cfg::STAGES; ++s) {
       mbar_init(&full[s], TC_NUM_PRODUCER_THREADS + 1);
-      mbar_init(&empty[s], 1);
+      mbar_init(&empty[s], 8);
     }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(&tmem_full[b], 1);
-      mbar_init(&tmem_empty[b], 128);
-    }
+    mbar_init(stg_free, 8);
     mbar_fence_init();
   }
-  if (warp == 8) tmem_alloc<Cfg::TMEM_COLS>(tmem_ptr);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp >= 4 && warp < 8) {
+  if (warp >= 8 && warp < 12) {
     // ============================ A producers ============================
     // thread = tile row, the 8 chunks of a k-block in sequence: for one chunk the 32 lanes of a warp are 32
     // consecutive tokens, i.e. one contiguous 512-byte run of the source field per load instruction, and the
     // 16-byte shared-memory stores of a quarter warp fall into 8 different swizzled chunk slots
-    const int row = threadIdx.x - 128;
-    int s = 0; uint32_t ph = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const int row = threadIdx.x - 256;
+    int s = 0; uint32_t ph = 0; int it = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
       const long long m0 = (long long)(tile / num_n_tiles) * TC_BLOCK_M;
       const RowInfo ri = prod.prep(m0 + row);
+      if (it > 0) mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&empty[s], ph ^ 1);
         uint8_t* a_s = smem + s * Cfg::STAGE_BYTES;
@@ -102,12 +84,13 @@ k_gemm_tc(const Prod prod, const Epi epi, const uint8_t* __restrict__ Wimg, long
         if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 9) {
+  } else if (warp == 12) {
     // ============================ B loader (TMA engine) ============================
-    int s = 0; uint32_t ph = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    int s = 0; uint32_t ph = 0; int it = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
       const int nt = tile % num_n_tiles;
       const uint8_t* src = Wimg + (size_t)nt * num_kb * Cfg::B_BYTES;
+      if (it > 0) mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
       for (int kb = 0; kb < num_kb; ++kb) {
         mbar_wait(&empty[s], ph ^ 1);
         if (lane == 0) {
@@ -119,61 +102,21 @@ k_gemm_tc(const Prod prod, const Epi epi, const uint8_t* __restrict__ Wimg, long
         if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 8) {
-    // ============================ MMA issuer ============================
-    constexpr uint32_t idesc = make_idesc_f16(TC_BLOCK_M, Cfg::N_INST);
-    int s = 0; uint32_t ph = 0; int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int buf = it % Cfg::NBUF;
-      const uint32_t use = (uint32_t)(it / Cfg::NBUF);
-      mbar_wait(&tmem_empty[buf], (use & 1) ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BLOCK_N);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full[s], ph);
-        tc_fence_after();
-        {  // descriptors on the uniform datapath, one elected thread issues the MMAs and the commits that track them
-          const uint32_t a_addr = smem_u32(smem + s * Cfg::STAGE_BYTES);
-          const uint64_t da = make_desc_sw128(a_addr);
-          const uint64_t db = make_desc_sw128(a_addr + TC_A_BYTES);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < TC_BLOCK_K / 16; ++k) {
-#pragma unroll
-              for (int ni = 0; ni < Cfg::N_SPLIT; ++ni)
-                tc_mma_f16(d_tmem + ni * Cfg::N_INST, da + 2 * k, db + (uint64_t)(ni * Cfg::N_INST * 8 + 2 * k), idesc,
-                           (kb | k) != 0 ? 1u : 0u);
-            }
-            tc_commit(&empty[s]);
-            if (kb == num_kb - 1) tc_commit(&tmem_full[buf]);
-          }
-        }
-        __syncwarp();
-        if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
-      }
-    }
   } else {
-    // ============================ epilogue warps 0..3 ============================
-    int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int buf = it % Cfg::NBUF;
-      const uint32_t use = (uint32_t)(it / Cfg::NBUF);
+    // ============================ consumer warpgroups: MMA, then epilogue in warps 0..3 ============================
+    const int wg = warp >> 2;
+    WgAcc<BLOCK_N> acc;
+    int s = 0; uint32_t ph = 0;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const long long m0 = (long long)(tile / num_n_tiles) * TC_BLOCK_M;
       const int n0 = (tile % num_n_tiles) * BLOCK_N;
-      mbar_wait(&tmem_full[buf], use & 1);
-      tc_fence_after();
-      AccTmem acc{tmem_base + ((uint32_t)(warp * 32) << 16) + (uint32_t)(buf * BLOCK_N)};
-      epi.run(acc, m0 + warp * 32 + lane, n0, BLOCK_N);
-      tc_fence_before();
-      mbar_arrive(&tmem_empty[buf]);
+      wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, num_kb, wg, lane);
+      wg_epilogue<128>(acc, smem, Cfg::STG_LD, wg, warp, lane, [&](AccSmem a) {
+        if (warp < 4) epi.run(a, m0 + warp * 32 + lane, n0, BLOCK_N);
+      });
+      __syncwarp();
+      if (lane == 0) mbar_arrive(stg_free);
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  if (warp == 8) {
-    __syncwarp();
-    tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
   }
 }
 

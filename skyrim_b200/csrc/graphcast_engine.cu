@@ -1,13 +1,13 @@
-// GraphCast 6-h step operator on sm_100a (SURVEY.md §8(a) A9 / §8(f) N1): replaces what
-// /root/reference/skyrim/core/models/graphcast.py:118 (`self.stepper.step(state)`) runs inside earth2mip's JAX wrapper.
+// GraphCast 6-h step operator on sm_90a (SURVEY.md §8(a) A9 / §8(f) N1): replaces what Skyrim's GraphCast model
+// (skyrim/core/models/graphcast.py, `self.stepper.step(state)`) runs inside earth2mip's JAX wrapper.
 //
 // State tensor of one member: (2 x 83, nlat, nlon) fp32 = the two time slices (t-6h, t) of the reference's 83-channel
 // field (graphcast.py:17-41; 82 prognostic channels + the toa-radiation forcing the reference labels "tp06").
 // One step = encoder (grid -> mesh), 16 message-passing layers on the multimesh, decoder (mesh -> grid), residual update.
 //
-// B200 mapping.  Every MLP is two persistent TMA-fed tcgen05 GEMMs: hidden = swish(A W1^T + ...) (k_gemm_pair: A-stationary
-// CTA pairs, cta_group::2; k_gemm2 where K != 512) written as the fp16 operand image of the second GEMM (k_gemm_split:
-// column-split CTA pairs, LayerNorm statistics over DSMEM), whose epilogue does bias + LayerNorm (+ residual, read from the
+// H100 mapping.  Every MLP is two persistent TMA-fed wgmma GEMMs: hidden = swish(A W1^T + ...) (k_gemm2) written as the
+// fp16 operand image of the second GEMM (k_gemm_split: column-split CTA pairs of a cluster, LayerNorm statistics over
+// DSMEM), whose epilogue does bias + LayerNorm (+ residual, read from the
 // stream's own fp16 image for grid nodes and mesh edges) and writes the operand image of whatever consumes it next.  The concatenations of the published formulation never exist:
 //   * [edge, sender, receiver] W1^T = edge W1e^T + (v W1s^T)[sender] + (v W1r^T)[receiver]: the per-NODE products are
 //     small GEMMs into fp16 tables, gathered by edge index inside the hidden GEMM's epilogue (row-owner lanes);
@@ -22,7 +22,6 @@
 
 #include "engine.h"
 #include "graphcast_ops.cuh"
-#include "gemm_pair.cuh"
 #include "gemm_split.cuh"
 
 namespace sky {
@@ -33,7 +32,7 @@ static inline size_t img_bytes(long long rows, int nkb) { return (size_t)(pad128
 struct WImg { uint8_t* img = nullptr; int N = 0, Kp = 0, BN = 0; };
 struct Mlp {
   WImg w1, w2;
-  WImg w2s;   // second layer packed in 256-row halves for the column-split pair kernel (k_gemm_split)
+  WImg w2s;   // second layer of the LayerNorm MLPs, packed in 256-row halves for the column-split pair kernel (k_gemm_split)
   const float *b1 = nullptr, *b2 = nullptr, *g = nullptr, *be = nullptr;
 };
 
@@ -59,10 +58,8 @@ struct GraphCastEngine : Engine {
   uint8_t *e_g2m_img = nullptr, *e_m2g_img = nullptr, *e_mesh_img = nullptr, *vm0_img = nullptr;
   float* vm0_f32 = nullptr;
   __half* g2m_tr = nullptr;             // (Nm, 512): embedded mesh nodes x W1r(g2m_edge)^T
-  bool use_pair = true;   // debug_set("gc_pair", 0): hidden GEMMs on k_gemm2 (A/B timing, bisection)
   cudaStream_t prep_stream = nullptr;   // stream of the running prepare() (dalloc's zero fills)
   bool l2_prefetch = true;  // debug_set("gc_prefetch", 0)
-  bool use_split = true;  // debug_set("gc_split", 0): LayerNorm GEMMs on k_gemm2 with one 512-column accumulator
   // clock
   double* clock_dev = nullptr;
   GcClock* clk_dev = nullptr;
@@ -107,7 +104,7 @@ struct GraphCastEngine : Engine {
     return 0;
   }
   int load_mlp(Mlp& m, const char* name, int fan_in, int k_in /*columns of w1 kept in the A-operand GEMM*/, int fan_out, bool ln,
-               cudaStream_t st, int w2_bn = GC_L) {
+               cudaStream_t st, int w2_bn = 256) {
     char nm[96];
     auto N = [&](const char* s) { snprintf(nm, sizeof nm, "%s.%s", name, s); return nm; };
     int rc;
@@ -115,17 +112,18 @@ struct GraphCastEngine : Engine {
       if ((rc = walloc(m.w1, GC_L, k_in, 256))) return rc;
       if ((rc = wfill(m.w1, N("w1"), GC_L, fan_in, 0, k_in, 0, 0, st))) return rc;
     }
-    if ((rc = walloc(m.w2, fan_out, GC_L, w2_bn))) return rc;
-    if ((rc = wfill(m.w2, N("w2"), fan_out, GC_L, 0, GC_L, 0, 0, st))) return rc;
-    if (ln && fan_out == GC_L) {
+    if (ln && fan_out == GC_L) {   // LayerNorm over 512 columns: column-split pair kernel, 256-row halves
       if ((rc = walloc(m.w2s, GC_L, GC_L, 256))) return rc;
       if ((rc = wfill(m.w2s, N("w2"), GC_L, GC_L, 0, GC_L, 0, 0, st))) return rc;
+    } else {
+      if ((rc = walloc(m.w2, fan_out, GC_L, w2_bn))) return rc;
+      if ((rc = wfill(m.w2, N("w2"), fan_out, GC_L, 0, GC_L, 0, 0, st))) return rc;
     }
     if (!(m.b1 = keep(N("b1"), GC_L, st))) return SKY_ERR_ARG;
     {   // b2 / gamma / beta padded to the n-tile width (the kernel stages BLOCK_N entries)
       const float* b2 = param(N("b2"), (uint64_t)fan_out);
       if (!b2) return SKY_ERR_ARG;
-      float* p = dalloc<float>((size_t)m.w2.N, true);
+      float* p = dalloc<float>((size_t)(m.w2.img ? m.w2.N : m.w2s.N), true);
       if (!p) return SKY_ERR_NOMEM;
       SKY_CUDA_OK(cudaMemcpyAsync(p, b2, (size_t)fan_out * 4, cudaMemcpyDeviceToDevice, st));
       m.b2 = p;
@@ -193,14 +191,7 @@ struct GraphCastEngine : Engine {
     epi.l2_prefetch = l2_prefetch && M > 4 * Nm ? 1 : 0;   // grid-sized tables only (the mesh tables are L2 resident)
     prof_begin(tag, st);
     count_launch();
-    int rc;
-    if (Kp == GC_L && A.nkb0 == GC_NKB && use_pair)
-      // K = 512 from one operand image (edge updates, grid2mesh grid update, output head): A-stationary CTA pairs,
-      // cta_group::2 M = 256 — each CTA keeps its 128 x 512 A tile for both n-tiles and streams half of every weight item
-      // (k_gemm2 moves 768 KB of L2 -> SM traffic per 128 rows here, the pair 384 KB)
-      rc = launch_gemm_pair<EpiGcSiluImg<kG>, GC_L, 256>(A.img0, epi, w.img, M, GC_L, num_sms, st);
-    else
-      rc = launch_gemm2<EpiGcSiluImg<kG>, 256, 8>(A, epi, w.img, M, GC_L, Kp, num_sms, st);
+    const int rc = launch_gemm2<EpiGcSiluImg<kG>, 256, 8>(A, epi, w.img, M, GC_L, Kp, num_sms, st);
     prof_end(tag, st);
     // fp16-range guard (engine.h; a no-op unless enabled): class 5 hidden images, 0 latent / update images, 6 per-node tables
     return rc ? rc : range_scan(5, out, (size_t)(M / 128) * GC_NKB * G2_A_BYTES, st);
@@ -210,8 +201,7 @@ struct GraphCastEngine : Engine {
                 const uint8_t* xin_img, cudaStream_t st) {
     EpiGcLn<kRes> epi{xin, xout, img, yimg, m.b2, m.g, m.be, cfg.ln_eps};
     epi.xin_img = xin_img;
-    return use_split ? launch_gemm_split<EpiGcLn<kRes>, 8>(A1(hid, GC_NKB), epi, m.w2s.img, M, GC_L, num_sms, st)
-                     : launch_gemm2<EpiGcLn<kRes>, GC_L, 8>(A1(hid, GC_NKB), epi, m.w2.img, M, GC_L, GC_L, num_sms, st);
+    return launch_gemm_split<EpiGcLn<kRes>, 8>(A1(hid, GC_NKB), epi, m.w2s.img, M, GC_L, num_sms, st);
   }
   // xin (fp32 rows) or xin_img (fp16 image) is the residual source; at most one of them
   int ln_gemm(int tag, const uint8_t* hid, const Mlp& m, long long M, const float* xin, float* xout, uint8_t* img, uint8_t* yimg,
@@ -488,8 +478,6 @@ struct GraphCastEngine : Engine {
   }
 
   int debug_set(const char* key, long long value) override {
-    if (!strcmp(key, "gc_pair")) { use_pair = value != 0; drop_graphs(); return 0; }
-    if (!strcmp(key, "gc_split")) { use_split = value != 0; drop_graphs(); return 0; }
     if (!strcmp(key, "gc_prefetch")) { l2_prefetch = value != 0; drop_graphs(); return 0; }
     return Engine::debug_set(key, value);
   }

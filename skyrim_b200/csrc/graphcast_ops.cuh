@@ -48,13 +48,10 @@ __device__ __forceinline__ void add_h8(float* v, const uint4& p) {
 }
 
 // hidden = swish(acc + bias + Ta[ia[row]] + Tb[ib[row]])  ->  fp16 tile image (GC_NKB k-blocks per row tile).
-// kG = number of gathered tables (0, 1, 2).  Everything after the TMEM read happens in the RE-TILED domain (lane ->
+// kG = number of gathered tables (0, 1, 2).  Everything after the accumulator read happens in the RE-TILED domain (lane ->
 // row = it * 8 + lane / 4, 8 columns = lane % 4): there four lanes read 64 contiguous bytes of one table row, so a gather
-// instruction touches 8 cache lines instead of 32 (row-owner gathers kept the L1TEX tag stage 67 % busy).
-// Latency structure (profiles/r2e_graphcast.md): a gather is an L2 round trip of 1 - 2 us, and tcgen05.wait::ld also waits
-// for the thread's outstanding global loads, so a register prefetch of the NEXT chunk is waited for at the current chunk's
-// TMEM read and hides nothing (measured: no change).  What does help is fewer exposures: the table rows of TWO 32-column
-// chunks are requested together, in front of the first chunk's TMEM read; the second chunk then finds its rows in
+// instruction touches 8 cache lines instead of 32.  A gather is an L2 round trip, so the table rows of TWO 32-column
+// chunks are requested together, in front of the first chunk's accumulator read; the second chunk then finds its rows in
 // registers.  A warp handles 4 chunks per 256-column tile: 2 exposed round trips instead of 4.
 template <int kG>
 struct EpiGcSiluImg {

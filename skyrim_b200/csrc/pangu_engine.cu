@@ -1,6 +1,6 @@
-// Pangu-Weather 6-h step operator on sm_100a: weight repacking + the per-step kernel
-// sequence.  Replaces what /root/reference/skyrim/core/models/pangu.py:45-46 loads
-// (two ONNXRuntime sessions) and what utils.py:34 steps.
+// Pangu-Weather 6-h step operator on sm_90a: weight repacking + the per-step kernel
+// sequence.  Replaces the two ONNX Runtime sessions that Skyrim's Pangu model
+// (skyrim/core/models/pangu.py) loads and steps.
 //
 // Data flow (v2): every token matrix lives in NATURAL token order (member, z, lat, lon).
 //   x   fp32 row-major (rows, C)                  the residual stream
@@ -16,15 +16,12 @@
 #include "engine.h"
 #include "gemm2.cuh"
 #include "gemm_tc.cuh"
-#include "mlp_fused2.cuh"
-#include "gemm_pair.cuh"
 #include "gemm_split.cuh"
 #ifdef SKY_EXPERIMENTS
 // development build only (libskyrim_b200_dev.so): CUDA-core reference GEMMs under the same epilogues, the single-CTA
 // kernel variants and the result-invalidating timing switches.  None of this is compiled into the product library.
 #include "gemm2_ref.cuh"
 #include "gemm_ref.cuh"
-#include "mlp_fused.cuh"
 #endif
 
 namespace sky {
@@ -139,8 +136,7 @@ struct GemmW {
 };
 struct BlockW {
   GemmW qkv, proj, fc1, fc2;
-  GemmW proj_s;  // C = 384: the projection packed in 192-row halves for the column-split pair kernel (gemm_split.cuh)
-  GemmW fc1f;  // fc1 packed in hidden-chunk tiles for the fused MLP kernel
+  GemmW proj_s, fc2_s;  // C = 384: projection and fc2 packed in 192-row halves for the column-split pair kernel (gemm_split.cuh)
   const float *qkv_b, *proj_b, *fc1_b, *fc2_b, *ln1_g, *ln1_b, *ln2_g, *ln2_b;
   __half* bias_tab;  // (n_type, heads, 3312), fp16, pre-scaled by log2 e
 };
@@ -154,11 +150,7 @@ struct PanguEngine : Engine {
   // per token and feature of the projection / MLP epilogues disappear; step error 5.8e-4 instead of 5.1e-4 at 721x1440),
   // false = fp32 rows beside the image (round-1 / early round-2 data flow; for weights whose error margin is tighter)
   bool img_stream = true;
-  bool proj_split = true;   // C = 384 projection on column-split CTA pairs ("proj_split" 0: one 384-column accumulator)
-  // fused MLP on CTA pairs (cta_group::2) per channel width; SKY_MLP=1cta|pair192|pair384 selects for A/B timing
-  bool mlp_pair192 = true, mlp_pair384 = true;
-  bool qkv_pair = true;     // SKY_QKV=1cta selects k_gemm2 for the QKV projection (A/B timing)
-  bool prof_split = false;  // SKY_PROF_SPLIT: report the C=384 MLP launches under the (otherwise unused) fc2 tag
+  bool proj_split = true;   // C = 384 LayerNorm GEMMs (projection, fc2) on column-split CTA pairs ("proj_split" 0: one 384-column tile)
   int exp_qkv = 0, exp_ln = 0;  // dev build only: result-invalidating timing experiments
   bool attn_ref = false;        // dev build only (SKY_ATTN=ref): CUDA-core reference attention on the same window image
   std::vector<void*> owned;
@@ -186,13 +178,6 @@ struct PanguEngine : Engine {
 #ifdef SKY_EXPERIMENTS   // read once, at creation; the product library reads no environment variable at all
     const char* e = getenv("SKY_GEMM");
     use_ref = e && !strcmp(e, "ref");
-    const char* m = getenv("SKY_MLP");
-    if (m && !strcmp(m, "1cta")) mlp_pair192 = mlp_pair384 = false;
-    if (m && !strcmp(m, "pair192")) mlp_pair384 = false;
-    if (m && !strcmp(m, "pair384")) mlp_pair192 = false;
-    prof_split = getenv("SKY_PROF_SPLIT") != nullptr;
-    const char* qv = getenv("SKY_QKV");
-    qkv_pair = !(qv && !strcmp(qv, "1cta"));
     exp_qkv = getenv("SKY_QKV_EXP") ? atoi(getenv("SKY_QKV_EXP")) : 0;
     exp_ln = getenv("SKY_LN_EXP") ? atoi(getenv("SKY_LN_EXP")) : 0;
     const char* at = getenv("SKY_ATTN");
@@ -270,12 +255,7 @@ struct PanguEngine : Engine {
         if (c == 384 && (rc = pack(b.proj_s, N("proj.w"), c, c, 192, false, st))) return rc;
         if ((rc = pack(b.fc1, N("fc1.w"), 4 * c, c, 192, false, st))) return rc;
         if ((rc = pack(b.fc2, N("fc2.w"), c, 4 * c, c, false, st))) return rc;
-#ifdef SKY_EXPERIMENTS
-        const int hc = (c == 192 ? mlp_pair192 : mlp_pair384) ? 128 : (c == 192 ? MlpCfg<192>::HC : MlpCfg<384>::HC);
-#else
-        const int hc = 128;   // hidden-chunk width of k_mlp_fused_pair
-#endif
-        if ((rc = pack(b.fc1f, N("fc1.w"), 4 * c, c, hc, false, st))) return rc;
+        if (c == 384 && (rc = pack(b.fc2_s, N("fc2.w"), c, 4 * c, 192, false, st))) return rc;
         P(b.qkv_b, N("qkv.b"), 3 * c); P(b.proj_b, N("proj.b"), c);
         P(b.fc1_b, N("fc1.b"), 4 * c); P(b.fc2_b, N("fc2.b"), c);
         P(b.ln1_g, N("ln1.g"), c); P(b.ln1_b, N("ln1.b"), c);
@@ -388,18 +368,8 @@ struct PanguEngine : Engine {
       EpiQkvWin e{ws.qkv, part_stride, b.qkv_b, g, roll, C, pairs};
 #ifdef SKY_EXPERIMENTS
       e.exp = exp_qkv;
-      if (use_ref || !qkv_pair) {
-        if ((rc = gemm2<192, 8>(KT_QKV, A, e, b.qkv, R, ws.scratch, st))) return rc;
-      } else
 #endif
-      {  // A-stationary CTA-pair kernel: a third of the L2 traffic of the tile-streaming kernel
-        prof_begin(KT_QKV, st);
-        count_launch();
-        rc = C == 192 ? launch_gemm_pair<EpiQkvWin, 192>(xh, e, b.qkv.img, R, 3 * C, num_sms, st)
-                      : launch_gemm_pair<EpiQkvWin, 384>(xh, e, b.qkv.img, R, 3 * C, num_sms, st);
-        prof_end(KT_QKV, st);
-        if (rc) return rc;
-      }
+      if ((rc = gemm2<192, 8>(KT_QKV, A, e, b.qkv, R, ws.scratch, st))) return rc;
       if (g.Hp > g.H) {   // latitude-padding tokens (x = 0): their q, k, v rows are the projection's bias.  (Writing them from
                           // the GEMM epilogue of the neighbouring tokens instead cost the GEMM 0.5 ms/step: measured, reverted.)
         const long long total = 3LL * B * g.Z * (g.Hp - g.H) * g.W * pairs * 8;
@@ -432,8 +402,8 @@ struct PanguEngine : Engine {
       e.exp = exp_ln;
 #endif
       if (C == 384 && proj_split && !use_ref) {
-        // one 384-column accumulator cannot be double buffered in TMEM: the two CTAs of a cluster take 192 columns each of the
-        // same 128 rows (epilogue of tile i under the main loop of tile i + 1), LayerNorm statistics cross through DSMEM
+        // a 128 x 384 accumulator takes 192 registers per consumer thread: the two CTAs of a cluster take 192 columns each of
+        // the same 128 rows, LayerNorm statistics cross through DSMEM
         prof_begin(KT_PROJ, st);
         count_launch();
         rc = launch_gemm_split<ELn, 8, 192>(A, e, b.proj_s.img, R, C, num_sms, st);
@@ -444,36 +414,24 @@ struct PanguEngine : Engine {
       }
       if (rc) return rc;
     }
-#ifdef SKY_EXPERIMENTS
-    if (use_ref) {  // two plain GEMMs through an HBM-resident hidden image (reference path only)
+    {  // MLP: fc1 + GELU into the fp16 hidden image, then fc2 + LayerNorm + residual
       AImage A{xh, xh, nkb, 0};
       Epi2F16<true, true> e{reinterpret_cast<__half*>(ws.hidh), 0, 4 * nkb, b.fc1_b};
       if ((rc = gemm2<192, 8>(KT_FC1, A, e, b.fc1, R, ws.scratch, st))) return rc;
       AImage A2{ws.hidh, ws.hidh, 4 * nkb, 0};
       ELn e2{x, C, xh, nkb, b.fc2_b, b.ln2_g, b.ln2_b, cfg.ln_eps};
-      rc = C == 192 ? gemm2<192, 8>(KT_FC2, A2, e2, b.fc2, R, ws.scratch, st)
-                    : gemm2<384, 8>(KT_FC2, A2, e2, b.fc2, R, ws.scratch, st);
-      return rc;
-    }
-#endif
-    {  // fused MLP: fc1 + GELU + fc2 + LayerNorm + residual, hidden stays on the SM
-      ELn e2{x, C, xh, nkb, b.fc2_b, b.ln2_g, b.ln2_b, cfg.ln_eps};
-      KTag tag = KT_MLP;
 #ifdef SKY_EXPERIMENTS
       e2.exp = exp_ln;
-      if (prof_split && C == 384) tag = KT_FC2;
 #endif
-      prof_begin(tag, st);
-      count_launch();
-#ifdef SKY_EXPERIMENTS
-      if (!(C == 192 ? mlp_pair192 : mlp_pair384))
-        rc = C == 192 ? launch_mlp_fused<192, ELn>(xh, e2, b.fc1f.img, b.fc2.img, b.fc1_b, R, num_sms, st)
-                      : launch_mlp_fused<384, ELn>(xh, e2, b.fc1f.img, b.fc2.img, b.fc1_b, R, num_sms, st);
-      else
-#endif
-        rc = C == 192 ? launch_mlp_fused_pair<192, ELn>(xh, e2, b.fc1f.img, b.fc2.img, b.fc1_b, R, num_sms, st)
-                      : launch_mlp_fused_pair<384, ELn>(xh, e2, b.fc1f.img, b.fc2.img, b.fc1_b, R, num_sms, st);
-      prof_end(tag, st);
+      if (C == 384 && proj_split && !use_ref) {
+        prof_begin(KT_FC2, st);
+        count_launch();
+        rc = launch_gemm_split<ELn, 8, 192>(A2, e2, b.fc2_s.img, R, 4 * C, num_sms, st);
+        prof_end(KT_FC2, st);
+      } else {
+        rc = C == 192 ? gemm2<192, 8>(KT_FC2, A2, e2, b.fc2, R, ws.scratch, st)
+                      : gemm2<384, 8>(KT_FC2, A2, e2, b.fc2, R, ws.scratch, st);
+      }
       if (rc) return rc;
     }
     if (range_guard) {   // fp16 operand images of this block (whole tiles only: the tail rows of the last tile are never written)

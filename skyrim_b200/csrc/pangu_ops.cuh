@@ -1,6 +1,6 @@
 // Pangu-Weather step: the A-operand producers (gather + normalise + fp32->fp16) and the
 // accumulator epilogues (bias / GELU / LayerNorm + residual / scatter) that are fused
-// into the GEMM kernels.  Both the tcgen05 GEMM (gemm_tc.cuh) and the plain reference
+// into the GEMM kernels.  Both the wgmma GEMM (gemm_tc.cuh) and the plain reference
 // GEMM (gemm_ref.cuh, test infrastructure on the device) are templated on these, so the
 // index arithmetic is written once.
 //
@@ -184,7 +184,7 @@ struct ProdEmbedSurf {
 
 // ======================================================================================
 // Epilogues.  Model: one lane owns one accumulator row; `acc.load32(col, v)` is a
-// warp-collective read of 32 consecutive columns of the lane's row (TMEM or scratch).
+// warp-collective read of 32 consecutive columns of the lane's row (staged accumulator or scratch).
 // `row` may be >= M (tail tile): loads still execute, stores are predicated off.
 // n0 = first column of this tile in the full N, BN = tile width.
 // ======================================================================================

@@ -1,11 +1,11 @@
-// FourCastNet-v2-small SFNO 6-h step operator on sm_100a.  Replaces what
-// /root/reference/skyrim/core/models/fourcastnet_v2.py:36-37 loads (earth2mip fcnv2_sm: torch +
-// torch_harmonics) and what models/utils.py:34 steps.  Architecture: SURVEY.md Appendix B,
+// FourCastNet-v2-small SFNO 6-h step operator on sm_90a.  Replaces what Skyrim's FourCastNet-v2
+// model (skyrim/core/models/fourcastnet_v2.py) loads (earth2mip fcnv2_sm: torch + torch_harmonics)
+// and what models/utils.py steps.  Architecture: SURVEY.md Appendix B,
 // free choices in DESIGN.md §2; oracle: oracle/sfno_ref.py.
 //
 // Every contraction of the step — per-pixel MLPs, the truncated longitude DFT, the Legendre
 // transforms (one GEMM per zonal wavenumber m), the per-degree complex channel mixing (one GEMM
-// per l) and their inverses — runs on the batched TMA-fed tcgen05 GEMMs (gemm_batched.cuh, gemm_tb.cuh) with
+// per l) and their inverses — runs on the batched TMA-fed wgmma GEMMs (gemm_batched.cuh, gemm_tb.cuh) with
 // 3-term fp16 splitting (a_hi*w_hi + a_lo*w_hi + a_hi*w_lo, ~22-bit mantissa: single-pass fp16
 // misses the 1e-3 budget on this network, DESIGN.md §2).
 // The spherical transforms are a chain of four "table x data" GEMMs around the mixing GEMM; the data is always the

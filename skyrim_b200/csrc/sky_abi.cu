@@ -95,7 +95,7 @@ __global__ void __launch_bounds__(256) k_absmax_half(const uint4* __restrict__ p
 int Engine::range_scan(int slot, const void* img, size_t bytes, cudaStream_t st) {
   if (!range_guard || !range_dev || !img || bytes < 16) return 0;
   const size_t n16 = bytes / 16;
-  const unsigned grid = (unsigned)std::min<size_t>((n16 + 255) / 256, 148 * 8);
+  const unsigned grid = (unsigned)std::min<size_t>((n16 + 255) / 256, (size_t)num_sms * 8);
   k_absmax_half<<<grid, 256, 0, st>>>(reinterpret_cast<const uint4*>(img), n16, range_dev + slot);
   SKY_CUDA_OK(cudaGetLastError());
   return 0;
@@ -267,8 +267,8 @@ int sky_model_create(sky_model_t** out, int kind, const void* cfg, size_t cfg_by
   DeviceGuard guard(device);
   cudaDeviceProp prop;
   SKY_CUDA_OK(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) {
-    set_error("device %d is sm_%d%d; this library contains sm_100a code only", device, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("device %d is sm_%d%d; this library contains sm_90a code only", device, prop.major, prop.minor);
     return SKY_ERR_CUDA;
   }
   Engine* e = nullptr;

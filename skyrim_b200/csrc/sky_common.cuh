@@ -1,5 +1,5 @@
-// Common device helpers for the sm_100a kernels: mbarrier, bulk-copy (TMA engine),
-// tcgen05 / TMEM wrappers, swizzle math, small math utilities.
+// Common device helpers for the sm_90a kernels: mbarrier, bulk-copy (TMA engine), wgmma
+// descriptors and fences, swizzle math, small math utilities.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -72,8 +72,7 @@ __device__ __forceinline__ bool elect_one() {
 //     gelu(x) = relu(x) - |x| h(|x|),   h(a) = Phi(-a) = 0.5 erfcx(a/sqrt 2) exp(-a^2/2)
 // with 0.5 erfcx(a/sqrt 2) replaced by a degree-7 polynomial fitted on [0, 6] under the weight
 // exp(-a^2/2) (tools/fit_gelu.py): max abs error 1.2e-5, 20x below the fp16 rounding the value
-// receives next.  One MUFU (ex2) per element — the earlier rcp+ex2 form made the fused-MLP
-// epilogue MUFU bound (16 lanes/clk/SM on sm_100).
+// receives next.  One MUFU (ex2) per element instead of an rcp + ex2 pair.
 __device__ __forceinline__ float mufu_rcp(float x) {
   float r;
   asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x));
@@ -102,47 +101,10 @@ __device__ __forceinline__ float gelu_erf(float x) {
   p = fmaf(p, a, SKY_GELU_C0);
   return fmaf(-a, p * e, fmaxf(x, 0.f));
 }
-// two lanes of the same formula on the packed fp32x2 pipe (FFMA2 / FMUL2, sm_100)
-__device__ __forceinline__ uint64_t pack_f32x2(float a, float b) {
-  uint64_t d;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(d) : "f"(a), "f"(b));
-  return d;
-}
-__device__ __forceinline__ void unpack_f32x2(uint64_t d, float& a, float& b) {
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(a), "=f"(b) : "l"(d));
-}
-__device__ __forceinline__ uint64_t fma_f32x2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-__device__ __forceinline__ uint64_t mul_f32x2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-__device__ __forceinline__ uint64_t add_f32x2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
 // (x0, x1) <- gelu(x0 + b0), gelu(x1 + b1)
 __device__ __forceinline__ void gelu_erf_x2(float& x0, float& x1, float b0, float b1) {
-  const uint64_t x = add_f32x2(pack_f32x2(x0, x1), pack_f32x2(b0, b1));
-  float y0, y1, a0, a1;
-  unpack_f32x2(x, y0, y1);
-  unpack_f32x2(mul_f32x2(mul_f32x2(x, x), pack_f32x2(SKY_GELU_EC, SKY_GELU_EC)), a0, a1);
-  const uint64_t e = pack_f32x2(mufu_ex2(a0), mufu_ex2(a1));
-  const uint64_t ax = pack_f32x2(fabsf(y0), fabsf(y1));
-#define SKY_P2(c) pack_f32x2(c, c)
-  uint64_t p = fma_f32x2(SKY_P2(SKY_GELU_C7), ax, SKY_P2(SKY_GELU_C6));
-  p = fma_f32x2(p, ax, SKY_P2(SKY_GELU_C5)); p = fma_f32x2(p, ax, SKY_P2(SKY_GELU_C4));
-  p = fma_f32x2(p, ax, SKY_P2(SKY_GELU_C3)); p = fma_f32x2(p, ax, SKY_P2(SKY_GELU_C2));
-  p = fma_f32x2(p, ax, SKY_P2(SKY_GELU_C1)); p = fma_f32x2(p, ax, SKY_P2(SKY_GELU_C0));
-#undef SKY_P2
-  const uint64_t q = mul_f32x2(p, e);
-  const uint64_t r = fma_f32x2(pack_f32x2(-fabsf(y0), -fabsf(y1)), q, pack_f32x2(fmaxf(y0, 0.f), fmaxf(y1, 0.f)));
-  unpack_f32x2(r, x0, x1);
+  x0 = gelu_erf(x0 + b0);
+  x1 = gelu_erf(x1 + b1);
 }
 
 // explicit shared-space accessors (a generic LD/ST through a pointer kept in a struct costs a
@@ -168,21 +130,22 @@ __device__ __forceinline__ void sts_f32(uint32_t a, float v) {
   asm volatile("st.shared.f32 [%0], %1;" ::"r"(a), "f"(v) : "memory");
 }
 
-// 256-bit global accesses (sm_100, PTX 8.8): one full 32-byte sector per lane.  Used by the
-// row-owner epilogues, where lane i owns token row i and the warp touches 32 different lines.
+// 32-byte global accesses as two 128-bit halves.  Used by the row-owner epilogues, where lane i
+// owns token row i and the warp touches 32 different lines.
 __device__ __forceinline__ void ldg_f32x8(const float* p, float* v) {
-  asm volatile("ld.global.L1::no_allocate.v8.f32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]), "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7])
-               : "l"(p));
+  asm volatile("ld.global.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"
+               : "=f"(v[0]), "=f"(v[1]), "=f"(v[2]), "=f"(v[3]) : "l"(p));
+  asm volatile("ld.global.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"
+               : "=f"(v[4]), "=f"(v[5]), "=f"(v[6]), "=f"(v[7]) : "l"(p + 4));
 }
 __device__ __forceinline__ void stg_f32x8(float* p, const float* v) {
-  asm volatile("st.global.v8.f32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]),
-               "f"(v[3]), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7])
-               : "memory");
+  asm volatile("st.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v[0]), "f"(v[1]), "f"(v[2]), "f"(v[3]) : "memory");
+  asm volatile("st.global.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p + 4), "f"(v[4]), "f"(v[5]), "f"(v[6]), "f"(v[7]) : "memory");
 }
 __device__ __forceinline__ void stg_b32x8(void* p, uint4 lo, uint4 hi) {
-  asm volatile("st.global.v8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"l"(p), "r"(lo.x), "r"(lo.y), "r"(lo.z),
-               "r"(lo.w), "r"(hi.x), "r"(hi.y), "r"(hi.z), "r"(hi.w)
+  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(p), "r"(lo.x), "r"(lo.y), "r"(lo.z), "r"(lo.w) : "memory");
+  asm volatile("st.global.v4.b32 [%0], {%1, %2, %3, %4};" ::"l"(static_cast<char*>(p) + 16), "r"(hi.x), "r"(hi.y), "r"(hi.z),
+               "r"(hi.w)
                : "memory");
 }
 
@@ -234,7 +197,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "r"(parity), "r"(0x989680)
       : "memory");
 }
-// generic-proxy smem writes -> visible to the async proxy (UMMA / bulk copy)
+// generic-proxy smem writes -> visible to the async proxy (wgmma / bulk copy)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -253,81 +216,59 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
 }
 
 // ---------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (warpgroup MMA).  A warpgroup of four consecutive warps issues m64nNk16 products
+// (wgmma_ops.cuh) with both operands read from shared memory through 64-bit descriptors and
+// fp32 accumulators in its registers: thread (warp w of the group, lane l) holds, per 8-column
+// group i, rows 16w + l/4 and 16w + l/4 + 8, columns 8i + 2(l%4) and 8i + 2(l%4) + 1.
 // ---------------------------------------------------------------------------------------
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]^T, fp16 operands, fp32 accumulate
-__device__ __forceinline__ void tc_mma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b,
-                                           uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// shared-memory matrix descriptor: K-major operand, SWIZZLE_128B, rows of 128 bytes,
-// 8-row groups 1024 bytes apart (cute::UMMA::SmemDescriptor, version 1 = Blackwell)
+// K-major operand, SWIZZLE_128B, rows of 128 bytes, 8-row groups 1024 bytes apart (SBO);
+// +2 in the address field = +32 B = one K=16 step inside the swizzle row
 __device__ __forceinline__ uint64_t make_desc_sw128(uint32_t smem_addr_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((smem_addr_bytes & 0x3FFFFu) >> 4);  // start address  [0,14)
-  d |= (uint64_t)1 << 16;                              // LBO (unused for swizzled K-major) = 1
+  d |= (uint64_t)1 << 16;                              // LBO (unused for swizzled K-major)
   d |= (uint64_t)(1024 >> 4) << 32;                    // SBO = 1024 B
-  d |= (uint64_t)1 << 46;                              // descriptor version (sm_100)
-  d |= (uint64_t)2 << 61;                              // layout type SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                              // layout type SWIZZLE_128B
   return d;
 }
-// instruction descriptor: A,B = F16 K-major, D = F32, shape M x N
-__host__ __device__ constexpr uint32_t make_idesc_f16(int M, int N) {
-  return (1u << 4) | (0u << 7) | (0u << 10) | (0u << 15) | (0u << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
+// MN-major operand, SWIZZLE_128B: atoms of [8 k-rows][64 elements = 128 B], 8-row K groups SBO = 1024 B apart,
+// 64-element MN blocks `lbo` bytes apart; +128 in the address field = +2048 B = one K=16 step
+__device__ __forceinline__ uint64_t make_desc_sw128_mn(uint32_t smem_addr_bytes, uint32_t lbo) {
+  uint64_t d = make_desc_sw128(smem_addr_bytes);
+  return (d & ~((uint64_t)0x3FFF << 16)) | ((uint64_t)(lbo >> 4) << 16);
 }
-// 32 lanes x 32 columns of fp32: thread i of the warp receives lane (base_lane + i),
-// columns [col, col+32).  The warp may only touch lanes 32*(warp_id%4) .. +31.
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float (&v)[32]) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  __syncwarp();  // .sync.aligned: the warp must be converged
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// pin accumulator registers behind the preceding wait (register reads may not be hoisted above it)
+template <int N>
+__device__ __forceinline__ void wgmma_fence_operands(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+__device__ __forceinline__ void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
+// Accumulator tile staged in shared memory, row-major fp32 with `ld` floats per row (ld % 32 == 4: the
+// row-owner reads of a quarter warp hit 8 different bank quads).  acc.load32(c, v): the calling lane's
+// row, columns [c, c+32) — the interface every epilogue is written against.
+struct AccSmem {
+  uint32_t row_s;  // shared-space address of the lane's row
+  __device__ void load32(int c, float (&v)[32]) const {
+    const uint32_t a = row_s + (uint32_t)c * 4u;
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];"
+                   : "=f"(v[4 * j]), "=f"(v[4 * j + 1]), "=f"(v[4 * j + 2]), "=f"(v[4 * j + 3])
+                   : "r"(a + 16u * j));
+    }
+  }
+};
+
 // ---------------------------------------------------------------------------------------
-// CTA pairs (cluster of 2): tcgen05 cta_group::2.  One thread of the even CTA issues an
-// M=256 MMA; each CTA supplies its own 128 rows of A and N/2 rows of B from its own shared
-// memory (same offsets in both) and receives its own 128 rows x N of D in its own TMEM.
+// clusters: distributed shared memory and cluster-scope barriers
 // ---------------------------------------------------------------------------------------
 __device__ __forceinline__ uint32_t cluster_ctarank() {
   uint32_t r;
@@ -342,71 +283,6 @@ __device__ __forceinline__ uint32_t mapa_u32(uint32_t local_smem_addr, uint32_t 
   uint32_t r;
   asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_smem_addr), "r"(rank));
   return r;
-}
-// Remote arrive on an mbarrier of another CTA of the cluster.  .relaxed on purpose: the default
-// .release.cluster compiles to MEMBAR.ALL.GPU in front of every arrive (~1k cycles each, measured:
-// profiles/r1_mlp_pair.md).  Every use here signals "my TMEM reads finished" or "data that a bulk
-// copy / my fenced st.shared put into MY shared memory is ready for the tensor core", none of which
-// publishes generic-proxy global writes, so no cumulativity is needed.
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.relaxed.cluster.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// wait with cluster-scope acquire (the arrivals may come from the peer CTA)
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "SKY_WAITC_%=:\n\t"
-      "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1, %2;\n\t"
-      "@p bra SKY_DONEC_%=;\n\t"
-      "bra SKY_WAITC_%=;\n\t"
-      "SKY_DONEC_%=:\n\t}\n" ::"r"(smem_u32(bar)),
-      "r"(parity), "r"(0x989680)
-      : "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_result) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_result)),
-               "n"(kCols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-// arrive on the mbarrier at this offset in BOTH CTAs of the pair once the MMAs issued so far are done
-__device__ __forceinline__ void tc_commit_pair(uint64_t* bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-          smem_u32(bar)),
-      "h"((uint16_t)3)
-      : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16_pair(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                                                uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// two 32-column TMEM loads in flight, one wait
-__device__ __forceinline__ void tmem_ld32_nowait(uint32_t taddr, float (&v)[32]) {
-  uint32_t* r = reinterpret_cast<uint32_t*>(v);
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 }
 
 }  // namespace sky

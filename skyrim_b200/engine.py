@@ -63,7 +63,7 @@ class StepEngine:
     def __init__(self, cfg, device: int = 0, lib: str | None = None, graph=None):
         import torch
         if not torch.cuda.is_available():
-            raise _ffi.SkyError("skyrim_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise _ffi.SkyError("skyrim_b200 needs a CUDA device (sm_90a, H100); there is no CPU fallback")
         self.cfg = cfg
         self.device = device
         self.torch = torch

@@ -1,5 +1,5 @@
 """`forecast` command line — mirrors /root/reference/skyrim/forecast.py:19-151 (same option names, short flags and
-defaults; same `run_forecast` signature and return value) on top of the B200 engine:
+defaults; same `run_forecast` signature and return value) on top of the H100 engine:
 
     python -m skyrim_b200.forecast -m pangu -d 20240507 -t 0000 -l 24 -o outputs
 

@@ -39,8 +39,9 @@ def pangu_bytes(cfg: PanguConfig) -> dict:
       qkv    read xh 2 B, write q|k|v window images 3 x 2 B (padded tokens included)
       attn   read q|k|v 6 B, write the projection's operand image 2 B
       proj   read operand image 2 B, residual read from xh 2 B, xh written in place 2 B
-      mlp    read xh 2 B (operand; the epilogue re-reads the same image as the residual: an L2 hit, ncu profiles/r2f_traffic.json),
-             xh written in place 2 B (the 4C hidden activation never leaves the SM)
+      mlp    read xh 2 B (operand; the epilogue re-reads the same image as the residual: an L2 hit), xh written in place 2 B
+             (the 4C hidden activation is not mandatory traffic: the H100 engine moves it through HBM as fc1's fp16 image,
+             8 B written and 8 B read per token and feature, which these figures do not count)
     (with the fp32 token stream, "fp32_stream", proj and mlp move 12 B)"""
     C = cfg.dim
     HW = cfg.H * cfg.W

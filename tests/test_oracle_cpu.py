@@ -90,7 +90,7 @@ def test_operator_is_periodic_in_longitude():
 
 
 def test_fp16_operand_error_budget(small):
-    """What tcgen05 kind::f16 does (fp16 operands, fp32 accumulate) stays inside the 1e-3 budget;
+    """What the tensor-core GEMMs do (fp16 operands, fp32 accumulate) stays inside the 1e-3 budget;
     bf16 operands would not — the reason the engine computes in fp16."""
     cfg, w, x0 = small
     y64 = PanguRef(cfg, w, torch.float64).step(x0).numpy()

@@ -127,12 +127,13 @@ def test_full_size_fixtures_match_the_seeded_inputs():
     """tests/golden/*_721x1440_seed0.npz (one real oracle step each, tools/make_golden_full.py): the committed IC
     sample must equal what skyrim_b200.weights regenerates, or the GPU-side comparison would be meaningless."""
     from skyrim_b200.config import PANGU_CHANNELS
-    from skyrim_b200.verify import load_fixture
+    from skyrim_b200.verify import BLOCK_PX, SAMPLE_STEP, load_fixture
     for model, names in (("pangu", PANGU_CHANNELS), ("sfno", FCNV2_CHANNELS)):
         fx = load_fixture(model)
         x0 = synthetic_state(names, 721, 1440, 0)
         np.testing.assert_array_equal(x0[:, ::64, ::64], fx["x0_sample"])
-        assert fx["y_sample"].shape == (len(names), 56, 85) and np.isfinite(fx["y_block"]).all()
+        assert fx["y_sample"].shape == (len(names), -(-721 // SAMPLE_STEP[0]), -(-1440 // SAMPLE_STEP[1]))
+        assert fx["y_block"].shape == (len(names), 720 // BLOCK_PX, 1440 // BLOCK_PX) and np.isfinite(fx["y_block"]).all()
         assert (fx["y_std"] > 0).all() and float(fx["oracle_seconds"]) > 1.0
 
 

@@ -18,7 +18,7 @@ ref = PanguRef(cfg, w, torch.float32)
 stages = ref.stages(x0)
 names = ["embed", "layer0", "down", "layer1", "layer2", "up", "layer3"]
 xin = torch.from_numpy(x0)[None].cuda()
-# modes: tc = product library; ref = dev library, CUDA-core GEMMs + tcgen05 attention; refattn = dev library,
+# modes: tc = product library; ref = dev library, CUDA-core GEMMs + tensor-core attention; refattn = dev library,
 # CUDA-core GEMMs + CUDA-core attention (bisects window image / index math from the tensor pipelines)
 for mode in (sys.argv[3:] or ["refattn", "ref", "tc"]):
     os.environ["SKY_GEMM"] = "ref" if mode.startswith("ref") else "tc"   # read by the development library only

@@ -7,15 +7,14 @@
                                                 # of the network's tendency (state = x + 0.1 sigma x tendency: a 1e-3 bound on the
                                                 # state alone would hide a 1e-2 error of the network)
 
-writes tests/golden/{pangu,sfno}_721x1440_seed0.npz holding, per channel,
-  y_sample   y[:, ::13, ::17]                   point values (56 x 85): strides 13 / 17 are coprime to the 4x4 patch and the 12-token windows, so the
-                                                sample visits every intra-patch position (a stride of 16 saw only position (0, 0))
-  y_block    16x16 block means of y[:, :720]    every pixel of rows 0..719 enters exactly one mean (45 x 90)
-  y_last     y[:, 720, ::4]                     the odd last latitude row (padding edge of the patch grid)
+writes tests/golden/{pangu,sfno,graphcast}_721x1440_seed0.npz holding, per channel (skyrim_b200/verify.py summarise_field),
+  y_sample   y[:, ::39, ::51]                   point values (19 x 29): odd strides, so the sample visits every position
+                                                inside a 4x4 patch (a stride of 16 saw only position (0, 0))
+  y_block    48x48 block means of y[:, :720]    every pixel of rows 0..719 enters exactly one mean (15 x 30)
+  y_last     y[:, 720, ::8]                     the odd last latitude row (padding edge of the patch grid)
   y_norm, y_mean, y_std                         per-channel L2 norm / mean / standard deviation of the full field
 so that tests/test_fullsize_gpu.py and bench.py can compare a full-size CUDA step with the oracle without
-re-running it (the GPU box has no /root/reference and its minutes are budgeted).  Seeded weights and IC are
-regenerated bit-identically from skyrim_b200/weights.py; x0_sample pins that.
+re-running it.  Seeded weights and IC are regenerated bit-identically from skyrim_b200/weights.py; x0_sample pins that.
 """
 import os, sys, time
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -23,12 +22,7 @@ sys.path.insert(0, ROOT)
 import numpy as np, torch
 
 
-def summarise(y):
-    y = np.asarray(y, dtype=np.float64)
-    blk = y[:, :720].reshape(y.shape[0], 45, 16, 90, 16).mean(axis=(2, 4))
-    return dict(y_sample=y[:, ::13, ::17].astype(np.float32), y_block=blk.astype(np.float32),
-                y_last=y[:, 720, ::4].astype(np.float32), y_norm=np.sqrt((y ** 2).sum(axis=(1, 2))),
-                y_mean=y.mean(axis=(1, 2)), y_std=y.std(axis=(1, 2)))
+from skyrim_b200.verify import summarise_field  # noqa: E402
 
 
 def main(which):
@@ -58,7 +52,7 @@ def main(which):
         print(f"graph + weights + IC: {time.time() - t0:.1f} s", flush=True)
         ynew, tend = GraphCastRef(cfg, w, graph, torch.float32).step(x0, T0, return_tendency=True)
         y = ynew.numpy()[cfg.n_state:cfg.n_state + cfg.n_prog]
-        extra = {"t_" + k[2:]: v for k, v in summarise(tend.numpy().T.reshape(cfg.n_prog, cfg.nlat, cfg.nlon)).items()}
+        extra = summarise_field(tend.numpy().T.reshape(cfg.n_prog, cfg.nlat, cfg.nlon), "t_")
         extra["t0"] = np.float64(T0)
     else:
         from skyrim_b200.config import FCNV2_CHANNELS, sfno_full
@@ -68,7 +62,7 @@ def main(which):
         w = make_sfno_weights(cfg, 0)
         x0 = synthetic_state(FCNV2_CHANNELS, cfg.nlat, cfg.nlon, 0)
         y = SFNORef(cfg, w, torch.float32).step(x0).numpy()
-    d = summarise(y)
+    d = summarise_field(y)
     if which == "graphcast":
         d.update(extra)
     d["x0_sample"] = x0[:, ::64, ::64].astype(np.float32)
