@@ -81,7 +81,6 @@ __device__ __forceinline__ long long at_row_token(const Geo& g, int roll, int b,
 // ---------------------------------------------------------------------------------------------------------------
 struct EpiQkvWin {
   static constexpr bool kNeedsBias = false;
-  static constexpr bool kHasPre = false;
   uint8_t* out; long long part_stride; const float* bias; Geo g; int roll; int C; int pairs;
   const float* gamma = nullptr; const float* beta = nullptr;   // unused (uniform epilogue interface)
 #ifdef SKY_EXPERIMENTS

@@ -1,13 +1,14 @@
-// TMA-fed persistent wgmma GEMM (v2 data flow):
+// TMA-fed persistent wgmma GEMM (v2 data flow), k_gemm2 / k_gemm2_pair:
 //
-//   D[M, N] = A[M, K] * W[N, K]^T -> fused epilogue
+//   D[M, N] = A[M, K] * W[N, K]^T -> fused epilogue        (optionally per batch)
 //
 // Both operands arrive as pre-built SWIZZLE_128B "tile images" and are fetched by ONE thread
 // with 1-D bulk copies through the TMA engine (cp.async.bulk + mbarrier complete_tx):
 //   A image  [ceil(M/128)][K/64][128 rows x 128 B]   fp16 activations, written in this layout
 //                                                     by the epilogue of the producing kernel
 //   W image  [N/BLOCK_N][K/64][BLOCK_N rows x 128 B]  packed once at weight load
-// so no warp ever touches the operands with ld/st.  Warp roles: 0..7 = two consumer warpgroups,
+// so no warp ever touches the operands with ld/st.  A schedule (SchedW here, SchedTB in gemm_tb.cuh) decides which
+// images a tile's k-blocks come from; the pipeline is the same for all.  Warp roles: 0..7 = two consumer warpgroups,
 // 8 = loader.  Warpgroup g issues the wgmma products of rows 64g .. 64g+63 of the 128-row tile
 // over all BLOCK_N columns (fp32 accumulators in registers, BLOCK_N / 2 per thread).  At the end of
 // a tile both warpgroups stage their accumulators in shared memory — over the operand ring, which
@@ -16,6 +17,10 @@
 // accumulator blocks through a padded smem patch so that every global access is a full
 // 64/128-byte row segment.
 #pragma once
+#include <climits>
+#include <type_traits>
+
+#include "../../include/skyrim_b200.h"
 #include "pangu_ops.cuh"
 #include "wgmma_ops.cuh"
 
@@ -34,21 +39,33 @@ __device__ __forceinline__ size_t img_offset(long long row, int col, int nkb) {
   return ((size_t)tile * nkb + (col >> 6)) * (size_t)G2_A_BYTES + sw128_offset(r, (col & 63) >> 3) + (col & 7) * 2;
 }
 
-// A operand made of one or two images concatenated along K (patch recovery reads
-// concat(skip, x) without materialising it)
-struct AImage {
-  const uint8_t* img0; const uint8_t* img1;
-  int nkb0, nkb1;  // k-blocks per row tile in each image
-  // optional third / fourth part (GraphCast's mesh2grid node update: [v | e0 | e1 | e2]); nkb2 = nkb3 = 0 when unused
-  const uint8_t* img2 = nullptr; const uint8_t* img3 = nullptr;
-  int nkb2 = 0, nkb3 = 0;
-  __device__ const uint8_t* kblock(int mt, int kb) const {
-    if (kb < nkb0) return img0 + ((size_t)mt * nkb0 + kb) * G2_A_BYTES;
-    kb -= nkb0;
-    if (kb < nkb1 || nkb2 == 0) return img1 + ((size_t)mt * nkb1 + kb) * G2_A_BYTES;
-    kb -= nkb1;
-    if (kb < nkb2) return img2 + ((size_t)mt * nkb2 + kb) * G2_A_BYTES;
-    return img3 + ((size_t)mt * nkb3 + (kb - nkb2)) * G2_A_BYTES;
+// A operand: up to 6 fp16 tile images concatenated along K, so that a concatenation is never materialised (patch
+// recovery: concat(skip, x); GraphCast's mesh2grid node update: [v | e0 | e1 | e2]; SFNO: the 3-term fp16 split
+// A = [hi | lo | hi], DESIGN.md §2, and the decoder's concat(x, input)).  In a batched launch every segment has its own
+// image per batch, batch_stride bytes apart.
+struct AOperand {
+  const uint8_t* seg[6] = {};
+  int nkb[6] = {};                 // k-blocks per row tile of each segment
+  long long batch_stride[6] = {};  // bytes between batches of each segment
+  int nseg = 0;
+  AOperand() = default;
+  AOperand(const uint8_t* img, int k) { add(img, k); }
+  // appends a segment of k k-blocks per row tile
+  AOperand& add(const uint8_t* img, int k, long long bstride = 0) {
+    seg[nseg] = img; nkb[nseg] = k; batch_stride[nseg] = bstride; ++nseg;
+    return *this;
+  }
+  // The loader calls this once per k-block, so it is kept short: a single image needs no walk, and the walk over several
+  // is done by selects (unused segments have nkb = 0), without branches.
+  __device__ const uint8_t* kblock(int batch, int mt, int kb) const {
+    if (nseg == 1) return seg[0] + (size_t)batch * batch_stride[0] + ((size_t)mt * nkb[0] + kb) * G2_A_BYTES;
+    const uint8_t* p = seg[0];
+    long long bs = batch_stride[0];
+    int n = nkb[0];
+#pragma unroll
+    for (int s = 1; s < 6; ++s)
+      if (kb >= n) { kb -= n; p = seg[s]; bs = batch_stride[s]; n = nkb[s]; }
+    return p + (size_t)batch * bs + ((size_t)mt * n + kb) * G2_A_BYTES;
   }
 };
 
@@ -78,6 +95,7 @@ struct EpiCtx {
   long long row0;   // first row of this warp's 32-row group
   long long M;
   int lane;
+  int batch = 0;    // batch of the tile (batched launches; 0 otherwise)
   int n0;           // first column of the tile in the full N
   int part, nparts; // column-chunk partition among the warps sharing a lane quarter
   float* patch;     // [32][33] floats, private to the warp
@@ -88,7 +106,7 @@ struct EpiCtx {
   // per-row-group scratch an epilogue may cache across the n-tiles of one m-tile (EpiQkvWin: destination row of this lane)
   mutable long long aux_row0 = -1;
   mutable int aux = 0, aux2 = 0;
-  // row-statistics exchange with the peer CTA of a column-split pair (gemm_split.cuh); x_own_bar == nullptr elsewhere
+  // row-statistics exchange with the peer CTA of a column-split pair (k_gemm2_pair); x_own_bar == nullptr elsewhere
   uint64_t* x_own_bar = nullptr;   // completes when the peer's 32 (sum, sum of squares) pairs of this lane quarter landed
   uint32_t x_own_stat = 0;         // shared-space address of this CTA's slot: 32 x {float s, ss}
   uint32_t x_peer_stat = 0, x_peer_bar = 0;   // shared::cluster addresses of the same slot / barrier in the peer CTA
@@ -189,10 +207,103 @@ __device__ __forceinline__ void wg_epilogue(const Acc& acc, uint8_t* smem, int l
   fence_proxy_async_smem();   // the staging's generic accesses are ordered before the next bulk copies into the ring
 }
 
-template <class Epi, int BLOCK_N, int EPI_WARPS>
-__global__ void __launch_bounds__((EPI_WARPS + 1) * 32, 1)
-k_gemm2(const AImage A, const Epi epi, const uint8_t* __restrict__ Wimg, long long M, int num_kb,
-        int num_m_tiles, int num_n_tiles) {
+// ---------------------------------------------------------------------------------------------------------------
+// Per-channel statistics of the CTA (SFNO epilogues with kCtaStats)
+// ---------------------------------------------------------------------------------------------------------------
+// Epilogues that gather per-channel statistics keep them in shared memory for the CTA's whole (persistent) life and flush
+// them with ONE fp64 atomic per channel and CTA at kernel end: per-chunk global atomics (26 M on 768 addresses for a
+// full-resolution GEMM) were the bottleneck of those epilogues (ncu r2b: 2.0 ms against 1.07 ms for the same GEMM with a
+// plain store).  Layout of the CTA accumulators (fp64): sums at [0, 384), sums of squares at [384, 768) of the bias region.
+template <class E, class = void> struct has_cta_stats : std::false_type {};
+template <class E> struct has_cta_stats<E, std::void_t<decltype(E::kCtaStats)>> : std::true_type {};
+constexpr int CTA_STATS_MAX = 384;   // channels: 2 x 384 fp64 accumulators fill the 6 KB bias region
+// fp64 accumulators: the order in which the warps of a CTA (and then the CTAs) add their fp32 partial sums is not fixed;
+// in fp64 the order changes the result by ~1e-16 relative, i.e. the fp32 scale / shift derived from it are reproducible
+// from run to run (fp32 accumulators were not: 1e-7 differences in the statistics)
+__device__ __forceinline__ void red_shared_f64(uint32_t addr, double v) {
+  asm volatile("red.shared.add.f64 [%0], %1;" ::"r"(addr), "d"(v) : "memory");
+}
+template <class Epi>
+__device__ __forceinline__ void cta_stats_flush(const Epi& epi, const float* sbias) {
+  if constexpr (has_cta_stats<Epi>::value) {
+    if (epi.sums) {
+      const double* acc = reinterpret_cast<const double*>(sbias);
+      for (int i = threadIdx.x; i < 2 * epi.n_valid; i += blockDim.x)
+        atomicAdd(epi.sums + i, acc[(i < epi.n_valid ? 0 : CTA_STATS_MAX) + (i < epi.n_valid ? i : i - epi.n_valid)]);
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Schedules: which bytes the loader fetches for a tile.  The kernel walks the tiles of D[batches][M, N] (n-tile fastest)
+// persistently; a schedule maps a tile to (batch, m-tile, n-tile, skip) and issues the bulk copies of its k-blocks.
+// ---------------------------------------------------------------------------------------------------------------
+struct G2Grid {
+  long long M;
+  int num_m_tiles, num_n_tiles, batches;
+  __host__ __device__ long long num_tiles() const { return (long long)num_m_tiles * num_n_tiles * batches; }
+};
+struct G2Tile {
+  int b, mt, nt;
+  bool skip;
+  __device__ static G2Tile at(const G2Grid& g, int tile) {
+    const int tiles_per_batch = g.num_m_tiles * g.num_n_tiles;
+    const int b = tile / tiles_per_batch, t = tile % tiles_per_batch;
+    return {b, t / g.num_n_tiles, t % g.num_n_tiles, false};
+  }
+};
+
+// Weights: D_b = A_b W_b^T with A an AOperand and W the image [batches][N / BLOCK_N][num_kb - w_rep][BLOCK_N rows x 128 B]
+// packed at weight load.  w_rep > 0: W = [hi | lo] with w_rep k-blocks each, consumed as hi, hi, lo against A = [hi | lo | hi]
+// (the 3-term split of the SFNO GEMMs).
+// kTri: batch b only has rows 0 .. b (degree l of a spectrum holds orders m <= l): row tiles that start past row b are
+// skipped by every role (their output is multiplied by zeros downstream).  A compile-time choice: the run-time test in
+// the consumers' tile loop alone costs registers (and spills) in every other instantiation.
+template <bool kTri = false>
+struct SchedW {
+  static constexpr bool kBMN = false;
+  AOperand A;
+  const uint8_t* W;
+  int num_kb;
+  long long w_batch_stride = 0;   // bytes
+  int w_rep = 0;
+  struct Tile : G2Tile {
+    const uint8_t* w;   // the tile's W image: k-block 0 of its batch and n-tile
+  };
+  template <int BN>
+  __device__ Tile tile(const G2Grid& g, int i) const {
+    Tile t{G2Tile::at(g, i), nullptr};
+    t.skip = kTri && t.mt * G2_BLOCK_M > t.b;
+    t.w = W + (size_t)t.b * w_batch_stride + (size_t)t.nt * (num_kb - w_rep) * (BN * 128);
+    return t;
+  }
+  template <int BN>
+  __device__ __forceinline__ void issue(uint8_t* dst, uint64_t* full, const Tile& t, int kb, int lane) const {
+    constexpr int B_BYTES = BN * 128;
+    if (lane == 0) {
+      mbar_arrive_expect_tx(full, G2_A_BYTES + B_BYTES);
+      bulk_g2s(dst, A.kblock(t.b, t.mt, kb), G2_A_BYTES, full);
+      bulk_g2s(dst + G2_A_BYTES, t.w + (size_t)(kb < w_rep ? kb : kb - w_rep) * B_BYTES, B_BYTES, full);
+    }
+  }
+};
+
+// ---------------------------------------------------------------------------------------------------------------
+// The TMA-fed persistent GEMM.  One loader warp fills the stage ring (stage = A tile | B tile) through the schedule; two
+// consumer warpgroups run the main loop and the epilogue of each tile.  The loader starts the next tile's copies once the
+// previous tile's epilogue has left the ring (stg_free); a tile the schedule skips counts for no role.
+// kPair (k_gemm2_pair): the two CTAs of a cluster take the same m-tile and n-tiles 0 / 1 (N = 2 BLOCK_N; the persistent
+// walk over 2 n-tiles with an even grid gives CTA rank r exactly the tiles (mt, r)), and exchange LayerNorm row statistics
+// through distributed shared memory (EpiCtx::x_*).  A 128 x 512 fp32 accumulator is the whole register file of an SM;
+// this way the epilogue still sees whole rows.  Exchange slots and barriers are double buffered by tile parity; a CTA
+// runs at most one tile ahead of its peer, because its next statistics wait needs the peer's sums of that tile.
+// ---------------------------------------------------------------------------------------------------------------
+constexpr int G2_EPI_WARPS = 8;
+constexpr int G2_PAIR_SMEM = 2048;   // the pair's exchange slots, behind the barrier block
+
+template <class Sched, class Epi, int BLOCK_N, bool kPair>
+__device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, const G2Grid& g) {
+  constexpr int EPI_WARPS = G2_EPI_WARPS;
   using Cfg = G2Cfg<BLOCK_N, EPI_WARPS>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -202,37 +313,44 @@ k_gemm2(const AImage A, const Epi epi, const uint8_t* __restrict__ Wimg, long lo
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::STAGES;
   uint64_t* stg_free = bars + 2 * Cfg::STAGES;   // consumers -> loader: the tile's epilogue has left the ring
+  uint64_t* xbar = bars + 2 * Cfg::STAGES + 1;                                          // pair: [2 tile parities][4 lane quarters]
+  float* xstat = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);     // pair: [2][4][32 lanes][2]
+  static_assert(!kPair || (2 * Cfg::STAGES + 1 + 8) * 8 <= 256, "barrier block");
 
   // warp index through a shuffle: provably warp-uniform, so the role branches are uniform control flow
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0), lane = threadIdx.x % 32;
-  const int num_tiles = num_m_tiles * num_n_tiles;
+  const uint32_t rank = kPair ? cluster_ctarank() : 0u;
+  const int num_tiles = (int)g.num_tiles();   // < 2^31 (launch_gemm2)
   constexpr int LOADER = EPI_WARPS;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], EPI_WARPS); }
     mbar_init(stg_free, EPI_WARPS);
+    if (kPair) for (int i = 0; i < 8; ++i) mbar_init(&xbar[i], 1);
     mbar_fence_init();
   }
   if constexpr (Epi::kNeedsBias) if (threadIdx.x < EPI_WARPS * 32)
     for (int i = threadIdx.x; i < BLOCK_N; i += EPI_WARPS * 32) {
-      sbias[i] = epi.bias[i]; sbias[512 + i] = epi.gamma[i]; sbias[1024 + i] = epi.beta[i];
+      const uint32_t c = rank * BLOCK_N + i;   // this CTA's columns
+      sbias[i] = epi.bias[c]; sbias[512 + i] = epi.gamma[c]; sbias[1024 + i] = epi.beta[c];
     }
+  if constexpr (has_cta_stats<Epi>::value)
+    for (int i = threadIdx.x; i < 3 * 512; i += blockDim.x) sbias[i] = 0.f;
   __syncthreads();
+  if (kPair) cluster_sync_all();   // the peer's exchange barriers exist before anything is posted to them
 
   if (warp == LOADER) {
     int s = 0; uint32_t ph = 0; int it = 0;
-    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int mt = tile / num_n_tiles, nt = tile % num_n_tiles;
-      const uint8_t* wsrc = Wimg + (size_t)nt * num_kb * Cfg::B_BYTES;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+      const auto t = sc.template tile<BLOCK_N>(g, tile);
+      if (t.skip) continue;
+      // the tile's indices are computed while the previous tile's epilogue still runs, not after it has left the ring
+      asm volatile("" ::"r"(t.b), "r"(t.mt), "r"(t.nt));
       if (it > 0) mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
-      for (int kb = 0; kb < num_kb; ++kb) {
+      ++it;
+      for (int kb = 0; kb < sc.num_kb; ++kb) {
         mbar_wait(&empty[s], ph ^ 1);
-        if (lane == 0) {
-          uint8_t* dst = smem + s * Cfg::STAGE_BYTES;
-          mbar_arrive_expect_tx(&full[s], Cfg::STAGE_BYTES);
-          bulk_g2s(dst, A.kblock(mt, kb), G2_A_BYTES, &full[s]);
-          bulk_g2s(dst + G2_A_BYTES, wsrc + (size_t)kb * Cfg::B_BYTES, Cfg::B_BYTES, &full[s]);
-        }
+        sc.template issue<BLOCK_N>(smem + s * Cfg::STAGE_BYTES, &full[s], t, kb, lane);
         __syncwarp();
         if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
       }
@@ -241,36 +359,81 @@ k_gemm2(const AImage A, const Epi epi, const uint8_t* __restrict__ Wimg, long lo
     // ---------------- consumer warpgroups: MMA, then epilogue ----------------
     const int q = warp & 3, part = warp >> 2, wg = warp >> 2;
     EpiCtx ctx;
-    ctx.M = M; ctx.lane = lane; ctx.part = part; ctx.nparts = EPI_WARPS / 4;
+    ctx.M = g.M; ctx.lane = lane; ctx.part = part; ctx.nparts = EPI_WARPS / 4;
     ctx.patch = patches + warp * G2_PATCH_FLOATS;
     ctx.patch_s = smem_u32(ctx.patch);
     ctx.svec_s = smem_u32(sbias);
-    WgAcc<BLOCK_N> acc;
-    int s = 0; uint32_t ph = 0;
+    WgAcc<BLOCK_N, Sched::kBMN> acc;
+    int s = 0; uint32_t ph = 0; int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      ctx.row0 = (long long)(tile / num_n_tiles) * G2_BLOCK_M + q * 32;
-      ctx.n0 = (tile % num_n_tiles) * BLOCK_N;
+      const auto t = sc.template tile<BLOCK_N>(g, tile);
+      if (t.skip) continue;
+      ctx.batch = t.b;
+      ctx.row0 = (long long)t.mt * G2_BLOCK_M + q * 32;
+      ctx.n0 = t.nt * BLOCK_N;
+      if constexpr (kPair) {
+        const int buf = it & 1;
+        ctx.x_own_bar = &xbar[buf * 4 + q];
+        ctx.x_own_stat = smem_u32(xstat + (buf * 4 + q) * 64);
+        ctx.x_peer_stat = mapa_u32(ctx.x_own_stat, rank ^ 1u);
+        ctx.x_peer_bar = mapa_u32(smem_u32(ctx.x_own_bar), rank ^ 1u);
+        ctx.x_parity = (uint32_t)(it >> 1) & 1;
+      }
+      ++it;
       if constexpr (Epi::kNeedsBias) epi.template prefetch<BLOCK_N>(ctx);  // LN + residual epilogues
-      wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, num_kb, wg, lane);
+      wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, sc.num_kb, wg, lane);
       wg_epilogue<Cfg::STG_ROWS>(acc, smem, Cfg::STG_LD, wg, warp, lane, [&](AccSmem a) { epi.template run<BLOCK_N>(a, ctx); });
       __syncwarp();
       if (lane == 0) mbar_arrive(stg_free);
     }
   }
+  if constexpr (kPair) {
+    __syncthreads();
+    cluster_sync_all();   // nobody leaves while the peer may still post into this CTA's slots
+  }
+  if constexpr (has_cta_stats<Epi>::value) {
+    __syncthreads();
+    cta_stats_flush(epi, sbias);
+  }
 }
 
-template <class Epi, int BLOCK_N, int EPI_WARPS>
-int launch_gemm2(const AImage& A, const Epi& epi, const uint8_t* Wimg, long long M, int N, int Kp, int num_sms,
-                 cudaStream_t st) {
-  using Cfg = G2Cfg<BLOCK_N, EPI_WARPS>;
-  auto kern = k_gemm2<Epi, BLOCK_N, EPI_WARPS>;
+template <class Sched, class Epi, int BLOCK_N>
+__global__ void __launch_bounds__((G2_EPI_WARPS + 1) * 32, 1) k_gemm2(const Sched sc, const Epi epi, const G2Grid g) {
+  gemm2_body<Sched, Epi, BLOCK_N, false>(sc, epi, g);
+}
+template <class Sched, class Epi, int BLOCK_N>
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__((G2_EPI_WARPS + 1) * 32, 1)
+k_gemm2_pair(const Sched sc, const Epi epi, const G2Grid g) {
+  gemm2_body<Sched, Epi, BLOCK_N, true>(sc, epi, g);
+}
+
+// D[batches][M, N] through schedule sc.  kPair: N = 2 BLOCK_N on the column-split CTA pairs (W packed as two BLOCK_N-row
+// halves: 256 for GraphCast's 512-wide latents, 192 for Pangu's C = 384 projection and fc2).
+template <int BLOCK_N, bool kPair = false, class Sched, class Epi>
+int launch_gemm2(const Sched& sc, const Epi& epi, long long M, int N, int batches, int num_sms, cudaStream_t st) {
+  using Cfg = G2Cfg<BLOCK_N, G2_EPI_WARPS>;
+  constexpr int SMEM = Cfg::SMEM_BYTES + (kPair ? G2_PAIR_SMEM : 0);
+  static_assert(SMEM <= 232448, "smem budget");
+  auto kern = [] {   // instantiates only the entry that is launched
+    if constexpr (kPair) return k_gemm2_pair<Sched, Epi, BLOCK_N>;
+    else return k_gemm2<Sched, Epi, BLOCK_N>;
+  }();
   static std::atomic<uint64_t> configured{0};   // one bit per device: the attribute is per (function, device)
-  if (int rc = smem_opt_in(configured, reinterpret_cast<const void*>(kern), Cfg::SMEM_BYTES)) return rc;
-  const int num_m_tiles = (int)((M + G2_BLOCK_M - 1) / G2_BLOCK_M);
-  const int num_n_tiles = N / BLOCK_N;
-  const int tiles = num_m_tiles * num_n_tiles;
-  const int grid = tiles < num_sms ? tiles : num_sms;
-  kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(A, epi, Wimg, M, Kp / 64, num_m_tiles, num_n_tiles);
+  if (int rc = smem_opt_in(configured, reinterpret_cast<const void*>(kern), SMEM)) return rc;
+  const G2Grid g{M, (int)((M + G2_BLOCK_M - 1) / G2_BLOCK_M), N / BLOCK_N, batches};
+  const long long tiles = g.num_tiles();
+  if (N % BLOCK_N || (kPair && N != 2 * BLOCK_N) || tiles > INT_MAX) {
+    set_error("internal: GEMM shape M=%lld N=%d BN=%d batches=%d%s", M, N, BLOCK_N, batches, kPair ? " (pair)" : "");
+    return SKY_ERR_STATE;
+  }
+  int grid;
+  if (kPair) {
+    const int pairs = g.num_m_tiles < num_sms / 2 ? g.num_m_tiles : num_sms / 2;
+    grid = 2 * pairs;
+  } else {
+    grid = (int)(tiles < num_sms ? tiles : num_sms);
+  }
+  kern<<<grid, Cfg::THREADS, SMEM, st>>>(sc, epi, g);
   SKY_CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -496,7 +659,7 @@ struct Epi2F32Img {
       }
       float width = (float)BN;
       if (e.x_own_bar) {
-        // column-split CTA pair (gemm_split.cuh): the other half of these rows is in the peer CTA — post this CTA's sums into
+        // column-split CTA pair (k_gemm2_pair): the other half of these rows is in the peer CTA — post this CTA's sums into
         // the peer's slot (st.async completes the peer's mbarrier transaction), wait for the peer's, add
         if (e.part == 0) {
           if (e.lane == 0) mbar_arrive_expect_tx(e.x_own_bar, 32 * 8);

@@ -8,7 +8,7 @@
 namespace sky {
 
 // scratch[M, N] = A(image)[M, Kp] * W[N, Kp]^T   (W plain fp16 row-major, K zero-padded)
-__global__ void __launch_bounds__(256) k_gemm2_ref(AImage A, const __half* __restrict__ W,
+__global__ void __launch_bounds__(256) k_gemm2_ref(AOperand A, const __half* __restrict__ W,
                                                    float* __restrict__ scratch, long long M, int N, int Kp) {
   constexpr int BM = 64, BN = 64, BK = 32;
   __shared__ float As[BK][BM + 1];
@@ -24,7 +24,7 @@ __global__ void __launch_bounds__(256) k_gemm2_ref(AImage A, const __half* __res
     const long long row = m0 + lr;
     if (row < M) {
       const int k = k0 + lc * 8;
-      const uint8_t* kbp = A.kblock((int)(row >> 7), k >> 6);
+      const uint8_t* kbp = A.kblock(0, (int)(row >> 7), k >> 6);
       a = __ldg(reinterpret_cast<const uint4*>(kbp + sw128_offset((uint32_t)(row & 127), (k & 63) >> 3)));
     }
     if (n0 + lr < N) b = __ldg(reinterpret_cast<const uint4*>(W + (long long)(n0 + lr) * Kp + k0 + lc * 8));
@@ -88,7 +88,7 @@ __global__ void __launch_bounds__(128) k_epi2_ref(Epi epi, const float* __restri
 }
 
 template <class Epi, int BLOCK_N>
-int launch_gemm2_ref(const AImage& A, const Epi& epi, const __half* Wplain, float* scratch, long long M, int N,
+int launch_gemm2_ref(const AOperand& A, const Epi& epi, const __half* Wplain, float* scratch, long long M, int N,
                      int Kp, cudaStream_t st) {
   dim3 g1((unsigned)((M + 63) / 64), (unsigned)((N + 63) / 64));
   k_gemm2_ref<<<g1, 256, 0, st>>>(A, Wplain, scratch, M, N, Kp);

@@ -1,4 +1,4 @@
-// "Table x data" variant of the batched wgmma GEMM (SFNO transforms):
+// "Table x data" schedule of the wgmma GEMM k_gemm2 (gemm2.cuh) and its epilogues (SFNO transforms):
 //
 //   for b in batches:  D_b[M, N] = T_b[M, Ktot] * X_b[Ktot, N]        -> fused epilogue
 //
@@ -27,113 +27,42 @@ struct BData {
   long long batch_bytes;       // at byte offset b * batch_bytes (one image per batch)
 };
 
-template <class Epi, int BLOCK_N, int EPI_WARPS>
-__global__ void __launch_bounds__((EPI_WARPS + 1) * 32, 1)
-k_gemm_tb(const uint8_t* __restrict__ Timg, long long t_batch_stride, const BData B, const Epi epi, long long M, int nkb,
-          int num_m_tiles, int num_n_tiles, int batches) {
-  using Cfg = G2Cfg<BLOCK_N, EPI_WARPS>;
-  static_assert(BLOCK_N % 64 == 0 && BLOCK_N <= 256, "whole 64-channel atoms, one MMA per k-step");
-  constexpr int ATOMS = BLOCK_N / 64;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  float* patches = reinterpret_cast<float*>(smem + Cfg::RING_BYTES);
-  float* sbias = patches + EPI_WARPS * G2_PATCH_FLOATS;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sbias + 3 * 512);
-  uint64_t* full = bars;
-  uint64_t* empty = bars + Cfg::STAGES;
-  uint64_t* stg_free = bars + 2 * Cfg::STAGES;
-
-  const int warp = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0), lane = threadIdx.x % 32;
-  const int tiles_per_batch = num_m_tiles * num_n_tiles;
-  const long long num_tiles = (long long)tiles_per_batch * batches;
-  const int num_kb = 3 * nkb;
-  constexpr int LOADER = EPI_WARPS;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], EPI_WARPS); }
-    mbar_init(stg_free, EPI_WARPS);
-    mbar_fence_init();
-  }
-  if constexpr (has_cta_stats<Epi>::value)
-    for (int i = threadIdx.x; i < 3 * 512; i += blockDim.x) sbias[i] = 0.f;
-  __syncthreads();
-
-  if (warp == LOADER) {
-    int s = 0; uint32_t ph = 0; int it = 0;
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x, ++it) {
-      const int b = (int)(tile / tiles_per_batch), t = (int)(tile % tiles_per_batch);
-      const int mt = t / num_n_tiles, nt = t % num_n_tiles;
-      const uint8_t* tsrc = Timg + (size_t)b * t_batch_stride + (size_t)mt * (2 * nkb) * G2_A_BYTES;   // [hi | lo] image
-      const long long row_b = (long long)b * B.rows_per_batch;
-      const size_t boff = (size_t)b * B.batch_bytes;
-      if (it > 0) mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&empty[s], ph ^ 1);
-        uint8_t* dst = smem + s * Cfg::STAGE_BYTES;
-        if (lane == 0) {
-          mbar_arrive_expect_tx(&full[s], Cfg::STAGE_BYTES);
-          bulk_g2s(dst, tsrc + (size_t)(kb < nkb ? kb : kb - nkb) * G2_A_BYTES, G2_A_BYTES, &full[s]);   // hi, hi, lo
-        }
-        __syncwarp();
-        // data rows [r0, r0 + 64) of segment hi | lo | hi; lanes 0 .. ATOMS-1 fetch one 64-channel atom each
-        const int seg = kb / nkb;
-        const long long r0 = row_b + (long long)(kb - seg * nkb) * 64;
-        const long long rt = r0 >> 7;
-        const uint32_t off = (uint32_t)(r0 & 127);
-        const uint32_t rows1 = off <= 64 ? 64u : 128u - off;
-        if (lane < ATOMS) {
-          const uint8_t* img = (seg == 1 ? B.lo : B.hi) + boff;
-          const size_t cb = (size_t)nt * ATOMS + lane;
-          uint8_t* d = dst + G2_A_BYTES + lane * 8192;
-          bulk_g2s(d, img + ((size_t)rt * B.nkb_img + cb) * G2_A_BYTES + off * 128u, rows1 * 128u, &full[s]);
-          if (rows1 < 64u)
-            bulk_g2s(d + rows1 * 128u, img + ((size_t)(rt + 1) * B.nkb_img + cb) * G2_A_BYTES, (64u - rows1) * 128u, &full[s]);
-        }
-        __syncwarp();
-        if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
-      }
+// Schedule of k_gemm2 (gemm2.cuh) for T_b x X_b.  T: [batches][M/128][hi | lo: 2 x num_kb/3 k-blocks][128 rows x 128 B],
+// t_batch_stride bytes apart (0: one table for all batches).
+struct SchedTB {
+  static constexpr bool kBMN = true;   // B = the data, MN-major
+  const uint8_t* T; long long t_batch_stride;
+  BData B;
+  int num_kb;                          // 3 x the k-blocks of one table segment
+  template <int BN>
+  __device__ G2Tile tile(const G2Grid& g, int i) const { return G2Tile::at(g, i); }
+  template <int BN>
+  __device__ __forceinline__ void issue(uint8_t* dst, uint64_t* full, const G2Tile& t, int kb, int lane) const {
+    static_assert(BN % 64 == 0 && BN <= 256, "whole 64-channel atoms, one MMA per k-step");
+    constexpr int ATOMS = BN / 64;
+    const int nkb = num_kb / 3;
+    if (lane == 0) {
+      const uint8_t* tsrc = T + (size_t)t.b * t_batch_stride + (size_t)t.mt * (2 * nkb) * G2_A_BYTES;   // [hi | lo] image
+      mbar_arrive_expect_tx(full, G2_A_BYTES + BN * 128);
+      bulk_g2s(dst, tsrc + (size_t)(kb < nkb ? kb : kb - nkb) * G2_A_BYTES, G2_A_BYTES, full);   // hi, hi, lo
     }
-  } else {
-    const int q = warp & 3, part = warp >> 2, wg = warp >> 2;
-    EpiCtxB ctx;
-    ctx.M = M; ctx.lane = lane; ctx.part = part; ctx.nparts = EPI_WARPS / 4;
-    ctx.patch = patches + warp * G2_PATCH_FLOATS;
-    ctx.patch_s = smem_u32(ctx.patch);
-    ctx.svec_s = smem_u32(sbias);
-    WgAcc<BLOCK_N, true> acc;   // B = the data, MN-major
-    int s = 0; uint32_t ph = 0;
-    for (long long tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-      const int b = (int)(tile / tiles_per_batch), t = (int)(tile % tiles_per_batch);
-      ctx.batch = b;
-      ctx.row0 = (long long)(t / num_n_tiles) * G2_BLOCK_M + q * 32;
-      ctx.n0 = (t % num_n_tiles) * BLOCK_N;
-      wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, num_kb, wg, lane);
-      wg_epilogue<Cfg::STG_ROWS>(acc, smem, Cfg::STG_LD, wg, warp, lane, [&](AccSmem a) { epi.template run<BLOCK_N>(a, ctx); });
-      __syncwarp();
-      if (lane == 0) mbar_arrive(stg_free);
+    __syncwarp();
+    // data rows [r0, r0 + 64) of segment hi | lo | hi; lanes 0 .. ATOMS-1 fetch one 64-channel atom each
+    const int seg = kb / nkb;
+    const long long r0 = (long long)t.b * B.rows_per_batch + (long long)(kb - seg * nkb) * 64;
+    const long long rt = r0 >> 7;
+    const uint32_t off = (uint32_t)(r0 & 127);
+    const uint32_t rows1 = off <= 64 ? 64u : 128u - off;
+    if (lane < ATOMS) {
+      const uint8_t* img = (seg == 1 ? B.lo : B.hi) + (size_t)t.b * B.batch_bytes;
+      const size_t cb = (size_t)t.nt * ATOMS + lane;
+      uint8_t* d = dst + G2_A_BYTES + lane * 8192;
+      bulk_g2s(d, img + ((size_t)rt * B.nkb_img + cb) * G2_A_BYTES + off * 128u, rows1 * 128u, full);
+      if (rows1 < 64u)
+        bulk_g2s(d + rows1 * 128u, img + ((size_t)(rt + 1) * B.nkb_img + cb) * G2_A_BYTES, (64u - rows1) * 128u, full);
     }
   }
-  __syncthreads();
-  cta_stats_flush(epi, sbias);
-}
-
-// T: W3-style image with 128-row tiles (N = padded table rows, Kp = padded K of one segment)
-template <class Epi, int BLOCK_N, int EPI_WARPS>
-int launch_gemm_tb(const uint8_t* Timg, long long t_batch_stride, int t_rows_pad, int Kp, const BData& B, const Epi& epi,
-                   long long M, int N, int batches, int num_sms, cudaStream_t st) {
-  using Cfg = G2Cfg<BLOCK_N, EPI_WARPS>;
-  auto kern = k_gemm_tb<Epi, BLOCK_N, EPI_WARPS>;
-  static std::atomic<uint64_t> configured{0};
-  if (int rc = smem_opt_in(configured, reinterpret_cast<const void*>(kern), Cfg::SMEM_BYTES)) return rc;
-  if (N % BLOCK_N || t_rows_pad % 128 || Kp % 64) { set_error("internal: gemm_tb shape N=%d BN=%d rows=%d Kp=%d", N, BLOCK_N, t_rows_pad, Kp); return SKY_ERR_STATE; }
-  const int num_m_tiles = (int)((M + G2_BLOCK_M - 1) / G2_BLOCK_M);
-  const int num_n_tiles = N / BLOCK_N;
-  const long long tiles = (long long)num_m_tiles * num_n_tiles * batches;
-  const int grid = (int)(tiles < num_sms ? tiles : num_sms);
-  kern<<<grid, Cfg::THREADS, Cfg::SMEM_BYTES, st>>>(Timg, t_batch_stride, B, epi, M, Kp / 64, num_m_tiles, num_n_tiles, batches);
-  SKY_CUDA_OK(cudaGetLastError());
-  return 0;
-}
+};
 
 // acc -> hi / lo fp16 rows of the NEXT contraction's data (or A) image, with the index roles permuted:
 //   source element (batch b, row r, column c)  ->  image of batch' = r / bdiv,
@@ -153,7 +82,7 @@ struct EpiSplitRemap {
   // per-column scale / shift and the table's row sums t1[r] (forward DFT: only the m = 0 real row is non-zero)
   const float* csc = nullptr; const float* csh = nullptr; const float* t1 = nullptr;
   template <int BN, class Acc>
-  __device__ void run(Acc& acc, const EpiCtxB& x) const {
+  __device__ void run(Acc& acc, const EpiCtx& x) const {
     const int rsub = x.lane >> 2, ch = x.lane & 3;
     for (int c = x.part * 32; c < BN; c += 32 * x.nparts) {
       const int col = x.n0 + c + ch * 8;
@@ -220,7 +149,7 @@ struct EpiGeluStatsImg {
   double* sums;               // [n_valid] sums, then [n_valid] sums of squares
   int n_valid;
   template <int BN, class Acc>
-  __device__ void run(Acc& acc, const EpiCtxB& x) const {
+  __device__ void run(Acc& acc, const EpiCtx& x) const {
     const int rsub = x.lane >> 2, ch = x.lane & 3;
     const long long p0 = (long long)x.batch * rows_per_batch + x.row0;   // pixel row of this warp's first accumulator row
     for (int c = x.part * 32; c < BN; c += 32 * x.nparts) {
@@ -306,7 +235,7 @@ struct EpiF32ImgStats {
   double* sums;                                           // may be null (last block: no norm follows)
   int n_valid;
   template <int BN, class Acc>
-  __device__ void run(Acc& acc, const EpiCtxB& x) const {
+  __device__ void run(Acc& acc, const EpiCtx& x) const {
     const int rsub = x.lane >> 2, ch = x.lane & 3;
     for (int c = x.part * 32; c < BN; c += 32 * x.nparts) {
       const int col = x.n0 + c + ch * 8;

@@ -6,12 +6,12 @@
 // One step = encoder (grid -> mesh), 16 message-passing layers on the multimesh, decoder (mesh -> grid), residual update.
 //
 // H100 mapping.  Every MLP is two persistent TMA-fed wgmma GEMMs: hidden = swish(A W1^T + ...) (k_gemm2) written as the
-// fp16 operand image of the second GEMM (k_gemm_split: column-split CTA pairs of a cluster, LayerNorm statistics over
+// fp16 operand image of the second GEMM (k_gemm2_pair: column-split CTA pairs of a cluster, LayerNorm statistics over
 // DSMEM), whose epilogue does bias + LayerNorm (+ residual, read from the
 // stream's own fp16 image for grid nodes and mesh edges) and writes the operand image of whatever consumes it next.  The concatenations of the published formulation never exist:
 //   * [edge, sender, receiver] W1^T = edge W1e^T + (v W1s^T)[sender] + (v W1r^T)[receiver]: the per-NODE products are
 //     small GEMMs into fp16 tables, gathered by edge index inside the hidden GEMM's epilogue (row-owner lanes);
-//   * [node, sum of incoming edges] is a K-concatenation of two operand images (AImage), the sum produced by a
+//   * [node, sum of incoming edges] is a K-concatenation of two operand images (AOperand), the sum produced by a
 //     deterministic CSR reduction over the edge-update image (mesh, grid2mesh) or, for mesh2grid where every grid point has
 //     exactly three incoming edges stored k-major, by a K-concatenation of the three edge-update images with W1a repeated;
 //   * embeddings of mesh nodes and of the three edge sets do not depend on the input: computed once at load.
@@ -22,7 +22,6 @@
 
 #include "engine.h"
 #include "graphcast_ops.cuh"
-#include "gemm_split.cuh"
 
 namespace sky {
 
@@ -32,7 +31,7 @@ static inline size_t img_bytes(long long rows, int nkb) { return (size_t)(pad128
 struct WImg { uint8_t* img = nullptr; int N = 0, Kp = 0, BN = 0; };
 struct Mlp {
   WImg w1, w2;
-  WImg w2s;   // second layer of the LayerNorm MLPs, packed in 256-row halves for the column-split pair kernel (k_gemm_split)
+  WImg w2s;   // second layer of the LayerNorm MLPs, packed in 256-row halves for the column-split pair kernel (k_gemm2_pair)
   const float *b1 = nullptr, *b2 = nullptr, *g = nullptr, *be = nullptr;
 };
 
@@ -59,7 +58,6 @@ struct GraphCastEngine : Engine {
   float* vm0_f32 = nullptr;
   __half* g2m_tr = nullptr;             // (Nm, 512): embedded mesh nodes x W1r(g2m_edge)^T
   cudaStream_t prep_stream = nullptr;   // stream of the running prepare() (dalloc's zero fills)
-  bool l2_prefetch = true;  // debug_set("gc_prefetch", 0)
   // clock
   double* clock_dev = nullptr;
   GcClock* clk_dev = nullptr;
@@ -179,19 +177,15 @@ struct GraphCastEngine : Engine {
   }
 
   // ---- GEMM wrappers --------------------------------------------------------------------------------------------
-  static AImage A1(const uint8_t* img, int nkb) { AImage a{}; a.img0 = img; a.img1 = img; a.nkb0 = nkb; a.nkb1 = 0; return a; }
-  static AImage A2(const uint8_t* i0, const uint8_t* i1) { AImage a{}; a.img0 = i0; a.img1 = i1; a.nkb0 = GC_NKB; a.nkb1 = GC_NKB; return a; }
-
   template <int kG>
-  int hidden(int tag, const AImage& A, int Kp, const WImg& w, const float* b1, long long M, uint8_t* out, const __half* ta, int lda,
+  int hidden(int tag, const AOperand& A, int Kp, const WImg& w, const float* b1, long long M, uint8_t* out, const __half* ta, int lda,
              const int* ia, const __half* tb, int ldb, const int* ib, cudaStream_t st) {
     if (w.BN != 256 || w.Kp != Kp) { set_error("internal: hidden GEMM weight shape"); return SKY_ERR_STATE; }
     EpiGcSiluImg<kG> epi{};
     epi.out = out; epi.bias = b1; epi.ta = ta; epi.lda = lda; epi.ia = ia; epi.tb = tb; epi.ldb = ldb; epi.ib = ib;
-    epi.l2_prefetch = l2_prefetch && M > 4 * Nm ? 1 : 0;   // grid-sized tables only (the mesh tables are L2 resident)
     prof_begin(tag, st);
     count_launch();
-    const int rc = launch_gemm2<EpiGcSiluImg<kG>, 256, 8>(A, epi, w.img, M, GC_L, Kp, num_sms, st);
+    const int rc = launch_gemm2<256>(SchedW<>{A, w.img, Kp / 64}, epi, M, GC_L, 1, num_sms, st);
     prof_end(tag, st);
     // fp16-range guard (engine.h; a no-op unless enabled): class 5 hidden images, 0 latent / update images, 6 per-node tables
     return rc ? rc : range_scan(5, out, (size_t)(M / 128) * GC_NKB * G2_A_BYTES, st);
@@ -201,7 +195,7 @@ struct GraphCastEngine : Engine {
                 const uint8_t* xin_img, cudaStream_t st) {
     EpiGcLn<kRes> epi{xin, xout, img, yimg, m.b2, m.g, m.be, cfg.ln_eps};
     epi.xin_img = xin_img;
-    return launch_gemm_split<EpiGcLn<kRes>, 8>(A1(hid, GC_NKB), epi, m.w2s.img, M, GC_L, num_sms, st);
+    return launch_gemm2<256, true>(SchedW<>{AOperand(hid, GC_NKB), m.w2s.img, GC_NKB}, epi, M, GC_L, 1, num_sms, st);
   }
   // xin (fp32 rows) or xin_img (fp16 image) is the residual source; at most one of them
   int ln_gemm(int tag, const uint8_t* hid, const Mlp& m, long long M, const float* xin, float* xout, uint8_t* img, uint8_t* yimg,
@@ -223,7 +217,7 @@ struct GraphCastEngine : Engine {
     epi.out = out; epi.ldo = w.N; epi.nkb = 0; epi.bias = zero_bias;
     prof_begin(tag, st);
     count_launch();
-    const int rc = launch_gemm2<Epi2F16<false, false>, 256, 8>(A1(aimg, GC_NKB), epi, w.img, M, w.N, GC_L, num_sms, st);
+    const int rc = launch_gemm2<256>(SchedW<>{AOperand(aimg, GC_NKB), w.img, GC_NKB}, epi, M, w.N, 1, num_sms, st);
     prof_end(tag, st);
     return rc ? rc : range_scan(6, out, (size_t)M * w.N * 2, st);
   }
@@ -253,7 +247,7 @@ struct GraphCastEngine : Engine {
     if (!fimg || !hid) return SKY_ERR_NOMEM;
     k_gc_pack_rows<<<(unsigned)((rows * 8 + 255) / 256), 256, 0, st>>>(feat_dev, rows, F, fimg);
     count_launch();
-    if ((rc = hidden<0>(KT_GC_MISC, A1(fimg, 1), 64, m.w1, m.b1, rows, hid, nullptr, 0, nullptr, nullptr, 0, nullptr, st))) return rc;
+    if ((rc = hidden<0>(KT_GC_MISC, AOperand(fimg, 1), 64, m.w1, m.b1, rows, hid, nullptr, 0, nullptr, nullptr, 0, nullptr, st))) return rc;
     if ((rc = ln_gemm(KT_GC_MISC, hid, m, rows, nullptr, out_f32, out_img, nullptr, st))) return rc;
     SKY_CUDA_OK(cudaStreamSynchronize(st));
     dfree(fimg); dfree(hid); dfree(m.w1.img); dfree(m.w2.img); dfree(m.w2s.img); dfree(const_cast<float*>(m.b2));
@@ -413,17 +407,17 @@ struct GraphCastEngine : Engine {
                                                             cfg.n_state, cfg.n_prog, cfg.n_static);
       prof_end(KT_GC_FEAT, st);
       SKY_CUDA_OK(cudaGetLastError());
-      if ((rc = hidden<0>(KT_GC_HIDDEN, A1(w.feat, GC_FEAT_KP / 64), GC_FEAT_KP, grid_embed.w1, grid_embed.b1, Ng, w.hid, nullptr, 0, nullptr,
+      if ((rc = hidden<0>(KT_GC_HIDDEN, AOperand(w.feat, GC_FEAT_KP / 64), GC_FEAT_KP, grid_embed.w1, grid_embed.b1, Ng, w.hid, nullptr, 0, nullptr,
                           nullptr, 0, nullptr, st))) return rc;
       if ((rc = ln_gemm(KT_GC_LN, w.hid, grid_embed, Ng, nullptr, nullptr, w.vg_img, nullptr, st))) return rc;
       if (stop_after == 0) continue;
       if ((rc = table(KT_GC_TABLE, w.vg_img, g2m_ws, Ng, w.tg, st))) return rc;
-      if ((rc = hidden<2>(KT_GC_HIDDEN, A1(e_g2m_img, GC_NKB), L, g2m_edge.w1, g2m_edge.b1, Eg, w.hid, w.tg, L, g2m_s, g2m_tr, L, g2m_r, st))) return rc;
+      if ((rc = hidden<2>(KT_GC_HIDDEN, AOperand(e_g2m_img, GC_NKB), L, g2m_edge.w1, g2m_edge.b1, Eg, w.hid, w.tg, L, g2m_s, g2m_tr, L, g2m_r, st))) return rc;
       if ((rc = ln_gemm(KT_GC_LN, w.hid, g2m_edge, Eg, nullptr, nullptr, nullptr, w.yimg, st))) return rc;
       if ((rc = segsum(KT_GC_AGG, w.yimg, g2m_seg, w.agg_img, st))) return rc;
-      if ((rc = hidden<0>(KT_GC_HIDDEN, A2(vm0_img, w.agg_img), 2 * L, g2m_mesh.w1, g2m_mesh.b1, Nm, w.hid_m, nullptr, 0, nullptr, nullptr, 0, nullptr, st))) return rc;
+      if ((rc = hidden<0>(KT_GC_HIDDEN, AOperand(vm0_img, GC_NKB).add(w.agg_img, GC_NKB), 2 * L, g2m_mesh.w1, g2m_mesh.b1, Nm, w.hid_m, nullptr, 0, nullptr, nullptr, 0, nullptr, st))) return rc;
       if ((rc = ln_gemm(KT_GC_LN, w.hid_m, g2m_mesh, Nm, vm0_f32, w.vm, w.vm_img, nullptr, st))) return rc;
-      if ((rc = hidden<0>(KT_GC_HIDDEN, A1(w.vg_img, GC_NKB), L, g2m_grid.w1, g2m_grid.b1, Ng, w.hid, nullptr, 0, nullptr, nullptr, 0, nullptr, st))) return rc;
+      if ((rc = hidden<0>(KT_GC_HIDDEN, AOperand(w.vg_img, GC_NKB), L, g2m_grid.w1, g2m_grid.b1, Ng, w.hid, nullptr, 0, nullptr, nullptr, 0, nullptr, st))) return rc;
       if ((rc = ln_gemm(KT_GC_LN, w.hid, g2m_grid, Ng, nullptr, nullptr, w.vg_img, nullptr, st, w.vg_img))) return rc;
       if (stop_after == 1) continue;
       // ---------------- processor
@@ -431,14 +425,14 @@ struct GraphCastEngine : Engine {
       for (int i = 0; i < cfg.layers; ++i) {
         const uint8_t* em_in_img = i ? w.em_img : e_mesh_img;
         if ((rc = table(KT_GC_TABLE, w.vm_img, proc_wsr[i], Nm, w.tm, st))) return rc;
-        if ((rc = hidden<2>(KT_GC_HIDDEN, A1(em_in_img, GC_NKB), L, proc_edge[i].w1, proc_edge[i].b1, Em, w.hid_m, w.tm, 2 * L, mesh_s, w.tm + L,
+        if ((rc = hidden<2>(KT_GC_HIDDEN, AOperand(em_in_img, GC_NKB), L, proc_edge[i].w1, proc_edge[i].b1, Em, w.hid_m, w.tm, 2 * L, mesh_s, w.tm + L,
                             2 * L, mesh_r, st))) return rc;
         // the edge latents are not read after the last layer: only the update image (for the aggregation) is produced there
         const bool last = i == cfg.layers - 1 && stop_after == 99;
         if ((rc = ln_gemm(KT_GC_LN, w.hid_m, proc_edge[i], Em, nullptr, nullptr, last ? nullptr : w.em_img, w.ym_img, st,
                           last ? nullptr : em_in_img))) return rc;
         if ((rc = segsum(KT_GC_AGG, w.ym_img, mesh_seg, w.agg_img, st))) return rc;
-        if ((rc = hidden<0>(KT_GC_HIDDEN, A2(w.vm_img, w.agg_img), 2 * L, proc_node[i].w1, proc_node[i].b1, Nm, w.hid_m, nullptr, 0, nullptr, nullptr, 0,
+        if ((rc = hidden<0>(KT_GC_HIDDEN, AOperand(w.vm_img, GC_NKB).add(w.agg_img, GC_NKB), 2 * L, proc_node[i].w1, proc_node[i].b1, Nm, w.hid_m, nullptr, 0, nullptr, nullptr, 0,
                             nullptr, st))) return rc;
         if ((rc = ln_gemm(KT_GC_LN, w.hid_m, proc_node[i], Nm, w.vm, w.vm, w.vm_img, nullptr, st))) return rc;
         if (stop_after == 2 + i) { stopped = true; break; }
@@ -447,39 +441,30 @@ struct GraphCastEngine : Engine {
       // ---------------- decoder
       if ((rc = table(KT_GC_TABLE, w.vm_img, m2g_ws, Nm, w.tm, st))) return rc;
       if ((rc = table(KT_GC_TABLE, w.vg_img, m2g_wr, Ng, w.tg, st))) return rc;
-      if ((rc = hidden<2>(KT_GC_HIDDEN, A1(e_m2g_img, GC_NKB), L, m2g_edge.w1, m2g_edge.b1, E3, w.hid, w.tm, L, m2g_s, w.tg, L, m2g_r, st))) return rc;
+      if ((rc = hidden<2>(KT_GC_HIDDEN, AOperand(e_m2g_img, GC_NKB), L, m2g_edge.w1, m2g_edge.b1, E3, w.hid, w.tm, L, m2g_s, w.tg, L, m2g_r, st))) return rc;
       if ((rc = ln_gemm(KT_GC_LN, w.hid, m2g_edge, E3, nullptr, nullptr, nullptr, w.yimg, st))) return rc;
       {
-        AImage a{};
         const size_t seg = img_bytes(Ngp, GC_NKB);
-        a.img0 = w.vg_img; a.nkb0 = GC_NKB;
-        a.img1 = w.yimg; a.nkb1 = GC_NKB;
-        a.img2 = w.yimg + seg; a.nkb2 = GC_NKB;
-        a.img3 = w.yimg + 2 * seg; a.nkb3 = GC_NKB;
+        const AOperand a = AOperand(w.vg_img, GC_NKB).add(w.yimg, GC_NKB).add(w.yimg + seg, GC_NKB).add(w.yimg + 2 * seg, GC_NKB);
         if ((rc = hidden<0>(KT_GC_HIDDEN, a, 4 * L, m2g_grid.w1, m2g_grid.b1, Ng, w.hid, nullptr, 0, nullptr, nullptr, 0, nullptr, st))) return rc;
       }
       if ((rc = ln_gemm(KT_GC_LN, w.hid, m2g_grid, Ng, nullptr, nullptr, w.vg_img, nullptr, st, w.vg_img))) return rc;
       if ((rc = range_scan(0, w.feat, img_bytes(Ng, GC_FEAT_KP / 64), st))) return rc;
       if (stop_after == 100) continue;
-      if ((rc = hidden<0>(KT_GC_HIDDEN, A1(w.vg_img, GC_NKB), L, out_mlp.w1, out_mlp.b1, Ng, w.hid, nullptr, 0, nullptr, nullptr, 0, nullptr, st))) return rc;
+      if ((rc = hidden<0>(KT_GC_HIDDEN, AOperand(w.vg_img, GC_NKB), L, out_mlp.w1, out_mlp.b1, Ng, w.hid, nullptr, 0, nullptr, nullptr, 0, nullptr, st))) return rc;
       {
         EpiGcOut epi{};
         epi.xout = xo + (size_t)cfg.n_state * plane; epi.xin = xi + (size_t)cfg.n_state * plane;
         epi.bias = out_mlp.b2; epi.dstd = dstd; epi.plane = plane; epi.nprog = cfg.n_prog;
         prof_begin(KT_GC_OUT, st);
         count_launch();
-        rc = launch_gemm2<EpiGcOut, 128, 8>(A1(w.hid, GC_NKB), epi, out_mlp.w2.img, Ng, 128, L, num_sms, st);
+        rc = launch_gemm2<128>(SchedW<>{AOperand(w.hid, GC_NKB), out_mlp.w2.img, L / 64}, epi, Ng, 128, 1, num_sms, st);
         prof_end(KT_GC_OUT, st);
         if (rc) return rc;
       }
     }
     SKY_CUDA_OK(cudaGetLastError());
     return 0;
-  }
-
-  int debug_set(const char* key, long long value) override {
-    if (!strcmp(key, "gc_prefetch")) { l2_prefetch = value != 0; drop_graphs(); return 0; }
-    return Engine::debug_set(key, value);
   }
 
   int debug_copy(const char* what, float* dst, uint64_t max_floats, void* ws_base, int, cudaStream_t st) override {

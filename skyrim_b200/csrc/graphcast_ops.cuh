@@ -56,34 +56,10 @@ __device__ __forceinline__ void add_h8(float* v, const uint4& p) {
 template <int kG>
 struct EpiGcSiluImg {
   static constexpr bool kNeedsBias = false;
-  static constexpr bool kHasPre = kG > 0;
   uint8_t* out; const float* bias;
   const float* gamma = nullptr; const float* beta = nullptr;   // unused (uniform epilogue interface)
   const __half* ta = nullptr; int lda = 0; const int* ia = nullptr;
   const __half* tb = nullptr; int ldb = 0; const int* ib = nullptr;
-  int l2_prefetch = 0;   // pre(): pull this tile's table rows into L2 before the accumulator wait (tables larger than L2)
-  // Before the accumulator of (row group, n-tile) is waited for: fetch the edge indices of the row group once per m-tile
-  // (cached in the context for the following n-tiles) and, optionally, prefetch the table rows of this n-tile into L2.
-  template <int BN>
-  __device__ void pre(const EpiCtx& x) const {
-    if (x.aux_row0 != x.row0) {
-      const long long row = x.row0 + x.lane;
-      const bool valid = row < x.M;
-      x.aux = (kG >= 1 && valid) ? __ldg(ia + row) : 0;
-      x.aux2 = (kG >= 2 && valid) ? __ldg(ib + row) : 0;
-      x.aux_row0 = x.row0;
-    }
-    if (l2_prefetch) {
-      const char* pa = reinterpret_cast<const char*>(ta + (size_t)x.aux * lda + x.n0);
-#pragma unroll
-      for (int i = x.part; i < BN * 2 / 128; i += x.nparts) asm volatile("prefetch.global.L2 [%0];" ::"l"(pa + i * 128));
-      if (kG >= 2) {
-        const char* pb = reinterpret_cast<const char*>(tb + (size_t)x.aux2 * ldb + x.n0);
-#pragma unroll
-        for (int i = x.part; i < BN * 2 / 128; i += x.nparts) asm volatile("prefetch.global.L2 [%0];" ::"l"(pb + i * 128));
-      }
-    }
-  }
   template <int BN, class Acc>
   __device__ void run(Acc& acc, const EpiCtx& x) const {
     const int rsub = x.lane >> 2, ch = x.lane & 3;
@@ -94,9 +70,8 @@ struct EpiGcSiluImg {
     {
       const long long row = x.row0 + x.lane;
       const bool valid = row < x.M;
-      const bool cached = kG > 0 && x.aux_row0 == x.row0;     // pre() ran for this row group (k_gemm_pair)
-      const int ja = cached ? x.aux : (kG >= 1 && valid) ? __ldg(ia + row) : 0;
-      const int jb = cached ? x.aux2 : (kG >= 2 && valid) ? __ldg(ib + row) : 0;
+      const int ja = (kG >= 1 && valid) ? __ldg(ia + row) : 0;
+      const int jb = (kG >= 2 && valid) ? __ldg(ib + row) : 0;
 #pragma unroll
       for (int it = 0; it < 4; ++it) {
         if (kG >= 1) pa[it] = ta + (size_t)__shfl_sync(0xffffffffu, ja, it * 8 + rsub) * lda + x.n0 + ch * 8;

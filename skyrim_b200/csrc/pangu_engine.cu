@@ -16,7 +16,6 @@
 #include "engine.h"
 #include "gemm2.cuh"
 #include "gemm_tc.cuh"
-#include "gemm_split.cuh"
 #ifdef SKY_EXPERIMENTS
 // development build only (libskyrim_b200_dev.so): CUDA-core reference GEMMs under the same epilogues, the single-CTA
 // kernel variants and the result-invalidating timing switches.  None of this is compiled into the product library.
@@ -136,7 +135,7 @@ struct GemmW {
 };
 struct BlockW {
   GemmW qkv, proj, fc1, fc2;
-  GemmW proj_s, fc2_s;  // C = 384: projection and fc2 packed in 192-row halves for the column-split pair kernel (gemm_split.cuh)
+  GemmW proj_s, fc2_s;  // C = 384: projection and fc2 packed in 192-row halves for the column-split pair kernel (k_gemm2_pair)
   const float *qkv_b, *proj_b, *fc1_b, *fc2_b, *ln1_g, *ln1_b, *ln2_g, *ln2_b;
   __half* bias_tab;  // (n_type, heads, 3312), fp16, pre-scaled by log2 e
 };
@@ -313,8 +312,8 @@ struct PanguEngine : Engine {
   size_t workspace_bytes(int batch) const override { return carve(nullptr, batch).total; }
 
   // ---- GEMM dispatch -----------------------------------------------------------------------
-  template <int BN, int EW, class Epi>
-  int gemm2(int tag, const AImage& A, const Epi& epi, const GemmW& w, long long M, float* scratch, cudaStream_t st) {
+  template <int BN, class Epi>
+  int gemm2(int tag, const AOperand& A, const Epi& epi, const GemmW& w, long long M, float* scratch, cudaStream_t st) {
     if (w.BN != BN) { set_error("internal: weight packed for BLOCK_N=%d used with %d", w.BN, BN); return SKY_ERR_STATE; }
     int rc;
     prof_begin(tag, st);
@@ -326,7 +325,7 @@ struct PanguEngine : Engine {
 #endif
     {
       count_launch();
-      rc = launch_gemm2<Epi, BN, EW>(A, epi, w.img, M, w.N, w.Kp, num_sms, st);
+      rc = launch_gemm2<BN>(SchedW<>{A, w.img, w.Kp / 64}, epi, M, w.N, 1, num_sms, st);
     }
     prof_end(tag, st);
     return rc;
@@ -364,12 +363,12 @@ struct PanguEngine : Engine {
     const int pairs = g.heads / 2;
     const long long part_stride = (long long)B * g.nWin * pairs * AT_TILE_B;
     {  // QKV projection: natural-order tokens in, window image out (windowing / shift / padding applied by the epilogue)
-      AImage A{xh, xh, nkb, 0};
+      AOperand A(xh, nkb);
       EpiQkvWin e{ws.qkv, part_stride, b.qkv_b, g, roll, C, pairs};
 #ifdef SKY_EXPERIMENTS
       e.exp = exp_qkv;
 #endif
-      if ((rc = gemm2<192, 8>(KT_QKV, A, e, b.qkv, R, ws.scratch, st))) return rc;
+      if ((rc = gemm2<192>(KT_QKV, A, e, b.qkv, R, ws.scratch, st))) return rc;
       if (g.Hp > g.H) {   // latitude-padding tokens (x = 0): their q, k, v rows are the projection's bias.  (Writing them from
                           // the GEMM epilogue of the neighbouring tokens instead cost the GEMM 0.5 ms/step: measured, reverted.)
         const long long total = 3LL * B * g.Z * (g.Hp - g.H) * g.W * pairs * 8;
@@ -396,7 +395,7 @@ struct PanguEngine : Engine {
       if (rc) return rc;
     }
     {  // projection + LayerNorm + residual
-      AImage A{ws.atth, ws.atth, nkb, 0};
+      AOperand A(ws.atth, nkb);
       ELn e{x, C, xh, nkb, b.proj_b, b.ln1_g, b.ln1_b, cfg.ln_eps};
 #ifdef SKY_EXPERIMENTS
       e.exp = exp_ln;
@@ -406,19 +405,19 @@ struct PanguEngine : Engine {
         // the same 128 rows, LayerNorm statistics cross through DSMEM
         prof_begin(KT_PROJ, st);
         count_launch();
-        rc = launch_gemm_split<ELn, 8, 192>(A, e, b.proj_s.img, R, C, num_sms, st);
+        rc = launch_gemm2<192, true>(SchedW<>{A, b.proj_s.img, C / 64}, e, R, C, 1, num_sms, st);
         prof_end(KT_PROJ, st);
       } else {
-        rc = C == 192 ? gemm2<192, 8>(KT_PROJ, A, e, b.proj, R, ws.scratch, st)
-                      : gemm2<384, 8>(KT_PROJ, A, e, b.proj, R, ws.scratch, st);
+        rc = C == 192 ? gemm2<192>(KT_PROJ, A, e, b.proj, R, ws.scratch, st)
+                      : gemm2<384>(KT_PROJ, A, e, b.proj, R, ws.scratch, st);
       }
       if (rc) return rc;
     }
     {  // MLP: fc1 + GELU into the fp16 hidden image, then fc2 + LayerNorm + residual
-      AImage A{xh, xh, nkb, 0};
+      AOperand A(xh, nkb);
       Epi2F16<true, true> e{reinterpret_cast<__half*>(ws.hidh), 0, 4 * nkb, b.fc1_b};
-      if ((rc = gemm2<192, 8>(KT_FC1, A, e, b.fc1, R, ws.scratch, st))) return rc;
-      AImage A2{ws.hidh, ws.hidh, 4 * nkb, 0};
+      if ((rc = gemm2<192>(KT_FC1, A, e, b.fc1, R, ws.scratch, st))) return rc;
+      AOperand A2(ws.hidh, 4 * nkb);
       ELn e2{x, C, xh, nkb, b.fc2_b, b.ln2_g, b.ln2_b, cfg.ln_eps};
 #ifdef SKY_EXPERIMENTS
       e2.exp = exp_ln;
@@ -426,11 +425,11 @@ struct PanguEngine : Engine {
       if (C == 384 && proj_split && !use_ref) {
         prof_begin(KT_FC2, st);
         count_launch();
-        rc = launch_gemm_split<ELn, 8, 192>(A2, e2, b.fc2_s.img, R, 4 * C, num_sms, st);
+        rc = launch_gemm2<192, true>(SchedW<>{A2, b.fc2_s.img, 4 * C / 64}, e2, R, C, 1, num_sms, st);
         prof_end(KT_FC2, st);
       } else {
-        rc = C == 192 ? gemm2<192, 8>(KT_FC2, A2, e2, b.fc2, R, ws.scratch, st)
-                      : gemm2<384, 8>(KT_FC2, A2, e2, b.fc2, R, ws.scratch, st);
+        rc = C == 192 ? gemm2<192>(KT_FC2, A2, e2, b.fc2, R, ws.scratch, st)
+                      : gemm2<384>(KT_FC2, A2, e2, b.fc2, R, ws.scratch, st);
       }
       if (rc) return rc;
     }
@@ -478,13 +477,13 @@ struct PanguEngine : Engine {
       prof_end(KT_DOWN, st);
       count_launch();
       SKY_CUDA_OK(cudaGetLastError());
-      AImage A{ws.hidh, ws.hidh, 4 * C / 64, 0};
+      AOperand A(ws.hidh, 4 * C / 64);
       if (img_stream) {
         Epi2F32Img<false, false, true> e{ws.x2, 2 * C, ws.x2h, 2 * C / 64, nullptr, nullptr, nullptr, 0.f};
-        rc = gemm2<192, 8>(KT_DOWN, A, e, down, R2, ws.scratch, st);
+        rc = gemm2<192>(KT_DOWN, A, e, down, R2, ws.scratch, st);
       } else {
         Epi2F32Img<false, false, false> e{ws.x2, 2 * C, ws.x2h, 2 * C / 64, nullptr, nullptr, nullptr, 0.f};
-        rc = gemm2<192, 8>(KT_DOWN, A, e, down, R2, ws.scratch, st);
+        rc = gemm2<192>(KT_DOWN, A, e, down, R2, ws.scratch, st);
       }
       if (rc) return rc;
       if ((rc = range_scan(3, ws.x2h, (size_t)(R2 / 128) * (2 * C / 64) * G2_A_BYTES, st))) return rc;
@@ -497,16 +496,16 @@ struct PanguEngine : Engine {
     }
     // ---- up-sample ----
     {
-      AImage A{ws.x2h, ws.x2h, 2 * C / 64, 0};
+      AOperand A(ws.x2h, 2 * C / 64);
       Epi2UpShuffle e{ws.hidh, C / 64, C, up_g, up_b, cfg.ln_eps, nullptr, g1.H, g1.W, g2.H, g2.W};
-      if ((rc = gemm2<192, 8>(KT_UP, A, e, up1, R2, ws.scratch, st))) return rc;
-      AImage A2{ws.hidh, ws.hidh, C / 64, 0};
+      if ((rc = gemm2<192>(KT_UP, A, e, up1, R2, ws.scratch, st))) return rc;
+      AOperand A2(ws.hidh, C / 64);
       if (img_stream) {
         Epi2F32Img<false, false, true> e2{ws.x1, C, ws.x1h, C / 64, nullptr, nullptr, nullptr, 0.f};
-        rc = gemm2<192, 8>(KT_UP, A2, e2, up2, R1, ws.scratch, st);
+        rc = gemm2<192>(KT_UP, A2, e2, up2, R1, ws.scratch, st);
       } else {
         Epi2F32Img<false, false, false> e2{ws.x1, C, ws.x1h, C / 64, nullptr, nullptr, nullptr, 0.f};
-        rc = gemm2<192, 8>(KT_UP, A2, e2, up2, R1, ws.scratch, st);
+        rc = gemm2<192>(KT_UP, A2, e2, up2, R1, ws.scratch, st);
       }
       if (rc) return rc;
     }
@@ -516,9 +515,9 @@ struct PanguEngine : Engine {
     if (stop == 6) return 0;
     // ---- patch recovery: concat(skip, x) along K, one GEMM for upper-air + surface ----
     {
-      AImage A{ws.skiph, ws.x1h, C / 64, C / 64};
+      const AOperand A = AOperand(ws.skiph, C / 64).add(ws.x1h, C / 64);
       Epi2Recover e{x_out, rec_b, mean, stdv, cfg.nlat, cfg.nlon, nch, nup, cfg.n_levels, g1.H, g1.W, g1.T};
-      if ((rc = gemm2<224, 8>(KT_RECOVER, A, e, rec, R1, ws.scratch, st))) return rc;
+      if ((rc = gemm2<224>(KT_RECOVER, A, e, rec, R1, ws.scratch, st))) return rc;
     }
     return 0;
   }

@@ -1,8 +1,8 @@
-// Pangu-Weather step: the A-operand producers (gather + normalise + fp32->fp16) and the
-// accumulator epilogues (bias / GELU / LayerNorm + residual / scatter) that are fused
-// into the GEMM kernels.  Both the wgmma GEMM (gemm_tc.cuh) and the plain reference
-// GEMM (gemm_ref.cuh, test infrastructure on the device) are templated on these, so the
-// index arithmetic is written once.
+// Pangu-Weather step: the token geometry, and the patch embedding's A-operand producers
+// (gather + normalise + fp32->fp16) and epilogue.  Both the producer-fed wgmma GEMM
+// (gemm_tc.cuh) and the plain reference GEMM (gemm_ref.cuh, test infrastructure on the
+// device) are templated on these, so the index arithmetic is written once.  The epilogues
+// of the TMA-fed GEMM are in gemm2.cuh and attention_tc.cuh.
 //
 // Architecture restated from SURVEY.md Appendix A; the reference reaches it through
 // /root/reference/skyrim/core/models/pangu.py:45-46.
@@ -23,27 +23,6 @@ struct Geo {
 constexpr int WZ = 2, WH = 6, WW = 12, WIN_TOK = WZ * WH * WW;  // 144
 constexpr int SZ = WZ / 2, SH = WH / 2, SW = WW / 2;
 
-// row r of the window-ordered token matrix (all members stacked) -> natural token index
-// (member*T + t) or -1 for a latitude-padding token.
-__device__ __forceinline__ long long win_row_to_token(const Geo& g, int roll, long long r) {
-  int n = (int)(r % WIN_TOK);
-  long long wq = r / WIN_TOK;
-  int win = (int)(wq % g.nWin);
-  long long b = wq / g.nWin;
-  int wwi = win % g.nWw;
-  int t2 = win / g.nWw;
-  int whi = t2 % g.nWh, wzi = t2 / g.nWh;
-  int wi = n % WW, hi = (n / WW) % WH, zi = n / (WW * WH);
-  int z = wzi * WZ + zi, h = whi * WH + hi, w = wwi * WW + wi;
-  if (roll) {
-    z += SZ; if (z >= g.Z) z -= g.Z;
-    h += SH; if (h >= g.Hp) h -= g.Hp;
-    w += SW; if (w >= g.W) w -= g.W;
-  }
-  if (h >= g.H) return -1;
-  return b * g.T + ((long long)z * g.H + h) * g.W + w;
-}
-
 struct RowInfo {
   long long base;  // element offset of the row's source, or -1 (row contributes zeros)
   int aux;
@@ -59,57 +38,6 @@ __device__ __forceinline__ uint4 f32x8_to_h8(float4 a, float4 b) {
 // ======================================================================================
 // A-operand producers:  prep(row) once per row, load8(info, k) -> 8 halves (k multiple of 8)
 // ======================================================================================
-struct ProdPlainF32 {
-  const float* A; int lda; long long M; int K;
-  __device__ RowInfo prep(long long row) const { return {row < M ? row * lda : -1, 0}; }
-  __device__ uint4 load8(const RowInfo& ri, int k) const {
-    if (ri.base < 0 || k >= K) return make_uint4(0, 0, 0, 0);
-    const float4* p = reinterpret_cast<const float4*>(A + ri.base + k);
-    return f32x8_to_h8(__ldg(p), __ldg(p + 1));
-  }
-};
-
-struct ProdPlainF16 {
-  const __half* A; int lda; long long M; int K;
-  __device__ RowInfo prep(long long row) const { return {row < M ? row * lda : -1, 0}; }
-  __device__ uint4 load8(const RowInfo& ri, int k) const {
-    if (ri.base < 0 || k >= K) return make_uint4(0, 0, 0, 0);
-    return __ldg(reinterpret_cast<const uint4*>(A + ri.base + k));
-  }
-};
-
-// window partition (+ cyclic shift + latitude padding) of the fp32 residual stream
-struct ProdWindow {
-  const float* x; Geo g; int roll; long long M;
-  __device__ RowInfo prep(long long row) const {
-    if (row >= M) return {-1, 0};
-    long long t = win_row_to_token(g, roll, row);
-    return {t < 0 ? -1 : t * g.C, 0};
-  }
-  __device__ uint4 load8(const RowInfo& ri, int k) const {
-    if (ri.base < 0) return make_uint4(0, 0, 0, 0);
-    const float4* p = reinterpret_cast<const float4*>(x + ri.base + k);
-    return f32x8_to_h8(__ldg(p), __ldg(p + 1));
-  }
-};
-
-// concat(skip, x) rows of one z-range (patch recovery); rows enumerate (member, z-zoff, h, w)
-struct ProdConcat {
-  const float* skip; const float* x; int C; int T; int HW; int zoff; int nz; long long M;
-  __device__ RowInfo prep(long long row) const {
-    if (row >= M) return {-1, 0};
-    long long rpb = (long long)nz * HW;
-    long long b = row / rpb, rem = row % rpb;
-    return {(b * T + (long long)zoff * HW + rem) * C, 0};
-  }
-  __device__ uint4 load8(const RowInfo& ri, int k) const {
-    if (ri.base < 0) return make_uint4(0, 0, 0, 0);
-    const float* src = k < C ? skip + ri.base + k : x + ri.base + (k - C);
-    const float4* p = reinterpret_cast<const float4*>(src);
-    return f32x8_to_h8(__ldg(p), __ldg(p + 1));
-  }
-};
-
 // patch embedding, upper-air: row = (member, zt, h, w), k = ((v*2+dz)*4+dh)*4+dw  (K=160)
 struct ProdEmbedUpper {
   const float* state;            // (B, nch, nlat, nlon)
@@ -233,164 +161,6 @@ struct EpiStoreF32 {
             const uint32_t pr = ((cb >> 1) + m) ^ (r7 >> 1);
             if (r7 & 1u) stg_b32x8(base + pr * 32, c1, c0); else stg_b32x8(base + pr * 32, c0, c1);
           }
-        }
-      }
-    }
-  }
-};
-
-// out_f16[row, n0+col] = half(act(acc + bias))   (QKV projection, MLP fc1 with GELU)
-template <bool kGelu>
-struct EpiStoreF16 {
-  __half* out; int ldo; const float* bias; long long M;
-  template <class Acc>
-  __device__ void run(Acc& acc, long long row, int n0, int BN) const {
-    for (int c = 0; c < BN; c += 32) {
-      float v[32];
-      acc.load32(c, v);
-      if (row < M) {
-        uint4* o = reinterpret_cast<uint4*>(out + row * ldo + n0 + c);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float t[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            float y = v[8 * j + e] + __ldg(bias + n0 + c + 8 * j + e);
-            t[e] = kGelu ? gelu_erf(y) : y;
-          }
-          uint4 pk;
-          pk.x = pack_half2(t[0], t[1]); pk.y = pack_half2(t[2], t[3]);
-          pk.z = pack_half2(t[4], t[5]); pk.w = pack_half2(t[6], t[7]);
-          o[j] = pk;
-        }
-      }
-    }
-  }
-};
-
-// x[dst, :] += LayerNorm(acc + bias) * gamma + beta     (attention proj, MLP fc2)
-// The tile must span the full feature width (BN == C, n0 == 0).
-struct EpiLnResidual {
-  float* x; int C; const float* bias; const float* gamma; const float* beta; float eps;
-  long long M;
-  int windowed; Geo g; int roll;  // windowed: rows are window-ordered -> scatter, skip padding
-  template <class Acc>
-  __device__ void run(Acc& acc, long long row, int n0, int BN) const {
-    float s = 0.f, ss = 0.f;
-    for (int c = 0; c < BN; c += 32) {
-      float v[32];
-      acc.load32(c, v);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) {
-        float y = v[j] + __ldg(bias + c + j);
-        s += y; ss += y * y;
-      }
-    }
-    float mean = s / BN;
-    float var = fmaxf(ss / BN - mean * mean, 0.f);
-    float rstd = rsqrtf(var + eps);
-    long long dst = -1;
-    if (row < M) dst = windowed ? win_row_to_token(g, roll, row) : row;
-    for (int c = 0; c < BN; c += 32) {
-      float v[32];
-      acc.load32(c, v);
-      if (dst >= 0) {
-        float4* o = reinterpret_cast<float4*>(x + dst * C + c);
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          float4 r = o[j];
-          float4 bb = __ldg(reinterpret_cast<const float4*>(bias + c) + j);
-          float4 gg = __ldg(reinterpret_cast<const float4*>(gamma + c) + j);
-          float4 be = __ldg(reinterpret_cast<const float4*>(beta + c) + j);
-          r.x += (v[4 * j + 0] + bb.x - mean) * rstd * gg.x + be.x;
-          r.y += (v[4 * j + 1] + bb.y - mean) * rstd * gg.y + be.y;
-          r.z += (v[4 * j + 2] + bb.z - mean) * rstd * gg.z + be.z;
-          r.w += (v[4 * j + 3] + bb.w - mean) * rstd * gg.w + be.w;
-          o[j] = r;
-        }
-      }
-    }
-  }
-};
-
-// up-sample linear1: N = 4*C as (hs, ws, C); tile = one (hs, ws) sub-position (BN == C):
-// LayerNorm over the C features, store half to the fine token (z, 2*h2+hs, 2*w2+ws) if it
-// survives the crop.  Rows are coarse tokens (member, z, h2, w2).
-struct EpiUpShuffleLn {
-  __half* out;  // (B*T1, C) fp16
-  int C; const float* gamma; const float* beta; float eps; long long M;
-  int Z, H, W, H2, W2;  // fine H,W and coarse H2,W2
-  template <class Acc>
-  __device__ void run(Acc& acc, long long row, int n0, int BN) const {
-    float s = 0.f, ss = 0.f;
-    for (int c = 0; c < BN; c += 32) {
-      float v[32];
-      acc.load32(c, v);
-#pragma unroll
-      for (int j = 0; j < 32; ++j) { s += v[j]; ss += v[j] * v[j]; }
-    }
-    float mean = s / BN;
-    float rstd = rsqrtf(fmaxf(ss / BN - mean * mean, 0.f) + eps);
-    int sub = n0 / C, hs = sub >> 1, ws = sub & 1;
-    long long dst = -1;
-    if (row < M) {
-      int w2 = (int)(row % W2); long long q = row / W2;
-      int h2 = (int)(q % H2); q /= H2;  // q = member*Z + z
-      int h = 2 * h2 + hs, w = 2 * w2 + ws;
-      if (h < H) dst = (q * H + h) * W + w;
-    }
-    for (int c = 0; c < BN; c += 32) {
-      float v[32];
-      acc.load32(c, v);
-      if (dst >= 0) {
-        uint4* o = reinterpret_cast<uint4*>(out + dst * C + c);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          float t[8];
-#pragma unroll
-          for (int e = 0; e < 8; ++e)
-            t[e] = (v[8 * j + e] - mean) * rstd * __ldg(gamma + c + 8 * j + e) + __ldg(beta + c + 8 * j + e);
-          uint4 pk;
-          pk.x = pack_half2(t[0], t[1]); pk.y = pack_half2(t[2], t[3]);
-          pk.z = pack_half2(t[4], t[5]); pk.w = pack_half2(t[6], t[7]);
-          o[j] = pk;
-        }
-      }
-    }
-  }
-};
-
-// patch recovery (transposed conv with stride == kernel): scatter + crop + de-normalise.
-// upper: rows (member, zt, h, w), cols ((v*2+dz)*4+dh)*4+dw ; surface: rows (member, h, w),
-// cols (v*4+dh)*4+dw with pz == 1.
-struct EpiRecover {
-  float* out;  // (B, nch, nlat, nlon)
-  const float* bias; const float* mean; const float* stdv;
-  int nlat, nlon, nch, ch0, nlev, pz, H, W, nzt, ncols; long long M;
-  template <class Acc>
-  __device__ void run(Acc& acc, long long row, int n0, int BN) const {
-    int w = (int)(row % W); long long q = row / W;
-    int h = (int)(q % H); q /= H;
-    int zt = (int)(q % nzt); long long b = q / nzt;
-    for (int c = 0; c < BN; c += 32) {
-      float v[32];
-      acc.load32(c, v);
-      if (row < M) {
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          int col = n0 + c + 4 * j;
-          if (col >= ncols) continue;
-          int dh = (col >> 2) & 3;
-          int dz = pz == 2 ? (col >> 4) & 1 : 0;
-          int vv = pz == 2 ? col >> 5 : col >> 4;
-          int lev = pz * zt + dz, lat = 4 * h + dh;
-          if (lev >= nlev || lat >= nlat) continue;
-          int ch = ch0 + vv * nlev + lev;
-          float bsv = __ldg(bias + vv), mu = __ldg(mean + ch), sd = __ldg(stdv + ch);
-          float4 t;
-          t.x = (v[4 * j + 0] + bsv) * sd + mu; t.y = (v[4 * j + 1] + bsv) * sd + mu;
-          t.z = (v[4 * j + 2] + bsv) * sd + mu; t.w = (v[4 * j + 3] + bsv) * sd + mu;
-          *reinterpret_cast<float4*>(out + ((b * nch + ch) * (long long)nlat + lat) * nlon + 4 * w) = t;
         }
       }
     }

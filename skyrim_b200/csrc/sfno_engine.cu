@@ -5,7 +5,7 @@
 //
 // Every contraction of the step — per-pixel MLPs, the truncated longitude DFT, the Legendre
 // transforms (one GEMM per zonal wavenumber m), the per-degree complex channel mixing (one GEMM
-// per l) and their inverses — runs on the batched TMA-fed wgmma GEMMs (gemm_batched.cuh, gemm_tb.cuh) with
+// per l) and their inverses — runs on the TMA-fed wgmma GEMM (gemm2.cuh: batched weights; gemm_tb.cuh: table x data) with
 // 3-term fp16 splitting (a_hi*w_hi + a_lo*w_hi + a_hi*w_lo, ~22-bit mantissa: single-pass fp16
 // misses the 1e-3 budget on this network, DESIGN.md §2).
 // The spherical transforms are a chain of four "table x data" GEMMs around the mixing GEMM; the data is always the
@@ -309,7 +309,7 @@ struct EpiStateOut {
   static constexpr bool kNeedsBias = false;
   float* out; long long P; int C; const float* bias; const float* mean; const float* stdv;
   template <int BN, class Acc>
-  __device__ void run(Acc& acc, const EpiCtxB& e) const {
+  __device__ void run(Acc& acc, const EpiCtx& e) const {
     const long long row = e.row0 + e.lane;
     for (int c = e.part * 32; c < BN; c += 32 * e.nparts) {
       float v[32];
@@ -580,25 +580,20 @@ struct SfnoEngine : Engine {
   }
 
   // D[batch][M, N] (=|+=) [hi|lo|hi](A) * W3^T (+bias)
-  template <class Epi>
-  int gemm_epi(int tag, const Img2& A, int nkbA, long long a_bstride, int a_mtiles, const Epi& epi, const W3& w,
-               long long M, cudaStream_t st, int tri = 0) {
+  template <bool kTri = false, class Epi>
+  int gemm_epi(int tag, const Img2& A, int nkbA, long long a_bstride, const Epi& epi, const W3& w, long long M, cudaStream_t st) {
     AOperand a;
-    a.tri = tri;
-    a.nseg = 3; a.m_tiles_per_batch = a_mtiles;
-    a.seg[0] = A.hi; a.seg[1] = A.lo; a.seg[2] = A.hi;
-    for (int s = 0; s < 3; ++s) { a.nkb[s] = nkbA; a.batch_stride[s] = a_bstride; }
-    for (int s = 3; s < 6; ++s) { a.seg[s] = nullptr; a.nkb[s] = 0; a.batch_stride[s] = 0; }
+    a.add(A.hi, nkbA, a_bstride).add(A.lo, nkbA, a_bstride).add(A.hi, nkbA, a_bstride);
     if (nkbA * 64 != w.Kp) { set_error("internal: K mismatch (A %d vs W %d)", nkbA * 64, w.Kp); return SKY_ERR_STATE; }
-    return gemm_op(tag, a, epi, w, M, st);
+    return gemm_op<kTri>(tag, a, epi, w, M, st);
   }
-  template <class Epi>
+  template <bool kTri = false, class Epi>
   int gemm_op(int tag, const AOperand& a, const Epi& epi, const W3& w, long long M, cudaStream_t st) {
     int rc;
     prof_begin(tag, st);
     count_launch();
-    const int Kt = 3 * w.Kp;
-#define SKY_BN(bn) case bn: rc = launch_gemm_batched<Epi, bn, 8>(a, epi, w.img, w.batch_stride, M, w.N, Kt, w.batches, num_sms, st); break;
+    const SchedW<kTri> sc{a, w.img, 3 * w.Kp / 64, w.batch_stride, w.Kp / 64};   // W = [hi | lo], read as hi, hi, lo
+#define SKY_BN(bn) case bn: rc = launch_gemm2<bn>(sc, epi, M, w.N, w.batches, num_sms, st); break;
     switch (w.BN) {
       SKY_BN(16) SKY_BN(32) SKY_BN(64) SKY_BN(80) SKY_BN(192) SKY_BN(240) SKY_BN(256)
       default: set_error("internal: unsupported BLOCK_N %d", w.BN); rc = SKY_ERR_STATE;
@@ -614,10 +609,10 @@ struct SfnoEngine : Engine {
     const int mt = pad_to((int)rows_per_batch, 128) / 128;
     if (accumulate) {
       EpiF32Batched<true> e{out, ldo, out_bstride, bias, w.N, add};
-      return gemm_epi(tag, A, nkb, a_bstride_bytes, mt, e, w, M, st);
+      return gemm_epi(tag, A, nkb, a_bstride_bytes, e, w, M, st);
     }
     EpiF32Batched<false> e{out, ldo, out_bstride, bias, w.N, add};
-    return gemm_epi(tag, A, nkb, a_bstride_bytes, mt, e, w, M, st);
+    return gemm_epi(tag, A, nkb, a_bstride_bytes, e, w, M, st);
   }
 
   // D (+bias, optional GELU) written directly as the hi / lo operand images of the next GEMM (no fp32 round trip, no pack)
@@ -626,9 +621,9 @@ struct SfnoEngine : Engine {
     const int nkb = pad_to(K, 64) / 64, mt = pad_to((int)rows, 128) / 128;
     const size_t need = (size_t)mt * (pad_to(Nout, 64) / 64) * G2_A_BYTES;
     if (need > out.bytes || Nout % 64) { set_error("internal: split-image epilogue target (%zu > %zu, N=%d)", need, out.bytes, Nout); return SKY_ERR_STATE; }
-    if (gelu) { EpiSplitImg<true> e{out.hi, out.lo, Nout / 64, bias, w.N}; return gemm_epi(tag, A, nkb, 0, mt, e, w, rows, st); }
+    if (gelu) { EpiSplitImg<true> e{out.hi, out.lo, Nout / 64, bias, w.N}; return gemm_epi(tag, A, nkb, 0, e, w, rows, st); }
     EpiSplitImg<false> e{out.hi, out.lo, Nout / 64, bias, w.N};
-    return gemm_epi(tag, A, nkb, 0, mt, e, w, rows, st);
+    return gemm_epi(tag, A, nkb, 0, e, w, rows, st);
   }
 
   int norm_stats(const float* x, long long P, int act, const float* g, const float* b, cudaStream_t st) {
@@ -650,10 +645,11 @@ struct SfnoEngine : Engine {
     int rc;
     prof_begin(tag, st);
     count_launch();
-    const long long tbs = T.batches > 1 ? T.batch_stride : 0;
+    const SchedTB sc{T.img, T.batches > 1 ? T.batch_stride : 0, B, 3 * T.Kp / 64};
     const int bn = N % 256 == 0 ? 256 : (N % 192 == 0 ? 192 : (N % 128 == 0 ? 128 : 64));
-#define SKY_TB(v) case v: rc = launch_gemm_tb<Epi, v, 8>(T.img, tbs, T.N, T.Kp, B, epi, M, N, batches, num_sms, st); break;
-    switch (bn) { SKY_TB(64) SKY_TB(128) SKY_TB(192) default: rc = launch_gemm_tb<Epi, 256, 8>(T.img, tbs, T.N, T.Kp, B, epi, M, N, batches, num_sms, st); }
+#define SKY_TB(v) case v: rc = launch_gemm2<v>(sc, epi, M, N, batches, num_sms, st); break;
+    if (T.N % 128 || T.Kp % 64) { set_error("internal: gemm_tb shape N=%d BN=%d rows=%d Kp=%d", N, bn, T.N, T.Kp); rc = SKY_ERR_STATE; }
+    else switch (bn) { SKY_TB(64) SKY_TB(128) SKY_TB(192) default: rc = launch_gemm2<256>(sc, epi, M, N, batches, num_sms, st); }
 #undef SKY_TB
     prof_end(tag, st);
     return rc;
@@ -738,7 +734,7 @@ struct SfnoEngine : Engine {
       EpiSplitRemap e{MI.hi, MI.lo, tile_img_bytes(lmax, n2), n2 / 64, 1, 0, 1 << 30, 1, n2};
       // degree l only has orders m <= l: row tiles past l are skipped (what they would write meets zeros of the inverse
       // Legendre table)
-      if ((rc = gemm_epi(KT_SFNO_SPEC, SI, n2 / 64, tile_img_bytes(mmax, n2), pad_to(mmax, 128) / 128, e, b.spec, mmax, st, 1))) return rc;
+      if ((rc = gemm_epi<true>(KT_SFNO_SPEC, SI, n2 / 64, tile_img_bytes(mmax, n2), e, b.spec, mmax, st))) return rc;
     }
     // g = GELU(iSHT(mixed) + inner_skip(residual) + bias) -> pixel image I_b + norm1 statistics, from the epilogue that
     // produces y (the inner-skip GEMM on an unchanged grid, the inverse DFT when the inner skip is folded)
@@ -746,7 +742,7 @@ struct SfnoEngine : Engine {
     if (Hi == Ho) {
       if ((rc = inverse_sht(MI, Ho, Wo, to_field(F1, Wo), st))) return rc;
       EpiGeluStatsImg e{I_b.hi, I_b.lo, E / 64, inner_bs, F1, E, 0, sums, E};
-      if ((rc = gemm_epi(KT_SFNO_MLP, I_x, E / 64, 0, 0, e, b.inner, Po, st))) return rc;
+      if ((rc = gemm_epi(KT_SFNO_MLP, I_x, E / 64, 0, e, b.inner, Po, st))) return rc;
     } else {
       EpiGeluStatsImg e{I_b.hi, I_b.lo, E / 64, b.inner_b, nullptr, E, Wo, sums, E};
       if ((rc = inverse_sht(MI, Ho, Wo, e, st))) return rc;
@@ -767,7 +763,7 @@ struct SfnoEngine : Engine {
       const bool same = Hi == Ho;
       EpiF32ImgStats e{i + 1 < L ? xout : nullptr, E, I_x.hi, I_x.lo, E / 64, b.fc2_b, same ? xin : Rpm, same ? n0_sc : nullptr, same ? n0_sh : nullptr,
                        i + 1 < L ? sums0 : nullptr, E};
-      if ((rc = gemm_epi(KT_SFNO_MLP, I_a, Hd / 64, 0, 0, e, b.fc2, Po, st))) return rc;
+      if ((rc = gemm_epi(KT_SFNO_MLP, I_a, Hd / 64, 0, e, b.fc2, Po, st))) return rc;
     }
     if (range_guard) {   // fp16 (hi) operand images this block produced: pixel images, hidden image, spectral images
       if ((rc = range_scan(4, I_x.hi, (size_t)(Po / 128) * (E / 64) * G2_A_BYTES, st))) return rc;
@@ -791,24 +787,21 @@ struct SfnoEngine : Engine {
     {   // + positional embedding; fp32 state, pixel image and the first block's norm0 statistics from one epilogue
       // (the fp32 copy is only read by an unchanged-grid first block's outer skip, i.e. when there is a single block)
       EpiF32ImgStats e{L > 1 ? nullptr : X, E, I_x.hi, I_x.lo, E / 64, enc2_b, pos_pm, nullptr, nullptr, sums0, E};
-      if ((rc = gemm_epi(KT_SFNO_ENC, I_a, E / 64, 0, 0, e, enc2, P1, st))) return rc;
+      if ((rc = gemm_epi(KT_SFNO_ENC, I_a, E / 64, 0, e, enc2, P1, st))) return rc;
     }
     float *a = X, *b = Xn;
     for (int i = 0; i < L; ++i)
       if ((rc = run_block(i, a, b, st))) return rc;
     // decoder on concat(x, normalised input): x is already there as the last fc2's pixel image
     {
-      AOperand op;
-      op.nseg = 6; op.m_tiles_per_batch = 0;
       const int kx = E / 64, ki = pad_to(Cin, 64) / 64;
-      const uint8_t* segs[6] = {I_x.hi, I_in.hi, I_x.lo, I_in.lo, I_x.hi, I_in.hi};
-      for (int s = 0; s < 6; ++s) { op.seg[s] = segs[s]; op.nkb[s] = (s & 1) ? ki : kx; op.batch_stride[s] = 0; }
+      const AOperand op = AOperand(I_x.hi, kx).add(I_in.hi, ki).add(I_x.lo, kx).add(I_in.lo, ki).add(I_x.hi, kx).add(I_in.hi, ki);
       EpiSplitImg<true> e{I_b.hi, I_b.lo, E / 64, dec1_b, dec1.N};   // GELU(fc1) -> operand images of fc2
       if ((rc = gemm_op(KT_SFNO_DEC, op, e, dec1, P1, st))) return rc;
     }
     {
       EpiStateOut e{x_out, P1, Cin, dec2_b, mean, stdv};
-      if ((rc = gemm_epi(KT_SFNO_DEC, I_b, E / 64, 0, 0, e, dec2, P1, st))) return rc;
+      if ((rc = gemm_epi(KT_SFNO_DEC, I_b, E / 64, 0, e, dec2, P1, st))) return rc;
     }
     return 0;
   }

@@ -193,7 +193,7 @@ def _engine_env(cfg, w, **env):
 
 
 def test_projection_on_column_split_pairs_matches_single_accumulator(small):
-    """C = 384 LayerNorm GEMMs (projection, fc2) run on column-split CTA pairs (gemm_split.cuh: 2 x 192 columns, LayerNorm
+    """C = 384 LayerNorm GEMMs (projection, fc2) run on column-split CTA pairs (k_gemm2_pair: 2 x 192 columns, LayerNorm
     statistics exchanged through distributed shared memory); the one-tile k_gemm2<.., 384> path differs in the summation order of the row
     statistics — 1e-7 differences that the fp16 rounding of the operand images turns into occasional one-ulp flips, which 16
     layers spread to a few 1e-4 per channel (both variants meet the oracle parity on their own).  121 x 384: 48 row tiles at

@@ -26,12 +26,6 @@ def main():
     eng.load_weights(w)
     torch.cuda.synchronize()
     t_load = time.time() - t0
-    if "nopair" in sys.argv:
-        eng.debug_set("gc_pair", 0)
-    if "noprefetch" in sys.argv:
-        eng.debug_set("gc_prefetch", 0)
-    if "nosplit" in sys.argv:
-        eng.debug_set("gc_split", 0)
     loop = GraphcastTimeLoop(eng)
     T0 = 1714521600.0
     x = torch.from_numpy(synthetic_graphcast_state(cfg, 0)).reshape(1, 2, cfg.n_state, cfg.nlat, cfg.nlon).cuda()
