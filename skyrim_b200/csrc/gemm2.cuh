@@ -50,11 +50,14 @@ struct AOperand {
   int nseg = 0;
   AOperand() = default;
   AOperand(const uint8_t* img, int k) { add(img, k); }
-  // appends a segment of k k-blocks per row tile
+  // appends a segment of k k-blocks per row tile; a seventh segment is not stored and marks the operand invalid
+  // (launch_gemm2 refuses it)
   AOperand& add(const uint8_t* img, int k, long long bstride = 0) {
+    if (nseg >= 6) { nseg = 7; return *this; }
     seg[nseg] = img; nkb[nseg] = k; batch_stride[nseg] = bstride; ++nseg;
     return *this;
   }
+  bool valid() const { return nseg >= 1 && nseg <= 6; }
   // The loader calls this once per k-block, so it is kept short: a single image needs no walk, and the walk over several
   // is done by selects (unused segments have nkb = 0), without branches.
   __device__ const uint8_t* kblock(int batch, int mt, int kb) const {
@@ -267,6 +270,7 @@ struct SchedW {
   int num_kb;
   long long w_batch_stride = 0;   // bytes
   int w_rep = 0;
+  bool valid() const { return A.valid(); }
   struct Tile : G2Tile {
     const uint8_t* w;   // the tile's W image: k-block 0 of its batch and n-tile
   };
@@ -424,6 +428,10 @@ int launch_gemm2(const Sched& sc, const Epi& epi, long long M, int N, int batche
   const long long tiles = g.num_tiles();
   if (N % BLOCK_N || (kPair && N != 2 * BLOCK_N) || tiles > INT_MAX) {
     set_error("internal: GEMM shape M=%lld N=%d BN=%d batches=%d%s", M, N, BLOCK_N, batches, kPair ? " (pair)" : "");
+    return SKY_ERR_STATE;
+  }
+  if (!sc.valid()) {   // an operand the loader cannot walk: more than 6 A segments, a misaligned data batch (SchedTB)
+    set_error("internal: GEMM operands (M=%lld N=%d BN=%d): schedule rejected", M, N, BLOCK_N);
     return SKY_ERR_STATE;
   }
   int grid;

@@ -34,6 +34,9 @@ struct SchedTB {
   const uint8_t* T; long long t_batch_stride;
   BData B;
   int num_kb;                          // 3 x the k-blocks of one table segment
+  // a batch starts at a multiple of 8 data rows: the MN-major swizzle atom is 8 rows, and the bulk copies of a k-block
+  // split at a 128-row tile boundary only on an 8-row boundary
+  bool valid() const { return num_kb > 0 && num_kb % 3 == 0 && B.rows_per_batch % 8 == 0; }
   template <int BN>
   __device__ G2Tile tile(const G2Grid& g, int i) const { return G2Tile::at(g, i); }
   template <int BN>

@@ -340,6 +340,7 @@ struct EpiGcOut {
   }
 };
 
+#ifndef SKY_GC_EPILOGUES_ONLY   // the GEMM epilogues above are all a test build of the GEMM (gemm_probe.cu) takes
 // ---------------------------------------------------------------------------------------------------------------
 // set-up kernels (weight / table packing; run once at load)
 // ---------------------------------------------------------------------------------------------------------------
@@ -614,4 +615,5 @@ __global__ void __launch_bounds__(256) k_gc_segsum_fin(const float* __restrict__
   gc_img_st(out, m.node, lane + 32, a + 8);
 }
 
+#endif  // SKY_GC_EPILOGUES_ONLY
 }  // namespace sky

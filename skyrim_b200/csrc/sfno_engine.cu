@@ -649,6 +649,7 @@ struct SfnoEngine : Engine {
     const int bn = N % 256 == 0 ? 256 : (N % 192 == 0 ? 192 : (N % 128 == 0 ? 128 : 64));
 #define SKY_TB(v) case v: rc = launch_gemm2<v>(sc, epi, M, N, batches, num_sms, st); break;
     if (T.N % 128 || T.Kp % 64) { set_error("internal: gemm_tb shape N=%d BN=%d rows=%d Kp=%d", N, bn, T.N, T.Kp); rc = SKY_ERR_STATE; }
+    else if (B.rows_per_batch % 8) { set_error("internal: gemm_tb data batches %lld rows apart (not a multiple of 8)", B.rows_per_batch); rc = SKY_ERR_STATE; }
     else switch (bn) { SKY_TB(64) SKY_TB(128) SKY_TB(192) default: rc = launch_gemm2<256>(sc, epi, M, N, batches, num_sms, st); }
 #undef SKY_TB
     prof_end(tag, st);
