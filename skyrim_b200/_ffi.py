@@ -11,8 +11,6 @@ import os
 from pathlib import Path
 
 LIB_PATH = Path(__file__).resolve().parent / "libskyrim_b200.so"
-# development build (-DSKY_EXPERIMENTS: CUDA-core reference GEMM and attention, timing-experiment switches).  Never loaded unless a test asks for it with lib("dev") / SKYRIM_B200_LIB=dev.
-DEV_LIB_PATH = Path(__file__).resolve().parent / "libskyrim_b200_dev.so"
 
 SKY_MODEL_PANGU6 = 1
 SKY_MODEL_SFNO73 = 2
@@ -69,24 +67,23 @@ EXPORTS = {
     "sky_model_destroy": (C.c_int, [C.c_void_p]),
 }
 
-_libs = {}
+_lib = None
 
 
-def lib(variant: str | None = None) -> C.CDLL:
-    """The product library (default) or, for tests that bisect against the reference kernels, the dev build."""
-    variant = variant or os.environ.get("SKYRIM_B200_LIB", "prod")
-    if variant not in _libs:
-        path = DEV_LIB_PATH if variant == "dev" else LIB_PATH
-        if not path.exists():
-            raise SkyError(f"{path} not found — build it with `python -c 'import __graft_entry__ as g; "
+def lib() -> C.CDLL:
+    """The product library, loaded once."""
+    global _lib
+    if _lib is None:
+        if not LIB_PATH.exists():
+            raise SkyError(f"{LIB_PATH} not found — build it with `python -c 'import __graft_entry__ as g; "
                            f"g.build()'` (there is no CPU fallback)")
-        L = C.CDLL(os.fspath(path))
+        L = C.CDLL(os.fspath(LIB_PATH))
         for name, (res, args) in EXPORTS.items():
             fn = getattr(L, name)
             fn.restype = res
             fn.argtypes = args
-        _libs[variant] = L
-    return _libs[variant]
+        _lib = L
+    return _lib
 
 
 def check(rc: int, what: str = "", L=None):

@@ -83,11 +83,6 @@ struct EpiQkvWin {
   static constexpr bool kNeedsBias = false;
   uint8_t* out; long long part_stride; const float* bias; Geo g; int roll; int C; int pairs;
   const float* gamma = nullptr; const float* beta = nullptr;   // unused (uniform epilogue interface)
-#ifdef SKY_EXPERIMENTS
-  int exp = 0;
-#else
-  static constexpr int exp = 0;
-#endif
   template <int BN, class Acc>
   __device__ void run(Acc& acc, const EpiCtx& x) const {
     // this lane's own token row -> index of its 128-byte row inside a part, pair 0 (tile stride = 144 rows); computed once
@@ -139,7 +134,7 @@ struct EpiQkvWin {
         pk.x = pack_half2(t0.x, t0.y); pk.y = pack_half2(t0.z, t0.w);
         pk.z = pack_half2(t1.x, t1.y); pk.w = pack_half2(t1.z, t1.w);
         const int drow = __shfl_sync(0xffffffffu, myrow, rr);
-        if (drow >= 0 && !(exp & 2))
+        if (drow >= 0)
           *reinterpret_cast<uint4*>(pbase + (size_t)drow * 128 + ((cpos ^ ((uint32_t)drow & 7u)) << 4)) = pk;
       }
       __syncwarp();
@@ -302,57 +297,6 @@ __global__ void __launch_bounds__(AT_THREADS) k_window_attention_tc(const AttnAr
     }
   }
 }
-
-#ifdef SKY_EXPERIMENTS
-// CUDA-core reference of the same operator on the same window image (development library, SKY_ATTN=ref): one thread
-// per query row, fp32 scores, bias gathered from the compact table.  Bisects "window image / index arithmetic" from
-// "tensor pipeline" failures; never benchmarked.
-__global__ void __launch_bounds__(WIN_TOK) k_window_attention_ref(const AttnArgs a) {
-  const Geo& g = a.g;
-  const long long item = blockIdx.x;
-  const int hd = blockIdx.y;   // 0 / 1 of the pair
-  const long long key = item / (a.B * g.nWw);
-  const int type = (int)(key / a.pairs), pair = (int)(key % a.pairs), wz = type / g.nWh, wh = type % g.nWh;
-  const int ww = (int)(item % g.nWw), b = (int)((item / g.nWw) % a.B);
-  const uint8_t* src = a.qkv + ((size_t)(((long long)b * g.nWin + (long long)type * g.nWw + ww) * a.pairs + pair)) * AT_TILE_B;
-  __shared__ float ks[WIN_TOK][33], vs[WIN_TOK][33];
-  const int i = threadIdx.x;
-  auto elem = [&](int part, int row, int d) {
-    const uint32_t c = (uint32_t)(hd * 4 + d / 8);
-    return __half2float(*reinterpret_cast<const __half*>(src + (size_t)part * a.part_stride + (size_t)row * 128 + ((c ^ ((uint32_t)row & 7u)) << 4) + (d % 8) * 2));
-  };
-  float q[32];
-  for (int d = 0; d < 32; ++d) { q[d] = elem(0, i, d); ks[i][d] = elem(1, i, d); vs[i][d] = elem(2, i, d); }
-  __syncthreads();
-  const int fmask = a.roll ? ((wz == g.nWz - 1 ? 1 : 0) | (wh == g.nWh - 1 ? 2 : 0)) : 0;
-  const int wi = i % WW, hi = (i / WW) % WH, zi = i / (WW * WH);
-  const int rflag = (zi >= WZ - SZ ? 1 : 0) | (hi >= WH - SH ? 2 : 0);
-  const __half* tab = a.bias_tab + ((long long)type * g.heads + 2 * pair + hd) * AT_TABLE;
-  float sc[WIN_TOK], mx = -INFINITY;
-  for (int j = 0; j < WIN_TOK; ++j) {
-    float d = 0.f;
-    for (int e = 0; e < 32; ++e) d += q[e] * ks[j][e];
-    const int wj = j % WW, hj = (j / WW) % WH, zj = j / (WW * WH);
-    const int idx = (zi + WZ * zj) * ((2 * WW - 1) * WH * WH) + (hi + WH * hj) * (2 * WW - 1) + wi - wj + WW - 1;
-    const int cflag = (zj >= WZ - SZ ? 1 : 0) | (hj >= WH - SH ? 2 : 0);
-    d = d * a.sl2 + __half2float(tab[idx]) + (((rflag ^ cflag) & fmask) ? a.mask_l2 : 0.f);
-    sc[j] = d; mx = fmaxf(mx, d);
-  }
-  float sum = 0.f, o[32];
-  for (int e = 0; e < 32; ++e) o[e] = 0.f;
-  for (int j = 0; j < WIN_TOK; ++j) {
-    const float p = exp2f(sc[j] - mx);
-    sum += p;
-    const float ph = __half2float(__float2half_rn(p));
-    for (int e = 0; e < 32; ++e) o[e] += ph * vs[j][e];
-  }
-  const long long tok = at_row_token(g, a.roll, b, wz, wh, ww, i);
-  if (tok < 0) return;
-  uint8_t* row = a.att_img + ((size_t)(tok >> 7) * a.att_nkb + pair) * (size_t)G2_A_BYTES + (size_t)(tok & 127) * 128;
-  for (int e = 0; e < 32; ++e)
-    *reinterpret_cast<__half*>(row + ((((uint32_t)(hd * 4 + e / 8)) ^ ((uint32_t)tok & 7u)) << 4) + (e % 8) * 2) = __float2half_rn(o[e] / sum);
-}
-#endif
 
 inline int launch_window_attention_tc(const AttnArgs& a, int num_sms, cudaStream_t st) {
   (void)num_sms;

@@ -82,15 +82,14 @@ struct G2Cfg {
   static constexpr int MAXS = (232448 - FIXED) / STAGE_BYTES;
   static constexpr int STAGES = MAXS > 6 ? 6 : MAXS;
   static constexpr int RING_BYTES = STAGES * STAGE_BYTES;
-  // accumulator staging over the drained ring: all 128 rows when they fit, else 64 rows (one warpgroup) at a time
+  // accumulator staging over the drained ring: all 128 rows at once
   static constexpr int STG_LD = (BLOCK_N + 31) / 32 * 32 + 4;
-  static constexpr int STG_ROWS = 128 * STG_LD * 4 <= RING_BYTES ? 128 : 64;
   static constexpr int SMEM_BYTES = RING_BYTES + FIXED;
   static constexpr int THREADS = (EPI_WARPS + 1) * 32;
-  static_assert(BLOCK_N % 8 == 0 && BLOCK_N <= 384, "wgmma N, accumulator registers");
+  static_assert(BLOCK_N % 8 == 0 && BLOCK_N <= 256, "wgmma N, accumulator registers");
   static_assert(STAGE_BYTES % 1024 == 0, "stage alignment");
   static_assert(STAGES >= 2, "pipeline depth");
-  static_assert(STG_ROWS * STG_LD * 4 <= RING_BYTES, "accumulator staging");
+  static_assert(128 * STG_LD * 4 <= RING_BYTES, "accumulator staging");
   static_assert(EPI_WARPS == 8, "two consumer warpgroups");
 };
 
@@ -119,19 +118,15 @@ struct EpiCtx {
 // ---------------------------------------------------------------------------------------------------------------
 // consumer side shared by the wgmma GEMM kernels
 // ---------------------------------------------------------------------------------------------------------------
-// Accumulators of warpgroup wg: rows 64 wg .. 64 wg + 63 of the 128-row tile, all BN columns (N > 256: two products of N/2).
+// Accumulators of warpgroup wg: rows 64 wg .. 64 wg + 63 of the 128-row tile, all BN columns.
 template <int BN, bool kBMN = false>
 struct WgAcc {
-  static constexpr int NI = BN <= 256 ? BN : BN / 2;
-  static constexpr int NS = BN / NI;
-  float d[NS][NI / 2];
+  float d[BN / 2];
   // zeroed at the start of every tile (rather than a scale-d = 0 first product): the registers are then dead between the
   // staging of one tile and the main loop of the next, i.e. free for the epilogue
   __device__ __forceinline__ void zero() {
 #pragma unroll
-    for (int ni = 0; ni < NS; ++ni)
-#pragma unroll
-      for (int i = 0; i < NI / 2; ++i) d[ni][i] = 0.f;
+    for (int i = 0; i < BN / 2; ++i) d[i] = 0.f;
   }
   // one k-block: A = 128 rows x 64 halves at a_addr; B = BN rows x 64 halves, K-major, at b_addr, or (kBMN) 64 k-rows x BN
   // columns in 64-column atoms 8 KB apart
@@ -140,33 +135,26 @@ struct WgAcc {
     const uint64_t da = make_desc_sw128(a_addr + (uint32_t)wg * 8192u);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-#pragma unroll
-      for (int ni = 0; ni < NS; ++ni) {
-        const uint64_t db = kBMN ? make_desc_sw128_mn(b_addr, 8192) + (uint64_t)(k * (2048 >> 4))
-                                 : make_desc_sw128(b_addr + (uint32_t)(ni * NI * 128)) + (uint64_t)(2 * k);
-        Wgmma<NI, kBMN>::mma(d[ni], da + 2 * k, db);
-      }
+      const uint64_t db = kBMN ? make_desc_sw128_mn(b_addr, 8192) + (uint64_t)(k * (2048 >> 4))
+                               : make_desc_sw128(b_addr) + (uint64_t)(2 * k);
+      Wgmma<BN, kBMN>::mma(d, da + 2 * k, db);
     }
     wgmma_commit();
   }
   __device__ __forceinline__ void settle() {
     wgmma_wait<0>();
-#pragma unroll
-    for (int ni = 0; ni < NS; ++ni) wgmma_fence_operands(d[ni]);
+    wgmma_fence_operands(d);
   }
-  // fragment -> staging (row-major, ld floats per row); row_off = first row of this warpgroup minus the staging's first row
-  __device__ __forceinline__ void dump(uint32_t stg_s, int ld, int row_off) const {
+  // fragment -> staging (row-major, ld floats per row, 128 rows); this warpgroup's rows start at 64 wg
+  __device__ __forceinline__ void dump(uint32_t stg_s, int ld, int wg) const {
     const int w = (threadIdx.x >> 5) & 3, l = threadIdx.x & 31;
-    const uint32_t r = (uint32_t)(16 * w + (l >> 2) + row_off);
+    const uint32_t r = (uint32_t)(64 * wg + 16 * w + (l >> 2));
     const uint32_t a0 = stg_s + (r * (uint32_t)ld + 2u * (uint32_t)(l & 3)) * 4u, a8 = a0 + 8u * (uint32_t)ld * 4u;
 #pragma unroll
-    for (int ni = 0; ni < NS; ++ni) {
-#pragma unroll
-      for (int i = 0; i < NI / 8; ++i) {
-        const uint32_t o = (uint32_t)(ni * NI + 8 * i) * 4u;
-        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a0 + o), "f"(d[ni][4 * i]), "f"(d[ni][4 * i + 1]) : "memory");
-        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a8 + o), "f"(d[ni][4 * i + 2]), "f"(d[ni][4 * i + 3]) : "memory");
-      }
+    for (int i = 0; i < BN / 8; ++i) {
+      const uint32_t o = (uint32_t)(8 * i) * 4u;
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a0 + o), "f"(d[4 * i]), "f"(d[4 * i + 1]) : "memory");
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a8 + o), "f"(d[4 * i + 2]), "f"(d[4 * i + 3]) : "memory");
     }
   }
 };
@@ -191,22 +179,16 @@ __device__ __forceinline__ void wg_mainloop(Acc& acc, uint8_t* smem, uint64_t* f
   if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(&empty[prev]); }
 }
 
-// Stage the accumulators at the base of the (drained) ring and run fn(AccSmem) in every consumer warp whose 32-row quarter
-// (warp % 4) is staged; STG_ROWS = 64 stages and finishes one warpgroup's rows at a time.  The caller signals the loader
-// afterwards (the ring is free again).
-template <int STG_ROWS, class Acc, class Fn>
+// Stage all 128 rows of accumulators at the base of the (drained) ring and run fn(AccSmem) in every consumer warp on its
+// 32-row quarter (warp % 4).  The caller signals the loader afterwards (the ring is free again).
+template <class Acc, class Fn>
 __device__ __forceinline__ void wg_epilogue(const Acc& acc, uint8_t* smem, int ld, int wg, int warp, int lane, Fn&& fn) {
   const uint32_t stg = smem_u32(smem);
-  const int q = warp & 3;
   named_bar_sync(1, 256);   // both warpgroups' products have completed: no wgmma still reads the ring the staging overwrites
-#pragma unroll 1
-  for (int h = 0; h < 128 / STG_ROWS; ++h) {
-    if (STG_ROWS == 128 || wg == h) acc.dump(stg, ld, 64 * wg - h * STG_ROWS);
-    named_bar_sync(1, 256);
-    if (q * 32 >= h * STG_ROWS && q * 32 < (h + 1) * STG_ROWS)
-      fn(AccSmem{stg + (uint32_t)((q * 32 + lane - h * STG_ROWS) * ld) * 4u});
-    named_bar_sync(1, 256);
-  }
+  acc.dump(stg, ld, wg);
+  named_bar_sync(1, 256);
+  fn(AccSmem{stg + (uint32_t)(((warp & 3) * 32 + lane) * ld) * 4u});
+  named_bar_sync(1, 256);
   fence_proxy_async_smem();   // the staging's generic accesses are ordered before the next bulk copies into the ring
 }
 
@@ -386,7 +368,7 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
       ++it;
       if constexpr (Epi::kNeedsBias) epi.template prefetch<BLOCK_N>(ctx);  // LN + residual epilogues
       wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, sc.num_kb, wg, lane);
-      wg_epilogue<Cfg::STG_ROWS>(acc, smem, Cfg::STG_LD, wg, warp, lane, [&](AccSmem a) { epi.template run<BLOCK_N>(a, ctx); });
+      wg_epilogue(acc, smem, Cfg::STG_LD, wg, warp, lane, [&](AccSmem a) { epi.template run<BLOCK_N>(a, ctx); });
       __syncwarp();
       if (lane == 0) mbar_arrive(stg_free);
     }
@@ -491,15 +473,6 @@ struct Epi2F16 {
   static constexpr bool kNeedsBias = false;
   __half* out; int ldo; int nkb; const float* bias;
   const float* gamma = nullptr; const float* beta = nullptr;  // unused (uniform epilogue interface)
-#ifdef SKY_EXPERIMENTS
-  int exp = 0;  // timing experiments only (results invalid): 2 = no global stores
-#else
-  static constexpr int exp = 0;
-#endif
-  // head_major (row-major mode only): column block j of 32 goes to out[j][row][0..32), i.e. (part, head, token, 32) for
-  // the QKV projection.  A warp store then covers 8 consecutive tokens x 64 B = 512 contiguous bytes instead of 8
-  // half lines 2*ldo bytes apart, and the attention kernel reads 64-byte rows that are contiguous along longitude.
-  int head_major = 0;
   template <int BN, class Acc>
   __device__ void run(Acc& acc, const EpiCtx& x) const {
     const int rsub = x.lane >> 2, ch = x.lane & 3;
@@ -540,15 +513,11 @@ struct Epi2F16 {
         uint4 pk;
         pk.x = pack_half2(t0.x, t0.y); pk.y = pack_half2(t0.z, t0.w);
         pk.z = pack_half2(t1.x, t1.y); pk.w = pack_half2(t1.z, t1.w);
-        if (x.row0 + rr < x.M && !(exp & 2)) {
+        if (x.row0 + rr < x.M) {
           if (kImage)
             *reinterpret_cast<uint4*>(ibase + rr * 128 + (((((col & 63) >> 3) + ch) ^ (rr & 7)) << 4)) = pk;
-          else if (head_major)
-            *reinterpret_cast<uint4*>(out + ((size_t)((col + ch * 8) >> 5) * x.M + (x.row0 + rr)) * 32 + ((col + ch * 8) & 31)) = pk;
           else
             *reinterpret_cast<uint4*>(out + (x.row0 + rr) * ldo + col + ch * 8) = pk;
-        } else if (exp & 2) {
-          asm volatile("" ::"r"(pk.x), "r"(pk.y), "r"(pk.z), "r"(pk.w));   // keep the value alive
         }
       }
       __syncwarp();
@@ -571,11 +540,6 @@ struct Epi2F32Img {
   float* x; int ldx;            // fp32 row-major (unused when kImgStream)
   uint8_t* img; int nkb;        // fp16 image of the same rows (may be null unless kImgStream)
   const float* bias; const float* gamma; const float* beta; float eps;  // bias may be null when !kLn
-#ifdef SKY_EXPERIMENTS
-  int exp = 0;  // timing experiments only (results invalid): 1 = no residual loads, 2 = no fp32 stores, 4 = no image stores
-#else
-  static constexpr int exp = 0;
-#endif
   // Pull this warp's residual rows into L2 ahead of time, while the tile's main loop runs.
   // four residual values of row (row0 + rr) at tile column n0 + c + 4 * c4, read from the fp16 image
   __device__ __forceinline__ uint2 img_res_raw(const EpiCtx& e, int rr, int c, int c4) const {
@@ -609,22 +573,21 @@ struct Epi2F32Img {
   // LayerNorm statistics of the 8 rows a lane touches come from their owner lanes by shuffle; the
   // fp16 image chunks (8 columns = 16 bytes) are assembled from lane pairs by shuffle, not through
   // shared memory.  Every warp reduces the statistics of its own column groups only; the warps that
-  // share a lane quarter exchange partial sums through their patches.
-  // kPrefetch: load the residual of the next column group while this one is processed (32 more registers)
-  template <int BN, bool kPrefetch = true, class Acc>
+  // share a lane quarter exchange partial sums through their patches.  The residual of the next column group is loaded
+  // while this one is processed (32 more registers).
+  template <int BN, class Acc>
   __device__ void run(Acc& acc, const EpiCtx& e) const {
     constexpr int NG = BN / 32;
     const int rsub4 = e.lane >> 3, c4 = e.lane & 7;
     const long long rows_left = e.M - e.row0;          // >= 32 for every tile but the last
     float* xp = x + e.row0 * ldx + e.n0 + c4 * 4;
-    const bool ld_on = kResidual && !(exp & 1);
     float4 xin[8];
     if constexpr (kImgStream) {
       uint2 raw[8];
 #pragma unroll
       for (int it = 0; it < 8; ++it) {
         const int rr = it * 4 + rsub4;
-        raw[it] = (kPrefetch && ld_on && rr < rows_left && e.part < NG) ? img_res_raw(e, rr, e.part * 32, c4) : make_uint2(0u, 0u);
+        raw[it] = (kResidual && rr < rows_left && e.part < NG) ? img_res_raw(e, rr, e.part * 32, c4) : make_uint2(0u, 0u);
       }
 #pragma unroll
       for (int it = 0; it < 8; ++it) xin[it] = h4_to_f4(raw[it]);
@@ -632,8 +595,8 @@ struct Epi2F32Img {
 #pragma unroll
       for (int it = 0; it < 8; ++it) {
         const int rr = it * 4 + rsub4;
-        xin[it] = (kPrefetch && ld_on && rr < rows_left && e.part < NG) ? *reinterpret_cast<const float4*>(xp + (size_t)rr * ldx + e.part * 32)
-                                                                       : make_float4(0.f, 0.f, 0.f, 0.f);
+        xin[it] = (kResidual && rr < rows_left && e.part < NG) ? *reinterpret_cast<const float4*>(xp + (size_t)rr * ldx + e.part * 32)
+                                                               : make_float4(0.f, 0.f, 0.f, 0.f);
       }
     }
     float rs[8], ns[8];   // rstd and -mean*rstd of row it*4 + rsub4
@@ -695,24 +658,6 @@ struct Epi2F32Img {
     const int odd = e.lane & 1;
     for (int g = e.part; g < NG; g += e.nparts) {
       const int c = g * 32;
-      if (!kPrefetch && kResidual) {
-        if constexpr (kImgStream) {
-          uint2 raw[8];
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int rr = it * 4 + rsub4;
-            raw[it] = (ld_on && rr < rows_left) ? img_res_raw(e, rr, c, c4) : make_uint2(0u, 0u);
-          }
-#pragma unroll
-          for (int it = 0; it < 8; ++it) xin[it] = h4_to_f4(raw[it]);
-        } else {
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int rr = it * 4 + rsub4;
-            xin[it] = (ld_on && rr < rows_left) ? *reinterpret_cast<const float4*>(xp + (size_t)rr * ldx + c) : make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-        }
-      }
       {
         float v[32];
         acc.load32(c, v);
@@ -728,14 +673,14 @@ struct Epi2F32Img {
         bs = __ldg(reinterpret_cast<const float4*>(bias + e.n0 + c + c4 * 4));
       }
       const bool more = g + e.nparts < NG;
-      float4 xnext[kPrefetch ? 8 : 1];
-      if constexpr (kResidual && kPrefetch) {
+      float4 xnext[8];
+      if constexpr (kResidual) {
         if constexpr (kImgStream) {
           uint2 raw[8];
 #pragma unroll
           for (int it = 0; it < 8; ++it) {
             const int rr = it * 4 + rsub4;
-            raw[it] = (more && ld_on && rr < rows_left) ? img_res_raw(e, rr, c + 32 * e.nparts, c4) : make_uint2(0u, 0u);
+            raw[it] = (more && rr < rows_left) ? img_res_raw(e, rr, c + 32 * e.nparts, c4) : make_uint2(0u, 0u);
           }
 #pragma unroll
           for (int it = 0; it < 8; ++it) xnext[it] = h4_to_f4(raw[it]);
@@ -743,8 +688,8 @@ struct Epi2F32Img {
 #pragma unroll
           for (int it = 0; it < 8; ++it) {
             const int rr = it * 4 + rsub4;
-            xnext[it] = (more && ld_on && rr < rows_left) ? *reinterpret_cast<const float4*>(xp + (size_t)rr * ldx + c + 32 * e.nparts)
-                                                          : make_float4(0.f, 0.f, 0.f, 0.f);
+            xnext[it] = (more && rr < rows_left) ? *reinterpret_cast<const float4*>(xp + (size_t)rr * ldx + c + 32 * e.nparts)
+                                                 : make_float4(0.f, 0.f, 0.f, 0.f);
           }
         }
       }
@@ -763,10 +708,10 @@ struct Epi2F32Img {
           y.x = fmaf(fmaf(t.x + bs.x, rs[it], ns[it]), ga.x, be.x); y.y = fmaf(fmaf(t.y + bs.y, rs[it], ns[it]), ga.y, be.y);
           y.z = fmaf(fmaf(t.z + bs.z, rs[it], ns[it]), ga.z, be.z); y.w = fmaf(fmaf(t.w + bs.w, rs[it], ns[it]), ga.w, be.w);
           if (kResidual) { y.x += xin[it].x; y.y += xin[it].y; y.z += xin[it].z; y.w += xin[it].w; }
-          if (!kImgStream && rr < rows_left && !(exp & 2)) *reinterpret_cast<float4*>(xp + (size_t)rr * ldx + c) = y;
+          if (!kImgStream && rr < rows_left) *reinterpret_cast<float4*>(xp + (size_t)rr * ldx + c) = y;
           h[u].x = pack_half2(y.x, y.y); h[u].y = pack_half2(y.z, y.w);
         }
-        if (ibase && !(exp & 4)) {
+        if (ibase) {
           // even lane assembles the chunk of row it2, odd lane the chunk of row it2+1: swap the other halves
           const uint2 send = odd ? h[0] : h[1];
           uint2 recv;
@@ -778,18 +723,13 @@ struct Epi2F32Img {
         }
       }
       __syncwarp();
-      if constexpr (kResidual && kPrefetch) {
+      if constexpr (kResidual) {
 #pragma unroll
         for (int it = 0; it < 8; ++it) xin[it] = xnext[it];
       }
     }
   }
 };
-
-// post-norm residual of the attention projection and of the MLP: fp32 row-major token stream (EpiLnRes) or the stream kept
-// only as its fp16 operand image (EpiLnResImg); the engine picks one per handle (pangu_engine.cu, "fp32_stream")
-using EpiLnRes = Epi2F32Img<true, true, false>;
-using EpiLnResImg = Epi2F32Img<true, true, true>;
 
 // up-sample linear1 (N = 4C as (hs, ws, C); one n-tile = one sub-position): LayerNorm over
 // the C features of the tile, written as fp16 image rows of the FINE token

@@ -378,13 +378,12 @@ int by_bn(const Case& c, const Sched& sc, cudaStream_t st, BnList<BNs...>) {
 // The (schedule, epilogue, BLOCK_N) lists mirror what the engines instantiate:
 //   SFNO SfnoEngine::gemm_op: SchedW / SchedW<true> x its epilogues x {16, 32, 64, 80, 192, 240, 256};
 //   SFNO SfnoEngine::gemm_tb: SchedTB x {EpiSplitRemap, EpiF32Batched<false>, EpiGeluStatsImg} x {64, 128, 192, 256};
-//   Pangu: SchedW x Epi2F32Img<true, true, *> x {192, 384}, and the pair kernel at 192; fc1's Epi2F16<true, true> at 192;
+//   Pangu: SchedW x Epi2F32Img<true, true, *> at 192, and the pair kernel at 192; fc1's Epi2F16<true, true> at 192;
 //   GraphCast: EpiGcSiluImg<0 / 2> and the node tables' Epi2F16<false, false> at 256, EpiGcOut at 128, and the pair kernel
 //   with EpiGcLn<0 / 1 / 2> at 256 (GraphCast never gathers exactly one table: EpiGcSiluImg<1> is not instantiated).
 using BnSfno = BnList<16, 32, 64, 80, 192, 240, 256>;
 using BnSfnoMain = BnList<64, 192>;
 using BnTb = BnList<64, 128, 192, 256>;
-using BnLn = BnList<192, 384>;
 using BnPair = BnList<192>;
 
 int dispatch(const Case& c, cudaStream_t st) {
@@ -422,8 +421,8 @@ int dispatch(const Case& c, cudaStream_t st) {
           case SKY_PROBE_EPI_SPLIT_GELU: return by_bn<false, EpiSplitImg<true>>(c, sc, st, BnSfnoMain{});
           case SKY_PROBE_EPI_F32_STATS: return by_bn<false, EpiF32ImgStats>(c, sc, st, BnSfnoMain{});
           case SKY_PROBE_EPI_GELU_STATS: return by_bn<false, EpiGeluStatsImg>(c, sc, st, BnSfnoMain{});
-          case SKY_PROBE_EPI_LN: return by_bn<false, Epi2F32Img<true, true, false>>(c, sc, st, BnLn{});
-          case SKY_PROBE_EPI_LN_IMG: return by_bn<false, Epi2F32Img<true, true, true>>(c, sc, st, BnLn{});
+          case SKY_PROBE_EPI_LN: return by_bn<false, Epi2F32Img<true, true, false>>(c, sc, st, BnList<192>{});
+          case SKY_PROBE_EPI_LN_IMG: return by_bn<false, Epi2F32Img<true, true, true>>(c, sc, st, BnList<192>{});
           case SKY_PROBE_EPI_F16_GELU_IMG: return by_bn<false, Epi2F16<true, true>>(c, sc, st, BnList<192>{});
           case SKY_PROBE_EPI_F16_ROWS: return by_bn<false, Epi2F16<false, false>>(c, sc, st, BnList<256>{});
           case SKY_PROBE_EPI_GC_SILU0: return by_bn<false, EpiGcSiluImg<0>>(c, sc, st, BnList<256>{});

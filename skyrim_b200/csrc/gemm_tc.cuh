@@ -111,7 +111,7 @@ k_gemm_tc(const Prod prod, const Epi epi, const uint8_t* __restrict__ Wimg, long
       const long long m0 = (long long)(tile / num_n_tiles) * TC_BLOCK_M;
       const int n0 = (tile % num_n_tiles) * BLOCK_N;
       wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, num_kb, wg, lane);
-      wg_epilogue<128>(acc, smem, Cfg::STG_LD, wg, warp, lane, [&](AccSmem a) {
+      wg_epilogue(acc, smem, Cfg::STG_LD, wg, warp, lane, [&](AccSmem a) {
         if (warp < 4) epi.run(a, m0 + warp * 32 + lane, n0, BLOCK_N);
       });
       __syncwarp();

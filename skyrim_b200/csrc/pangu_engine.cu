@@ -16,12 +16,6 @@
 #include "engine.h"
 #include "gemm2.cuh"
 #include "gemm_tc.cuh"
-#ifdef SKY_EXPERIMENTS
-// development build only (libskyrim_b200_dev.so): CUDA-core reference GEMMs under the same epilogues, the single-CTA
-// kernel variants and the result-invalidating timing switches.  None of this is compiled into the product library.
-#include "gemm2_ref.cuh"
-#include "gemm_ref.cuh"
-#endif
 
 namespace sky {
 
@@ -29,10 +23,9 @@ namespace sky {
 // weight repacking (runs once, at load)
 // ======================================================================================
 // fp32 W (logical [Nsrc, K]; stored [Nsrc,K] or, if transposed, [K,Nsrc]) -> rows
-// [n_off, n_off+Nsrc) of   plain fp16 [Ntot, Kp]   and   tile image
-// [Ntot/BN][Kp/64][BN rows x 128 B, SWIZZLE_128B]
+// [n_off, n_off+Nsrc) of the fp16 tile image [Ntot/BN][Kp/64][BN rows x 128 B, SWIZZLE_128B]
 __global__ void k_pack_weight(const float* __restrict__ W, int Nsrc, int K, int Kp, int BN, int transposed,
-                              int n_off, __half* __restrict__ plain, uint8_t* __restrict__ img) {
+                              int n_off, uint8_t* __restrict__ img) {
   long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;  // one 8-half chunk each
   int chunks_per_row = Kp / 8;
   if (idx >= (long long)Nsrc * chunks_per_row) return;
@@ -47,7 +40,6 @@ __global__ void k_pack_weight(const float* __restrict__ W, int Nsrc, int K, int 
   }
   uint4 pk = *reinterpret_cast<uint4*>(h);
   const int n = n_off + ns;
-  *reinterpret_cast<uint4*>(plain + (long long)n * Kp + kc * 8) = pk;
   int nt = n / BN, nr = n % BN, kb = kc / 8, ch = kc % 8;
   size_t tile = ((size_t)nt * (Kp / 64) + kb) * (size_t)BN * 128;
   *reinterpret_cast<uint4*>(img + tile + sw128_offset(nr, ch)) = pk;
@@ -130,12 +122,10 @@ __global__ void k_image_to_rows(const uint8_t* __restrict__ img, int nkb, float*
 // ======================================================================================
 struct GemmW {
   uint8_t* img = nullptr;
-  __half* plain = nullptr;
   int N = 0, K = 0, Kp = 0, BN = 0;
 };
 struct BlockW {
-  GemmW qkv, proj, fc1, fc2;
-  GemmW proj_s, fc2_s;  // C = 384: projection and fc2 packed in 192-row halves for the column-split pair kernel (k_gemm2_pair)
+  GemmW qkv, proj, fc1, fc2;   // all at BLOCK_N 192: at C = 384 projection and fc2 are the two halves of a CTA pair
   const float *qkv_b, *proj_b, *fc1_b, *fc2_b, *ln1_g, *ln1_b, *ln2_g, *ln2_b;
   __half* bias_tab;  // (n_type, heads, 3312), fp16, pre-scaled by log2 e
 };
@@ -144,14 +134,10 @@ struct PanguEngine : Engine {
   sky_pangu_config_t cfg;
   Geo g1, g2;
   int nch, nup;
-  bool use_ref = false;
   // Token stream storage (sky_model_debug_set "fp32_stream"): true = only the fp16 operand image (default: 8 of the 12 bytes
   // per token and feature of the projection / MLP epilogues disappear; step error 5.8e-4 instead of 5.1e-4 at 721x1440),
   // false = fp32 rows beside the image (round-1 / early round-2 data flow; for weights whose error margin is tighter)
   bool img_stream = true;
-  bool proj_split = true;   // C = 384 LayerNorm GEMMs (projection, fc2) on column-split CTA pairs ("proj_split" 0: one 384-column tile)
-  int exp_qkv = 0, exp_ln = 0;  // dev build only: result-invalidating timing experiments
-  bool attn_ref = false;        // dev build only (SKY_ATTN=ref): CUDA-core reference attention on the same window image
   std::vector<void*> owned;
   GemmW embed_u, embed_s, down, up1, up2, rec;
   std::vector<BlockW> blocks[4];
@@ -174,14 +160,6 @@ struct PanguEngine : Engine {
     int H = (c.nlat + 3) / 4, W = c.nlon / 4;
     g1 = mk(H, W, c.dim, c.heads[0]);
     g2 = mk((H + 1) / 2, W / 2, 2 * c.dim, c.heads[1]);
-#ifdef SKY_EXPERIMENTS   // read once, at creation; the product library reads no environment variable at all
-    const char* e = getenv("SKY_GEMM");
-    use_ref = e && !strcmp(e, "ref");
-    exp_qkv = getenv("SKY_QKV_EXP") ? atoi(getenv("SKY_QKV_EXP")) : 0;
-    exp_ln = getenv("SKY_LN_EXP") ? atoi(getenv("SKY_LN_EXP")) : 0;
-    const char* at = getenv("SKY_ATTN");
-    attn_ref = at && !strcmp(at, "ref");
-#endif
   }
   ~PanguEngine() override {
     for (void* p : owned) cudaFree(p);
@@ -198,16 +176,14 @@ struct PanguEngine : Engine {
   int pack_alloc(GemmW& g, int N, int K, int BN) {
     g.N = N; g.K = K; g.Kp = (K + 63) / 64 * 64; g.BN = BN;
     if (N % BN) { set_error("N=%d not a multiple of BLOCK_N=%d", N, BN); return SKY_ERR_ARG; }
-    g.plain = dalloc<__half>((size_t)N * g.Kp);
     g.img = dalloc<uint8_t>((size_t)N * g.Kp * 2);
-    return (g.plain && g.img) ? 0 : SKY_ERR_NOMEM;
+    return g.img ? 0 : SKY_ERR_NOMEM;
   }
   int pack_rows(GemmW& g, const char* name, int Nsrc, int n_off, bool transposed, cudaStream_t st) {
     const float* w = param(name, (uint64_t)Nsrc * g.K);
     if (!w) return SKY_ERR_ARG;
     long long chunks = (long long)Nsrc * g.Kp / 8;
-    k_pack_weight<<<(unsigned)((chunks + 255) / 256), 256, 0, st>>>(w, Nsrc, g.K, g.Kp, g.BN, transposed ? 1 : 0, n_off,
-                                                                 g.plain, g.img);
+    k_pack_weight<<<(unsigned)((chunks + 255) / 256), 256, 0, st>>>(w, Nsrc, g.K, g.Kp, g.BN, transposed ? 1 : 0, n_off, g.img);
     count_launch();
     SKY_CUDA_OK(cudaGetLastError());
     return 0;
@@ -250,11 +226,9 @@ struct PanguEngine : Engine {
         char nm[96];
         auto N = [&](const char* s) { snprintf(nm, sizeof nm, "layer%d.block%d.%s", li, bi, s); return nm; };
         if ((rc = pack(b.qkv, N("qkv.w"), 3 * c, c, 192, false, st))) return rc;
-        if ((rc = pack(b.proj, N("proj.w"), c, c, c, false, st))) return rc;
-        if (c == 384 && (rc = pack(b.proj_s, N("proj.w"), c, c, 192, false, st))) return rc;
+        if ((rc = pack(b.proj, N("proj.w"), c, c, 192, false, st))) return rc;
         if ((rc = pack(b.fc1, N("fc1.w"), 4 * c, c, 192, false, st))) return rc;
-        if ((rc = pack(b.fc2, N("fc2.w"), c, 4 * c, c, false, st))) return rc;
-        if (c == 384 && (rc = pack(b.fc2_s, N("fc2.w"), c, 4 * c, 192, false, st))) return rc;
+        if ((rc = pack(b.fc2, N("fc2.w"), c, 4 * c, 192, false, st))) return rc;
         P(b.qkv_b, N("qkv.b"), 3 * c); P(b.proj_b, N("proj.b"), c);
         P(b.fc1_b, N("fc1.b"), 4 * c); P(b.fc2_b, N("fc2.b"), c);
         P(b.ln1_g, N("ln1.g"), c); P(b.ln1_b, N("ln1.b"), c);
@@ -276,7 +250,7 @@ struct PanguEngine : Engine {
 
   // ---- workspace carving -----------------------------------------------------------------
   struct Ws {
-    float *x1, *x2, *scratch;
+    float *x1, *x2;
     uint8_t *x1h, *skiph, *x2h, *atth, *hidh;
     uint8_t* qkv;
     size_t x1h_bytes;
@@ -303,48 +277,28 @@ struct PanguEngine : Engine {
     w.atth = (uint8_t*)take(att_b * G2_A_BYTES);
     size_t hid_b = t1 * (4 * C / 64) > t2 * (8 * C / 64) ? t1 * (4 * C / 64) : t2 * (8 * C / 64);
     w.hidh = (uint8_t*)take(hid_b * G2_A_BYTES);  // MLP hidden; also the down-sample / up-sample staging images
-    size_t scr = 0;
-    if (use_ref) scr = (size_t)R1 * 4 * C * 4;
-    w.scratch = (float*)take(scr);
     w.total = off;
     return w;
   }
   size_t workspace_bytes(int batch) const override { return carve(nullptr, batch).total; }
 
   // ---- GEMM dispatch -----------------------------------------------------------------------
-  template <int BN, class Epi>
-  int gemm2(int tag, const AOperand& A, const Epi& epi, const GemmW& w, long long M, float* scratch, cudaStream_t st) {
+  // kPair: N = 2 BN on the column-split CTA pairs (k_gemm2_pair)
+  template <int BN, bool kPair = false, class Epi>
+  int gemm2(int tag, const AOperand& A, const Epi& epi, const GemmW& w, long long M, cudaStream_t st) {
     if (w.BN != BN) { set_error("internal: weight packed for BLOCK_N=%d used with %d", w.BN, BN); return SKY_ERR_STATE; }
-    int rc;
     prof_begin(tag, st);
-#ifdef SKY_EXPERIMENTS
-    if (use_ref) {
-      count_launch(2);
-      rc = launch_gemm2_ref<Epi, BN>(A, epi, w.plain, scratch, M, w.N, w.Kp, st);
-    } else
-#endif
-    {
-      count_launch();
-      rc = launch_gemm2<BN>(SchedW<>{A, w.img, w.Kp / 64}, epi, M, w.N, 1, num_sms, st);
-    }
+    count_launch();
+    const int rc = launch_gemm2<BN, kPair>(SchedW<>{A, w.img, w.Kp / 64}, epi, M, w.N, 1, num_sms, st);
     prof_end(tag, st);
     return rc;
   }
   // patch embedding keeps warp producers (im2col + normalisation of the fp32 state)
   template <int BN, class Prod, class Epi>
-  int gemm_prod(int tag, const Prod& prod, const Epi& epi, const GemmW& w, long long M, float* scratch, cudaStream_t st) {
-    int rc;
+  int gemm_prod(int tag, const Prod& prod, const Epi& epi, const GemmW& w, long long M, cudaStream_t st) {
     prof_begin(tag, st);
-#ifdef SKY_EXPERIMENTS
-    if (use_ref) {
-      count_launch(2);
-      rc = launch_gemm_ref(prod, epi, w.plain, scratch, M, w.N, w.Kp, BN, st);
-    } else
-#endif
-    {
-      count_launch();
-      rc = launch_gemm_tc<Prod, Epi, BN>(prod, epi, w.img, M, w.N, w.Kp, num_sms, st);
-    }
+    count_launch();
+    const int rc = launch_gemm_tc<Prod, Epi, BN>(prod, epi, w.img, M, w.N, w.Kp, num_sms, st);
     prof_end(tag, st);
     return rc;
   }
@@ -365,10 +319,7 @@ struct PanguEngine : Engine {
     {  // QKV projection: natural-order tokens in, window image out (windowing / shift / padding applied by the epilogue)
       AOperand A(xh, nkb);
       EpiQkvWin e{ws.qkv, part_stride, b.qkv_b, g, roll, C, pairs};
-#ifdef SKY_EXPERIMENTS
-      e.exp = exp_qkv;
-#endif
-      if ((rc = gemm2<192>(KT_QKV, A, e, b.qkv, R, ws.scratch, st))) return rc;
+      if ((rc = gemm2<192>(KT_QKV, A, e, b.qkv, R, st))) return rc;
       if (g.Hp > g.H) {   // latitude-padding tokens (x = 0): their q, k, v rows are the projection's bias.  (Writing them from
                           // the GEMM epilogue of the neighbouring tokens instead cost the GEMM 0.5 ms/step: measured, reverted.)
         const long long total = 3LL * B * g.Z * (g.Hp - g.H) * g.W * pairs * 8;
@@ -384,53 +335,24 @@ struct PanguEngine : Engine {
                  rsqrtf(32.f) * 1.4426950408889634f, cfg.mask_value * 1.4426950408889634f, (long long)B * g.nWin * pairs};
       prof_begin(KT_ATTN, st);
       count_launch();
-#ifdef SKY_EXPERIMENTS
-      if (attn_ref) {
-        k_window_attention_ref<<<dim3((unsigned)a.items, 2), WIN_TOK, 0, st>>>(a);
-        rc = cudaGetLastError() == cudaSuccess ? 0 : SKY_ERR_CUDA;
-      } else
-#endif
-        rc = launch_window_attention_tc(a, num_sms, st);
+      rc = launch_window_attention_tc(a, num_sms, st);
       prof_end(KT_ATTN, st);
       if (rc) return rc;
     }
-    {  // projection + LayerNorm + residual
+    {  // projection + LayerNorm + residual.  At C = 384 a 128 x 384 accumulator would take 192 registers per consumer thread:
+       // the two CTAs of a cluster take 192 columns each of the same 128 rows, LayerNorm statistics cross through DSMEM
       AOperand A(ws.atth, nkb);
       ELn e{x, C, xh, nkb, b.proj_b, b.ln1_g, b.ln1_b, cfg.ln_eps};
-#ifdef SKY_EXPERIMENTS
-      e.exp = exp_ln;
-#endif
-      if (C == 384 && proj_split && !use_ref) {
-        // a 128 x 384 accumulator takes 192 registers per consumer thread: the two CTAs of a cluster take 192 columns each of
-        // the same 128 rows, LayerNorm statistics cross through DSMEM
-        prof_begin(KT_PROJ, st);
-        count_launch();
-        rc = launch_gemm2<192, true>(SchedW<>{A, b.proj_s.img, C / 64}, e, R, C, 1, num_sms, st);
-        prof_end(KT_PROJ, st);
-      } else {
-        rc = C == 192 ? gemm2<192>(KT_PROJ, A, e, b.proj, R, ws.scratch, st)
-                      : gemm2<384>(KT_PROJ, A, e, b.proj, R, ws.scratch, st);
-      }
+      rc = C == 192 ? gemm2<192>(KT_PROJ, A, e, b.proj, R, st) : gemm2<192, true>(KT_PROJ, A, e, b.proj, R, st);
       if (rc) return rc;
     }
     {  // MLP: fc1 + GELU into the fp16 hidden image, then fc2 + LayerNorm + residual
       AOperand A(xh, nkb);
       Epi2F16<true, true> e{reinterpret_cast<__half*>(ws.hidh), 0, 4 * nkb, b.fc1_b};
-      if ((rc = gemm2<192>(KT_FC1, A, e, b.fc1, R, ws.scratch, st))) return rc;
+      if ((rc = gemm2<192>(KT_FC1, A, e, b.fc1, R, st))) return rc;
       AOperand A2(ws.hidh, 4 * nkb);
       ELn e2{x, C, xh, nkb, b.fc2_b, b.ln2_g, b.ln2_b, cfg.ln_eps};
-#ifdef SKY_EXPERIMENTS
-      e2.exp = exp_ln;
-#endif
-      if (C == 384 && proj_split && !use_ref) {
-        prof_begin(KT_FC2, st);
-        count_launch();
-        rc = launch_gemm2<192, true>(SchedW<>{A2, b.fc2_s.img, 4 * C / 64}, e2, R, C, 1, num_sms, st);
-        prof_end(KT_FC2, st);
-      } else {
-        rc = C == 192 ? gemm2<192>(KT_FC2, A2, e2, b.fc2, R, ws.scratch, st)
-                      : gemm2<384>(KT_FC2, A2, e2, b.fc2, R, ws.scratch, st);
-      }
+      rc = C == 192 ? gemm2<192>(KT_FC2, A2, e2, b.fc2, R, st) : gemm2<192, true>(KT_FC2, A2, e2, b.fc2, R, st);
       if (rc) return rc;
     }
     if (range_guard) {   // fp16 operand images of this block (whole tiles only: the tail rows of the last tile are never written)
@@ -457,11 +379,11 @@ struct PanguEngine : Engine {
       long long M = (long long)B * nzt * HW;
       ProdEmbedUpper p{x_in, mean, stdv, cfg.nlat, cfg.nlon, cfg.n_levels, 5, nch, g1.H, g1.W, nzt, M};
       EpiStoreF32 e{img_stream ? nullptr : ws.x1, C, embed_u_b, M, g1.T, HW, 1, (long long)nzt * HW, ws.skiph, C / 64};
-      if ((rc = gemm_prod<192>(KT_EMBED, p, e, embed_u, M, ws.scratch, st))) return rc;
+      if ((rc = gemm_prod<192>(KT_EMBED, p, e, embed_u, M, st))) return rc;
       long long Ms = (long long)B * HW;
       ProdEmbedSurf ps{x_in, masks, mean, stdv, cfg.nlat, cfg.nlon, nch, nup, 4, 3, g1.H, g1.W, Ms};
       EpiStoreF32 es{img_stream ? nullptr : ws.x1, C, embed_s_b, Ms, g1.T, HW, 0, (long long)HW, ws.skiph, C / 64};
-      if ((rc = gemm_prod<192>(KT_EMBED, ps, es, embed_s, Ms, ws.scratch, st))) return rc;
+      if ((rc = gemm_prod<192>(KT_EMBED, ps, es, embed_s, Ms, st))) return rc;
     }
     if (stop == 0) return 0;
     for (size_t i = 0; i < blocks[0].size(); ++i)
@@ -480,10 +402,10 @@ struct PanguEngine : Engine {
       AOperand A(ws.hidh, 4 * C / 64);
       if (img_stream) {
         Epi2F32Img<false, false, true> e{ws.x2, 2 * C, ws.x2h, 2 * C / 64, nullptr, nullptr, nullptr, 0.f};
-        rc = gemm2<192>(KT_DOWN, A, e, down, R2, ws.scratch, st);
+        rc = gemm2<192>(KT_DOWN, A, e, down, R2, st);
       } else {
         Epi2F32Img<false, false, false> e{ws.x2, 2 * C, ws.x2h, 2 * C / 64, nullptr, nullptr, nullptr, 0.f};
-        rc = gemm2<192>(KT_DOWN, A, e, down, R2, ws.scratch, st);
+        rc = gemm2<192>(KT_DOWN, A, e, down, R2, st);
       }
       if (rc) return rc;
       if ((rc = range_scan(3, ws.x2h, (size_t)(R2 / 128) * (2 * C / 64) * G2_A_BYTES, st))) return rc;
@@ -498,14 +420,14 @@ struct PanguEngine : Engine {
     {
       AOperand A(ws.x2h, 2 * C / 64);
       Epi2UpShuffle e{ws.hidh, C / 64, C, up_g, up_b, cfg.ln_eps, nullptr, g1.H, g1.W, g2.H, g2.W};
-      if ((rc = gemm2<192>(KT_UP, A, e, up1, R2, ws.scratch, st))) return rc;
+      if ((rc = gemm2<192>(KT_UP, A, e, up1, R2, st))) return rc;
       AOperand A2(ws.hidh, C / 64);
       if (img_stream) {
         Epi2F32Img<false, false, true> e2{ws.x1, C, ws.x1h, C / 64, nullptr, nullptr, nullptr, 0.f};
-        rc = gemm2<192>(KT_UP, A2, e2, up2, R1, ws.scratch, st);
+        rc = gemm2<192>(KT_UP, A2, e2, up2, R1, st);
       } else {
         Epi2F32Img<false, false, false> e2{ws.x1, C, ws.x1h, C / 64, nullptr, nullptr, nullptr, 0.f};
-        rc = gemm2<192>(KT_UP, A2, e2, up2, R1, ws.scratch, st);
+        rc = gemm2<192>(KT_UP, A2, e2, up2, R1, st);
       }
       if (rc) return rc;
     }
@@ -517,14 +439,13 @@ struct PanguEngine : Engine {
     {
       const AOperand A = AOperand(ws.skiph, C / 64).add(ws.x1h, C / 64);
       Epi2Recover e{x_out, rec_b, mean, stdv, cfg.nlat, cfg.nlon, nch, nup, cfg.n_levels, g1.H, g1.W, g1.T};
-      if ((rc = gemm2<224>(KT_RECOVER, A, e, rec, R1, ws.scratch, st))) return rc;
+      if ((rc = gemm2<224>(KT_RECOVER, A, e, rec, R1, st))) return rc;
     }
     return 0;
   }
 
   int debug_set(const char* key, long long value) override {
     if (!strcmp(key, "fp32_stream")) { img_stream = value == 0; drop_graphs(); return 0; }
-    if (!strcmp(key, "proj_split")) { proj_split = value != 0; drop_graphs(); return 0; }
     return Engine::debug_set(key, value);
   }
 

@@ -1,8 +1,7 @@
 // Pangu-Weather step: the token geometry, and the patch embedding's A-operand producers
-// (gather + normalise + fp32->fp16) and epilogue.  Both the producer-fed wgmma GEMM
-// (gemm_tc.cuh) and the plain reference GEMM (gemm_ref.cuh, test infrastructure on the
-// device) are templated on these, so the index arithmetic is written once.  The epilogues
-// of the TMA-fed GEMM are in gemm2.cuh and attention_tc.cuh.
+// (gather + normalise + fp32->fp16) and epilogue, on which the producer-fed wgmma GEMM
+// (gemm_tc.cuh) is templated.  The epilogues of the TMA-fed GEMM are in gemm2.cuh and
+// attention_tc.cuh.
 //
 // Architecture restated from SURVEY.md Appendix A; the reference reaches it through
 // /root/reference/skyrim/core/models/pangu.py:45-46.

@@ -60,14 +60,14 @@ def _graphcast_cfg_c(cfg: GraphCastConfig, graph) -> _ffi.GraphCastConfigC:
 class StepEngine:
     """One 6-h step operator resident on one GPU."""
 
-    def __init__(self, cfg, device: int = 0, lib: str | None = None, graph=None):
+    def __init__(self, cfg, device: int = 0, graph=None):
         import torch
         if not torch.cuda.is_available():
             raise _ffi.SkyError("skyrim_b200 needs a CUDA device (sm_90a, H100); there is no CPU fallback")
         self.cfg = cfg
         self.device = device
         self.torch = torch
-        L = self._L = _ffi.lib(lib)
+        L = self._L = _ffi.lib()
         if isinstance(cfg, PanguConfig):
             kind, cc = _ffi.SKY_MODEL_PANGU6, _pangu_cfg_c(cfg)
         elif isinstance(cfg, SFNOConfig):

@@ -18,32 +18,27 @@ ref = PanguRef(cfg, w, torch.float32)
 stages = ref.stages(x0)
 names = ["embed", "layer0", "down", "layer1", "layer2", "up", "layer3"]
 xin = torch.from_numpy(x0)[None].cuda()
-# modes: tc = product library; ref = dev library, CUDA-core GEMMs + tensor-core attention; refattn = dev library,
-# CUDA-core GEMMs + CUDA-core attention (bisects window image / index math from the tensor pipelines)
-for mode in (sys.argv[3:] or ["refattn", "ref", "tc"]):
-    os.environ["SKY_GEMM"] = "ref" if mode.startswith("ref") else "tc"   # read by the development library only
-    os.environ["SKY_ATTN"] = "ref" if mode == "refattn" else "tc"
-    eng = StepEngine(cfg, 0, lib="dev" if mode.startswith("ref") else None)
-    eng.load_weights(w)
-    print(f"== SKY_GEMM={mode}  grid {nlat}x{nlon}", flush=True)
-    for i, nm in enumerate(names):
-        eng.debug_set("stop_after", i)
-        try:
-            eng.step(xin)
-            torch.cuda.synchronize()
-        except Exception as e:
-            print("  stage", nm, "FAILED:", e, flush=True)
-            break
-        r = stages[nm]
-        which = "tokens2" if nm in ("down", "layer1", "layer2") else "tokens1"
-        t = eng.debug_tensor(which, tuple(r.shape)).cpu()
-        err = (t - r).norm() / r.norm()
-        print(f"  {nm:7s} rel l2 err {err:.3e}  max abs {float((t - r).abs().max()):.3e}  nan={bool(torch.isnan(t).any())}", flush=True)
-    eng.debug_set("stop_after", 99)
+eng = StepEngine(cfg, 0)
+eng.load_weights(w)
+print(f"== grid {nlat}x{nlon}", flush=True)
+for i, nm in enumerate(names):
+    eng.debug_set("stop_after", i)
     try:
-        y = eng.step(xin); torch.cuda.synchronize()
-        e = rel_err_per_channel(y[0].cpu().numpy(), stages["out"].numpy())
-        print(f"  OUTPUT per-channel rel err max {e.max():.3e} (ch {PANGU_CHANNELS[int(e.argmax())]}) median {np.median(e):.3e}", flush=True)
+        eng.step(xin)
+        torch.cuda.synchronize()
     except Exception as e:
-        print("  full step FAILED:", e, flush=True)
-    eng.close()
+        print("  stage", nm, "FAILED:", e, flush=True)
+        break
+    r = stages[nm]
+    which = "tokens2" if nm in ("down", "layer1", "layer2") else "tokens1"
+    t = eng.debug_tensor(which, tuple(r.shape)).cpu()
+    err = (t - r).norm() / r.norm()
+    print(f"  {nm:7s} rel l2 err {err:.3e}  max abs {float((t - r).abs().max()):.3e}  nan={bool(torch.isnan(t).any())}", flush=True)
+eng.debug_set("stop_after", 99)
+try:
+    y = eng.step(xin); torch.cuda.synchronize()
+    e = rel_err_per_channel(y[0].cpu().numpy(), stages["out"].numpy())
+    print(f"  OUTPUT per-channel rel err max {e.max():.3e} (ch {PANGU_CHANNELS[int(e.argmax())]}) median {np.median(e):.3e}", flush=True)
+except Exception as e:
+    print("  full step FAILED:", e, flush=True)
+eng.close()
