@@ -153,6 +153,31 @@ SKY_API int sky_model_debug_set(sky_model_t* m, const char* key, int64_t value);
 SKY_API int sky_perturb_ic(float* x, const float* sigma_c, float amp, uint64_t seed, int32_t member0,
                    int32_t members, int32_t channels, int64_t plane, void* stream);
 
+/* Spherically correlated perturbation: x[m, c, :, :] += amp * sigma[c] * f, f a Gaussian random field on the sphere with
+ * unit pointwise variance, per field (global member g = member0 + m, channel c):
+ *   a_l0 = s_l z0,  a_lm = s_l (z0 + i z1) / sqrt 2 (0 < m <= l <= lmax),  z0, z1 = fp64 Box-Muller of the first two
+ *   words of Philox4x32-10 with key = seed and counter = (l | m << 16, 0x47524631 "GRF1", c, g),
+ *   f = the inverse real SHT of a_lm on the equiangular (nlat, nlon) grid, torch-harmonics conventions
+ *   (skyrim_b200/sht.py RealSHT.inverse).
+ * A draw depends only on (seed, g, c, l, m): not on lmax, on the batch or on the rank layout.  Channels with
+ * sigma[c] == 0 are left bit-identical.  All pointers are device memory on the device that owns x:
+ *   spec_std   fp32 [lmax + 1], s_l (skyrim_b200.engine.grf_spectrum: s_0 = 0, sum_l s_l^2 (2l + 1) / 4 pi = 1);
+ *   legendre   fp32 Pbar_l^m(cos theta_k) for m = 0..lmax, k < nlat, l = m..lmax, stored m-major, then k, then l
+ *              (block m holds nlat * (lmax + 1 - m) values);
+ *   workspace  at least sky_grf_workspace_bytes(members, channels, nlat, nlon, lmax) bytes (at most 512 MB whenever one
+ *              field fits; the fields are processed in chunks).
+ * Requires 1 <= lmax < nlat and nlon >= 2 lmax + 1; other shapes, a short workspace and host pointers are refused
+ * (SKY_ERR_ARG) before anything is launched.  Asynchronous and stream-ordered; launches on the device that owns x. */
+SKY_API size_t sky_grf_workspace_bytes(int32_t members, int32_t channels, int32_t nlat, int32_t nlon, int32_t lmax);
+SKY_API int sky_perturb_ic_grf(float* x, const float* sigma_c, float amp, uint64_t seed, int32_t member0, int32_t members,
+                       int32_t channels, int32_t nlat, int32_t nlon, int32_t lmax, const float* spec_std,
+                       const float* legendre, void* workspace, size_t workspace_bytes, void* stream);
+/* The coefficients sky_perturb_ic_grf draws, for inspection: coeffs = device complex64
+ * [members * channels][(lmax + 1)(lmax + 2) / 2], (m, l) triangle m-major (entry (m, l) at m (lmax + 1) - m (m - 1) / 2
+ * + l - m), each a_lm rounded once from fp64 to fp32. */
+SKY_API int sky_grf_draw(float* coeffs, const float* spec_std, uint64_t seed, int32_t member0, int32_t members,
+                 int32_t channels, int32_t lmax, void* stream);
+
 /* Per-kernel-family device timing (CUDA events recorded on the launching stream around the
  * launches whose family bit is set in tag_mask).  profile_end synchronises on the recorded
  * events and returns the summed milliseconds and launch counts per family.  Used by bench.py

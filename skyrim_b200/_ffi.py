@@ -59,6 +59,12 @@ EXPORTS = {
     "sky_model_debug_set": (C.c_int, [C.c_void_p, C.c_char_p, C.c_int64]),
     "sky_perturb_ic": (C.c_int, [C.c_void_p, C.c_void_p, C.c_float, C.c_uint64, C.c_int32, C.c_int32, C.c_int32,
                                  C.c_int64, C.c_void_p]),
+    "sky_grf_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "sky_perturb_ic_grf": (C.c_int, [C.c_void_p, C.c_void_p, C.c_float, C.c_uint64, C.c_int32, C.c_int32, C.c_int32,
+                                     C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                     C.c_void_p]),
+    "sky_grf_draw": (C.c_int, [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                               C.c_void_p]),
     "sky_model_profile_begin": (C.c_int, [C.c_void_p, C.c_uint64]),
     "sky_model_profile_end": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int32]),
     "sky_profile_tag_count": (C.c_int, []),

@@ -5,6 +5,7 @@
 #include <cstring>
 
 #include "engine.h"
+#include "philox.cuh"
 #include "sky_common.cuh"
 
 namespace sky {
@@ -201,20 +202,6 @@ const float* Engine::param(const char* name, uint64_t expect) {
 // ---------------------------------------------------------------------------------------
 // Philox4x32-10 Gaussian perturbation (K11)
 // ---------------------------------------------------------------------------------------
-__device__ __forceinline__ void philox_round(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
-  const uint32_t M0 = 0xD2511F53u, M1 = 0xCD9E8D57u;
-  uint32_t hi0 = __umulhi(M0, c[0]), lo0 = M0 * c[0];
-  uint32_t hi1 = __umulhi(M1, c[2]), lo1 = M1 * c[2];
-  uint32_t n0 = hi1 ^ c[1] ^ k0, n2 = hi0 ^ c[3] ^ k1;
-  c[0] = n0; c[1] = lo1; c[2] = n2; c[3] = lo0;
-}
-__device__ __forceinline__ void philox4x32_10(uint32_t (&c)[4], uint32_t k0, uint32_t k1) {
-#pragma unroll
-  for (int r = 0; r < 10; ++r) {
-    philox_round(c, k0, k1);
-    k0 += 0x9E3779B9u; k1 += 0xBB67AE85u;
-  }
-}
 // each thread perturbs 4 consecutive floats of one (member, channel) plane
 __global__ void k_perturb_ic(float* __restrict__ x, const float* __restrict__ sigma, float amp, uint64_t seed,
                              int member0, int channels, long long plane, long long n_quads_per_plane,

@@ -6,6 +6,7 @@ PyTorch tensors are used as device-memory containers only: the engine receives r
 from __future__ import annotations
 
 import ctypes as C
+import functools
 from collections import OrderedDict
 
 import numpy as np
@@ -233,6 +234,77 @@ def perturb_ic(x, sigma_c, amp: float, seed: int, member0: int = 0):
     st = torch.cuda.current_stream(x.device).cuda_stream
     _ffi.check(_ffi.lib().sky_perturb_ic(x.data_ptr(), sigma_c.data_ptr(), float(amp), int(seed), int(member0), M,
                                          Cn, plane, st), "sky_perturb_ic")
+    return x
+
+
+def grf_spectrum(alpha: float = 2.0, tau: float = 3.0, lmax: int = 180):
+    """Per-degree standard deviations of the spherical Gaussian random field, float64 [lmax + 1]:
+    s_l = k (l (l + 1) + tau^2)^(-alpha / 2) for 1 <= l <= lmax, s_0 = 0 (zero mean over the sphere), with k chosen so that
+    sum_l s_l^2 (2l + 1) / (4 pi) = 1 (unit pointwise variance).  Also returns the fraction of the untruncated field's
+    variance that degrees <= lmax keep (alpha > 1, else the untruncated variance is infinite)."""
+    if not alpha > 1.0:
+        raise ValueError(f"alpha = {alpha} must exceed 1 for the field's variance to be finite")
+    if lmax < 1:
+        raise ValueError(f"lmax = {lmax} must be at least 1")
+    l = np.arange(lmax + 1, dtype=np.float64)
+    s = (l * (l + 1) + tau * tau) ** (-alpha / 2)
+    s[0] = 0.0
+    var = np.sum(s * s * (2 * l + 1))
+    # untruncated sum: exact terms up to 2^20, then the integral of (2l + 1) u^-alpha du / dl from u(N + 1/2)
+    big = np.arange(1, 1 << 20, dtype=np.float64)
+    u = lambda x: x * (x + 1) + tau * tau  # noqa: E731
+    total = np.sum((2 * big + 1) * u(big) ** -alpha) + u(big[-1] + 0.5) ** (1 - alpha) / (alpha - 1)
+    return s / np.sqrt(var / (4 * np.pi)), float(var / total)
+
+
+_GRF_TABLES: "OrderedDict[tuple, object]" = OrderedDict()
+
+
+def grf_legendre_table(nlat: int, lmax: int, device):
+    """Pbar_l^m(cos theta_k) on the equiangular grid (sht.legpoly), fp32 on ``device``, m-major triangle
+    [m][k][l - m] (the layout sky_perturb_ic_grf reads; 47 MB at nlat 721, lmax 180).  The last four are cached."""
+    import torch
+    from . import sht
+    key = (nlat, lmax, str(device))
+    if key not in _GRF_TABLES:
+        p = sht.legpoly(lmax + 1, lmax + 1, sht.clenshaw_curtis(nlat)[0])          # [m, l, k]
+        tab = np.concatenate([p[m, m:].T.astype(np.float32).reshape(-1) for m in range(lmax + 1)])
+        _GRF_TABLES[key] = torch.from_numpy(tab).to(device)
+        while len(_GRF_TABLES) > 4:
+            _GRF_TABLES.popitem(last=False)
+    return _GRF_TABLES[key]
+
+
+@functools.lru_cache(maxsize=16)
+def _grf_spectrum_device(alpha: float, tau: float, lmax: int, device):
+    import torch
+    return torch.from_numpy(grf_spectrum(alpha, tau, lmax)[0].astype(np.float32)).to(device)
+
+
+def perturb_ic_grf(x, sigma_c, amp: float, seed: int, member0: int = 0, alpha: float = 2.0, tau: float = 3.0,
+                   lmax: int = 180):
+    """In-place spherically correlated perturbation of (M, C, nlat, nlon) CUDA fp32 members on the equiangular grid:
+    x[m, c] += amp sigma_c f, f a Gaussian random field with unit pointwise variance and the spectrum of
+    ``grf_spectrum(alpha, tau, lmax)``, drawn per (seed, member0 + m, c) (include/skyrim_b200.h sky_perturb_ic_grf).
+    Channels with sigma_c == 0 stay bit-identical.  lmax may be at most (nlat - 1) / 2, the finest degree the grid's
+    latitudes resolve (360 at 0.25 degrees)."""
+    import torch
+    assert x.is_cuda and x.dtype == torch.float32 and x.is_contiguous() and x.dim() == 4
+    M, Cn, nlat, nlon = x.shape
+    assert sigma_c.is_cuda and sigma_c.dtype == torch.float32 and sigma_c.is_contiguous() and sigma_c.numel() == Cn
+    if not 1 <= lmax <= (nlat - 1) // 2:
+        raise ValueError(f"lmax = {lmax} must lie in [1, {(nlat - 1) // 2}] on {nlat} latitudes")
+    L = _ffi.lib()
+    s = _grf_spectrum_device(float(alpha), float(tau), lmax, x.device)
+    leg = grf_legendre_table(nlat, lmax, x.device)
+    nbytes = L.sky_grf_workspace_bytes(M, Cn, nlat, nlon, lmax)
+    if nbytes == 0:
+        _ffi.check(-1, "sky_grf_workspace_bytes", L)
+    ws = torch.empty(nbytes, dtype=torch.uint8, device=x.device)
+    st = torch.cuda.current_stream(x.device).cuda_stream
+    _ffi.check(L.sky_perturb_ic_grf(x.data_ptr(), sigma_c.data_ptr(), float(amp), int(seed), int(member0), M, Cn, nlat,
+                                    nlon, lmax, s.data_ptr(), leg.data_ptr(), ws.data_ptr(), nbytes, st),
+               "sky_perturb_ic_grf", L)
     return x
 
 

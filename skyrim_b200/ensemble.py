@@ -38,14 +38,25 @@ class EnsembleRunner:
     """Per-rank driver: M members resident on this GPU, chained device-resident steps."""
 
     def __init__(self, engine, base_state, sigma_c, members_per_gpu: int, rank: int = 0, amp: float = 0.05,
-                 seed: int = 0):
+                 seed: int = 0, perturbation: str = "gaussian", grf: dict | None = None):
+        """``perturbation``: "gaussian" adds independent N(0, 1) amp sigma_c noise at every grid point (K11);
+        "spherical_grf" adds amp sigma_c times a spherical Gaussian random field of unit pointwise variance,
+        ``grf`` = keyword arguments of ``engine.perturb_ic_grf`` (alpha, tau, lmax)."""
         import torch
-        from .engine import perturb_ic
+        from .engine import perturb_ic, perturb_ic_grf
+        if perturbation not in ("gaussian", "spherical_grf"):
+            raise ValueError(f"unknown perturbation {perturbation!r} (gaussian, spherical_grf)")
+        if grf and perturbation != "spherical_grf":
+            raise ValueError("grf options need perturbation='spherical_grf'")
         self.engine, self.M, self.rank = engine, members_per_gpu, rank
         dev = torch.device("cuda", engine.device)
         x = torch.as_tensor(base_state, dtype=torch.float32)[None].repeat(self.M, 1, 1, 1).to(dev).contiguous()
         self.sigma = torch.as_tensor(sigma_c, dtype=torch.float32, device=dev)
-        perturb_ic(x, self.sigma, amp, seed=seed, member0=rank * self.M)  # Philox keyed by the GLOBAL member id
+        # Philox keyed by the GLOBAL member id
+        if perturbation == "gaussian":
+            perturb_ic(x, self.sigma, amp, seed=seed, member0=rank * self.M)
+        else:
+            perturb_ic_grf(x, self.sigma, amp, seed=seed, member0=rank * self.M, **(grf or {}))
         self.x, self.y = x, torch.empty_like(x)
         self.steps = 0
 
