@@ -18,6 +18,8 @@
 #include "gemm_tb.cuh"
 #define SKY_GC_EPILOGUES_ONLY   // graphcast_ops.cuh: the epilogues, not the engine's kernels (defined in graphcast_engine.o)
 #include "graphcast_ops.cuh"
+#include "attention_tc.cuh"   // EpiQkvWin (the attention kernels are defined in pangu_engine.o)
+#include "probe_geo.cuh"
 
 extern "C" {
 
@@ -40,6 +42,7 @@ enum {
   SKY_PROBE_EPI_GC_LN0 = 14,      // EpiGcLn<0>
   SKY_PROBE_EPI_GC_LN1 = 15,      // EpiGcLn<1>
   SKY_PROBE_EPI_GC_LN2 = 16,      // EpiGcLn<2>
+  SKY_PROBE_EPI_QKV_WIN = 17,     // EpiQkvWin (Pangu's QKV projection -> q | k | v window image)
 };
 
 // Every pointer is a device pointer; every *_bytes / *_floats field is the size of the allocation behind it, which the
@@ -77,6 +80,11 @@ typedef struct {
   void* yimg; const float* xin; const void* xin_img; const float* dstd;
   int64_t xin_bytes, plane;
   int32_t nprog;
+  // EpiQkvWin: the token grid (M = members x T), the cyclic shift, head pairs and the bytes between the q, k and v parts
+  // of the window image `hi` (img_bytes long); the projection's bias is `bias`
+  sky_probe_geo_t geo;
+  int32_t roll, pairs;
+  int64_t part_stride;
 } sky_probe_case_t;
 
 SKY_API int sky_probe_case_size(void) { return (int)sizeof(sky_probe_case_t); }
@@ -293,6 +301,21 @@ int check_epilogue(const Case& c) {
       if (c.epi == SKY_PROBE_EPI_GC_LN2) PROBE_REQUIRE(c.xin_img && aligned16(c.xin_img) && img_need <= c.xin_bytes, "residual image");
       return 0;
     }
+    case SKY_PROBE_EPI_QKV_WIN: {
+      const char* ge = probe_geo_error(c.geo, c.pairs);
+      PROBE_REQUIRE(!ge, "QKV window image: Geo: %s", ge ? ge : "");
+      PROBE_REQUIRE(c.n == 3 * c.geo.C && c.n_valid == c.n && c.batches == 1, "QKV window image: N=%d is not 3C=%d, or n_valid / batches",
+                    c.n, 3 * c.geo.C);
+      PROBE_REQUIRE(c.roll == 0 || c.roll == 1, "QKV window image: roll %d", c.roll);
+      PROBE_REQUIRE(c.m % c.geo.T == 0, "QKV window image: M=%lld is not members x T=%d", (long long)c.m, c.geo.T);
+      // the epilogue's 32-bit row arithmetic: members x tokens and members x windows x pairs x 144 rows below 2^31
+      const long long tiles = c.m / c.geo.T * c.geo.nWin * c.pairs;
+      PROBE_REQUIRE(c.m < (1LL << 31) && tiles * WIN_TOK < (1LL << 31), "QKV window image: %lld tiles overflow 32-bit rows", tiles);
+      PROBE_REQUIRE(c.part_stride >= tiles * AT_TILE_B && c.part_stride % 16 == 0, "QKV window image: part stride %lld (%lld tiles)",
+                    (long long)c.part_stride, tiles);
+      PROBE_REQUIRE(c.hi && aligned16(c.hi) && 2 * c.part_stride + tiles * AT_TILE_B <= c.img_bytes, "QKV window image too small");
+      return check_vec(c, c.bias, c.n, "bias");
+    }
     default:
       PROBE_REQUIRE(false, "unknown epilogue %d", c.epi);
   }
@@ -359,6 +382,9 @@ EpiGcLn<kRes> make_gcln(const Case& c) {
 template <> EpiGcLn<0> make_epi(const Case& c) { return make_gcln<0>(c); }
 template <> EpiGcLn<1> make_epi(const Case& c) { return make_gcln<1>(c); }
 template <> EpiGcLn<2> make_epi(const Case& c) { return make_gcln<2>(c); }
+template <> EpiQkvWin make_epi(const Case& c) {
+  return EpiQkvWin{(uint8_t*)c.hi, c.part_stride, c.bias, probe_geo(c.geo), c.roll, c.geo.C, c.pairs};
+}
 
 template <int... BNs> struct BnList {};
 
@@ -378,7 +404,8 @@ int by_bn(const Case& c, const Sched& sc, cudaStream_t st, BnList<BNs...>) {
 // The (schedule, epilogue, BLOCK_N) lists mirror what the engines instantiate:
 //   SFNO SfnoEngine::gemm_op: SchedW / SchedW<true> x its epilogues x {16, 32, 64, 80, 192, 240, 256};
 //   SFNO SfnoEngine::gemm_tb: SchedTB x {EpiSplitRemap, EpiF32Batched<false>, EpiGeluStatsImg} x {64, 128, 192, 256};
-//   Pangu: SchedW x Epi2F32Img<true, true, *> at 192, and the pair kernel at 192; fc1's Epi2F16<true, true> at 192;
+//   Pangu: SchedW x Epi2F32Img<true, true, *> at 192, and the pair kernel at 192; fc1's Epi2F16<true, true> at 192; the QKV
+//   projection's EpiQkvWin at 192;
 //   GraphCast: EpiGcSiluImg<0 / 2> and the node tables' Epi2F16<false, false> at 256, EpiGcOut at 128, and the pair kernel
 //   with EpiGcLn<0 / 1 / 2> at 256 (GraphCast never gathers exactly one table: EpiGcSiluImg<1> is not instantiated).
 using BnSfno = BnList<16, 32, 64, 80, 192, 240, 256>;
@@ -428,6 +455,7 @@ int dispatch(const Case& c, cudaStream_t st) {
           case SKY_PROBE_EPI_GC_SILU0: return by_bn<false, EpiGcSiluImg<0>>(c, sc, st, BnList<256>{});
           case SKY_PROBE_EPI_GC_SILU2: return by_bn<false, EpiGcSiluImg<2>>(c, sc, st, BnList<256>{});
           case SKY_PROBE_EPI_GC_OUT: return by_bn<false, EpiGcOut>(c, sc, st, BnList<128>{});
+          case SKY_PROBE_EPI_QKV_WIN: return by_bn<false, EpiQkvWin>(c, sc, st, BnList<192>{});
           default: break;
         }
       }

@@ -57,6 +57,192 @@ __global__ void k_pack_bias_table(const float* __restrict__ src, __half* __restr
   dst[idx] = __float2half_rn(src[(long long)l * n_type * heads + th] * 1.4426950408889634f);
 }
 
+int launch_pack_bias_table(const float* src, __half* dst, int n_type, int heads, cudaStream_t st) {
+  const long long tot = (long long)AT_TABLE * n_type * heads;
+  if (tot <= 0) return 0;
+  k_pack_bias_table<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(src, dst, AT_TABLE, n_type, heads);
+  SKY_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ======================================================================================
+// window image fill and window attention (layout, AttnArgs and EpiQkvWin: attention_tc.cuh)
+// ======================================================================================
+// latitude-padding rows of the window image (tokens with x = 0): q, k, v = the projection's bias
+__global__ void __launch_bounds__(256) k_qkv_fill_pad(uint8_t* __restrict__ out, long long part_stride, const float* __restrict__ bias,
+                                                      Geo g, int roll, int B, int pairs, int C, long long total) {
+  long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  const int chunk = (int)(t & 7); t >>= 3;
+  const int pair = (int)(t % pairs); t /= pairs;
+  int w = (int)(t % g.W); t /= g.W;
+  const int npad = g.Hp - g.H;
+  int h = g.H + (int)(t % npad); t /= npad;
+  int z = (int)(t % g.Z); t /= g.Z;
+  const int b = (int)(t % B); const int part = (int)(t / B);
+  if (roll) {
+    z -= SZ; if (z < 0) z += g.Z;
+    h -= SH; if (h < 0) h += g.Hp;
+    w -= SW; if (w < 0) w += g.W;
+  }
+  const int wz = z / WZ, zj = z % WZ, wh = h / WH, hj = h % WH, ww = w / WW, wj = w % WW;
+  const long long win = (long long)b * g.nWin + ((long long)wz * g.nWh + wh) * g.nWw + ww;
+  const int j = (zj * WH + hj) * WW + wj;
+  const float* bp = bias + part * C + pair * 64 + chunk * 8;
+  uint4 pk;
+  pk.x = pack_half2(bp[0], bp[1]); pk.y = pack_half2(bp[2], bp[3]);
+  pk.z = pack_half2(bp[4], bp[5]); pk.w = pack_half2(bp[6], bp[7]);
+  *reinterpret_cast<uint4*>(out + (size_t)part * part_stride + ((size_t)(win * pairs + pair) * WIN_TOK + j) * 128 +
+                            (((uint32_t)chunk ^ ((uint32_t)j & 7u)) << 4)) = pk;
+}
+
+int launch_qkv_fill_pad(uint8_t* out, long long part_stride, const float* bias, const Geo& g, int roll, int B, int pairs,
+                        cudaStream_t st) {
+  const long long total = 3LL * B * g.Z * (g.Hp - g.H) * g.W * pairs * 8;
+  if (total <= 0) return 0;
+  k_qkv_fill_pad<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(out, part_stride, bias, g, roll, B, pairs, g.C, total);
+  SKY_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// the attention kernel
+// ---------------------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(AT_THREADS) k_window_attention_tc(const AttnArgs a) {
+  extern __shared__ __align__(1024) uint8_t at_smem[];
+  const Geo& g = a.g;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  // item n = ((type * pairs + pair) * B + b) * nWw + ww
+  const long long n = blockIdx.x;
+  const long long key = n / ((long long)a.B * g.nWw);
+  const int type = (int)(key / a.pairs), pair = (int)(key % a.pairs);
+  const int wz = type / g.nWh, wh = type % g.nWh;
+  const int ww = (int)(n % g.nWw), b = (int)((n / g.nWw) % a.B);
+  const uint8_t* src = a.qkv + ((size_t)(((long long)b * g.nWin + (long long)type * g.nWw + ww) * a.pairs + pair)) * AT_TILE_B;
+
+  // ---- q, k, v tiles and the pair's two compact bias tables -> shared memory ----
+  for (int i = tid; i < 3 * AT_TILE_B / 16; i += AT_THREADS) {
+    const int part = i / (AT_TILE_B / 16), off = i - part * (AT_TILE_B / 16);
+    reinterpret_cast<uint4*>(at_smem)[i] = __ldg(reinterpret_cast<const uint4*>(src + (size_t)part * a.part_stride) + off);
+  }
+  {
+    const uint4* tsrc = reinterpret_cast<const uint4*>(a.bias_tab + ((long long)type * g.heads + 2 * pair) * AT_TABLE);
+    for (int i = tid; i < 2 * AT_TABLE * 2 / 16; i += AT_THREADS) reinterpret_cast<uint4*>(at_smem + AT_OFF_TAB)[i] = __ldg(tsrc + i);
+  }
+  int* kpart = reinterpret_cast<int*>(at_smem + AT_OFF_KEY);
+  int* kflag = kpart + WIN_TOK;
+  for (int j = tid; j < WIN_TOK; j += AT_THREADS) {
+    const int wj = j % WW, hj = (j / WW) % WH, zj = j / (WW * WH);
+    kpart[j] = (WZ * zj) * ((2 * WW - 1) * WH * WH) + (WH * hj) * (2 * WW - 1) - wj;
+    kflag[j] = (zj >= WZ - SZ ? 1 : 0) | (hj >= WH - SH ? 2 : 0);
+  }
+  __syncthreads();
+
+  const uint32_t q_s = smem_u32(at_smem), k_s = q_s + AT_TILE_B, v_s = q_s + 2 * AT_TILE_B;
+  const __half* tabs = reinterpret_cast<const __half*>(at_smem + AT_OFF_TAB);
+  const int fmask = a.roll ? ((wz == g.nWz - 1 ? 1 : 0) | (wh == g.nWh - 1 ? 2 : 0)) : 0;
+  const __half mask_h = __float2half_rn(a.mask_l2);
+  // this thread's two query rows (fragment rows l/4 and l/4 + 8 of the warp's 16)
+  int row[2], rpart[2], rflag[2];
+#pragma unroll
+  for (int u = 0; u < 2; ++u) {
+    const int i = 16 * warp + (lane >> 2) + 8 * u;
+    const int wi = i % WW, hi = (i / WW) % WH, zi = i / (WW * WH);
+    row[u] = i;
+    rpart[u] = zi * ((2 * WW - 1) * WH * WH) + hi * (2 * WW - 1) + wi + (WW - 1);
+    rflag[u] = (zi >= WZ - SZ ? 1 : 0) | (hi >= WH - SH ? 2 : 0);
+  }
+  const int c2 = 2 * (lane & 3);   // first of this thread's two columns in every 8-column fragment
+
+#pragma unroll 1
+  for (int hd = 0; hd < 2; ++hd) {
+    // ---- S = Q K^T: 16 rows x 144 keys, K = 32 (two k16 steps = the head's four 16-byte chunks) ----
+    uint32_t qa[2][4];
+#pragma unroll
+    for (int ks = 0; ks < 2; ++ks)
+      ldsm_x4(at_chunk(q_s, 16 * warp + (lane & 7) + 8 * ((lane >> 3) & 1), hd * 4 + 2 * ks + (lane >> 4)), qa[ks]);
+    float s[WIN_TOK / 8][4];
+#pragma unroll
+    for (int j = 0; j < WIN_TOK / 8; ++j) {
+      s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+      uint32_t kb[4];   // keys 8j .. 8j+7: dims 0-7 | 8-15 | 16-23 | 24-31
+      ldsm_x4(at_chunk(k_s, 8 * j + (lane & 7), hd * 4 + (lane >> 3)), kb);
+      mma_16816(s[j], qa[0], kb[0], kb[1]);
+      mma_16816(s[j], qa[1], kb[2], kb[3]);
+    }
+    // ---- scale + bias (+ shift mask), row max ----
+    const __half* tab = tabs + hd * AT_TABLE;
+    float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+    for (int j = 0; j < WIN_TOK / 8; ++j) {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        const int u = e >> 1, col = 8 * j + c2 + (e & 1);
+        __half bh = tab[rpart[u] + kpart[col]];
+        if ((rflag[u] ^ kflag[col]) & fmask) bh = __hadd(bh, mask_h);
+        s[j][e] = fmaf(s[j][e], a.sl2, __half2float(bh));
+        mx[u] = fmaxf(mx[u], s[j][e]);
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      mx[u] = fmaxf(mx[u], __shfl_xor_sync(0xffffffffu, mx[u], 1));
+      mx[u] = fmaxf(mx[u], __shfl_xor_sync(0xffffffffu, mx[u], 2));
+    }
+    // ---- P = exp2(s - max) in (0, 1]: fp16 into the tensor core, fp32 row sums ----
+    uint32_t p[WIN_TOK / 8][2];
+    float sum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < WIN_TOK / 8; ++j) {
+      const float e0 = mufu_ex2(s[j][0] - mx[0]), e1 = mufu_ex2(s[j][1] - mx[0]);
+      const float e2 = mufu_ex2(s[j][2] - mx[1]), e3 = mufu_ex2(s[j][3] - mx[1]);
+      sum[0] += e0 + e1; sum[1] += e2 + e3;
+      p[j][0] = pack_half2(e0, e1); p[j][1] = pack_half2(e2, e3);
+    }
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      sum[u] += __shfl_xor_sync(0xffffffffu, sum[u], 1);
+      sum[u] += __shfl_xor_sync(0xffffffffu, sum[u], 2);
+    }
+    // ---- O = P V: K = 144 keys (nine k16 steps), N = 32 dims (four n8 fragments) ----
+    float o[4][4];
+#pragma unroll
+    for (int c = 0; c < 4; ++c) o[c][0] = o[c][1] = o[c][2] = o[c][3] = 0.f;
+#pragma unroll
+    for (int t = 0; t < WIN_TOK / 16; ++t) {
+      const uint32_t pa[4] = {p[2 * t][0], p[2 * t][1], p[2 * t + 1][0], p[2 * t + 1][1]};
+      uint32_t v0[4], v1[4];   // keys 16t .. 16t+7 | 16t+8 .. 16t+15, dims 8c .. 8c+7 in register c
+      ldsm_x4_t(at_chunk(v_s, 16 * t + (lane & 7), hd * 4 + (lane >> 3)), v0);
+      ldsm_x4_t(at_chunk(v_s, 16 * t + 8 + (lane & 7), hd * 4 + (lane >> 3)), v1);
+#pragma unroll
+      for (int c = 0; c < 4; ++c) mma_16816(o[c], pa, v0[c], v1[c]);
+    }
+    // ---- 1/sum -> fp16 -> 64 bytes of the projection's operand image per row ----
+#pragma unroll
+    for (int u = 0; u < 2; ++u) {
+      const long long tok = at_row_token(g, a.roll, b, wz, wh, ww, row[u]);
+      if (tok < 0) continue;
+      const float inv = 1.f / sum[u];
+      uint8_t* dst = a.att_img + ((size_t)(tok >> 7) * a.att_nkb + pair) * (size_t)G2_A_BYTES + (size_t)(tok & 127) * 128;
+      const uint32_t r7 = (uint32_t)tok & 7u;
+#pragma unroll
+      for (int c = 0; c < 4; ++c)
+        *reinterpret_cast<uint32_t*>(dst + ((((uint32_t)(hd * 4 + c)) ^ r7) << 4) + 2 * c2) =
+            pack_half2(o[c][2 * u] * inv, o[c][2 * u + 1] * inv);
+    }
+  }
+}
+
+int launch_window_attention_tc(const AttnArgs& a, int num_sms, cudaStream_t st) {
+  (void)num_sms;
+  static std::atomic<uint64_t> configured{0};
+  if (int rc = smem_opt_in(configured, reinterpret_cast<const void*>(k_window_attention_tc), AT_SMEM_BYTES)) return rc;
+  if (a.items <= 0) return 0;
+  k_window_attention_tc<<<(unsigned)a.items, AT_THREADS, AT_SMEM_BYTES, st>>>(a);
+  SKY_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
 // DownSample front end: 2x2 (lat, lon) merge + zero pad + LayerNorm(4C) -> fp16 tile image.
 // One warp per output row; NPL = (4C)/32 values per lane.
 template <int NPL>
@@ -238,7 +424,7 @@ struct PanguEngine : Engine {
         if (!bt) return SKY_ERR_ARG;
         b.bias_tab = dalloc<__half>((size_t)tot);
         if (!b.bias_tab) return SKY_ERR_NOMEM;
-        k_pack_bias_table<<<(unsigned)((tot + 255) / 256), 256, 0, st>>>(bt, b.bias_tab, AT_TABLE, n_type, heads);
+        if ((rc = launch_pack_bias_table(bt, b.bias_tab, n_type, heads, st))) return rc;
         count_launch();
       }
     }
@@ -322,12 +508,11 @@ struct PanguEngine : Engine {
       if ((rc = gemm2<192>(KT_QKV, A, e, b.qkv, R, st))) return rc;
       if (g.Hp > g.H) {   // latitude-padding tokens (x = 0): their q, k, v rows are the projection's bias.  (Writing them from
                           // the GEMM epilogue of the neighbouring tokens instead cost the GEMM 0.5 ms/step: measured, reverted.)
-        const long long total = 3LL * B * g.Z * (g.Hp - g.H) * g.W * pairs * 8;
         prof_begin(KT_QKV, st);
-        k_qkv_fill_pad<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(ws.qkv, part_stride, b.qkv_b, g, roll, B, pairs, C, total);
+        rc = launch_qkv_fill_pad(ws.qkv, part_stride, b.qkv_b, g, roll, B, pairs, st);
         prof_end(KT_QKV, st);
         count_launch();
-        SKY_CUDA_OK(cudaGetLastError());
+        if (rc) return rc;
       }
     }
     {
