@@ -9,11 +9,19 @@
 //   Windowing, the cyclic shift and the latitude padding were applied by the producer, so one work item is three
 //   contiguous 18 KB tiles.
 //
-// One CTA per item (window, head pair), nine warps: warp w owns query rows 16w .. 16w+15 of both heads.  The q, k, v
-// tiles and the pair's two compact bias tables are copied to shared memory once; per head the warp computes its 16 x 144
-// score block in registers (ldmatrix + mma.sync), adds the bias gathered from the compact table (shift mask folded in,
-// in fp16), takes exp2 against the row max, and multiplies P (fp16, straight from the score registers) by V
-// (ldmatrix.trans).  1/sum is applied to the 32 outputs of each row, which go to the projection's operand image.
+// Work item n = ((type * pairs + pair) * B + b) * nWw + ww, one (window, head pair).  The kernel is persistent: CTA c
+// walks the contiguous item range [c items / G, (c+1) items / G) of a grid of G = min(items, SMs) CTAs, so consecutive
+// items of a CTA share their window type and head pair for B nWw items at a time.  Ten warps:
+//   * warp 9, the producer: one lane streams each item's q, k, v tiles (three contiguous 18 KB bulk copies) into a
+//     two-slot ring, so the next item's loads run under the current item's compute;
+//   * warps 0-8 compute: warp w owns query rows 16w .. 16w+15 of both heads.  Per head the warp computes its 16 x 144
+//     score block in registers (ldmatrix + mma.sync), adds the bias, takes exp2 against the row max, and multiplies P
+//     (fp16, straight from the score registers) by V (ldmatrix.trans).  1/sum is applied to the 32 outputs of each row.
+// The bias (compact table entry + shift mask, added in fp16) depends only on (type, head) and the thread's fragment
+// position, so each warp expands its 16 x 144 slice of both heads into shared memory in the order the score loop
+// consumes it (nine 16-byte loads per head) and rebuilds it only when the item's (type, pair) changes.  Once a warp
+// holds its q fragments in registers, its 16 q rows of the slot are free: the output rows are staged there and leave as
+// full 128-byte lines of the projection's operand image.
 // This header holds the layout, EpiQkvWin and the device helpers; the kernels themselves are in pangu_engine.cu.
 #pragma once
 #include <cstdio>
@@ -26,11 +34,16 @@ namespace sky {
 
 constexpr int AT_TABLE = (2 * WW - 1) * WH * WH * WZ * WZ;   // 3312 entries of the compact bias table per (type, head)
 constexpr int AT_TILE_B = WIN_TOK * 128;                     // 18432: one (window, head pair) tile of q, k or v
-constexpr int AT_OFF_TAB = 3 * AT_TILE_B;                    // q | k | v tiles, then the two heads' compact tables (fp16)
-constexpr int AT_OFF_KEY = AT_OFF_TAB + 2 * AT_TABLE * 2;    // per key: table offset and shift-region flags (int32 each)
-constexpr int AT_SMEM_BYTES = AT_OFF_KEY + 2 * WIN_TOK * 4;
-constexpr int AT_THREADS = 32 * (WIN_TOK / 16);              // one warp per 16 query rows
-static_assert(WIN_TOK % 16 == 0 && (2 * AT_TABLE * 2) % 16 == 0, "tile shapes");
+constexpr int AT_WARPS = WIN_TOK / 16;                       // compute warps, one per 16 query rows
+constexpr int AT_THREADS = 32 * (AT_WARPS + 1);              // + the producer warp
+constexpr int AT_STAGES = 2;                                 // ring slots
+constexpr int AT_SLOT_B = 3 * AT_TILE_B;                     // one item's q | k | v tiles
+constexpr int AT_BIAS_WARP_B = AT_WARPS * 32 * 16;           // a warp's 16 x 144 fp16 bias slice: uint4 [i < 9][lane]
+constexpr int AT_BIAS_HEAD_B = AT_WARPS * AT_BIAS_WARP_B;    // one head: 144 x 144 fp16
+constexpr int AT_OFF_BIAS = AT_STAGES * AT_SLOT_B;           // ring, then the bias [head][warp][i][lane], then the barriers
+constexpr int AT_OFF_BAR = AT_OFF_BIAS + 2 * AT_BIAS_HEAD_B;
+constexpr int AT_SMEM_BYTES = AT_OFF_BAR + 2 * AT_STAGES * 8;
+static_assert(WIN_TOK % 16 == 0 && AT_SMEM_BYTES <= 227 * 1024, "tile shapes");
 
 struct AttnArgs {
   const uint8_t* qkv;        // window image, 3 parts
@@ -67,6 +80,17 @@ __device__ __forceinline__ void mma_16816(float (&c)[4], const uint32_t (&a)[4],
 // shared address of 16-byte chunk c of row j of a window tile (swizzled: chunk c sits at c ^ (j & 7))
 __device__ __forceinline__ uint32_t at_chunk(uint32_t tile_s, int j, int c) {
   return tile_s + (uint32_t)j * 128u + ((uint32_t)(c ^ (j & 7)) << 4);
+}
+
+// shared-space 32- and 128-bit accesses (volatile: the bias slice and the staged rows are rewritten between reads)
+__device__ __forceinline__ void sts_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v) : "memory");
+}
+__device__ __forceinline__ void sts_b32x4(uint32_t addr, const uint32_t (&v)[4]) {
+  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]) : "memory");
+}
+__device__ __forceinline__ void lds_b32x4(uint32_t addr, uint32_t (&v)[4]) {
+  asm volatile("ld.shared.v4.b32 {%0, %1, %2, %3}, [%4];" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(addr) : "memory");
 }
 
 // window position (wz, wh, ww, row j) -> natural token of member b, or -1 for a latitude-padding row

@@ -106,139 +106,218 @@ int launch_qkv_fill_pad(uint8_t* out, long long part_stride, const float* bias, 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// the attention kernel
+// the attention kernel (work split, warp roles and shared-memory layout: attention_tc.cuh)
 // ---------------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(AT_THREADS) k_window_attention_tc(const AttnArgs a) {
+// item n = ((type * pairs + pair) * B + b) * nWw + ww; a CTA decodes its first item and steps through the rest
+struct AtItem {
+  int type, pair, b, ww;
+  __device__ AtItem(const AttnArgs& a, long long n) {
+    const long long key = n / ((long long)a.B * a.g.nWw);
+    type = (int)(key / a.pairs); pair = (int)(key % a.pairs); b = (int)((n / a.g.nWw) % a.B); ww = (int)(n % a.g.nWw);
+  }
+  __device__ void next(const AttnArgs& a) {
+    if (++ww < a.g.nWw) return;
+    ww = 0;
+    if (++b < a.B) return;
+    b = 0;
+    if (++pair < a.pairs) return;
+    pair = 0; ++type;
+  }
+};
+
+__global__ void __launch_bounds__(AT_THREADS, 1) k_window_attention_tc(const AttnArgs a) {
   extern __shared__ __align__(1024) uint8_t at_smem[];
   const Geo& g = a.g;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  // item n = ((type * pairs + pair) * B + b) * nWw + ww
-  const long long n = blockIdx.x;
-  const long long key = n / ((long long)a.B * g.nWw);
-  const int type = (int)(key / a.pairs), pair = (int)(key % a.pairs);
-  const int wz = type / g.nWh, wh = type % g.nWh;
-  const int ww = (int)(n % g.nWw), b = (int)((n / g.nWw) % a.B);
-  const uint8_t* src = a.qkv + ((size_t)(((long long)b * g.nWin + (long long)type * g.nWw + ww) * a.pairs + pair)) * AT_TILE_B;
-
-  // ---- q, k, v tiles and the pair's two compact bias tables -> shared memory ----
-  for (int i = tid; i < 3 * AT_TILE_B / 16; i += AT_THREADS) {
-    const int part = i / (AT_TILE_B / 16), off = i - part * (AT_TILE_B / 16);
-    reinterpret_cast<uint4*>(at_smem)[i] = __ldg(reinterpret_cast<const uint4*>(src + (size_t)part * a.part_stride) + off);
-  }
-  {
-    const uint4* tsrc = reinterpret_cast<const uint4*>(a.bias_tab + ((long long)type * g.heads + 2 * pair) * AT_TABLE);
-    for (int i = tid; i < 2 * AT_TABLE * 2 / 16; i += AT_THREADS) reinterpret_cast<uint4*>(at_smem + AT_OFF_TAB)[i] = __ldg(tsrc + i);
-  }
-  int* kpart = reinterpret_cast<int*>(at_smem + AT_OFF_KEY);
-  int* kflag = kpart + WIN_TOK;
-  for (int j = tid; j < WIN_TOK; j += AT_THREADS) {
-    const int wj = j % WW, hj = (j / WW) % WH, zj = j / (WW * WH);
-    kpart[j] = (WZ * zj) * ((2 * WW - 1) * WH * WH) + (WH * hj) * (2 * WW - 1) - wj;
-    kflag[j] = (zj >= WZ - SZ ? 1 : 0) | (hj >= WH - SH ? 2 : 0);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  uint64_t* full = reinterpret_cast<uint64_t*>(at_smem + AT_OFF_BAR);
+  uint64_t* empty = full + AT_STAGES;
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < AT_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], AT_WARPS); }
+    mbar_fence_init();
   }
   __syncthreads();
+  const long long n0 = a.items * blockIdx.x / gridDim.x, n1 = a.items * (blockIdx.x + 1) / gridDim.x;
 
-  const uint32_t q_s = smem_u32(at_smem), k_s = q_s + AT_TILE_B, v_s = q_s + 2 * AT_TILE_B;
-  const __half* tabs = reinterpret_cast<const __half*>(at_smem + AT_OFF_TAB);
-  const int fmask = a.roll ? ((wz == g.nWz - 1 ? 1 : 0) | (wh == g.nWh - 1 ? 2 : 0)) : 0;
-  const __half mask_h = __float2half_rn(a.mask_l2);
-  // this thread's two query rows (fragment rows l/4 and l/4 + 8 of the warp's 16)
-  int row[2], rpart[2], rflag[2];
-#pragma unroll
-  for (int u = 0; u < 2; ++u) {
-    const int i = 16 * warp + (lane >> 2) + 8 * u;
-    const int wi = i % WW, hi = (i / WW) % WH, zi = i / (WW * WH);
-    row[u] = i;
-    rpart[u] = zi * ((2 * WW - 1) * WH * WH) + hi * (2 * WW - 1) + wi + (WW - 1);
-    rflag[u] = (zi >= WZ - SZ ? 1 : 0) | (hi >= WH - SH ? 2 : 0);
-  }
-  const int c2 = 2 * (lane & 3);   // first of this thread's two columns in every 8-column fragment
-
-#pragma unroll 1
-  for (int hd = 0; hd < 2; ++hd) {
-    // ---- S = Q K^T: 16 rows x 144 keys, K = 32 (two k16 steps = the head's four 16-byte chunks) ----
-    uint32_t qa[2][4];
-#pragma unroll
-    for (int ks = 0; ks < 2; ++ks)
-      ldsm_x4(at_chunk(q_s, 16 * warp + (lane & 7) + 8 * ((lane >> 3) & 1), hd * 4 + 2 * ks + (lane >> 4)), qa[ks]);
-    float s[WIN_TOK / 8][4];
-#pragma unroll
-    for (int j = 0; j < WIN_TOK / 8; ++j) {
-      s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
-      uint32_t kb[4];   // keys 8j .. 8j+7: dims 0-7 | 8-15 | 16-23 | 24-31
-      ldsm_x4(at_chunk(k_s, 8 * j + (lane & 7), hd * 4 + (lane >> 3)), kb);
-      mma_16816(s[j], qa[0], kb[0], kb[1]);
-      mma_16816(s[j], qa[1], kb[2], kb[3]);
-    }
-    // ---- scale + bias (+ shift mask), row max ----
-    const __half* tab = tabs + hd * AT_TABLE;
-    float mx[2] = {-INFINITY, -INFINITY};
-#pragma unroll
-    for (int j = 0; j < WIN_TOK / 8; ++j) {
-#pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        const int u = e >> 1, col = 8 * j + c2 + (e & 1);
-        __half bh = tab[rpart[u] + kpart[col]];
-        if ((rflag[u] ^ kflag[col]) & fmask) bh = __hadd(bh, mask_h);
-        s[j][e] = fmaf(s[j][e], a.sl2, __half2float(bh));
-        mx[u] = fmaxf(mx[u], s[j][e]);
+  if (warp == AT_WARPS) {   // ---- producer: the q, k, v tiles of each item -> ring slot ----
+    if (lane == 0) {
+      int s = 0; uint32_t ph = 0;
+      AtItem it(a, n0);
+      for (long long n = n0; n < n1; ++n, it.next(a)) {
+        const uint8_t* src =
+            a.qkv + (size_t)(((long long)it.b * g.nWin + (long long)it.type * g.nWw + it.ww) * a.pairs + it.pair) * AT_TILE_B;
+        mbar_wait(&empty[s], ph ^ 1);
+        mbar_arrive_expect_tx(&full[s], AT_SLOT_B);
+        for (int p = 0; p < 3; ++p)
+          bulk_g2s(at_smem + s * AT_SLOT_B + p * AT_TILE_B, src + (size_t)p * a.part_stride, AT_TILE_B, &full[s]);
+        if (++s == AT_STAGES) { s = 0; ph ^= 1; }
       }
     }
+    return;
+  }
+
+  const int c2 = 2 * (lane & 3);   // first of this thread's two columns in every 8-column fragment
+  // this thread's nine 16-byte entries of the warp's head-0 bias slice, 512 bytes apart (head 1: + AT_BIAS_HEAD_B)
+  const uint32_t bias_s = smem_u32(at_smem + AT_OFF_BIAS + warp * AT_BIAS_WARP_B) + 16u * lane;
+  int held = -1;   // type * pairs + pair of the bias the slice holds
+  int slot = 0; uint32_t ph = 0;
+
+  AtItem it(a, n0);
+#pragma unroll 1
+  for (long long n = n0; n < n1; ++n, it.next(a)) {
+    const int wz = it.type / g.nWh, wh = it.type % g.nWh;
+    if (it.type * a.pairs + it.pair != held) {
+      // ---- bias slice of both heads: compact table entry (+ shift mask, in fp16) of every (row, key) this thread's
+      // score fragments hold, in the order the score loop consumes them.  A thread reads back only what it wrote, so
+      // the refill needs no barrier.  Runs while the item's tiles are in flight ----
+      held = it.type * a.pairs + it.pair;
+      const int fmask = a.roll ? ((wz == g.nWz - 1 ? 1 : 0) | (wh == g.nWh - 1 ? 2 : 0)) : 0;
+      const __half mask_h = __float2half_rn(a.mask_l2);
+      int rpart[2], rflag[2];   // this thread's two query rows (fragment rows l/4 and l/4 + 8 of the warp's 16)
 #pragma unroll
-    for (int u = 0; u < 2; ++u) {
-      mx[u] = fmaxf(mx[u], __shfl_xor_sync(0xffffffffu, mx[u], 1));
-      mx[u] = fmaxf(mx[u], __shfl_xor_sync(0xffffffffu, mx[u], 2));
+      for (int u = 0; u < 2; ++u) {
+        const int i = 16 * warp + (lane >> 2) + 8 * u;
+        const int wi = i % WW, hi = (i / WW) % WH, zi = i / (WW * WH);
+        rpart[u] = zi * ((2 * WW - 1) * WH * WH) + hi * (2 * WW - 1) + wi + (WW - 1);
+        rflag[u] = (zi >= WZ - SZ ? 1 : 0) | (hi >= WH - SH ? 2 : 0);
+      }
+#pragma unroll 1
+      for (int hd = 0; hd < 2; ++hd) {
+        const __half* tab = a.bias_tab + ((long long)it.type * g.heads + 2 * it.pair + hd) * AT_TABLE;
+#pragma unroll 1
+        for (int i = 0; i < WIN_TOK / 16; ++i) {   // not unrolled: 72 loads in flight at once spill the score registers
+          uint32_t w[4];
+#pragma unroll
+          for (int x = 0; x < 4; ++x) {   // word x: keys 8j + c2, 8j + c2 + 1 of row u, j = 2i + x/2, u = x%2
+            const int j = 2 * i + (x >> 1), u = x & 1;
+            __half bh[2];
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int col = 8 * j + c2 + e;
+              const int wj = col % WW, hj = (col / WW) % WH, zj = col / (WW * WH);
+              const int kpart = (WZ * zj) * ((2 * WW - 1) * WH * WH) + (WH * hj) * (2 * WW - 1) - wj;
+              const int kflag = (zj >= WZ - SZ ? 1 : 0) | (hj >= WH - SH ? 2 : 0);
+              bh[e] = __ldg(tab + rpart[u] + kpart);
+              if ((rflag[u] ^ kflag) & fmask) bh[e] = __hadd(bh[e], mask_h);
+            }
+            w[x] = (uint32_t)__half_as_ushort(bh[0]) | ((uint32_t)__half_as_ushort(bh[1]) << 16);
+          }
+          sts_b32x4(bias_s + hd * AT_BIAS_HEAD_B + i * 512, w);
+        }
+      }
     }
-    // ---- P = exp2(s - max) in (0, 1]: fp16 into the tensor core, fp32 row sums ----
-    uint32_t p[WIN_TOK / 8][2];
-    float sum[2] = {0.f, 0.f};
+
+    mbar_wait(&full[slot], ph);
+    const uint32_t q_s = smem_u32(at_smem + slot * AT_SLOT_B), k_s = q_s + AT_TILE_B, v_s = q_s + 2 * AT_TILE_B;
+    // the warp's 16 q rows stage its output rows, same swizzle: head hd's outputs overwrite exactly the chunks that held
+    // head hd's q, after the warp has them in registers
+    const uint32_t stage = q_s + 16 * warp * 128;
+
+#pragma unroll 1
+    for (int hd = 0; hd < 2; ++hd) {
+      // ---- S = Q K^T: 16 rows x 144 keys, K = 32 (two k16 steps = the head's four 16-byte chunks) ----
+      uint32_t qa[2][4];
 #pragma unroll
-    for (int j = 0; j < WIN_TOK / 8; ++j) {
-      const float e0 = mufu_ex2(s[j][0] - mx[0]), e1 = mufu_ex2(s[j][1] - mx[0]);
-      const float e2 = mufu_ex2(s[j][2] - mx[1]), e3 = mufu_ex2(s[j][3] - mx[1]);
-      sum[0] += e0 + e1; sum[1] += e2 + e3;
-      p[j][0] = pack_half2(e0, e1); p[j][1] = pack_half2(e2, e3);
+      for (int ks = 0; ks < 2; ++ks)
+        ldsm_x4(at_chunk(q_s, 16 * warp + (lane & 7) + 8 * ((lane >> 3) & 1), hd * 4 + 2 * ks + (lane >> 4)), qa[ks]);
+      __syncwarp();
+      float s[WIN_TOK / 8][4];
+#pragma unroll
+      for (int j = 0; j < WIN_TOK / 8; ++j) {
+        s[j][0] = s[j][1] = s[j][2] = s[j][3] = 0.f;
+        uint32_t kb[4];   // keys 8j .. 8j+7: dims 0-7 | 8-15 | 16-23 | 24-31
+        ldsm_x4(at_chunk(k_s, 8 * j + (lane & 7), hd * 4 + (lane >> 3)), kb);
+        mma_16816(s[j], qa[0], kb[0], kb[1]);
+        mma_16816(s[j], qa[1], kb[2], kb[3]);
+      }
+      // ---- scale + bias, row max.  Half x of entry i: s[2i + x/4][x%4] ----
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int i = 0; i < WIN_TOK / 16; ++i) {
+        uint32_t bw[4];
+        lds_b32x4(bias_s + hd * AT_BIAS_HEAD_B + i * 512, bw);
+#pragma unroll
+        for (int x = 0; x < 8; ++x) {
+          const int j = 2 * i + (x >> 2), e = x & 3;
+          const __half bh = __ushort_as_half((unsigned short)(bw[x >> 1] >> (16 * (x & 1))));
+          s[j][e] = fmaf(s[j][e], a.sl2, __half2float(bh));
+          mx[e >> 1] = fmaxf(mx[e >> 1], s[j][e]);
+        }
+      }
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        mx[u] = fmaxf(mx[u], __shfl_xor_sync(0xffffffffu, mx[u], 1));
+        mx[u] = fmaxf(mx[u], __shfl_xor_sync(0xffffffffu, mx[u], 2));
+      }
+      // ---- P = exp2(s - max) in (0, 1]: fp16 into the tensor core, fp32 row sums ----
+      uint32_t p[WIN_TOK / 8][2];
+      float sum[2] = {0.f, 0.f};
+#pragma unroll
+      for (int j = 0; j < WIN_TOK / 8; ++j) {
+        const float e0 = mufu_ex2(s[j][0] - mx[0]), e1 = mufu_ex2(s[j][1] - mx[0]);
+        const float e2 = mufu_ex2(s[j][2] - mx[1]), e3 = mufu_ex2(s[j][3] - mx[1]);
+        sum[0] += e0 + e1; sum[1] += e2 + e3;
+        p[j][0] = pack_half2(e0, e1); p[j][1] = pack_half2(e2, e3);
+      }
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        sum[u] += __shfl_xor_sync(0xffffffffu, sum[u], 1);
+        sum[u] += __shfl_xor_sync(0xffffffffu, sum[u], 2);
+      }
+      // ---- O = P V: K = 144 keys (nine k16 steps), N = 32 dims (four n8 fragments) ----
+      float o[4][4];
+#pragma unroll
+      for (int c = 0; c < 4; ++c) o[c][0] = o[c][1] = o[c][2] = o[c][3] = 0.f;
+#pragma unroll
+      for (int t = 0; t < WIN_TOK / 16; ++t) {
+        const uint32_t pa[4] = {p[2 * t][0], p[2 * t][1], p[2 * t + 1][0], p[2 * t + 1][1]};
+        uint32_t v0[4], v1[4];   // keys 16t .. 16t+7 | 16t+8 .. 16t+15, dims 8c .. 8c+7 in register c
+        ldsm_x4_t(at_chunk(v_s, 16 * t + (lane & 7), hd * 4 + (lane >> 3)), v0);
+        ldsm_x4_t(at_chunk(v_s, 16 * t + 8 + (lane & 7), hd * 4 + (lane >> 3)), v1);
+#pragma unroll
+        for (int c = 0; c < 4; ++c) mma_16816(o[c], pa, v0[c], v1[c]);
+      }
+      // ---- 1/sum -> fp16 -> the head's 64 bytes of the two staged rows ----
+#pragma unroll
+      for (int u = 0; u < 2; ++u) {
+        const int r = (lane >> 2) + 8 * u;
+        const float inv = 1.f / sum[u];
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+          sts_b32(stage + r * 128 + (((hd * 4 + c) ^ (r & 7)) << 4) + 2 * c2, pack_half2(o[c][2 * u] * inv, o[c][2 * u + 1] * inv));
+      }
     }
+    __syncwarp();
+    // ---- staged rows -> 128-byte lines of k-block `pair` of the projection's operand image, eight lanes per token row;
+    // latitude-padding rows are skipped ----
+    const long long my_tok = at_row_token(g, a.roll, it.b, wz, wh, it.ww, 16 * warp + (lane & 15));   // token of row lane % 16
 #pragma unroll
-    for (int u = 0; u < 2; ++u) {
-      sum[u] += __shfl_xor_sync(0xffffffffu, sum[u], 1);
-      sum[u] += __shfl_xor_sync(0xffffffffu, sum[u], 2);
-    }
-    // ---- O = P V: K = 144 keys (nine k16 steps), N = 32 dims (four n8 fragments) ----
-    float o[4][4];
-#pragma unroll
-    for (int c = 0; c < 4; ++c) o[c][0] = o[c][1] = o[c][2] = o[c][3] = 0.f;
-#pragma unroll
-    for (int t = 0; t < WIN_TOK / 16; ++t) {
-      const uint32_t pa[4] = {p[2 * t][0], p[2 * t][1], p[2 * t + 1][0], p[2 * t + 1][1]};
-      uint32_t v0[4], v1[4];   // keys 16t .. 16t+7 | 16t+8 .. 16t+15, dims 8c .. 8c+7 in register c
-      ldsm_x4_t(at_chunk(v_s, 16 * t + (lane & 7), hd * 4 + (lane >> 3)), v0);
-      ldsm_x4_t(at_chunk(v_s, 16 * t + 8 + (lane & 7), hd * 4 + (lane >> 3)), v1);
-#pragma unroll
-      for (int c = 0; c < 4; ++c) mma_16816(o[c], pa, v0[c], v1[c]);
-    }
-    // ---- 1/sum -> fp16 -> 64 bytes of the projection's operand image per row ----
-#pragma unroll
-    for (int u = 0; u < 2; ++u) {
-      const long long tok = at_row_token(g, a.roll, b, wz, wh, ww, row[u]);
+    for (int k = 0; k < 4; ++k) {
+      const int r = 4 * k + (lane >> 3), ch = lane & 7;
+      const long long tok = __shfl_sync(0xffffffffu, my_tok, r);
       if (tok < 0) continue;
-      const float inv = 1.f / sum[u];
-      uint8_t* dst = a.att_img + ((size_t)(tok >> 7) * a.att_nkb + pair) * (size_t)G2_A_BYTES + (size_t)(tok & 127) * 128;
-      const uint32_t r7 = (uint32_t)tok & 7u;
-#pragma unroll
-      for (int c = 0; c < 4; ++c)
-        *reinterpret_cast<uint32_t*>(dst + ((((uint32_t)(hd * 4 + c)) ^ r7) << 4) + 2 * c2) =
-            pack_half2(o[c][2 * u] * inv, o[c][2 * u + 1] * inv);
+      uint32_t v[4];
+      lds_b32x4(stage + r * 128 + ((ch ^ (r & 7)) << 4), v);
+      *reinterpret_cast<uint4*>(a.att_img + ((size_t)(tok >> 7) * a.att_nkb + it.pair) * (size_t)G2_A_BYTES +
+                                (size_t)(tok & 127) * 128 + (((uint32_t)ch ^ ((uint32_t)tok & 7u)) << 4)) = make_uint4(v[0], v[1], v[2], v[3]);
     }
+    fence_proxy_async_smem();   // the staging's generic writes are ordered before the next bulk copy into the slot
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[slot]);
+    if (++slot == AT_STAGES) { slot = 0; ph ^= 1; }
   }
 }
 
 int launch_window_attention_tc(const AttnArgs& a, int num_sms, cudaStream_t st) {
-  (void)num_sms;
   static std::atomic<uint64_t> configured{0};
   if (int rc = smem_opt_in(configured, reinterpret_cast<const void*>(k_window_attention_tc), AT_SMEM_BYTES)) return rc;
   if (a.items <= 0) return 0;
-  k_window_attention_tc<<<(unsigned)a.items, AT_THREADS, AT_SMEM_BYTES, st>>>(a);
+  if (num_sms <= 0) {
+    int dev = 0;
+    SKY_CUDA_OK(cudaGetDevice(&dev));
+    SKY_CUDA_OK(cudaDeviceGetAttribute(&num_sms, cudaDevAttrMultiProcessorCount, dev));
+  }
+  const long long grid = a.items < num_sms ? a.items : num_sms;
+  k_window_attention_tc<<<(unsigned)grid, AT_THREADS, AT_SMEM_BYTES, st>>>(a);
   SKY_CUDA_OK(cudaGetLastError());
   return 0;
 }

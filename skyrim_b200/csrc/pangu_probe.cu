@@ -3,7 +3,8 @@
 // sky_probe_pangu makes ONE launch of a kernel that is not a k_gemm2 epilogue, from raw device pointers, so that
 // tests/test_pangu_kernels_gpu.py can compare it element by element against oracle/pangu_kernels_ref.py:
 //   FILL_PAD    k_qkv_fill_pad: the q / k / v rows of latitude-padding tokens in the window image = the QKV bias
-//   ATTENTION   k_window_attention_tc: window image + compact fp16 bias tables -> (tokens, C) operand image
+//   ATTENTION   k_window_attention_tc: window image + compact fp16 bias tables -> (tokens, C) operand image; one CTA per
+//               SM, or a chosen number of CTAs through sky_probe_pangu_grid
 //   PACK_BIAS   k_pack_bias_table: fp32 (3312, type, head) -> fp16 (type, head, 3312) x log2 e
 // (The QKV projection's epilogue EpiQkvWin is reached through sky_probe_gemm.)  The kernels are launched through the
 // engine's own host launchers (attention_tc.cuh, defined in pangu_engine.o), so each has one definition.
@@ -37,6 +38,8 @@ typedef struct {
 
 SKY_API int sky_probe_pangu_size(void) { return (int)sizeof(sky_probe_pangu_t); }
 SKY_API int sky_probe_pangu(const sky_probe_pangu_t* c, void* stream);
+// sky_probe_pangu with the persistent attention kernel's grid set to grid_ctas CTAs (at most one per item); 0 = one per SM
+SKY_API int sky_probe_pangu_grid(const sky_probe_pangu_t* c, int32_t grid_ctas, void* stream);
 
 }  // extern "C"
 
@@ -45,7 +48,7 @@ namespace {
 
 // The compact table index the attention kernel forms, (query part) + (key part), spans exactly [0, AT_TABLE): the
 // largest is (zi, hi, wi) = (1, 5, 11) against (zj, hj, wj) = (1, 5, 0), the smallest wi = 0 against wj = 11.  So no
-// case can read a bias entry outside the pair's two tables in shared memory.
+// case can read a bias entry outside the (type, head) table it expands.
 static_assert((WZ - 1) * (1 + WZ) * ((2 * WW - 1) * WH * WH) + (WH - 1) * (1 + WH) * (2 * WW - 1) + 2 * (WW - 1) == AT_TABLE - 1,
               "bias table index range");
 
@@ -101,7 +104,7 @@ int check(const sky_probe_pangu_t& c) {
   return 0;
 }
 
-int dispatch(const sky_probe_pangu_t& c, cudaStream_t st) {
+int dispatch(const sky_probe_pangu_t& c, int grid_ctas, cudaStream_t st) {
   const Geo g = probe_geo(c.geo);
   switch (c.op) {
     case SKY_PROBE_PG_FILL_PAD:
@@ -109,7 +112,7 @@ int dispatch(const sky_probe_pangu_t& c, cudaStream_t st) {
     case SKY_PROBE_PG_ATTENTION: {
       const AttnArgs a{(const uint8_t*)c.qkv, c.part_stride, (uint8_t*)c.out, c.att_nkb, (const __half*)c.tab, g, c.roll, c.B, c.pairs,
                        c.sl2, c.mask_l2, (long long)c.B * g.nWin * c.pairs};
-      return launch_window_attention_tc(a, 0, st);
+      return launch_window_attention_tc(a, grid_ctas, st);
     }
     case SKY_PROBE_PG_PACK_BIAS:
       return launch_pack_bias_table(c.src, (__half*)c.out, c.n_type, g.heads, st);
@@ -120,9 +123,12 @@ int dispatch(const sky_probe_pangu_t& c, cudaStream_t st) {
 }  // namespace
 }  // namespace sky
 
-extern "C" SKY_API int sky_probe_pangu(const sky_probe_pangu_t* c, void* stream) {
+extern "C" SKY_API int sky_probe_pangu_grid(const sky_probe_pangu_t* c, int32_t grid_ctas, void* stream) {
   using namespace sky;
   if (!c) { set_error("pangu probe: null case"); return SKY_ERR_ARG; }
+  if (grid_ctas < 0) { set_error("pangu probe: grid of %d CTAs", grid_ctas); return SKY_ERR_ARG; }
   if (int rc = check(*c)) return rc;
-  return dispatch(*c, (cudaStream_t)stream);
+  return dispatch(*c, grid_ctas, (cudaStream_t)stream);
 }
+
+extern "C" SKY_API int sky_probe_pangu(const sky_probe_pangu_t* c, void* stream) { return sky_probe_pangu_grid(c, 0, stream); }
