@@ -15,7 +15,8 @@
 // is drained by then — and the same eight warps run the row-owner epilogue on the staged tile
 // (warp%4 selects the 32-row quarter, warp/4 the column partition).  Epilogues re-tile their 32x32
 // accumulator blocks through a padded smem patch so that every global access is a full
-// 64/128-byte row segment.
+// 64/128-byte row segment.  Epilogues wrapped in FragEpi run on the accumulator registers instead and leave through a
+// dedicated output tile that the loader bulk-stores, so the ring keeps streaming under them (Pangu's fc1, projection, fc2).
 #pragma once
 #include <climits>
 #include <type_traits>
@@ -72,11 +73,14 @@ struct AOperand {
   }
 };
 
-template <int BLOCK_N, int EPI_WARPS>
+// kFrag: the epilogue runs on the accumulator fragments (FragEpi below); the patches give way to the output tile,
+// BLOCK_N / 64 blocks of 128 rows x 128 B laid out as the destination image's blocks
+template <int BLOCK_N, int EPI_WARPS, bool kFrag = false>
 struct G2Cfg {
   static constexpr int B_BYTES = BLOCK_N * 128;
   static constexpr int STAGE_BYTES = G2_A_BYTES + B_BYTES;
-  static constexpr int PATCH_BYTES = EPI_WARPS * G2_PATCH_FLOATS * 4;
+  static constexpr int OUT_BYTES = BLOCK_N / 64 * G2_A_BYTES;
+  static constexpr int PATCH_BYTES = kFrag ? OUT_BYTES : EPI_WARPS * G2_PATCH_FLOATS * 4;
   static constexpr int VEC_BYTES = 3 * 512 * 4;  // smem copies of bias | gamma | beta (LN epilogues), <= 512 floats each
   static constexpr int FIXED = 1024 /*align*/ + 256 /*barriers*/ + PATCH_BYTES + VEC_BYTES;
   static constexpr int MAXS = (232448 - FIXED) / STAGE_BYTES;
@@ -89,8 +93,41 @@ struct G2Cfg {
   static_assert(BLOCK_N % 8 == 0 && BLOCK_N <= 256, "wgmma N, accumulator registers");
   static_assert(STAGE_BYTES % 1024 == 0, "stage alignment");
   static_assert(STAGES >= 2, "pipeline depth");
-  static_assert(128 * STG_LD * 4 <= RING_BYTES, "accumulator staging");
+  static_assert(kFrag || 128 * STG_LD * 4 <= RING_BYTES, "accumulator staging");
+  static_assert(!kFrag || BLOCK_N % 64 == 0, "output tile of whole 64-column blocks");
   static_assert(EPI_WARPS == 8, "two consumer warpgroups");
+};
+
+// Epilogue on the accumulator fragments: FragEpi<E> runs E::frag instead of E::run.  Each consumer thread applies the
+// epilogue to its own wgmma fragment (rows 64 wg + 16 w + l/4 and + 8, columns 8 i + 2 (l & 3) + {0, 1}) and writes the
+// fp16 results into the output tile, which the loader warp bulk-stores to E::tile_image.  Nothing is staged over the
+// ring, so the loader streams the next tile's k-blocks in under the epilogue.  E::kLoadsTile: the loader first fills the
+// output tile with the destination's current bytes (the residual of an in-place update).
+template <class E>
+struct FragEpi : E {
+  static constexpr bool kFragment = true;
+};
+template <class E, class = void> struct is_fragment_epi : std::false_type {};
+template <class E> struct is_fragment_epi<E, std::void_t<decltype(E::kFragment)>> : std::true_type {};
+
+// What a fragment epilogue sees of its tile
+struct FragCtx {
+  int row;              // the thread's first fragment row in the tile (64 wg + 16 w + l/4); the second is row + 8
+  int c2;               // 2 (l & 3): the thread's first column inside each 8-column group
+  int n0;               // first column of the tile in the full N
+  uint32_t out_s;       // shared-space address of the output tile
+  uint32_t svec_s;      // bias | gamma | beta of this CTA's columns, 512 floats apart (LN epilogues)
+  uint64_t* out_ready;  // completes when the output tile may be written (and, kLoadsTile, holds the destination's bytes)
+  uint32_t ready_parity;
+  // row statistics of a column-split CTA pair (k_gemm2_pair), indexed by tile row; x_own_bar == nullptr elsewhere
+  uint64_t* x_own_bar = nullptr;   // completes when the peer's (sum, sum of squares) of this thread's 32-row group landed
+  uint32_t x_own_stat = 0, x_peer_stat = 0, x_peer_bar = 0, x_parity = 0;
+  bool post_bar = false;           // this warp announces the barrier's transaction bytes (one of the group's two warps)
+  // byte offset inside the output tile of fragment row `row` (+ 8 with hi), 8-column group i
+  __device__ __forceinline__ uint32_t offset(int i, bool hi) const {
+    const uint32_t r = (uint32_t)(row + (hi ? 8 : 0));
+    return (uint32_t)(i >> 3) * G2_A_BYTES + r * 128u + ((((uint32_t)i & 7u) ^ (r & 7u)) << 4) + (uint32_t)c2 * 2u;
+  }
 };
 
 struct EpiCtx {
@@ -287,14 +324,33 @@ struct SchedW {
 constexpr int G2_EPI_WARPS = 8;
 constexpr int G2_PAIR_SMEM = 2048;   // the pair's exchange slots, behind the barrier block
 
+// Fragment epilogues (FragEpi): the loader warp stores the output tile of tile `t` (a finished tile) to the destination
+// image.  The three 16 KB blocks of a tile are contiguous there (n0 is a multiple of BLOCK_N); a partial last m-tile is
+// stored row by row, so that rows >= M are never written.  Every lane waits until its copies have read the tile.
+template <class Cfg, class Epi, class Tile>
+__device__ __forceinline__ void frag_store(const Epi& epi, const Tile& t, uint32_t out_s, long long M, int bn, int lane) {
+  uint8_t* dst = epi.tile_image(t.mt, t.nt * bn);
+  const long long rows = M - (long long)t.mt * G2_BLOCK_M;
+  if (rows >= G2_BLOCK_M) {
+    if (lane == 0) bulk_s2g(dst, out_s, Cfg::OUT_BYTES);
+  } else {
+    for (int r = lane; r < rows; r += 32)
+      for (int j = 0; j < Cfg::OUT_BYTES / G2_A_BYTES; ++j)
+        bulk_s2g(dst + j * G2_A_BYTES + r * 128, out_s + (uint32_t)(j * G2_A_BYTES + r * 128), 128);
+  }
+  bulk_commit();
+  bulk_wait_read<0>();
+}
+
 template <class Sched, class Epi, int BLOCK_N, bool kPair>
 __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, const G2Grid& g) {
   constexpr int EPI_WARPS = G2_EPI_WARPS;
-  using Cfg = G2Cfg<BLOCK_N, EPI_WARPS>;
+  constexpr bool kFrag = is_fragment_epi<Epi>::value;
+  using Cfg = G2Cfg<BLOCK_N, EPI_WARPS, kFrag>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   float* patches = reinterpret_cast<float*>(smem + Cfg::RING_BYTES);
-  float* sbias = patches + EPI_WARPS * G2_PATCH_FLOATS;
+  float* sbias = reinterpret_cast<float*>(smem + Cfg::RING_BYTES + Cfg::PATCH_BYTES);
   uint64_t* bars = reinterpret_cast<uint64_t*>(sbias + 3 * 512);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::STAGES;
@@ -302,6 +358,10 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
   uint64_t* xbar = bars + 2 * Cfg::STAGES + 1;                                          // pair: [2 tile parities][4 lane quarters]
   float* xstat = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(bars) + 256);     // pair: [2][4][32 lanes][2]
   static_assert(!kPair || (2 * Cfg::STAGES + 1 + 8) * 8 <= 256, "barrier block");
+  // fragment path: stg_free becomes out_full (consumers -> loader: the output tile is written), and out_ready (loader ->
+  // consumers: the output tile may be written) follows the pair's barriers
+  uint64_t* out_ready = bars + 2 * Cfg::STAGES + 9;
+  static_assert(!kFrag || (2 * Cfg::STAGES + 10) * 8 <= 256, "barrier block");
 
   // warp index through a shuffle: provably warp-uniform, so the role branches are uniform control flow
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x / 32, 0), lane = threadIdx.x % 32;
@@ -313,6 +373,7 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
     for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], EPI_WARPS); }
     mbar_init(stg_free, EPI_WARPS);
     if (kPair) for (int i = 0; i < 8; ++i) mbar_init(&xbar[i], 1);
+    if constexpr (kFrag) mbar_init(out_ready, 1);
     mbar_fence_init();
   }
   if constexpr (Epi::kNeedsBias) if (threadIdx.x < EPI_WARPS * 32)
@@ -325,7 +386,84 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
   __syncthreads();
   if (kPair) cluster_sync_all();   // the peer's exchange barriers exist before anything is posted to them
 
-  if (warp == LOADER) {
+  const uint32_t out_s = smem_u32(patches);   // fragment path: the output tile
+  if constexpr (kFrag) {
+    int it = 0;
+    if (warp == LOADER) {
+      // The first min(num_kb, STAGES) k-blocks of a tile only wait for ring slots that the previous tile's main loop
+      // releases.  After them the loader hands the output tile over: it stores the previous tile's once that epilogue is
+      // done (stg_free), then opens it for this tile (out_ready), after loading the destination's bytes if the epilogue
+      // reads them.  The rest of the tile's k-blocks follow.
+      const int head = sc.num_kb < Cfg::STAGES ? sc.num_kb : Cfg::STAGES;
+      int s = 0; uint32_t ph = 0;
+      decltype(sc.template tile<BLOCK_N>(g, 0)) prev{};
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const auto t = sc.template tile<BLOCK_N>(g, tile);
+        if (t.skip) continue;
+        // the destination's bytes of this tile are pulled into L2 a main loop ahead of their load into the output tile
+        if constexpr (Epi::kLoadsTile) if (lane == 0) bulk_prefetch_l2(epi.tile_image(t.mt, t.nt * BLOCK_N), Cfg::OUT_BYTES);
+        for (int kb = 0; kb < sc.num_kb; ++kb) {
+          mbar_wait(&empty[s], ph ^ 1);
+          sc.template issue<BLOCK_N>(smem + s * Cfg::STAGE_BYTES, &full[s], t, kb, lane);
+          __syncwarp();
+          if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
+          if (kb + 1 != head) continue;
+          if (it > 0) {
+            mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
+            frag_store<Cfg>(epi, prev, out_s, g.M, BLOCK_N, lane);
+          }
+          __syncwarp();
+          if (lane == 0) {
+            if constexpr (Epi::kLoadsTile) {
+              mbar_arrive_expect_tx(out_ready, Cfg::OUT_BYTES);
+              bulk_g2s(patches, epi.tile_image(t.mt, t.nt * BLOCK_N), Cfg::OUT_BYTES, out_ready);
+            } else {
+              mbar_arrive(out_ready);
+            }
+          }
+        }
+        prev = t;
+        ++it;
+      }
+      if (it > 0) {
+        mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
+        frag_store<Cfg>(epi, prev, out_s, g.M, BLOCK_N, lane);
+        bulk_wait<0>();
+      }
+    } else {
+      const int wg = warp >> 2, w = warp & 3;
+      FragCtx x;
+      x.row = 64 * wg + 16 * w + (lane >> 2);
+      x.c2 = 2 * (lane & 3);
+      x.out_s = out_s;
+      x.svec_s = smem_u32(sbias);
+      x.out_ready = out_ready;
+      x.post_bar = (w & 1) == 0;
+      WgAcc<BLOCK_N, Sched::kBMN> acc;
+      int s = 0; uint32_t ph = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const auto t = sc.template tile<BLOCK_N>(g, tile);
+        if (t.skip) continue;
+        x.n0 = t.nt * BLOCK_N;
+        x.ready_parity = (uint32_t)it & 1;
+        if constexpr (kPair) {
+          // the statistics slots keep the staged path's layout: [tile parity][32-row group][row % 32][sum, sum of squares]
+          const int buf = it & 1, q = x.row >> 5;
+          x.x_own_bar = &xbar[buf * 4 + q];
+          x.x_own_stat = smem_u32(xstat + (buf * 4 + q) * 64);
+          x.x_peer_stat = mapa_u32(x.x_own_stat, rank ^ 1u);
+          x.x_peer_bar = mapa_u32(smem_u32(x.x_own_bar), rank ^ 1u);
+          x.x_parity = (uint32_t)(it >> 1) & 1;
+        }
+        ++it;
+        wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, sc.num_kb, wg, lane);
+        epi.template frag<BLOCK_N>(acc, x);
+        fence_proxy_async_smem();   // the tile's generic writes are ordered before the loader's bulk store
+        __syncwarp();
+        if (lane == 0) mbar_arrive(stg_free);
+      }
+    }
+  } else if (warp == LOADER) {
     int s = 0; uint32_t ph = 0; int it = 0;
     for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       const auto t = sc.template tile<BLOCK_N>(g, tile);
@@ -397,7 +535,7 @@ k_gemm2_pair(const Sched sc, const Epi epi, const G2Grid g) {
 // halves: 256 for GraphCast's 512-wide latents, 192 for Pangu's C = 384 projection and fc2).
 template <int BLOCK_N, bool kPair = false, class Sched, class Epi>
 int launch_gemm2(const Sched& sc, const Epi& epi, long long M, int N, int batches, int num_sms, cudaStream_t st) {
-  using Cfg = G2Cfg<BLOCK_N, G2_EPI_WARPS>;
+  using Cfg = G2Cfg<BLOCK_N, G2_EPI_WARPS, is_fragment_epi<Epi>::value>;
   constexpr int SMEM = Cfg::SMEM_BYTES + (kPair ? G2_PAIR_SMEM : 0);
   static_assert(SMEM <= 232448, "smem budget");
   auto kern = [] {   // instantiates only the entry that is launched
@@ -521,6 +659,33 @@ struct Epi2F16 {
         }
       }
       __syncwarp();
+    }
+  }
+  // FragEpi (tile image only): the same arithmetic on the accumulator fragments, into the output tile
+  static constexpr bool kLoadsTile = false;
+  __device__ uint8_t* tile_image(int mt, int n0) const {
+    return reinterpret_cast<uint8_t*>(out) + ((size_t)mt * nkb + (n0 >> 6)) * (size_t)G2_A_BYTES;
+  }
+  template <int BN, class Acc>
+  __device__ void frag(Acc& acc, const FragCtx& x) const {
+    static_assert(kImage, "fragment path: tile image output");
+    const float* bp = bias + x.n0 + x.c2;
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      const float2 b = __ldg(reinterpret_cast<const float2*>(bp + 8 * i));
+      float* d = acc.d + 4 * i;
+      if (kGelu) {
+        gelu_erf_x2(d[0], d[1], b.x, b.y);
+        gelu_erf_x2(d[2], d[3], b.x, b.y);
+      } else {
+        d[0] += b.x; d[1] += b.y; d[2] += b.x; d[3] += b.y;
+      }
+    }
+    mbar_wait(x.out_ready, x.ready_parity);
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(x.out_s + x.offset(i, false)), "r"(pack_half2(acc.d[4 * i], acc.d[4 * i + 1])) : "memory");
+      asm volatile("st.shared.b32 [%0], %1;" ::"r"(x.out_s + x.offset(i, true)), "r"(pack_half2(acc.d[4 * i + 2], acc.d[4 * i + 3])) : "memory");
     }
   }
 };
@@ -726,6 +891,82 @@ struct Epi2F32Img {
       if constexpr (kResidual) {
 #pragma unroll
         for (int it = 0; it < 8; ++it) xin[it] = xnext[it];
+      }
+    }
+  }
+  // FragEpi (LayerNorm into the fp16 stream image): the same arithmetic on the accumulator fragments.  A warpgroup holds
+  // whole rows, so a row's statistics are the thread's sums added across its lane quad (and, in a CTA pair, the peer's).
+  // The residual is the output tile itself: the loader fills it with the destination's bytes, the sum overwrites them.
+  static constexpr bool kLoadsTile = kResidual;
+  __device__ uint8_t* tile_image(int mt, int n0) const { return img + ((size_t)mt * nkb + (n0 >> 6)) * (size_t)G2_A_BYTES; }
+  template <int BN, class Acc>
+  __device__ void frag(Acc& acc, const FragCtx& x) const {
+    static_assert(kLn && kImgStream, "fragment path: LayerNorm into the fp16 stream image");
+    float s[2] = {0.f, 0.f}, ss[2] = {0.f, 0.f};   // rows x.row, x.row + 8
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      float2 b;
+      asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(b.x), "=f"(b.y) : "r"(x.svec_s + (uint32_t)(8 * i + x.c2) * 4u));
+      float* d = acc.d + 4 * i;
+      d[0] += b.x; d[1] += b.y; d[2] += b.x; d[3] += b.y;
+      s[0] += d[0] + d[1]; ss[0] += d[0] * d[0] + d[1] * d[1];
+      s[1] += d[2] + d[3]; ss[1] += d[2] * d[2] + d[3] * d[3];
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int o = 1; o < 4; o <<= 1) {
+        s[h] += __shfl_xor_sync(0xffffffffu, s[h], o);
+        ss[h] += __shfl_xor_sync(0xffffffffu, ss[h], o);
+      }
+    float width = (float)BN;
+    if (x.x_own_bar) {
+      // column-split CTA pair: lane (l & 3) == h of each quad posts row x.row + 8 h into the peer's slot; the two warps of a
+      // 32-row group share one barrier, whose 256 transaction bytes one of them announces
+      const int lane = threadIdx.x & 31, h = lane & 3;
+      if (x.post_bar && lane == 0) mbar_arrive_expect_tx(x.x_own_bar, 32 * 8);
+      __syncwarp();
+      if (h < 2) {
+        const uint32_t slot = (uint32_t)((x.row + 8 * h) & 31) * 8u;
+        const float ps = h ? s[1] : s[0], pss = h ? ss[1] : ss[0];
+        asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];" ::"r"(x.x_peer_stat + slot),
+                     "f"(ps), "f"(pss), "r"(x.x_peer_bar)
+                     : "memory");
+      }
+      mbar_wait(x.x_own_bar, x.x_parity);   // CTA-scope acquire, as in run()
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        float ps, pss;
+        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ps), "=f"(pss) : "r"(x.x_own_stat + (uint32_t)((x.row + 8 * hh) & 31) * 8u));
+        s[hh] += ps; ss[hh] += pss;
+      }
+      width = (float)(2 * BN);
+    }
+    float rs[2], ns[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const float mean = s[h] / width;
+      rs[h] = rsqrtf(fmaxf(ss[h] / width - mean * mean, 0.f) + eps);
+      ns[h] = -mean * rs[h];
+    }
+    mbar_wait(x.out_ready, x.ready_parity);
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i) {
+      float2 ga, be;
+      asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ga.x), "=f"(ga.y) : "r"(x.svec_s + (uint32_t)(512 + 8 * i + x.c2) * 4u));
+      asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(be.x), "=f"(be.y) : "r"(x.svec_s + (uint32_t)(1024 + 8 * i + x.c2) * 4u));
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const uint32_t a = x.out_s + x.offset(i, h);
+        const float* d = acc.d + 4 * i + 2 * h;
+        float y0 = fmaf(fmaf(d[0], rs[h], ns[h]), ga.x, be.x), y1 = fmaf(fmaf(d[1], rs[h], ns[h]), ga.y, be.y);
+        if (kResidual) {
+          uint32_t r;
+          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(a));
+          const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(&r));
+          y0 += rf.x; y1 += rf.y;
+        }
+        asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(pack_half2(y0, y1)) : "memory");
       }
     }
   }

@@ -43,6 +43,8 @@ enum {
   SKY_PROBE_EPI_GC_LN1 = 15,      // EpiGcLn<1>
   SKY_PROBE_EPI_GC_LN2 = 16,      // EpiGcLn<2>
   SKY_PROBE_EPI_QKV_WIN = 17,     // EpiQkvWin (Pangu's QKV projection -> q | k | v window image)
+  SKY_PROBE_EPI_F16_GELU_IMG_FRAG = 18,   // FragEpi<Epi2F16<true, true>>: SKY_PROBE_EPI_F16_GELU_IMG on the fragment path
+  SKY_PROBE_EPI_LN_IMG_FRAG = 19,         // FragEpi<Epi2F32Img<true, true, true>>: SKY_PROBE_EPI_LN_IMG on the fragment path
 };
 
 // Every pointer is a device pointer; every *_bytes / *_floats field is the size of the allocation behind it, which the
@@ -248,7 +250,8 @@ int check_epilogue(const Case& c) {
       return 0;
     }
     case SKY_PROBE_EPI_LN:
-    case SKY_PROBE_EPI_LN_IMG: {
+    case SKY_PROBE_EPI_LN_IMG:
+    case SKY_PROBE_EPI_LN_IMG_FRAG: {
       PROBE_REQUIRE(c.n_valid == c.n && c.batches == 1 && c.n <= 512, "LayerNorm: whole rows, one batch, N <= 512");
       PROBE_REQUIRE(c.kernel == SKY_PROBE_PAIR || c.n == c.block_n, "LayerNorm: one n-tile spans the row (N=%d, BN=%d)", c.n, c.block_n);
       if ((rc = check_vec(c, c.bias, c.n, "bias")) || (rc = check_vec(c, c.gamma, c.n, "gamma")) || (rc = check_vec(c, c.beta, c.n, "beta")))
@@ -260,10 +263,11 @@ int check_epilogue(const Case& c) {
       return check_img(c, c.m, c.n);
     }
     case SKY_PROBE_EPI_F16_GELU_IMG:
+    case SKY_PROBE_EPI_F16_GELU_IMG_FRAG:
     case SKY_PROBE_EPI_F16_ROWS: {
       PROBE_REQUIRE(c.n_valid == c.n && c.batches == 1, "fp16 output: every column, one batch");
       if ((rc = check_vec(c, c.bias, c.n, "bias"))) return rc;
-      if (c.epi == SKY_PROBE_EPI_F16_GELU_IMG) {
+      if (c.epi != SKY_PROBE_EPI_F16_ROWS) {
         PROBE_REQUIRE(c.hi && aligned16(c.hi), "fp16 image");
         return check_img(c, c.m, c.n);
       }
@@ -359,6 +363,8 @@ template <> Epi2F32Img<true, true, true> make_epi(const Case& c) {
 
 template <> Epi2F16<true, true> make_epi(const Case& c) { return {(__half*)c.hi, 0, c.img_nkb, c.bias}; }
 template <> Epi2F16<false, false> make_epi(const Case& c) { return {(__half*)c.out, c.ldo, 0, c.bias}; }
+template <> FragEpi<Epi2F16<true, true>> make_epi(const Case& c) { return {make_epi<Epi2F16<true, true>>(c)}; }
+template <> FragEpi<Epi2F32Img<true, true, true>> make_epi(const Case& c) { return {make_epi<Epi2F32Img<true, true, true>>(c)}; }
 template <int kG>
 EpiGcSiluImg<kG> make_silu(const Case& c) {
   EpiGcSiluImg<kG> e{};
@@ -405,7 +411,9 @@ int by_bn(const Case& c, const Sched& sc, cudaStream_t st, BnList<BNs...>) {
 //   SFNO SfnoEngine::gemm_op: SchedW / SchedW<true> x its epilogues x {16, 32, 64, 80, 192, 240, 256};
 //   SFNO SfnoEngine::gemm_tb: SchedTB x {EpiSplitRemap, EpiF32Batched<false>, EpiGeluStatsImg} x {64, 128, 192, 256};
 //   Pangu: SchedW x Epi2F32Img<true, true, *> at 192, and the pair kernel at 192; fc1's Epi2F16<true, true> at 192; the QKV
-//   projection's EpiQkvWin at 192;
+//   projection's EpiQkvWin at 192; the fragment path of the projection / fc2 (FragEpi<Epi2F32Img<true, true, true>>, single
+//   CTA and pair) and of fc1 (FragEpi<Epi2F16<true, true>>) at 192.  The engine no longer launches the staged
+//   Epi2F32Img<true, true, true> and Epi2F16<true, true>; the probe keeps them as the reference of the fragment path;
 //   GraphCast: EpiGcSiluImg<0 / 2> and the node tables' Epi2F16<false, false> at 256, EpiGcOut at 128, and the pair kernel
 //   with EpiGcLn<0 / 1 / 2> at 256 (GraphCast never gathers exactly one table: EpiGcSiluImg<1> is not instantiated).
 using BnSfno = BnList<16, 32, 64, 80, 192, 240, 256>;
@@ -435,6 +443,7 @@ int dispatch(const Case& c, cudaStream_t st) {
         switch (c.epi) {
           case SKY_PROBE_EPI_LN: return by_bn<true, Epi2F32Img<true, true, false>>(c, sc, st, BnPair{});
           case SKY_PROBE_EPI_LN_IMG: return by_bn<true, Epi2F32Img<true, true, true>>(c, sc, st, BnPair{});
+          case SKY_PROBE_EPI_LN_IMG_FRAG: return by_bn<true, FragEpi<Epi2F32Img<true, true, true>>>(c, sc, st, BnPair{});
           case SKY_PROBE_EPI_GC_LN0: return by_bn<true, EpiGcLn<0>>(c, sc, st, BnList<256>{});
           case SKY_PROBE_EPI_GC_LN1: return by_bn<true, EpiGcLn<1>>(c, sc, st, BnList<256>{});
           case SKY_PROBE_EPI_GC_LN2: return by_bn<true, EpiGcLn<2>>(c, sc, st, BnList<256>{});
@@ -451,6 +460,8 @@ int dispatch(const Case& c, cudaStream_t st) {
           case SKY_PROBE_EPI_LN: return by_bn<false, Epi2F32Img<true, true, false>>(c, sc, st, BnList<192>{});
           case SKY_PROBE_EPI_LN_IMG: return by_bn<false, Epi2F32Img<true, true, true>>(c, sc, st, BnList<192>{});
           case SKY_PROBE_EPI_F16_GELU_IMG: return by_bn<false, Epi2F16<true, true>>(c, sc, st, BnList<192>{});
+          case SKY_PROBE_EPI_LN_IMG_FRAG: return by_bn<false, FragEpi<Epi2F32Img<true, true, true>>>(c, sc, st, BnList<192>{});
+          case SKY_PROBE_EPI_F16_GELU_IMG_FRAG: return by_bn<false, FragEpi<Epi2F16<true, true>>>(c, sc, st, BnList<192>{});
           case SKY_PROBE_EPI_F16_ROWS: return by_bn<false, Epi2F16<false, false>>(c, sc, st, BnList<256>{});
           case SKY_PROBE_EPI_GC_SILU0: return by_bn<false, EpiGcSiluImg<0>>(c, sc, st, BnList<256>{});
           case SKY_PROBE_EPI_GC_SILU2: return by_bn<false, EpiGcSiluImg<2>>(c, sc, st, BnList<256>{});

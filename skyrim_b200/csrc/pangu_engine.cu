@@ -575,7 +575,8 @@ struct PanguEngine : Engine {
   }
   template <bool IMG>
   int run_block_t(float* x, uint8_t* xh, const Geo& g, const BlockW& b, int roll, int B, const Ws& ws, cudaStream_t st) {
-    using ELn = Epi2F32Img<true, true, IMG>;
+    // projection and fc2: the epilogue runs on the accumulator fragments on the fp16 stream (the fp32 rows stay staged)
+    using ELn = std::conditional_t<IMG, FragEpi<Epi2F32Img<true, true, true>>, Epi2F32Img<true, true, false>>;
     const int C = g.C, nkb = C / 64;
     const long long R = (long long)B * g.T;
     int rc;
@@ -612,7 +613,7 @@ struct PanguEngine : Engine {
     }
     {  // MLP: fc1 + GELU into the fp16 hidden image, then fc2 + LayerNorm + residual
       AOperand A(xh, nkb);
-      Epi2F16<true, true> e{reinterpret_cast<__half*>(ws.hidh), 0, 4 * nkb, b.fc1_b};
+      FragEpi<Epi2F16<true, true>> e{reinterpret_cast<__half*>(ws.hidh), 0, 4 * nkb, b.fc1_b};
       if ((rc = gemm2<192>(KT_FC1, A, e, b.fc1, R, st))) return rc;
       AOperand A2(ws.hidh, 4 * nkb);
       ELn e2{x, C, xh, nkb, b.fc2_b, b.ln2_g, b.ln2_b, cfg.ln_eps};

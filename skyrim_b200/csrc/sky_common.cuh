@@ -214,6 +214,21 @@ __device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint3
       "l"(gsrc), "r"(bytes), "r"(smem_u32(bar))
       : "memory");
 }
+// bulk copy shared -> global (same alignment rules), tracked by the issuing thread's bulk async-groups: after
+// bulk_commit(), bulk_wait_read<0>() returns once the source bytes have been read (the shared memory may be rewritten),
+// bulk_wait<0>() once the writes are done
+__device__ __forceinline__ void bulk_s2g(void* gdst, uint32_t smem_src, uint32_t bytes) {
+  asm volatile("cp.async.bulk.global.shared::cta.bulk_group [%0], [%1], %2;" ::"l"(gdst), "r"(smem_src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// bulk prefetch of global memory into L2 (16-byte aligned, bytes multiple of 16)
+__device__ __forceinline__ void bulk_prefetch_l2(const void* gsrc, uint32_t bytes) {
+  asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(gsrc), "r"(bytes) : "memory");
+}
 
 // ---------------------------------------------------------------------------------------
 // wgmma (warpgroup MMA).  A warpgroup of four consecutive warps issues m64nNk16 products
