@@ -178,6 +178,31 @@ SKY_API int sky_perturb_ic_grf(float* x, const float* sigma_c, float amp, uint64
 SKY_API int sky_grf_draw(float* coeffs, const float* spec_std, uint64_t seed, int32_t member0, int32_t members,
                  int32_t channels, int32_t lmax, void* stream);
 
+/* Ensemble statistics of `members` states on one device, for the selected channels, into caller-owned device buffers:
+ *   member m, channel c is the plane x + m * member_stride + c * plane (plane = nlat * nlon floats), c < channel_count;
+ *   channels   host int32 [n_sel], 1 <= n_sel <= 128, each in [0, channel_count); the order of the outputs;
+ *   quantiles  host fp64 [n_q], 0 <= n_q <= 8, each in [0, 1];
+ *   event_sel  host int32 [n_events], 0 <= n_events <= 64: event e is about channels[event_sel[e]]; nondecreasing;
+ *   event_thr  host fp32 [n_events], finite thresholds;
+ *   stats      device fp32 [2 + n_q][n_sel][plane]: mean, spread, then one plane set per quantile;
+ *   prob       device fp32 [n_events][plane] (may be NULL when n_events == 0).
+ * Per (selected channel, point), over m < members, in fp64 and rounded once to fp32:
+ *   mean    = sum_m x_m / M, summed in member order;
+ *   spread  = sqrt(sum_m (x_m - mean)^2 / M) with the unrounded mean: the population standard deviation;
+ *   q_j     = numpy.quantile(x, q_j, method="linear"): h = q_j (M - 1), x_(floor h) and x_(ceil h) of the sorted members
+ *             linearly interpolated with numpy's lerp;
+ *   prob_e  = count(x_m > event_thr[e]) / M (strict: x == t does not count).
+ * A NaN member makes every output at that point NaN.  Results are bitwise reproducible (no atomics), a channel's outputs do
+ * not depend on which other channels are selected, and quantiles / probabilities do not depend on the member order.
+ * Refused with SKY_ERR_ARG before any launch: members outside 1..64, member_stride < channel_count * plane, a channel,
+ * quantile, event index or threshold out of range, a decreasing event_sel, too many channels / quantiles / events (all
+ * checked before any CUDA call), and x / stats / prob that are not device memory on one device.  Asynchronous and
+ * stream-ordered; launches on the device that owns x. */
+SKY_API int sky_ensemble_stats(const float* x, int32_t members, int64_t member_stride, int64_t plane, int32_t channel_count,
+                       const int32_t* channels, int32_t n_sel, const double* quantiles, int32_t n_q,
+                       const int32_t* event_sel, const float* event_thr, int32_t n_events, float* stats, float* prob,
+                       void* stream);
+
 /* Per-kernel-family device timing (CUDA events recorded on the launching stream around the
  * launches whose family bit is set in tag_mask).  profile_end synchronises on the recorded
  * events and returns the summed milliseconds and launch counts per family.  Used by bench.py

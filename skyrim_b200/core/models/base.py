@@ -136,6 +136,84 @@ class GlobalModel:
             logger.success(f"Rollout step {n+1}/{n_steps} completed")
         return pred, output_paths
 
+    def _ensemble_initial_state(self, start_time: datetime.datetime):
+        """(unperturbed state (C, H, W), per-channel perturbation sigma (C,), offset of the reduced channels in the state)"""
+        from ...weights import channel_stats
+        vals = np.asarray(self.data_source[start_time].values, dtype=np.float32)
+        return np.ascontiguousarray(vals[-1] if vals.ndim == 4 else vals), channel_stats(self.in_channel_names)[1], 0
+
+    def predict_ensemble(self, start_time: datetime.datetime, n_steps: int, members: int, perturbation: str = "spherical_grf",
+                         amp: float = 0.05, seed: int = 0, quantiles=(), events: dict = {}, channels: List[str] = [],
+                         save: bool = False, save_config: dict = {}, grf: dict | None = None):
+        """Perturbed-initial-condition ensemble of ``members`` (1..64) on this model's GPU, reduced on the device to
+        per-step statistics: mean, spread and ``quantiles`` of ``channels`` (default: save_config's filter_vars, else all),
+        and P(x > t) for ``events`` = {channel: threshold or [thresholds]} (their channels are reduced too).  Member m is
+        the state ``EnsembleRunner(members_per_gpu=members, rank=0, amp=amp, seed=seed, perturbation=...)`` produces;
+        "spherical_grf" defaults to the degree limit min(180, (nlat - 1) // 2) unless ``grf`` says otherwise.  Only the
+        statistics are copied to the host, each step's copy under the next step.  ``save`` writes one netCDF file of
+        statistics per step (model "<model>-ens<M>") and, with events, one of probabilities ("<model>-ens<M>-prob").
+        Returns (GlobalEnsemblePrediction of the last step with 2 time slices, paths)."""
+        from ... import engine as E
+        from .ensemble import GlobalEnsemblePrediction, event_name, quantile_name
+        names = list(self.out_channel_names)
+        if not 1 <= members <= E.ENS_MAX_MEMBERS:
+            raise ValueError(f"members = {members} must lie in [1, {E.ENS_MAX_MEMBERS}]")
+        if n_steps < 1:
+            raise ValueError(f"n_steps = {n_steps} must be at least 1")
+        q = [float(v) for v in quantiles]
+        if len(q) > E.ENS_MAX_QUANTILES or not all(0.0 <= v <= 1.0 for v in q):
+            raise ValueError(f"quantiles {q}: at most {E.ENS_MAX_QUANTILES}, each in [0, 1]")
+        ev = {c: [float(t) for t in np.atleast_1d(thr)] for c, thr in dict(events).items()}
+        filt = list(save_config.get("filter_vars", ()))
+        unknown = [c for c in list(channels) + filt + list(ev) if c not in names]
+        if unknown:
+            raise ValueError(f"unknown channel(s) {unknown} for {self.model_name}")
+        if not all(np.isfinite(t) for ts in ev.values() for t in ts):
+            raise ValueError(f"event thresholds must be finite: {ev}")
+        if save and save_config.get("file_type", "netcdf") == "zarr":
+            raise ValueError("ensemble statistics are written as netCDF only: the zarr writer holds one variable per "
+                             "forecast id")
+        wanted = set(channels or filt or names) | set(ev)
+        sel = [c for c in names if c in wanted]
+        ev_list = [(i, t) for i, c in enumerate(sel) for t in ev.get(c, ())]
+        if len(sel) > E.ENS_MAX_CHANNELS or len(ev_list) > E.ENS_MAX_EVENTS:
+            raise ValueError(f"{len(sel)} channels and {len(ev_list)} events: at most {E.ENS_MAX_CHANNELS} and "
+                             f"{E.ENS_MAX_EVENTS}")
+        from ...ensemble import EnsembleRunner
+        if perturbation == "spherical_grf" and grf is None:
+            grf = dict(lmax=min(180, (len(self.model.grid.lat) - 1) // 2))
+        base, sigma, offset = self._ensemble_initial_state(start_time)
+        runner = EnsembleRunner(self.model.engine, base, sigma, members_per_gpu=members, rank=0, amp=amp, seed=seed,
+                                perturbation=perturbation, grf=grf)
+        save_config = {k: v for k, v in save_config.items() if k != "filter_vars"}   # selected on the device already
+        save_config.setdefault("forecast_id", generate_forecast_id())
+        label, source = f"{self.model_name}-ens{members}", self.ic_source if isinstance(self.ic_source, str) else "file"
+        lat, lon = np.array(self.model.grid.lat), np.array(self.model.grid.lon)
+        stat_names = np.array(["mean", "spread"] + [quantile_name(v) for v in q])
+        ev_names = np.array([event_name(sel[i], t) for i, t in ev_list])
+        result, paths, prev, t_prev = None, [], None, start_time
+        # the host buffers of step n - 1 stay valid while step n is handled (iter_stats: rings of two)
+        for n, s, p in runner.iter_stats(n_steps, [names.index(c) for c in sel], q, ev_list, offset):
+            t_cur = start_time + n * self.time_step
+            if n > 0 and (save or n == n_steps):
+                times = np.array([np.datetime64(t_prev, "s"), np.datetime64(t_cur, "s")])
+                stats = xr.DataArray(np.stack([prev[0].numpy(), s.numpy()]), dims=["time", "statistic", "channel", "lat", "lon"],
+                                     coords=dict(time=times, statistic=stat_names, channel=np.array(sel), lat=lat, lon=lon))
+                prob = None
+                if ev_list:
+                    prob = xr.DataArray(np.stack([prev[1].numpy(), p.numpy()]), dims=["time", "event", "lat", "lon"],
+                                        coords=dict(time=times, event=ev_names, lat=lat, lon=lon))
+                if save:
+                    paths.append(save_forecast(stats, label, t_prev, t_cur, source, config=save_config))
+                    if prob is not None:
+                        paths.append(save_forecast(prob, f"{label}-prob", t_prev, t_cur, source, config=save_config))
+                result = GlobalEnsemblePrediction(stats, prob, self.model_name, members)
+            if n > 0:
+                source = "file"
+                logger.success(f"Ensemble step {n}/{n_steps} completed")
+            prev, t_prev = (s, p), t_cur
+        return result, paths
+
 
 class GlobalPrediction:
     filepath: Path | None = None

@@ -57,6 +57,21 @@ class GraphcastModel(GlobalModel):
 
     def _initial_state(self, start_time: datetime.datetime):
         """what get_initial_condition_for_model + stepper.initialize do upstream (graphcast.py:104-110)"""
+        return self.model.stepper.initialize(self._initial_fields(start_time), start_time)
+
+    def _ensemble_initial_state(self, start_time: datetime.datetime):
+        """both slices, forcing filled, as one (2 * 83, H, W) state; the toa channels are not perturbed (sigma 0), the
+        engine's clock is set, and the statistics are taken over slice 1 (the newest)"""
+        from ...weights import channel_stats
+        ns = self._cfg.n_state
+        x = self._initial_fields(start_time)
+        self.model.engine.set_clock(start_time)
+        sigma = np.tile(channel_stats(self.out_channel_names)[1], 2)
+        sigma[ns - 1] = sigma[2 * ns - 1] = 0.0
+        return x.reshape(2 * ns, self._cfg.nlat, self._cfg.nlon), sigma, ns
+
+    def _initial_fields(self, start_time: datetime.datetime):
+        """(1, 2, 83, H, W) device tensor of the slices at start_time - 6 h and start_time, toa forcing filled"""
         import torch
         cfg = self._cfg
         if self.data_source is None:
@@ -67,8 +82,7 @@ class GraphcastModel(GlobalModel):
             x = torch.from_numpy(np.stack([np.asarray(self.data_source[start_time - step].values, dtype=np.float32),
                                            np.asarray(self.data_source[start_time].values, dtype=np.float32)]))[None]
         x = x.to(self.model.device)
-        self.model.fill_forcing(x, start_time)
-        return self.model.stepper.initialize(x, start_time)
+        return self.model.fill_forcing(x, start_time)
 
     def _predict_one_step(self, start_time: datetime.datetime, initial_condition: tuple | None = None):
         self.stepper = self.model.stepper

@@ -47,3 +47,12 @@ class Skyrim:
                                                 save_config=save_config)
         logger.debug("Prediction completed successfully")
         return GlobalPrediction(pred, model_name=self.model_names), output_paths
+
+    def predict_ensemble(self, date: str, time: str, lead_time: int = 6, members: int = 4, **kw):
+        """Perturbed-initial-condition ensemble forecast reduced to per-step statistics on the GPU: the date, time and lead
+        time are read as ``predict`` reads them, ``kw`` goes to ``GlobalModel.predict_ensemble`` (perturbation, amp, seed,
+        quantiles, events, channels, save, save_config, grf).  Returns (GlobalEnsemblePrediction, paths)."""
+        start_time = datetime.datetime(int(date[:4]), int(date[4:6]), int(date[6:8]), int(time[:2]), int(time[2:4]))
+        n_steps = self.model.time_steps(lead_time)
+        logger.debug(f"Ensemble of {members} members, {n_steps} steps")
+        return self.model.predict_ensemble(start_time=start_time, n_steps=n_steps, members=members, **kw)

@@ -1,0 +1,187 @@
+// Per-step ensemble statistics of the M members resident on one GPU (DESIGN.md section 5).
+//
+// For each selected channel c and grid point p, over members m < M (fp64 inside, each output rounded once to fp32):
+//     mean      sum_m x_m / M, summed in member order
+//     spread    sqrt(sum_m (x_m - mu)^2 / M), mu the unrounded fp64 mean (two passes over the registers: population std)
+//     q_j       numpy quantile(method="linear"): h = q_j (M - 1), lo = floor h, hi = min(lo + 1, M - 1), g = h - lo, then
+//               numpy's lerp of the sorted x_(lo), x_(hi) (a + (b - a) g, or b - (b - a)(1 - g) when g >= 0.5), unfused
+//     P(x > t)  count(x_m > t_e) / M, strict
+// A NaN member makes every output at that point NaN.
+//
+// One thread owns one (channel, point) and holds its M values in registers, padded to MP (8, 16, 32, 64) with +inf; the
+// padding is excluded from every statistic and sorts behind the members.  Consecutive threads take consecutive points, so
+// each member's load is coalesced.  Quantiles come from a fully unrolled bitonic network (min / max on registers only);
+// the QUANT = false instantiation skips it.  No atomics: each output is one thread's fixed-order computation, so results
+// are bitwise reproducible and a channel's outputs do not depend on which other channels are selected.
+#include <algorithm>
+#include <cmath>
+
+#include "engine.h"
+#include "sky_common.cuh"
+
+namespace sky {
+namespace {
+
+constexpr int kMaxMembers = 64, kMaxSel = 128, kMaxQ = 8, kMaxEvents = 64, kThreads = 128;
+
+// travels by value (kernel parameter space): the host validates everything before any CUDA call
+struct EnsStatsParams {
+  const float* x;              // base: member m, selected channel s at x + m member_stride + chan[s] plane
+  float* stats;                // [2 + n_q][n_sel][plane]
+  float* prob;                 // [n_events][plane]
+  long long member_stride, plane;
+  int members, n_sel, n_q, n_events;
+  int chan[kMaxSel];
+  int q_lo[kMaxQ], q_hi[kMaxQ];
+  double q_g[kMaxQ];
+  int ev_sel[kMaxEvents];
+  float ev_thr[kMaxEvents];
+};
+
+template <int MP, bool QUANT>
+__global__ void __launch_bounds__(kThreads) k_ens_stats(const __grid_constant__ EnsStatsParams P) {
+  const long long p = (long long)blockIdx.x * kThreads + threadIdx.x;
+  if (p >= P.plane) return;
+  const int s = blockIdx.y, M = P.members;
+  const float* xp = P.x + (long long)P.chan[s] * P.plane + p;
+  float v[MP];
+#pragma unroll
+  for (int m = 0; m < MP; ++m) v[m] = m < M ? xp[m * P.member_stride] : __int_as_float(0x7f800000);
+
+  double sum = 0.0;
+  bool nan = false;
+#pragma unroll
+  for (int m = 0; m < MP; ++m)
+    if (m < M) { sum = __dadd_rn(sum, (double)v[m]); nan |= v[m] != v[m]; }
+  const double mu = __ddiv_rn(sum, (double)M);
+  double ss = 0.0;
+#pragma unroll
+  for (int m = 0; m < MP; ++m)
+    if (m < M) { const double d = __dsub_rn((double)v[m], mu); ss = __dadd_rn(ss, __dmul_rn(d, d)); }
+  const long long sp = (long long)P.n_sel * P.plane;
+  float* out = P.stats + (long long)s * P.plane + p;
+  out[0] = (float)mu;
+  out[sp] = (float)__dsqrt_rn(__ddiv_rn(ss, (double)M));
+
+  const float qnan = __int_as_float(0x7fc00000);
+  for (int e = 0; e < P.n_events; ++e) {
+    if (P.ev_sel[e] != s) continue;
+    const float t = P.ev_thr[e];
+    int cnt = 0;
+#pragma unroll
+    for (int m = 0; m < MP; ++m) cnt += (m < M && v[m] > t) ? 1 : 0;
+    P.prob[(long long)e * P.plane + p] = nan ? qnan : (float)__ddiv_rn((double)cnt, (double)M);
+  }
+
+  if constexpr (QUANT) {
+#pragma unroll
+    for (int k = 2; k <= MP; k <<= 1)
+#pragma unroll
+      for (int j = k >> 1; j > 0; j >>= 1)
+#pragma unroll
+        for (int i = 0; i < MP; ++i) {
+          const int l = i ^ j;
+          if (l > i) {
+            const float a = v[i], b = v[l];
+            const bool up = (i & k) == 0;
+            v[i] = up ? fminf(a, b) : fmaxf(a, b);
+            v[l] = up ? fmaxf(a, b) : fminf(a, b);
+          }
+        }
+    for (int q = 0; q < P.n_q; ++q) {
+      const int lo = P.q_lo[q], hi = P.q_hi[q];
+      float a = 0.f, b = 0.f;
+#pragma unroll
+      for (int i = 0; i < MP; ++i) { a = i == lo ? v[i] : a; b = i == hi ? v[i] : b; }
+      const double g = P.q_g[q], da = a, db = b, d = __dsub_rn(db, da);
+      const double r = g >= 0.5 ? __dsub_rn(db, __dmul_rn(d, __dsub_rn(1.0, g))) : __dadd_rn(da, __dmul_rn(d, g));
+      out[(2 + q) * sp] = nan ? qnan : (float)r;
+    }
+  }
+}
+
+template <int MP>
+void launch(const EnsStatsParams& P, dim3 grid, cudaStream_t st) {
+  if (P.n_q > 0) k_ens_stats<MP, true><<<grid, kThreads, 0, st>>>(P);
+  else k_ens_stats<MP, false><<<grid, kThreads, 0, st>>>(P);
+}
+
+int device_ptr(const void* p, const char* what, int* dev) {
+  cudaPointerAttributes attr;
+  SKY_CUDA_OK(cudaPointerGetAttributes(&attr, p));
+  if (attr.type != cudaMemoryTypeDevice) { set_error("%s must be device memory", what); return SKY_ERR_ARG; }
+  if (*dev >= 0 && attr.device != *dev) { set_error("%s is on device %d, x on device %d", what, attr.device, *dev); return SKY_ERR_ARG; }
+  *dev = attr.device;
+  return 0;
+}
+
+}  // namespace
+}  // namespace sky
+
+using namespace sky;
+
+extern "C" {
+
+int sky_ensemble_stats(const float* x, int32_t members, int64_t member_stride, int64_t plane, int32_t channel_count,
+                       const int32_t* channels, int32_t n_sel, const double* quantiles, int32_t n_q,
+                       const int32_t* event_sel, const float* event_thr, int32_t n_events, float* stats, float* prob,
+                       void* stream) {
+  if (members < 1 || members > kMaxMembers) { set_error("members = %d must lie in [1, %d]", members, kMaxMembers); return SKY_ERR_ARG; }
+  if (plane < 1 || channel_count < 1) { set_error("plane (%lld) and channel_count (%d) must be positive", (long long)plane, channel_count); return SKY_ERR_ARG; }
+  if (member_stride < (int64_t)channel_count * plane) {
+    set_error("member_stride = %lld is below channel_count x plane = %lld", (long long)member_stride, (long long)channel_count * plane);
+    return SKY_ERR_ARG;
+  }
+  if (n_sel < 1 || n_sel > kMaxSel || !channels) { set_error("n_sel = %d channels must lie in [1, %d]", n_sel, kMaxSel); return SKY_ERR_ARG; }
+  if (n_q < 0 || n_q > kMaxQ || (n_q && !quantiles)) { set_error("n_q = %d quantiles must lie in [0, %d]", n_q, kMaxQ); return SKY_ERR_ARG; }
+  if (n_events < 0 || n_events > kMaxEvents || (n_events && (!event_sel || !event_thr))) {
+    set_error("n_events = %d events must lie in [0, %d]", n_events, kMaxEvents);
+    return SKY_ERR_ARG;
+  }
+  EnsStatsParams P{};
+  P.member_stride = member_stride;
+  P.plane = plane;
+  P.members = members;
+  P.n_sel = n_sel;
+  P.n_q = n_q;
+  P.n_events = n_events;
+  for (int s = 0; s < n_sel; ++s) {
+    if (channels[s] < 0 || channels[s] >= channel_count) { set_error("channel %d is outside [0, %d)", channels[s], channel_count); return SKY_ERR_ARG; }
+    P.chan[s] = channels[s];
+  }
+  for (int q = 0; q < n_q; ++q) {
+    const double v = quantiles[q];
+    if (!(v >= 0.0 && v <= 1.0)) { set_error("quantile %g is outside [0, 1]", v); return SKY_ERR_ARG; }
+    const double h = (double)(members - 1) * v, lo = std::floor(h);
+    P.q_lo[q] = (int)lo;
+    P.q_hi[q] = std::min((int)lo + 1, members - 1);
+    P.q_g[q] = h - lo;
+  }
+  for (int e = 0; e < n_events; ++e) {
+    if (event_sel[e] < 0 || event_sel[e] >= n_sel) { set_error("event_sel[%d] = %d is outside [0, %d)", e, event_sel[e], n_sel); return SKY_ERR_ARG; }
+    if (e > 0 && event_sel[e] < event_sel[e - 1]) { set_error("event_sel decreases at %d", e); return SKY_ERR_ARG; }
+    if (!std::isfinite(event_thr[e])) { set_error("event threshold %d is not finite", e); return SKY_ERR_ARG; }
+    P.ev_sel[e] = event_sel[e];
+    P.ev_thr[e] = event_thr[e];
+  }
+  if (!x || !stats || (n_events && !prob)) { set_error("x, stats and (with events) prob must not be null"); return SKY_ERR_ARG; }
+  int dev = -1, rc;
+  if ((rc = device_ptr(x, "x", &dev)) || (rc = device_ptr(stats, "stats", &dev)) ||
+      (n_events && (rc = device_ptr(prob, "prob", &dev))))
+    return rc;
+  P.x = x;
+  P.stats = stats;
+  P.prob = prob;
+  DeviceGuard guard(dev);   // launch on the device that owns the members, whatever the caller's current device is
+  const dim3 grid((unsigned)((plane + kThreads - 1) / kThreads), (unsigned)n_sel);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (members <= 8) launch<8>(P, grid, st);
+  else if (members <= 16) launch<16>(P, grid, st);
+  else if (members <= 32) launch<32>(P, grid, st);
+  else launch<64>(P, grid, st);
+  count_launch();
+  SKY_CUDA_OK(cudaGetLastError());
+  return SKY_OK;
+}
+
+}  // extern "C"

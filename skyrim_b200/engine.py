@@ -308,6 +308,47 @@ def perturb_ic_grf(x, sigma_c, amp: float, seed: int, member0: int = 0, alpha: f
     return x
 
 
+ENS_MAX_MEMBERS, ENS_MAX_CHANNELS, ENS_MAX_QUANTILES, ENS_MAX_EVENTS = 64, 128, 8, 64
+
+
+def ensemble_statistics(x, channels=None, quantiles=(), events=(), channel_offset: int = 0, out=None):
+    """Per-point statistics over the members of a CUDA fp32 (M, C, H, W) tensor, or a view of one whose members each hold
+    contiguous (C, H, W) planes (include/skyrim_b200.h sky_ensemble_stats).  Channels are counted from ``channel_offset``
+    (a GraphCast state reduces its new time slice with offset 83); ``channels`` lists the reduced ones (default: all),
+    ``quantiles`` the numpy-"linear" quantiles, ``events`` (i, threshold) pairs for P(x > threshold) of ``channels[i]``
+    with i nondecreasing.  Returns (stats (2 + n_q, n_sel, H, W): mean, spread, quantiles; prob (n_events, H, W)), into
+    ``out`` = (stats, prob) when given.  Asynchronous on the current stream."""
+    import torch
+    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4):
+        raise ValueError("x must be a CUDA fp32 (members, channels, nlat, nlon) tensor")
+    M, Cn, H, W = x.shape
+    plane = H * W
+    if x.stride(3) != 1 or x.stride(2) != W or x.stride(1) != plane:
+        raise ValueError(f"each member of x must hold contiguous (C, H, W) planes (strides {x.stride()})")
+    if not 0 <= channel_offset < Cn:
+        raise ValueError(f"channel_offset = {channel_offset} is outside [0, {Cn})")
+    count = Cn - channel_offset
+    member_stride = x.stride(0) if M > 1 else max(x.stride(0), Cn * plane)
+    sel = list(range(count)) if channels is None else [int(c) for c in channels]
+    q = [float(v) for v in quantiles]
+    ev_sel, ev_thr = [int(i) for i, _ in events], [float(t) for _, t in events]
+    shapes = ((2 + len(q), len(sel), H, W), (len(ev_sel), H, W))
+    if out is None:
+        out = tuple(torch.empty(s, dtype=torch.float32, device=x.device) for s in shapes)
+    stats, prob = out
+    for t, s in zip(out, shapes):
+        if tuple(t.shape) != s or t.dtype != torch.float32 or not t.is_contiguous():
+            raise ValueError(f"output of shape {tuple(t.shape)} {t.dtype}: contiguous fp32 {s} needed")
+    arr = lambda ct, v: (ct * max(len(v), 1))(*v)  # noqa: E731
+    L = _ffi.lib()
+    st = torch.cuda.current_stream(x.device).cuda_stream
+    _ffi.check(L.sky_ensemble_stats(x.data_ptr() + 4 * channel_offset * plane, M, member_stride, plane, count,
+                                    arr(C.c_int32, sel), len(sel), arr(C.c_double, q), len(q), arr(C.c_int32, ev_sel),
+                                    arr(C.c_float, ev_thr), len(ev_sel), stats.data_ptr(),
+                                    prob.data_ptr() if prob.numel() else None, st), "sky_ensemble_stats", L)
+    return stats, prob
+
+
 def unix_seconds(when) -> float:
     """datetime (naive = UTC) / numpy datetime64 / number -> unix seconds"""
     import datetime as _dt

@@ -71,6 +71,36 @@ class EnsembleRunner:
         """ensemble mean / standard deviation over ALL members (two all-reduces, outside the step loop)"""
         return mean_and_spread(self.x, world)
 
+    def iter_stats(self, n_steps: int, channels=None, quantiles=(), events=(), channel_offset: int = 0):
+        """Steps ``n_steps`` times and yields (n, stats, prob) for the current state (n = 0) and after each step:
+        ``engine.ensemble_statistics`` of this rank's members, as pinned host tensors.  Only the statistics leave the
+        device, and the device->host copy of step n runs on a copy stream while step n + 1 computes (the event pattern of
+        ``timeloop._EngineTimeLoop.iter_host``, with rings of two statistics buffers on the device and on the host).  A
+        yielded pair is valid until the second next() after it."""
+        import torch
+        from .engine import ensemble_statistics
+        dev = self.x.device
+        main = torch.cuda.current_stream(dev)
+        copy = torch.cuda.Stream(dev)
+        ring = [ensemble_statistics(self.x, channels, quantiles, events, channel_offset)]
+        ring.append(tuple(torch.empty_like(t) for t in ring[0]))
+        host = [tuple(torch.empty(t.shape, dtype=t.dtype).pin_memory() for t in ring[0]) for _ in range(2)]
+        done = [torch.cuda.Event() for _ in range(2)]    # statistics i % 2 are complete on the main stream
+        copied = torch.cuda.Event()
+        done[0].record(main)
+        for n in range(n_steps + 1):
+            if n < n_steps:   # launch step n + 1 and its reduction before waiting for the copy of step n
+                self.step()
+                ensemble_statistics(self.x, channels, quantiles, events, channel_offset, out=ring[(n + 1) % 2])
+                done[(n + 1) % 2].record(main)
+            copy.wait_event(done[n % 2])
+            with torch.cuda.stream(copy):
+                for h, d in zip(host[n % 2], ring[n % 2]):
+                    h.copy_(d, non_blocking=True)
+                copied.record(copy)
+            copied.synchronize()   # also orders the next reduction into ring[n % 2] (launched at n + 1) after this copy
+            yield (n,) + host[n % 2]
+
 
 def mean_and_spread(x, world: int = 1):
     """x: this rank's members (M, C, H, W).  Two-pass: the mean is reduced first, then the sum of squared DEVIATIONS —

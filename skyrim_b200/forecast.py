@@ -2,6 +2,10 @@
 defaults; same `run_forecast` signature and return value) on top of the H100 engine:
 
     python -m skyrim_b200.forecast -m pangu -d 20240507 -t 0000 -l 24 -o outputs
+    python -m skyrim_b200.forecast -m pangu -l 24 --members 8 --quantiles 0.1,0.5,0.9 --exceed t2m:273.15 -o outputs
+
+The second form runs a perturbed-initial-condition ensemble and saves its per-step statistics (mean, spread, quantiles)
+and exceedance probabilities instead of the members.
 
 Differences, all forced by the scope of this build (SURVEY.md section 2): `--initial_conditions` accepts `synthetic`
 (the default here: the network IC providers cds / ifs / gfs are the reference's `libs/ic`, out of scope, and raise a clear
@@ -36,6 +40,37 @@ def run_forecast(model_name: str, date: str, time: str, lead_time: int, list_mod
     return output_paths
 
 
+def run_ensemble_forecast(model_name: str, date: str, time: str, lead_time: int, initial_conditions: str, output_dir: str,
+                          filter_vars: str, members: int, perturbation: str, amp: float, seed: int, quantiles=(),
+                          events: dict = {}, **model_kw):
+    """``--members`` > 1: ``Skyrim.predict_ensemble(save=True)``; returns the statistics and probability file paths"""
+    from .core import Skyrim
+    model = Skyrim(model_name, ic_source=initial_conditions, **model_kw)
+    _, paths = model.predict_ensemble(
+        date=date, time=time, lead_time=lead_time, members=members, perturbation=perturbation, amp=amp, seed=seed,
+        quantiles=quantiles, events=events, save=True,
+        save_config={"output_dir": output_dir or str(Path.cwd() / "outputs"),
+                     "filter_vars": [v.strip() for v in filter_vars.split(",") if v.strip()]})
+    return paths
+
+
+def parse_quantiles(text: str):
+    """"0.1,0.5,0.9" -> [0.1, 0.5, 0.9]"""
+    return [float(v) for v in text.split(",") if v.strip()]
+
+
+def parse_exceed(text: str):
+    """"t2m:273.15,u10m:15" -> {"t2m": [273.15], "u10m": [15.0]} (a channel may appear more than once)"""
+    events = {}
+    for item in (v.strip() for v in text.split(",")):
+        if item:
+            name, sep, thr = item.partition(":")
+            if not sep:
+                raise ValueError(f"--exceed item {item!r} is not channel:threshold")
+            events.setdefault(name.strip(), []).append(float(thr))
+    return events
+
+
 @click.command()
 @click.option("--model_name", "-m", type=click.Choice(AVAILABLE_MODELS, case_sensitive=False), default="pangu", help="Select model")
 @click.option("--date", "-d", type=str, default=yesterday, help="YYYYMMDD")
@@ -51,16 +86,36 @@ def run_forecast(model_name: str, date: str, time: str, lead_time: int, list_mod
 @click.option("--weight_seed", type=int, default=0, help="seed of the synthetic weights (no checkpoint download here)")
 @click.option("--device", type=int, default=0, help="CUDA device ordinal")
 @click.option("--grid", type=str, default="", help="NLATxNLON coarse test grid (default: the model's 721x1440)")
-def main(model_name, date, time, lead_time, list_models, initial_conditions, output_dir, filter_vars, modal, weight_seed, device, grid):
+@click.option("--members", type=int, default=1, help="Ensemble members (1..64); above 1, per-step ensemble statistics are saved")
+@click.option("--perturbation", type=click.Choice(["spherical_grf", "gaussian"]), default="spherical_grf",
+              help="Initial-condition perturbation of the ensemble members")
+@click.option("--amp", type=float, default=0.05, help="Perturbation amplitude in units of each channel's standard deviation")
+@click.option("--seed", type=int, default=0, help="Perturbation seed")
+@click.option("--quantiles", type=str, default="", help="Ensemble quantiles such as 0.1,0.5,0.9")
+@click.option("--exceed", type=str, default="", help="Exceedance events channel:threshold such as t2m:273.15,u10m:15")
+def main(model_name, date, time, lead_time, list_models, initial_conditions, output_dir, filter_vars, modal, weight_seed, device, grid,
+         members, perturbation, amp, seed, quantiles, exceed):
     if modal:
         raise click.UsageError("--modal: remote execution through Modal is outside this build (SURVEY.md section 2); run locally")
+    if not 1 <= members <= 64:
+        raise click.UsageError(f"--members {members}: an ensemble holds 1 to 64 members on one GPU")
+    try:
+        q, events = parse_quantiles(quantiles), parse_exceed(exceed)
+    except ValueError as e:
+        raise click.UsageError(str(e))
+    if members == 1 and (q or events):
+        raise click.UsageError("--quantiles and --exceed describe an ensemble: give --members > 1")
     kw = {"weight_seed": weight_seed, "device": device}
     if grid:
         from .config import graphcast_small, pangu_small, sfno_small
         nlat, nlon = (int(v) for v in grid.lower().split("x"))
         kw["cfg"] = (pangu_small(nlat, nlon) if model_name == "pangu" else graphcast_small(nlat, nlon) if model_name == "graphcast"
                      else sfno_small(nlat, nlon))
-    paths = run_forecast(model_name, date, time, lead_time, list_models, initial_conditions, output_dir, filter_vars, **kw)
+    if members > 1 and not list_models:
+        paths = run_ensemble_forecast(model_name, date, time, lead_time, initial_conditions, output_dir, filter_vars, members,
+                                      perturbation, amp, seed, q, events, **kw)
+    else:
+        paths = run_forecast(model_name, date, time, lead_time, list_models, initial_conditions, output_dir, filter_vars, **kw)
     for p in paths:
         print(p)
     return paths
