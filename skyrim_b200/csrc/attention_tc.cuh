@@ -106,73 +106,106 @@ __device__ __forceinline__ long long at_row_token(const Geo& g, int roll, int b,
   return (long long)b * g.T + ((long long)z * g.H + h) * g.W + w;
 }
 
+// natural token row (member b = row / T) -> row of its tile of the window image at head pair 0: win * pairs * 144 + j, win
+// the member's window and j the position in it, on the rolled grid when roll is set.  members * tokens < 2^31, and
+// members * windows * pairs * 144 < 2^31 (checked by the callers).
+__device__ __forceinline__ int qkv_window_row(const Geo& g, int roll, int pairs, unsigned row) {
+  const unsigned b = row / (unsigned)g.T, t = row - b * (unsigned)g.T;
+  const unsigned q2 = t / (unsigned)g.W;
+  int w = (int)(t - q2 * (unsigned)g.W);
+  int z = (int)(q2 / (unsigned)g.H), h = (int)(q2 - (unsigned)z * (unsigned)g.H);
+  if (roll) {   // natural -> rolled-grid coordinates
+    z -= SZ; if (z < 0) z += g.Z;
+    h -= SH; if (h < 0) h += g.Hp;
+    w -= SW; if (w < 0) w += g.W;
+  }
+  const int wz = z / WZ, zj = z % WZ, wh = h / WH, hj = h % WH, ww = w / WW, wj = w % WW;
+  const int win = (int)b * g.nWin + (wz * g.nWh + wh) * g.nWw + ww;
+  return win * pairs * WIN_TOK + (zj * WH + hj) * WW + wj;
+}
+
 // ---------------------------------------------------------------------------------------------------------------
-// QKV projection epilogue: accumulator (tokens in natural order) -> fp16 window image.  Re-tiled through the warp's
-// swizzled patch exactly like Epi2F16; only the destination address differs: row (window, j) of tile (part, pair).
-// A warp store covers 8 token rows x 64 B (one head of each row).
+// QKV projection epilogue, on the accumulator fragments (FragEpi<EpiQkvWin>, BLOCK_N 192): accumulator (tokens in
+// natural order) + bias -> fp16 window image.  C is a multiple of 192, so an n-tile is three consecutive head pairs
+// hp0 .. hp0 + 2 of one part (q, k or v at C = 192; half a part at C = 384).  The output tile holds them as
+// [pair p < 3][tile row r < 128][128 B], and row r of block p is byte for byte destination row drow (qkv_window_row of the
+// tile's row r) of pair hp0 + p: its 16-byte chunk c sits at c ^ (drow & 7), the swizzle of the destination row, not of r.
+// The loader stores the tile in runs of consecutive drow (kScatter): a run breaks at a window edge, at the end of a latitude
+// row or level, at a member boundary and at the roll's wrap, so most runs are one window row (12 rows, 1.5 KB) and a tile
+// has 10 to 15 of them.  One bulk copy per (run, pair) instead of one per (row, pair) is 30 to 45 copies instead of 384.
 // ---------------------------------------------------------------------------------------------------------------
 struct EpiQkvWin {
-  static constexpr bool kNeedsBias = false;
+  static constexpr bool kNeedsBias = false, kLoadsTile = false, kScatter = true;
   uint8_t* out; long long part_stride; const float* bias; Geo g; int roll; int C; int pairs;
   const float* gamma = nullptr; const float* beta = nullptr;   // unused (uniform epilogue interface)
+  // The loader, not the consumers, computes the destination rows: it has the time while it waits for ring slots, and
+  // the divisions by the grid's run-time sizes stay off the epilogue that keeps the tensor cores waiting.  -1: row >= M.
+  __device__ __forceinline__ int dest_row(long long row, long long M) const {
+    return row < M ? qkv_window_row(g, roll, pairs, (unsigned)row) : -1;
+  }
   template <int BN, class Acc>
-  __device__ void run(Acc& acc, const EpiCtx& x) const {
-    // this lane's own token row -> index of its 128-byte row inside a part, pair 0 (tile stride = 144 rows); computed once
-    // per row group and cached in the context across the n-tiles of the m-tile (the divisions are by run-time values)
-    if (x.aux_row0 != x.row0) {
-      int myrow = -1;
-      const long long row = x.row0 + x.lane;
-      if (row < x.M) {
-        const unsigned ur = (unsigned)row;             // members * tokens < 2^31
-        const unsigned b = ur / (unsigned)g.T, t = ur - b * (unsigned)g.T;
-        const unsigned q2 = t / (unsigned)g.W;
-        int w = (int)(t - q2 * (unsigned)g.W);
-        int z = (int)(q2 / (unsigned)g.H), h = (int)(q2 - (unsigned)z * (unsigned)g.H);
-        if (roll) {   // natural -> rolled-grid coordinates
-          z -= SZ; if (z < 0) z += g.Z;
-          h -= SH; if (h < 0) h += g.Hp;
-          w -= SW; if (w < 0) w += g.W;
-        }
-        const int wz = z / WZ, zj = z % WZ, wh = h / WH, hj = h % WH, ww = w / WW, wj = w % WW;
-        const int win = (int)b * g.nWin + (wz * g.nWh + wh) * g.nWw + ww;
-        myrow = win * pairs * WIN_TOK + (zj * WH + hj) * WW + wj;     // < 2^31 for members * windows * pairs * 144
-      }
-      x.aux = myrow;
-      x.aux_row0 = x.row0;
-    }
-    const int myrow = x.aux;
-    const int rsub = x.lane >> 2, ch = x.lane & 3;
-    for (int c = x.part * 32; c < BN; c += 32 * x.nparts) {
-      const int col = x.n0 + c;                       // first of the 32 columns = one head of one part
-      const int part = col / C, hd = (col - part * C) >> 5;
-      const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + col + ch * 8));
-      const float4 b1 = __ldg(reinterpret_cast<const float4*>(bias + col + ch * 8 + 4));
-      {
-        float v[32];
-        acc.load32(c, v);
-        patch_put_v(x.patch_s, x.lane, v);
-      }
-      __syncwarp();
-      uint8_t* pbase = out + (size_t)part * part_stride + (size_t)(hd >> 1) * AT_TILE_B;
-      const uint32_t cpos = (uint32_t)((hd & 1) * 4 + ch);
+  __device__ void frag(Acc& acc, const FragCtx& x) const {
+    static_assert(BN == 192, "an n-tile is three head pairs");
+    const float* bp = bias + x.n0 + x.c2;
 #pragma unroll
-      for (int it = 0; it < 4; ++it) {
-        const int rr = it * 8 + rsub;
-        float4 t0 = lds_f32x4(patchv_addr(x.patch_s, rr, 2 * ch));
-        float4 t1 = lds_f32x4(patchv_addr(x.patch_s, rr, 2 * ch + 1));
-        t0.x += b0.x; t0.y += b0.y; t0.z += b0.z; t0.w += b0.w;
-        t1.x += b1.x; t1.y += b1.y; t1.z += b1.z; t1.w += b1.w;
-        uint4 pk;
-        pk.x = pack_half2(t0.x, t0.y); pk.y = pack_half2(t0.z, t0.w);
-        pk.z = pack_half2(t1.x, t1.y); pk.w = pack_half2(t1.z, t1.w);
-        const int drow = __shfl_sync(0xffffffffu, myrow, rr);
-        if (drow >= 0)
-          *reinterpret_cast<uint4*>(pbase + (size_t)drow * 128 + ((cpos ^ ((uint32_t)drow & 7u)) << 4)) = pk;
-      }
-      __syncwarp();
+    for (int i = 0; i < BN / 8; ++i) {
+      const float2 b = __ldg(reinterpret_cast<const float2*>(bp + 8 * i));
+      float* d = acc.d + 4 * i;
+      d[0] += b.x; d[1] += b.y; d[2] += b.x; d[3] += b.y;
     }
+    mbar_wait(x.out_ready, x.ready_parity);   // also publishes the loader's map of destination rows (svec_s)
+    uint32_t row_s[2], sw[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const uint32_t r = (uint32_t)(x.row + 8 * h);
+      uint32_t drow;
+      asm volatile("ld.shared.b32 %0, [%1];" : "=r"(drow) : "r"(x.svec_s + r * 4u) : "memory");
+      sw[h] = drow & 7u;
+      row_s[h] = x.out_s + r * 128u + (uint32_t)x.c2 * 2u;
+    }
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        sts_b32(row_s[h] + (uint32_t)(i >> 3) * G2_A_BYTES + ((((uint32_t)i & 7u) ^ sw[h]) << 4),
+                pack_half2(acc.d[4 * i + 2 * h], acc.d[4 * i + 2 * h + 1]));
+  }
+  // Loader warp: store the output tile of the n-tile at column n0, with tile row r going to destination row map[r]
+  // (map_s + 4 r; -1 past M, those rows are not written).  Lane l looks at rows l + 32 k; every lane issues the copies of
+  // the runs that start at its rows and waits until they have read the tile.
+  __device__ void frag_store(int n0, uint32_t out_s, uint32_t map_s, int lane) const {
+    const int part = n0 / C, hp0 = (n0 - part * C) >> 6;
+    uint8_t* dst = out + (size_t)part * part_stride + (size_t)hp0 * AT_TILE_B;
+    int d[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) asm volatile("ld.shared.b32 %0, [%1];" : "=r"(d[k]) : "r"(map_s + (uint32_t)(lane + 32 * k) * 4u) : "memory");
+    // bit l of brk[k]: row 32 k + l does not continue the run of the row before it (it starts a run, or is past M)
+    uint32_t brk[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      int prev = __shfl_up_sync(0xffffffffu, d[k], 1);
+      const int last = __shfl_sync(0xffffffffu, d[k > 0 ? k - 1 : 0], 31);
+      if (lane == 0) prev = k > 0 ? last : -1;
+      brk[k] = __ballot_sync(0xffffffffu, d[k] < 0 || prev < 0 || d[k] != prev + 1);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (d[k] < 0 || !((brk[k] >> lane) & 1u)) continue;
+      const int r = 32 * k + lane;
+      int end = G2_BLOCK_M;   // the next break after row r
+#pragma unroll
+      for (int kk = 3; kk >= k; --kk) {
+        const uint32_t m = kk == k ? brk[kk] & (0xfffffffeu << lane) : brk[kk];
+        if (m) end = 32 * kk + __ffs((int)m) - 1;
+      }
+      const uint32_t bytes = (uint32_t)(end - r) * 128u;
+#pragma unroll
+      for (int p = 0; p < 3; ++p)
+        bulk_s2g(dst + (size_t)p * AT_TILE_B + (size_t)d[k] * 128, out_s + (uint32_t)(p * G2_A_BYTES + r * 128), bytes);
+    }
+    bulk_commit();
+    bulk_wait_read<0>();
   }
 };
-
 
 }  // namespace sky

@@ -16,7 +16,8 @@
 // (warp%4 selects the 32-row quarter, warp/4 the column partition).  Epilogues re-tile their 32x32
 // accumulator blocks through a padded smem patch so that every global access is a full
 // 64/128-byte row segment.  Epilogues wrapped in FragEpi run on the accumulator registers instead and leave through a
-// dedicated output tile that the loader bulk-stores, so the ring keeps streaming under them (Pangu's fc1, projection, fc2).
+// dedicated output tile that the loader bulk-stores, so the ring keeps streaming under them (Pangu's QKV projection, fc1,
+// projection, fc2).
 #pragma once
 #include <climits>
 #include <type_traits>
@@ -109,6 +110,13 @@ struct FragEpi : E {
 };
 template <class E, class = void> struct is_fragment_epi : std::false_type {};
 template <class E> struct is_fragment_epi<E, std::void_t<decltype(E::kFragment)>> : std::true_type {};
+// E::kScatter: the tile's rows do not land as three contiguous blocks at E::tile_image.  The loader looks up the destination
+// row of each tile row with E::dest_row (while it waits for the ring, ahead of the tile's epilogue), publishes the 128 rows
+// as a 512-byte map over the bias region (E::kNeedsBias is false), opens the output tile, and stores it later with
+// E::frag_store, which reads the same map.  The map is overwritten only after the previous tile's epilogue has finished
+// (stg_free) and that tile has been stored.
+template <class E, class = void> struct is_scatter_epi : std::false_type {};
+template <class E> struct is_scatter_epi<E, std::void_t<decltype(E::kScatter)>> : std::true_type {};
 
 // What a fragment epilogue sees of its tile
 struct FragCtx {
@@ -142,9 +150,6 @@ struct EpiCtx {
   uint32_t svec_s;     // shared-space address of bias | gamma | beta, vstride floats apart (LN epilogues)
   int vstride = 512;
   int patch_stride = G2_PATCH_FLOATS * 4;   // bytes between the patches of consecutive warps
-  // per-row-group scratch an epilogue may cache across the n-tiles of one m-tile (EpiQkvWin: destination row of this lane)
-  mutable long long aux_row0 = -1;
-  mutable int aux = 0, aux2 = 0;
   // row-statistics exchange with the peer CTA of a column-split pair (k_gemm2_pair); x_own_bar == nullptr elsewhere
   uint64_t* x_own_bar = nullptr;   // completes when the peer's 32 (sum, sum of squares) pairs of this lane quarter landed
   uint32_t x_own_stat = 0;         // shared-space address of this CTA's slot: 32 x {float s, ss}
@@ -326,7 +331,8 @@ constexpr int G2_PAIR_SMEM = 2048;   // the pair's exchange slots, behind the ba
 
 // Fragment epilogues (FragEpi): the loader warp stores the output tile of tile `t` (a finished tile) to the destination
 // image.  The three 16 KB blocks of a tile are contiguous there (n0 is a multiple of BLOCK_N); a partial last m-tile is
-// stored row by row, so that rows >= M are never written.  Every lane waits until its copies have read the tile.
+// stored row by row, so that rows >= M are never written.  Every lane waits until its copies have read the tile.  (Scatter
+// epilogues, E::kScatter, store the tile with E::frag_store instead.)
 template <class Cfg, class Epi, class Tile>
 __device__ __forceinline__ void frag_store(const Epi& epi, const Tile& t, uint32_t out_s, long long M, int bn, int lane) {
   uint8_t* dst = epi.tile_image(t.mt, t.nt * bn);
@@ -346,6 +352,8 @@ template <class Sched, class Epi, int BLOCK_N, bool kPair>
 __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, const G2Grid& g) {
   constexpr int EPI_WARPS = G2_EPI_WARPS;
   constexpr bool kFrag = is_fragment_epi<Epi>::value;
+  constexpr bool kScatter = is_scatter_epi<Epi>::value;
+  if constexpr (kScatter) static_assert(kFrag && !Epi::kNeedsBias && !Epi::kLoadsTile, "scatter: fragment path, map over the bias region");
   using Cfg = G2Cfg<BLOCK_N, EPI_WARPS, kFrag>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -397,11 +405,16 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
       const int head = sc.num_kb < Cfg::STAGES ? sc.num_kb : Cfg::STAGES;
       int s = 0; uint32_t ph = 0;
       decltype(sc.template tile<BLOCK_N>(g, 0)) prev{};
+      const uint32_t map_s = smem_u32(sbias);   // kScatter: destination row of tile row r at map_s + 4 r
+      int dst_row[4];                           // kScatter: of tile rows lane + 32 k
       for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         const auto t = sc.template tile<BLOCK_N>(g, tile);
         if (t.skip) continue;
         // the destination's bytes of this tile are pulled into L2 a main loop ahead of their load into the output tile
         if constexpr (Epi::kLoadsTile) if (lane == 0) bulk_prefetch_l2(epi.tile_image(t.mt, t.nt * BLOCK_N), Cfg::OUT_BYTES);
+        if constexpr (kScatter)
+#pragma unroll
+          for (int k = 0; k < 4; ++k) dst_row[k] = epi.dest_row((long long)t.mt * G2_BLOCK_M + lane + 32 * k, g.M);
         for (int kb = 0; kb < sc.num_kb; ++kb) {
           mbar_wait(&empty[s], ph ^ 1);
           sc.template issue<BLOCK_N>(smem + s * Cfg::STAGE_BYTES, &full[s], t, kb, lane);
@@ -410,8 +423,13 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
           if (kb + 1 != head) continue;
           if (it > 0) {
             mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
-            frag_store<Cfg>(epi, prev, out_s, g.M, BLOCK_N, lane);
+            if constexpr (kScatter) epi.frag_store(prev.nt * BLOCK_N, out_s, map_s, lane);
+            else frag_store<Cfg>(epi, prev, out_s, g.M, BLOCK_N, lane);
           }
+          if constexpr (kScatter)
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(map_s + (uint32_t)(lane + 32 * k) * 4u), "r"(dst_row[k]) : "memory");
           __syncwarp();
           if (lane == 0) {
             if constexpr (Epi::kLoadsTile) {
@@ -427,7 +445,8 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
       }
       if (it > 0) {
         mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
-        frag_store<Cfg>(epi, prev, out_s, g.M, BLOCK_N, lane);
+        if constexpr (kScatter) epi.frag_store(prev.nt * BLOCK_N, out_s, map_s, lane);
+        else frag_store<Cfg>(epi, prev, out_s, g.M, BLOCK_N, lane);
         bulk_wait<0>();
       }
     } else {

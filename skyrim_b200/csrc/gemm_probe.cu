@@ -42,7 +42,7 @@ enum {
   SKY_PROBE_EPI_GC_LN0 = 14,      // EpiGcLn<0>
   SKY_PROBE_EPI_GC_LN1 = 15,      // EpiGcLn<1>
   SKY_PROBE_EPI_GC_LN2 = 16,      // EpiGcLn<2>
-  SKY_PROBE_EPI_QKV_WIN = 17,     // EpiQkvWin (Pangu's QKV projection -> q | k | v window image)
+  SKY_PROBE_EPI_QKV_WIN = 17,     // FragEpi<EpiQkvWin> (Pangu's QKV projection -> q | k | v window image)
   SKY_PROBE_EPI_F16_GELU_IMG_FRAG = 18,   // FragEpi<Epi2F16<true, true>>: SKY_PROBE_EPI_F16_GELU_IMG on the fragment path
   SKY_PROBE_EPI_LN_IMG_FRAG = 19,         // FragEpi<Epi2F32Img<true, true, true>>: SKY_PROBE_EPI_LN_IMG on the fragment path
 };
@@ -311,6 +311,8 @@ int check_epilogue(const Case& c) {
       PROBE_REQUIRE(c.n == 3 * c.geo.C && c.n_valid == c.n && c.batches == 1, "QKV window image: N=%d is not 3C=%d, or n_valid / batches",
                     c.n, 3 * c.geo.C);
       PROBE_REQUIRE(c.roll == 0 || c.roll == 1, "QKV window image: roll %d", c.roll);
+      // an n-tile of the fragment epilogue is three head pairs of one part
+      PROBE_REQUIRE(c.geo.C % 192 == 0, "QKV window image: C=%d is not a multiple of 192", c.geo.C);
       PROBE_REQUIRE(c.m % c.geo.T == 0, "QKV window image: M=%lld is not members x T=%d", (long long)c.m, c.geo.T);
       // the epilogue's 32-bit row arithmetic: members x tokens and members x windows x pairs x 144 rows below 2^31
       const long long tiles = c.m / c.geo.T * c.geo.nWin * c.pairs;
@@ -388,8 +390,8 @@ EpiGcLn<kRes> make_gcln(const Case& c) {
 template <> EpiGcLn<0> make_epi(const Case& c) { return make_gcln<0>(c); }
 template <> EpiGcLn<1> make_epi(const Case& c) { return make_gcln<1>(c); }
 template <> EpiGcLn<2> make_epi(const Case& c) { return make_gcln<2>(c); }
-template <> EpiQkvWin make_epi(const Case& c) {
-  return EpiQkvWin{(uint8_t*)c.hi, c.part_stride, c.bias, probe_geo(c.geo), c.roll, c.geo.C, c.pairs};
+template <> FragEpi<EpiQkvWin> make_epi(const Case& c) {
+  return {EpiQkvWin{(uint8_t*)c.hi, c.part_stride, c.bias, probe_geo(c.geo), c.roll, c.geo.C, c.pairs}};
 }
 
 template <int... BNs> struct BnList {};
@@ -410,10 +412,11 @@ int by_bn(const Case& c, const Sched& sc, cudaStream_t st, BnList<BNs...>) {
 // The (schedule, epilogue, BLOCK_N) lists mirror what the engines instantiate:
 //   SFNO SfnoEngine::gemm_op: SchedW / SchedW<true> x its epilogues x {16, 32, 64, 80, 192, 240, 256};
 //   SFNO SfnoEngine::gemm_tb: SchedTB x {EpiSplitRemap, EpiF32Batched<false>, EpiGeluStatsImg} x {64, 128, 192, 256};
-//   Pangu: SchedW x Epi2F32Img<true, true, *> at 192, and the pair kernel at 192; fc1's Epi2F16<true, true> at 192; the QKV
-//   projection's EpiQkvWin at 192; the fragment path of the projection / fc2 (FragEpi<Epi2F32Img<true, true, true>>, single
-//   CTA and pair) and of fc1 (FragEpi<Epi2F16<true, true>>) at 192.  The engine no longer launches the staged
-//   Epi2F32Img<true, true, true> and Epi2F16<true, true>; the probe keeps them as the reference of the fragment path;
+//   Pangu: SchedW x Epi2F32Img<true, true, *> at 192, and the pair kernel at 192; fc1's Epi2F16<true, true> at 192; the
+//   fragment path of the QKV projection (FragEpi<EpiQkvWin>, which has no staged form), of the projection / fc2
+//   (FragEpi<Epi2F32Img<true, true, true>>, single CTA and pair) and of fc1 (FragEpi<Epi2F16<true, true>>) at 192.  The
+//   engine no longer launches the staged Epi2F32Img<true, true, true> and Epi2F16<true, true>; the probe keeps them as the
+//   reference of the fragment path;
 //   GraphCast: EpiGcSiluImg<0 / 2> and the node tables' Epi2F16<false, false> at 256, EpiGcOut at 128, and the pair kernel
 //   with EpiGcLn<0 / 1 / 2> at 256 (GraphCast never gathers exactly one table: EpiGcSiluImg<1> is not instantiated).
 using BnSfno = BnList<16, 32, 64, 80, 192, 240, 256>;
@@ -466,7 +469,7 @@ int dispatch(const Case& c, cudaStream_t st) {
           case SKY_PROBE_EPI_GC_SILU0: return by_bn<false, EpiGcSiluImg<0>>(c, sc, st, BnList<256>{});
           case SKY_PROBE_EPI_GC_SILU2: return by_bn<false, EpiGcSiluImg<2>>(c, sc, st, BnList<256>{});
           case SKY_PROBE_EPI_GC_OUT: return by_bn<false, EpiGcOut>(c, sc, st, BnList<128>{});
-          case SKY_PROBE_EPI_QKV_WIN: return by_bn<false, EpiQkvWin>(c, sc, st, BnList<192>{});
+          case SKY_PROBE_EPI_QKV_WIN: return by_bn<false, FragEpi<EpiQkvWin>>(c, sc, st, BnList<192>{});
           default: break;
         }
       }

@@ -584,7 +584,7 @@ struct PanguEngine : Engine {
     const long long part_stride = (long long)B * g.nWin * pairs * AT_TILE_B;
     {  // QKV projection: natural-order tokens in, window image out (windowing / shift / padding applied by the epilogue)
       AOperand A(xh, nkb);
-      EpiQkvWin e{ws.qkv, part_stride, b.qkv_b, g, roll, C, pairs};
+      FragEpi<EpiQkvWin> e{{ws.qkv, part_stride, b.qkv_b, g, roll, C, pairs}};
       if ((rc = gemm2<192>(KT_QKV, A, e, b.qkv, R, st))) return rc;
       if (g.Hp > g.H) {   // latitude-padding tokens (x = 0): their q, k, v rows are the projection's bias.  (Writing them from
                           // the GEMM epilogue of the neighbouring tokens instead cost the GEMM 0.5 ms/step: measured, reverted.)

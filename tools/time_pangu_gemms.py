@@ -5,7 +5,7 @@
 
 Each GEMM runs through libskyrim_b200_probe.so (oracle/gemm_probe.py) at the full 721 x 1440 token grids (C = 192 with
 M = 521,280 tokens per member, C = 384 with M = 131,040), on random fp16 operand images made on the device:
-  qkv    N = 3C, K = C,  window-image scatter (staged path only)
+  qkv    N = 3C, K = C,  window-image scatter (fragment path only: it has no staged form)
   proj   N = C,  K = C,  LayerNorm + residual into the fp16 token image (CTA pairs at C = 384)
   fc1    N = 4C, K = C,  GELU into the fp16 hidden image
   fc2    N = C,  K = 4C, LayerNorm + residual into the fp16 token image (CTA pairs at C = 384)
@@ -119,7 +119,7 @@ def main():
             case = gemm_case(gp.W, gp.EPI_QKV_WIN, 3 * C, M, x, nkb, w_qkv, hi=qkv.data_ptr(), img_bytes=nbytes(qkv),
                              bias=b3.data_ptr(), vec_floats=3 * C, geo=g.probe_geo(), roll=1, pairs=g.pairs,
                              part_stride=wt * pk.TILE_B)
-            res["gemms"].append(report("qkv", "staged", C, B, M, 3 * C, C, time_case(case), mt * 3 * C // BN))
+            res["gemms"].append(report("qkv", "fragment", C, B, M, 3 * C, C, time_case(case), mt * 3 * C // BN))
             del qkv
             for name, N, K in (("proj", C, C), ("fc1", 4 * C, C), ("fc2", C, 4 * C)):
                 cases = {}
