@@ -188,7 +188,8 @@ def col_stats(f_ref, f_bound, rows_per_sum: int = 32):
 
 
 def layer_norm(R, S, bias, gamma, beta, res, eps, tau=TAU):
-    """Epi2F32Img<kLn, kResidual> / EpiGcLn: out = LN(acc + bias) * gamma + beta + res over whole rows, with its bound"""
+    """Epi2F32Img<true, kRes> (Pangu's and GraphCast's LayerNorm epilogue): out = LN(acc + bias) * gamma + beta + res over
+    whole rows, with its bound; res = 0 for kRes 0"""
     y = R + bias
     e = tau * S + 2 * U32 * np.abs(y)
     mu = y.mean(1, keepdims=True)

@@ -33,6 +33,7 @@ constexpr int G2_A_BYTES = G2_BLOCK_M * 128;
 constexpr int G2_PATCH_LD = 33;    // scalar accessors (odd stride: conflict-free column reads)
 constexpr int G2_PATCH_FLOATS = 32 * G2_PATCH_LD;
 constexpr int G2_PATCHV_BYTES = 4096;   // 128-bit accessors: 32 rows x 128 B, 16-byte chunk index XOR (row & 7)
+constexpr int G2_VEC_FLOATS = 512;      // shared-memory copies of bias | gamma | beta (LN epilogues), this many floats apart
 
 // element (row, col) of an fp16 tile image with nkb k-blocks per row tile -> byte offset
 __device__ __forceinline__ size_t img_offset(long long row, int col, int nkb) {
@@ -82,7 +83,7 @@ struct G2Cfg {
   static constexpr int STAGE_BYTES = G2_A_BYTES + B_BYTES;
   static constexpr int OUT_BYTES = BLOCK_N / 64 * G2_A_BYTES;
   static constexpr int PATCH_BYTES = kFrag ? OUT_BYTES : EPI_WARPS * G2_PATCH_FLOATS * 4;
-  static constexpr int VEC_BYTES = 3 * 512 * 4;  // smem copies of bias | gamma | beta (LN epilogues), <= 512 floats each
+  static constexpr int VEC_BYTES = 3 * G2_VEC_FLOATS * 4;
   static constexpr int FIXED = 1024 /*align*/ + 256 /*barriers*/ + PATCH_BYTES + VEC_BYTES;
   static constexpr int MAXS = (232448 - FIXED) / STAGE_BYTES;
   static constexpr int STAGES = MAXS > 6 ? 6 : MAXS;
@@ -118,19 +119,58 @@ template <class E> struct is_fragment_epi<E, std::void_t<decltype(E::kFragment)>
 template <class E, class = void> struct is_scatter_epi : std::false_type {};
 template <class E> struct is_scatter_epi<E, std::void_t<decltype(E::kScatter)>> : std::true_type {};
 
+// LayerNorm row statistics of a column-split CTA pair (k_gemm2_pair): the two CTAs hold the two column halves of the same
+// 128 rows.  For each tile and 32-row group, a CTA posts its rows' (sum, sum of squares) into the peer's slot and reads
+// the peer's from its own.  Slots [tile parity][32-row group][row % 32][sum, sum of squares] and one barrier per (tile
+// parity, group) follow the barrier block (gemm2_body).  own_bar == nullptr outside a pair.
+struct PairStats {
+  uint64_t* own_bar = nullptr;            // completes when the peer's 32 rows of this group have landed
+  uint32_t own_stat = 0;                  // shared-space address of this CTA's slot
+  uint32_t peer_stat = 0, peer_bar = 0;   // shared::cluster addresses of the same slot / barrier in the peer CTA
+  uint32_t parity = 0;
+  // 32-row group q of the CTA's it-th tile
+  __device__ __forceinline__ static PairStats at(uint64_t* xbar, float* xstat, int it, int q, uint32_t rank) {
+    PairStats p;
+    const int buf = it & 1;
+    p.own_bar = &xbar[buf * 4 + q];
+    p.own_stat = smem_u32(xstat + (buf * 4 + q) * 64);
+    p.peer_stat = mapa_u32(p.own_stat, rank ^ 1u);
+    p.peer_bar = mapa_u32(smem_u32(p.own_bar), rank ^ 1u);
+    p.parity = (uint32_t)(it >> 1) & 1;
+    return p;
+  }
+  // one lane per group and tile: announces the bytes of the peer's 32 posts
+  __device__ __forceinline__ void expect() const { mbar_arrive_expect_tx(own_bar, 32 * 8); }
+  // tile row r's sums into the peer's slot.  st.async itself completes the peer's barrier transaction: no fence, no release
+  // arrive.
+  __device__ __forceinline__ void post(int r, float s, float ss) const {
+    asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];" ::"r"(
+                     peer_stat + (uint32_t)(r & 31) * 8u),
+                 "f"(s), "f"(ss), "r"(peer_bar)
+                 : "memory");
+  }
+  // CTA-scope acquire: the peer's sums arrive in THIS CTA's shared memory through st.async, whose completion the barrier
+  // phase carries (as for bulk copies); a cluster-scope wait added an L1 invalidate (CCTL.IVALL) per tile
+  __device__ __forceinline__ void wait() const { mbar_wait(own_bar, parity); }
+  // after wait(): adds the peer's sums of tile row r
+  __device__ __forceinline__ void add_peer(int r, float& s, float& ss) const {
+    float ps, pss;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ps), "=f"(pss) : "r"(own_stat + (uint32_t)(r & 31) * 8u));
+    s += ps; ss += pss;
+  }
+};
+
 // What a fragment epilogue sees of its tile
 struct FragCtx {
   int row;              // the thread's first fragment row in the tile (64 wg + 16 w + l/4); the second is row + 8
   int c2;               // 2 (l & 3): the thread's first column inside each 8-column group
   int n0;               // first column of the tile in the full N
   uint32_t out_s;       // shared-space address of the output tile
-  uint32_t svec_s;      // bias | gamma | beta of this CTA's columns, 512 floats apart (LN epilogues)
+  uint32_t svec_s;      // bias | gamma | beta of this CTA's columns, G2_VEC_FLOATS apart (LN epilogues)
   uint64_t* out_ready;  // completes when the output tile may be written (and, kLoadsTile, holds the destination's bytes)
   uint32_t ready_parity;
-  // row statistics of a column-split CTA pair (k_gemm2_pair), indexed by tile row; x_own_bar == nullptr elsewhere
-  uint64_t* x_own_bar = nullptr;   // completes when the peer's (sum, sum of squares) of this thread's 32-row group landed
-  uint32_t x_own_stat = 0, x_peer_stat = 0, x_peer_bar = 0, x_parity = 0;
-  bool post_bar = false;           // this warp announces the barrier's transaction bytes (one of the group's two warps)
+  PairStats pair;       // the thread's 32-row group (k_gemm2_pair)
+  bool post_bar = false;   // this warp announces the pair's transaction bytes (one of the group's two warps)
   // byte offset inside the output tile of fragment row `row` (+ 8 with hi), 8-column group i
   __device__ __forceinline__ uint32_t offset(int i, bool hi) const {
     const uint32_t r = (uint32_t)(row + (hi ? 8 : 0));
@@ -147,14 +187,8 @@ struct EpiCtx {
   int part, nparts; // column-chunk partition among the warps sharing a lane quarter
   float* patch;     // [32][33] floats, private to the warp
   uint32_t patch_s;    // the same patch as a shared-space address
-  uint32_t svec_s;     // shared-space address of bias | gamma | beta, vstride floats apart (LN epilogues)
-  int vstride = 512;
-  int patch_stride = G2_PATCH_FLOATS * 4;   // bytes between the patches of consecutive warps
-  // row-statistics exchange with the peer CTA of a column-split pair (k_gemm2_pair); x_own_bar == nullptr elsewhere
-  uint64_t* x_own_bar = nullptr;   // completes when the peer's 32 (sum, sum of squares) pairs of this lane quarter landed
-  uint32_t x_own_stat = 0;         // shared-space address of this CTA's slot: 32 x {float s, ss}
-  uint32_t x_peer_stat = 0, x_peer_bar = 0;   // shared::cluster addresses of the same slot / barrier in the peer CTA
-  uint32_t x_parity = 0;
+  uint32_t svec_s;     // shared-space address of bias | gamma | beta, G2_VEC_FLOATS apart (LN epilogues)
+  PairStats pair;      // the warp's 32-row group (k_gemm2_pair)
 };
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -322,7 +356,7 @@ struct SchedW {
 // previous tile's epilogue has left the ring (stg_free); a tile the schedule skips counts for no role.
 // kPair (k_gemm2_pair): the two CTAs of a cluster take the same m-tile and n-tiles 0 / 1 (N = 2 BLOCK_N; the persistent
 // walk over 2 n-tiles with an even grid gives CTA rank r exactly the tiles (mt, r)), and exchange LayerNorm row statistics
-// through distributed shared memory (EpiCtx::x_*).  A 128 x 512 fp32 accumulator is the whole register file of an SM;
+// through distributed shared memory (PairStats).  A 128 x 512 fp32 accumulator is the whole register file of an SM;
 // this way the epilogue still sees whole rows.  Exchange slots and barriers are double buffered by tile parity; a CTA
 // runs at most one tile ahead of its peer, because its next statistics wait needs the peer's sums of that tile.
 // ---------------------------------------------------------------------------------------------------------------
@@ -359,7 +393,7 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   float* patches = reinterpret_cast<float*>(smem + Cfg::RING_BYTES);
   float* sbias = reinterpret_cast<float*>(smem + Cfg::RING_BYTES + Cfg::PATCH_BYTES);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sbias + 3 * 512);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sbias + 3 * G2_VEC_FLOATS);
   uint64_t* full = bars;
   uint64_t* empty = bars + Cfg::STAGES;
   uint64_t* stg_free = bars + 2 * Cfg::STAGES;   // consumers -> loader: the tile's epilogue has left the ring
@@ -387,10 +421,10 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
   if constexpr (Epi::kNeedsBias) if (threadIdx.x < EPI_WARPS * 32)
     for (int i = threadIdx.x; i < BLOCK_N; i += EPI_WARPS * 32) {
       const uint32_t c = rank * BLOCK_N + i;   // this CTA's columns
-      sbias[i] = epi.bias[c]; sbias[512 + i] = epi.gamma[c]; sbias[1024 + i] = epi.beta[c];
+      sbias[i] = epi.bias[c]; sbias[G2_VEC_FLOATS + i] = epi.gamma[c]; sbias[2 * G2_VEC_FLOATS + i] = epi.beta[c];
     }
   if constexpr (has_cta_stats<Epi>::value)
-    for (int i = threadIdx.x; i < 3 * 512; i += blockDim.x) sbias[i] = 0.f;
+    for (int i = threadIdx.x; i < 3 * G2_VEC_FLOATS; i += blockDim.x) sbias[i] = 0.f;
   __syncthreads();
   if (kPair) cluster_sync_all();   // the peer's exchange barriers exist before anything is posted to them
 
@@ -465,15 +499,7 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
         if (t.skip) continue;
         x.n0 = t.nt * BLOCK_N;
         x.ready_parity = (uint32_t)it & 1;
-        if constexpr (kPair) {
-          // the statistics slots keep the staged path's layout: [tile parity][32-row group][row % 32][sum, sum of squares]
-          const int buf = it & 1, q = x.row >> 5;
-          x.x_own_bar = &xbar[buf * 4 + q];
-          x.x_own_stat = smem_u32(xstat + (buf * 4 + q) * 64);
-          x.x_peer_stat = mapa_u32(x.x_own_stat, rank ^ 1u);
-          x.x_peer_bar = mapa_u32(smem_u32(x.x_own_bar), rank ^ 1u);
-          x.x_parity = (uint32_t)(it >> 1) & 1;
-        }
+        if constexpr (kPair) x.pair = PairStats::at(xbar, xstat, it, x.row >> 5, rank);
         ++it;
         wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, sc.num_kb, wg, lane);
         epi.template frag<BLOCK_N>(acc, x);
@@ -514,14 +540,7 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
       ctx.batch = t.b;
       ctx.row0 = (long long)t.mt * G2_BLOCK_M + q * 32;
       ctx.n0 = t.nt * BLOCK_N;
-      if constexpr (kPair) {
-        const int buf = it & 1;
-        ctx.x_own_bar = &xbar[buf * 4 + q];
-        ctx.x_own_stat = smem_u32(xstat + (buf * 4 + q) * 64);
-        ctx.x_peer_stat = mapa_u32(ctx.x_own_stat, rank ^ 1u);
-        ctx.x_peer_bar = mapa_u32(smem_u32(ctx.x_own_bar), rank ^ 1u);
-        ctx.x_parity = (uint32_t)(it >> 1) & 1;
-      }
+      if constexpr (kPair) ctx.pair = PairStats::at(xbar, xstat, it, q, rank);
       ++it;
       if constexpr (Epi::kNeedsBias) epi.template prefetch<BLOCK_N>(ctx);  // LN + residual epilogues
       wg_mainloop<Cfg::STAGES, Cfg::STAGE_BYTES>(acc, smem, full, empty, s, ph, sc.num_kb, wg, lane);
@@ -709,80 +728,106 @@ struct Epi2F16 {
   }
 };
 
-// xf32[row, n0+col] (=|+=) f(acc)  and the fp16 tile image of the new rows.
-//   kLn:       y = LayerNorm(acc + bias) * gamma + beta  (tile spans the feature width: n0 == 0)
-//   kResidual: x += y, else x = y  (bias, if any, is applied when !kLn as well)
-// Global traffic is 128-bit: lane -> (row = it*4 + lane/8, float4 column group = lane%8), i.e.
-// eight lanes cover one 128-byte row segment.  bias / gamma / beta come from shared memory.
-// kImgStream: the rows exist ONLY as their fp16 operand image — the residual is read from `img` (in place), the sum is formed in
-// fp32 and rounded once back into `img`; nothing is read from or written to x.  Round 2 (late): on the oracle an fp16-only
-// residual stream moves the Pangu step error from 5.3e-4 to 5.9e-4 (tests/test_oracle_cpu.py) and removes 8 of the 12 bytes
-// per token and feature that the projection / MLP epilogues move through HBM.
-template <bool kLn, bool kResidual, bool kImgStream = false>
+// The staged LayerNorm / residual epilogue: Pangu's projection, fc2 and the second GEMMs of down- and up-sample, and every
+// GraphCast LayerNorm MLP.  For each row of the tile
+//   y   = LayerNorm(acc + bias) * gamma + beta   (kLn: the tile spans the row, or one column half of it in a CTA pair)
+//   y   = acc + bias                             (!kLn: no statistics; bias may be null)
+//   sum = res + y                                (kRes: the residual source, 0 none, 1 fp32 rows, 2 an fp16 tile image)
+// and it writes any of xout (fp32 rows of sum), img (fp16 tile image of sum: the A operand of the next GEMM) and yimg (fp16
+// tile image of y: what GraphCast's aggregation sums).  Each destination may be null; res may be one of them (an in-place
+// update).  The residual source is a template argument because a run-time branch per load serialised the loads and cost
+// the kernel 10 - 50 %.
+// A stream kept only as its fp16 image (Pangu by default, GraphCast's grid nodes and mesh edges) passes res = img and
+// xout = null: the sum is formed in fp32 and rounded once back into img.  On the oracle that moves the Pangu step error
+// from 5.3e-4 to 5.9e-4 (tests/test_oracle_cpu.py) and GraphCast's tendency error over 16 layers from 7.66e-4 to 7.95e-4
+// (tests/test_graphcast_cpu.py); it removes 8 of the 12 bytes per row and feature that Pangu's projection / MLP
+// epilogues move through HBM, and 3 KB per row and launch of GraphCast's.
+// Global traffic is 128-bit: lane -> (row = it*4 + lane/8, float4 column group = lane%8), i.e. eight lanes cover one
+// 128-byte row segment.  bias / gamma / beta come from shared memory (kLn) or bias from global memory (!kLn).
+template <bool kLn, int kRes>
 struct Epi2F32Img {
+  static_assert(kRes >= 0 && kRes <= 2, "residual source: none, fp32 rows, fp16 image");
   static constexpr bool kNeedsBias = kLn;
-  float* x; int ldx;            // fp32 row-major (unused when kImgStream)
-  uint8_t* img; int nkb;        // fp16 image of the same rows (may be null unless kImgStream)
-  const float* bias; const float* gamma; const float* beta; float eps;  // bias may be null when !kLn
+  const void* res;              // residual: fp32 rows ldx floats apart (kRes 1), or a tile image with nkb k-blocks (kRes 2)
+  float* xout; int ldx;         // fp32 rows of the sum, ldx floats apart
+  uint8_t* img; int nkb;        // fp16 tile image of the sum, nkb k-blocks per row tile
+  uint8_t* yimg;                // fp16 tile image of y, in img's layout
+  const float* bias; const float* gamma; const float* beta; float eps;
+  // residual of the lane's eight (row, 4-column) pieces of the 32-column group at tile column c: all eight loads are
+  // issued before any is used
+  __device__ __forceinline__ void residual8(const EpiCtx& e, int c, int rsub4, int c4, size_t rowoff, long long rows_left, bool on,
+                                            float4 (&r)[8]) const {
+    if constexpr (kRes == 1) {
+      const float* xin = static_cast<const float*>(res);
+#pragma unroll
+      for (int it = 0; it < 8; ++it) {
+        const int rr = it * 4 + rsub4;
+        r[it] = (on && rr < rows_left) ? *reinterpret_cast<const float4*>(xin + rowoff + (size_t)rr * ldx + c) : make_float4(0.f, 0.f, 0.f, 0.f);
+      }
+    } else if constexpr (kRes == 2) {
+      const int col = e.n0 + c + c4 * 4;
+      const uint8_t* base = static_cast<const uint8_t*>(res) + ((size_t)(e.row0 >> 7) * nkb + (col >> 6)) * (size_t)G2_A_BYTES +
+                            (uint32_t)(e.row0 & 127) * 128 + (c4 & 1) * 8;
+      const uint32_t chunk = (uint32_t)(col & 63) >> 3;
+      uint2 u[8];
+#pragma unroll
+      for (int it = 0; it < 8; ++it) {
+        const int rr = it * 4 + rsub4;
+        u[it] = (on && rr < rows_left) ? *reinterpret_cast<const uint2*>(base + rr * 128 + ((chunk ^ (uint32_t)(rr & 7)) << 4)) : make_uint2(0u, 0u);
+      }
+#pragma unroll
+      for (int it = 0; it < 8; ++it) {
+        const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u[it].x)), b = __half22float2(*reinterpret_cast<const __half2*>(&u[it].y));
+        r[it] = make_float4(a.x, a.y, b.x, b.y);
+      }
+    } else {
+#pragma unroll
+      for (int it = 0; it < 8; ++it) r[it] = make_float4(0.f, 0.f, 0.f, 0.f);
+    }
+  }
   // Pull this warp's residual rows into L2 ahead of time, while the tile's main loop runs.
-  // four residual values of row (row0 + rr) at tile column n0 + c + 4 * c4, read from the fp16 image
-  __device__ __forceinline__ uint2 img_res_raw(const EpiCtx& e, int rr, int c, int c4) const {
-    const int col = e.n0 + c + c4 * 4;
-    return *reinterpret_cast<const uint2*>(img + ((size_t)(e.row0 >> 7) * nkb + (col >> 6)) * (size_t)G2_A_BYTES +
-                                           ((uint32_t)(e.row0 & 127) + rr) * 128 + ((((uint32_t)(col & 63) >> 3) ^ (uint32_t)(rr & 7)) << 4) + (c4 & 1) * 8);
-  }
-  static __device__ __forceinline__ float4 h4_to_f4(const uint2& u) {
-    const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u.x)), b = __half22float2(*reinterpret_cast<const __half2*>(&u.y));
-    return make_float4(a.x, a.y, b.x, b.y);
-  }
   template <int BN>
   __device__ void prefetch(const EpiCtx& e) const {
-    if (!kResidual) return;
+    if (kRes == 0) return;
     const long long row = e.row0 + e.lane;
     if (row >= e.M) return;
-    if (kImgStream) {
-      const char* p = reinterpret_cast<const char*>(img) + ((size_t)(e.row0 >> 7) * nkb + (e.n0 >> 6)) * (size_t)G2_A_BYTES +
+    if (kRes == 2) {
+      const char* p = static_cast<const char*>(res) + ((size_t)(e.row0 >> 7) * nkb + (e.n0 >> 6)) * (size_t)G2_A_BYTES +
                       ((uint32_t)(e.row0 & 127) + e.lane) * 128;
 #pragma unroll
       for (int i = e.part; i < BN / 64; i += e.nparts) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + (size_t)i * G2_A_BYTES));
       return;
     }
-    const char* p = reinterpret_cast<const char*>(x + row * ldx + e.n0);
+    const char* p = reinterpret_cast<const char*>(static_cast<const float*>(res) + row * ldx + e.n0);
 #pragma unroll
     for (int i = e.part; i < BN * 4 / 128; i += e.nparts) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + i * 128));
   }
-  // Per 32x32 block: the row-owner lanes drop the raw accumulator into the warp's patch with 128-bit
-  // stores, then every lane works on (row = it*4 + lane/8, 4 columns = lane%8) pieces: 8 lanes cover a
-  // full 128-byte row segment of x, so residual loads and stores are coalesced 128-bit accesses.  The
-  // LayerNorm statistics of the 8 rows a lane touches come from their owner lanes by shuffle; the
-  // fp16 image chunks (8 columns = 16 bytes) are assembled from lane pairs by shuffle, not through
-  // shared memory.  Every warp reduces the statistics of its own column groups only; the warps that
-  // share a lane quarter exchange partial sums through their patches.  The residual of the next column group is loaded
-  // while this one is processed (32 more registers).
+  // The 16-byte image chunk (8 columns) of a lane pair: the even lane assembles the chunk of row it2, the odd lane that of
+  // row it2 + 1, and the pair swaps the other halves by shuffle.  h: this lane's 4 columns of rows it2, it2 + 1.
+  static __device__ __forceinline__ uint4 pair_chunk(const uint2 (&h)[2], int odd) {
+    const uint2 send = odd ? h[0] : h[1];
+    uint2 recv;
+    recv.x = __shfl_xor_sync(0xffffffffu, send.x, 1);
+    recv.y = __shfl_xor_sync(0xffffffffu, send.y, 1);
+    return odd ? make_uint4(recv.x, recv.y, h[1].x, h[1].y) : make_uint4(h[0].x, h[0].y, recv.x, recv.y);
+  }
+  // Per 32x32 block: the row-owner lanes drop the raw accumulator into the warp's patch with 128-bit stores, then every
+  // lane works on (row = it*4 + lane/8, 4 columns = lane%8) pieces.  The LayerNorm statistics of the 8 rows a lane touches
+  // come from their owner lanes by shuffle; the fp16 image chunks are assembled from lane pairs by shuffle, not through
+  // shared memory.  Every warp reduces the statistics of its own column groups only; the warps that share a lane quarter
+  // exchange partial sums through their patches.  The residual of the next column group is loaded while this one is
+  // processed (32 more registers).
   template <int BN, class Acc>
   __device__ void run(Acc& acc, const EpiCtx& e) const {
     constexpr int NG = BN / 32;
+    static_assert(NG >= 2, "a column group for each warp of a lane quarter");
     const int rsub4 = e.lane >> 3, c4 = e.lane & 7;
     const long long rows_left = e.M - e.row0;          // >= 32 for every tile but the last
-    float* xp = x + e.row0 * ldx + e.n0 + c4 * 4;
-    float4 xin[8];
-    if constexpr (kImgStream) {
-      uint2 raw[8];
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const int rr = it * 4 + rsub4;
-        raw[it] = (kResidual && rr < rows_left && e.part < NG) ? img_res_raw(e, rr, e.part * 32, c4) : make_uint2(0u, 0u);
-      }
-#pragma unroll
-      for (int it = 0; it < 8; ++it) xin[it] = h4_to_f4(raw[it]);
-    } else {
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const int rr = it * 4 + rsub4;
-        xin[it] = (kResidual && rr < rows_left && e.part < NG) ? *reinterpret_cast<const float4*>(xp + (size_t)rr * ldx + e.part * 32)
-                                                               : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    }
+    const size_t rowoff = (size_t)e.row0 * ldx + e.n0 + c4 * 4;   // fp32 rows: this lane's columns in row row0
+    const size_t ld4 = (size_t)4 * ldx;                             // from the lane's row it * 4 + rsub4 to its next
+    // residual rows of the first column group: requested before the statistics pass (they come from L2: prefetch())
+    float4 xr[8];
+    residual8(e, e.part * 32, rsub4, c4, rowoff, rows_left, true, xr);
     float rs[8], ns[8];   // rstd and -mean*rstd of row it*4 + rsub4
 #pragma unroll
     for (int it = 0; it < 8; ++it) { rs[it] = 1.f; ns[it] = 0.f; }
@@ -800,6 +845,7 @@ struct Epi2F32Img {
         }
       }
       if (e.nparts > 1) {
+        // the warps of a lane quarter are 4 warps apart, and so are their patches
         const uint32_t slot = e.patch_s + e.lane * 8;
         asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(slot), "f"(s), "f"(ss) : "memory");
         const int q = (int)((e.row0 >> 5) & 3);
@@ -807,26 +853,20 @@ struct Epi2F32Img {
         for (int p = 0; p < e.nparts; ++p) {
           if (p == e.part) continue;
           float ps, pss;
-          asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ps), "=f"(pss) : "r"(slot + (p - e.part) * 4 * e.patch_stride));
+          asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ps), "=f"(pss) : "r"(slot + (p - e.part) * 4 * (G2_PATCH_FLOATS * 4)));
           s += ps; ss += pss;
         }
         asm volatile("bar.sync %0, %1;" ::"r"(8 + q), "r"(32 * e.nparts) : "memory");   // the patches are reused below
       }
       float width = (float)BN;
-      if (e.x_own_bar) {
-        // column-split CTA pair (k_gemm2_pair): the other half of these rows is in the peer CTA — post this CTA's sums into
-        // the peer's slot (st.async completes the peer's mbarrier transaction), wait for the peer's, add
+      if (e.pair.own_bar) {   // column-split CTA pair: the other half of these rows is in the peer CTA
         if (e.part == 0) {
-          if (e.lane == 0) mbar_arrive_expect_tx(e.x_own_bar, 32 * 8);
+          if (e.lane == 0) e.pair.expect();
           __syncwarp();
-          asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];" ::"r"(e.x_peer_stat + e.lane * 8),
-                       "f"(s), "f"(ss), "r"(e.x_peer_bar)
-                       : "memory");
+          e.pair.post(e.lane, s, ss);
         }
-        mbar_wait(e.x_own_bar, e.x_parity);   // CTA-scope acquire: the peer's sums arrive in THIS CTA's shared memory through st.async, whose completion the barrier phase carries (as for bulk copies); the cluster-scope wait added an L1 invalidate (CCTL.IVALL) per tile
-        float ps, pss;
-        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ps), "=f"(pss) : "r"(e.x_own_stat + e.lane * 8));
-        s += ps; ss += pss;
+        e.pair.wait();
+        e.pair.add_peer(e.lane, s, ss);
         width = (float)(2 * BN);
       }
       const float mean = s / width;
@@ -842,6 +882,8 @@ struct Epi2F32Img {
     const int odd = e.lane & 1;
     for (int g = e.part; g < NG; g += e.nparts) {
       const int c = g * 32;
+      float4 xn[8];   // the next group's residual, in flight while this group is normalised and stored
+      residual8(e, c + 32 * e.nparts, rsub4, c4, rowoff, rows_left, g + e.nparts < NG, xn);
       {
         float v[32];
         acc.load32(c, v);
@@ -851,38 +893,18 @@ struct Epi2F32Img {
       float4 bs = make_float4(0.f, 0.f, 0.f, 0.f), ga = make_float4(1.f, 1.f, 1.f, 1.f), be = make_float4(0.f, 0.f, 0.f, 0.f);
       if (kLn) {
         bs = lds_f32x4_ro(e.svec_s + (c + c4 * 4) * 4);
-        ga = lds_f32x4_ro(e.svec_s + (e.vstride + c + c4 * 4) * 4);
-        be = lds_f32x4_ro(e.svec_s + (2 * e.vstride + c + c4 * 4) * 4);
+        ga = lds_f32x4_ro(e.svec_s + (G2_VEC_FLOATS + c + c4 * 4) * 4);
+        be = lds_f32x4_ro(e.svec_s + (2 * G2_VEC_FLOATS + c + c4 * 4) * 4);
       } else if (bias) {
         bs = __ldg(reinterpret_cast<const float4*>(bias + e.n0 + c + c4 * 4));
       }
-      const bool more = g + e.nparts < NG;
-      float4 xnext[8];
-      if constexpr (kResidual) {
-        if constexpr (kImgStream) {
-          uint2 raw[8];
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int rr = it * 4 + rsub4;
-            raw[it] = (more && rr < rows_left) ? img_res_raw(e, rr, c + 32 * e.nparts, c4) : make_uint2(0u, 0u);
-          }
-#pragma unroll
-          for (int it = 0; it < 8; ++it) xnext[it] = h4_to_f4(raw[it]);
-        } else {
-#pragma unroll
-          for (int it = 0; it < 8; ++it) {
-            const int rr = it * 4 + rsub4;
-            xnext[it] = (more && rr < rows_left) ? *reinterpret_cast<const float4*>(xp + (size_t)rr * ldx + c + 32 * e.nparts)
-                                                 : make_float4(0.f, 0.f, 0.f, 0.f);
-          }
-        }
-      }
       const int col = e.n0 + c;
-      uint8_t* ibase = img ? img + ((size_t)(e.row0 >> 7) * nkb + (col >> 6)) * (size_t)G2_A_BYTES + r0 * 128 : nullptr;
+      const size_t tile_off = ((size_t)(e.row0 >> 7) * nkb + (col >> 6)) * (size_t)G2_A_BYTES + r0 * 128;
       const uint32_t cb = (((uint32_t)col & 63u) >> 3) + (uint32_t)(c4 >> 1);   // 16-byte chunk of this lane pair inside the image row
+      size_t xo = rowoff + (size_t)rsub4 * ldx + c;   // xout offset of the lane's row it * 4 + rsub4: one add per row
 #pragma unroll
       for (int it2 = 0; it2 < 8; it2 += 2) {
-        uint2 h[2];
+        uint2 hs[2], hy[2];   // fp16 of the sum and of y, rows it2 and it2 + 1
 #pragma unroll
         for (int u = 0; u < 2; ++u) {
           const int it = it2 + u;
@@ -891,36 +913,39 @@ struct Epi2F32Img {
           float4 y;
           y.x = fmaf(fmaf(t.x + bs.x, rs[it], ns[it]), ga.x, be.x); y.y = fmaf(fmaf(t.y + bs.y, rs[it], ns[it]), ga.y, be.y);
           y.z = fmaf(fmaf(t.z + bs.z, rs[it], ns[it]), ga.z, be.z); y.w = fmaf(fmaf(t.w + bs.w, rs[it], ns[it]), ga.w, be.w);
-          if (kResidual) { y.x += xin[it].x; y.y += xin[it].y; y.z += xin[it].z; y.w += xin[it].w; }
-          if (!kImgStream && rr < rows_left) *reinterpret_cast<float4*>(xp + (size_t)rr * ldx + c) = y;
-          h[u].x = pack_half2(y.x, y.y); h[u].y = pack_half2(y.z, y.w);
+          hy[u].x = pack_half2(y.x, y.y); hy[u].y = pack_half2(y.z, y.w);
+          if (kRes) { y.x += xr[it].x; y.y += xr[it].y; y.z += xr[it].z; y.w += xr[it].w; }
+          if (xout && rr < rows_left) *reinterpret_cast<float4*>(xout + xo) = y;
+          xo += ld4;
+          hs[u].x = pack_half2(y.x, y.y); hs[u].y = pack_half2(y.z, y.w);
         }
-        if (ibase) {
-          // even lane assembles the chunk of row it2, odd lane the chunk of row it2+1: swap the other halves
-          const uint2 send = odd ? h[0] : h[1];
-          uint2 recv;
-          recv.x = __shfl_xor_sync(0xffffffffu, send.x, 1);
-          recv.y = __shfl_xor_sync(0xffffffffu, send.y, 1);
-          const int rr = (it2 + odd) * 4 + rsub4;
-          const uint4 pk = odd ? make_uint4(recv.x, recv.y, h[1].x, h[1].y) : make_uint4(h[0].x, h[0].y, recv.x, recv.y);
-          if (rr < rows_left) *reinterpret_cast<uint4*>(ibase + rr * 128 + ((cb ^ (uint32_t)(rr & 7)) << 4)) = pk;
+        const int rr = (it2 + odd) * 4 + rsub4;
+        const uint32_t coff = rr * 128 + ((cb ^ (uint32_t)(rr & 7)) << 4);
+        if (img) {
+          const uint4 pk = pair_chunk(hs, odd);
+          if (rr < rows_left) *reinterpret_cast<uint4*>(img + tile_off + coff) = pk;
+        }
+        if (yimg) {
+          const uint4 pk = pair_chunk(hy, odd);
+          if (rr < rows_left) *reinterpret_cast<uint4*>(yimg + tile_off + coff) = pk;
         }
       }
       __syncwarp();
-      if constexpr (kResidual) {
+      if (kRes) {
 #pragma unroll
-        for (int it = 0; it < 8; ++it) xin[it] = xnext[it];
+        for (int it = 0; it < 8; ++it) xr[it] = xn[it];
       }
     }
   }
-  // FragEpi (LayerNorm into the fp16 stream image): the same arithmetic on the accumulator fragments.  A warpgroup holds
-  // whole rows, so a row's statistics are the thread's sums added across its lane quad (and, in a CTA pair, the peer's).
-  // The residual is the output tile itself: the loader fills it with the destination's bytes, the sum overwrites them.
-  static constexpr bool kLoadsTile = kResidual;
+  // FragEpi: the same arithmetic on the accumulator fragments, only for LayerNorm with the residual read in place from the
+  // fp16 image (kLn, kRes == 2, res == img; xout and yimg are not written).  The loader fills the output tile with img's
+  // bytes, which are the residual, and the sum overwrites them.  A warpgroup holds whole rows, so a row's statistics are
+  // the thread's sums added across its lane quad (and, in a CTA pair, the peer's).
+  static constexpr bool kLoadsTile = kRes == 2;
   __device__ uint8_t* tile_image(int mt, int n0) const { return img + ((size_t)mt * nkb + (n0 >> 6)) * (size_t)G2_A_BYTES; }
   template <int BN, class Acc>
   __device__ void frag(Acc& acc, const FragCtx& x) const {
-    static_assert(kLn && kImgStream, "fragment path: LayerNorm into the fp16 stream image");
+    static_assert(kLn && kRes == 2, "fragment path: LayerNorm with the fp16 image's in-place residual");
     float s[2] = {0.f, 0.f}, ss[2] = {0.f, 0.f};   // rows x.row, x.row + 8
 #pragma unroll
     for (int i = 0; i < BN / 8; ++i) {
@@ -939,26 +964,16 @@ struct Epi2F32Img {
         ss[h] += __shfl_xor_sync(0xffffffffu, ss[h], o);
       }
     float width = (float)BN;
-    if (x.x_own_bar) {
-      // column-split CTA pair: lane (l & 3) == h of each quad posts row x.row + 8 h into the peer's slot; the two warps of a
-      // 32-row group share one barrier, whose 256 transaction bytes one of them announces
+    if (x.pair.own_bar) {
+      // column-split CTA pair: lane (l & 3) == h of each quad posts row x.row + 8 h; the two warps of a 32-row group share
+      // one barrier, whose transaction bytes one of them announces
       const int lane = threadIdx.x & 31, h = lane & 3;
-      if (x.post_bar && lane == 0) mbar_arrive_expect_tx(x.x_own_bar, 32 * 8);
+      if (x.post_bar && lane == 0) x.pair.expect();
       __syncwarp();
-      if (h < 2) {
-        const uint32_t slot = (uint32_t)((x.row + 8 * h) & 31) * 8u;
-        const float ps = h ? s[1] : s[0], pss = h ? ss[1] : ss[0];
-        asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];" ::"r"(x.x_peer_stat + slot),
-                     "f"(ps), "f"(pss), "r"(x.x_peer_bar)
-                     : "memory");
-      }
-      mbar_wait(x.x_own_bar, x.x_parity);   // CTA-scope acquire, as in run()
+      if (h < 2) x.pair.post(x.row + 8 * h, h ? s[1] : s[0], h ? ss[1] : ss[0]);
+      x.pair.wait();
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        float ps, pss;
-        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ps), "=f"(pss) : "r"(x.x_own_stat + (uint32_t)((x.row + 8 * hh) & 31) * 8u));
-        s[hh] += ps; ss[hh] += pss;
-      }
+      for (int hh = 0; hh < 2; ++hh) x.pair.add_peer(x.row + 8 * hh, s[hh], ss[hh]);
       width = (float)(2 * BN);
     }
     float rs[2], ns[2];
@@ -972,19 +987,17 @@ struct Epi2F32Img {
 #pragma unroll
     for (int i = 0; i < BN / 8; ++i) {
       float2 ga, be;
-      asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ga.x), "=f"(ga.y) : "r"(x.svec_s + (uint32_t)(512 + 8 * i + x.c2) * 4u));
-      asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(be.x), "=f"(be.y) : "r"(x.svec_s + (uint32_t)(1024 + 8 * i + x.c2) * 4u));
+      asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ga.x), "=f"(ga.y) : "r"(x.svec_s + (uint32_t)(G2_VEC_FLOATS + 8 * i + x.c2) * 4u));
+      asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(be.x), "=f"(be.y) : "r"(x.svec_s + (uint32_t)(2 * G2_VEC_FLOATS + 8 * i + x.c2) * 4u));
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const uint32_t a = x.out_s + x.offset(i, h);
         const float* d = acc.d + 4 * i + 2 * h;
         float y0 = fmaf(fmaf(d[0], rs[h], ns[h]), ga.x, be.x), y1 = fmaf(fmaf(d[1], rs[h], ns[h]), ga.y, be.y);
-        if (kResidual) {
-          uint32_t r;
-          asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(a));
-          const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(&r));
-          y0 += rf.x; y1 += rf.y;
-        }
+        uint32_t r;
+        asm volatile("ld.shared.b32 %0, [%1];" : "=r"(r) : "r"(a));
+        const float2 rf = __half22float2(*reinterpret_cast<const __half2*>(&r));
+        y0 += rf.x; y1 += rf.y;
         asm volatile("st.shared.b32 [%0], %1;" ::"r"(a), "r"(pack_half2(y0, y1)) : "memory");
       }
     }

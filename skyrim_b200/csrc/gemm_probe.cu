@@ -32,19 +32,19 @@ enum {
   SKY_PROBE_EPI_F32_STATS = 4,    // EpiF32ImgStats
   SKY_PROBE_EPI_GELU_STATS = 5,   // EpiGeluStatsImg
   SKY_PROBE_EPI_REMAP = 6,        // EpiSplitRemap
-  SKY_PROBE_EPI_LN = 7,           // Epi2F32Img<true, true, false>
-  SKY_PROBE_EPI_LN_IMG = 8,       // Epi2F32Img<true, true, true>
+  SKY_PROBE_EPI_LN = 7,           // Epi2F32Img<true, 1>: fp32 rows in place, and their image
+  SKY_PROBE_EPI_LN_IMG = 8,       // Epi2F32Img<true, 2>: the fp16 image in place
   SKY_PROBE_EPI_F16_GELU_IMG = 9, // Epi2F16<true, true>
   SKY_PROBE_EPI_F16_ROWS = 10,    // Epi2F16<false, false>
   SKY_PROBE_EPI_GC_SILU0 = 11,    // EpiGcSiluImg<0>
   SKY_PROBE_EPI_GC_SILU2 = 12,    // EpiGcSiluImg<2>
   SKY_PROBE_EPI_GC_OUT = 13,      // EpiGcOut
-  SKY_PROBE_EPI_GC_LN0 = 14,      // EpiGcLn<0>
-  SKY_PROBE_EPI_GC_LN1 = 15,      // EpiGcLn<1>
-  SKY_PROBE_EPI_GC_LN2 = 16,      // EpiGcLn<2>
+  SKY_PROBE_EPI_GC_LN0 = 14,      // Epi2F32Img<true, 0> at GraphCast's shapes
+  SKY_PROBE_EPI_GC_LN1 = 15,      // Epi2F32Img<true, 1> at GraphCast's shapes
+  SKY_PROBE_EPI_GC_LN2 = 16,      // Epi2F32Img<true, 2> at GraphCast's shapes
   SKY_PROBE_EPI_QKV_WIN = 17,     // FragEpi<EpiQkvWin> (Pangu's QKV projection -> q | k | v window image)
   SKY_PROBE_EPI_F16_GELU_IMG_FRAG = 18,   // FragEpi<Epi2F16<true, true>>: SKY_PROBE_EPI_F16_GELU_IMG on the fragment path
-  SKY_PROBE_EPI_LN_IMG_FRAG = 19,         // FragEpi<Epi2F32Img<true, true, true>>: SKY_PROBE_EPI_LN_IMG on the fragment path
+  SKY_PROBE_EPI_LN_IMG_FRAG = 19,         // FragEpi<Epi2F32Img<true, 2>>: SKY_PROBE_EPI_LN_IMG on the fragment path
 };
 
 // Every pointer is a device pointer; every *_bytes / *_floats field is the size of the allocation behind it, which the
@@ -74,8 +74,8 @@ typedef struct {
   int64_t rows_per_batch;    // EpiGeluStatsImg: pixel row = batch * rows_per_batch + row
   int32_t bdiv, kmul, kdiv, rb, same;
   float eps;
-  // GraphCast epilogues: gathered fp16 tables ta / tb [rows][ld] indexed by ia / ib [M]; EpiGcLn's residual and update
-  // images; EpiGcOut's channel planes
+  // GraphCast epilogues: gathered fp16 tables ta / tb [rows][ld] indexed by ia / ib [M]; the LayerNorm's residual source
+  // (xin or xin_img) and update image; EpiGcOut's channel planes
   const void* ta; const void* tb; const int32_t* ia; const int32_t* ib;
   int64_t ta_bytes, tb_bytes, ta_rows, tb_rows;
   int32_t lda, ldb;
@@ -356,17 +356,22 @@ template <> EpiGeluStatsImg make_epi(const Case& c) {
 template <> EpiSplitRemap make_epi(const Case& c) {
   return {(uint8_t*)c.hi, (uint8_t*)c.lo, c.img_batch_bytes, c.img_nkb, c.bdiv, c.kmul, c.kdiv, c.rb, c.n_valid, c.same, c.csc, c.csh, c.t1};
 }
-template <> Epi2F32Img<true, true, false> make_epi(const Case& c) {
-  return {(float*)c.out, c.ldo, (uint8_t*)c.hi, c.img_nkb, c.bias, c.gamma, c.beta, c.eps};
+// The LayerNorm epilogue as Pangu runs it (make_ln): in place on fp32 rows `out` and their image `hi`, or on the image
+// `hi` alone; and as GraphCast runs it (make_gcln): the residual from xin or xin_img, any of out, hi and yimg written, rows
+// of 512 and 8 k-blocks.  Epi2F32Img<true, 1 / 2> serves both, so these are not make_epi specialisations.
+template <int kRes>
+Epi2F32Img<true, kRes> make_ln(const Case& c) {
+  return {kRes == 1 ? c.out : c.hi, kRes == 1 ? (float*)c.out : nullptr, c.ldo, (uint8_t*)c.hi, c.img_nkb, nullptr, c.bias, c.gamma, c.beta, c.eps};
 }
-template <> Epi2F32Img<true, true, true> make_epi(const Case& c) {
-  return {nullptr, 0, (uint8_t*)c.hi, c.img_nkb, c.bias, c.gamma, c.beta, c.eps};
+template <int kRes>
+Epi2F32Img<true, kRes> make_gcln(const Case& c) {
+  const void* res = kRes == 1 ? static_cast<const void*>(c.xin) : c.xin_img;
+  return {res, (float*)c.out, GC_L, (uint8_t*)c.hi, GC_NKB, (uint8_t*)c.yimg, c.bias, c.gamma, c.beta, c.eps};
 }
 
 template <> Epi2F16<true, true> make_epi(const Case& c) { return {(__half*)c.hi, 0, c.img_nkb, c.bias}; }
 template <> Epi2F16<false, false> make_epi(const Case& c) { return {(__half*)c.out, c.ldo, 0, c.bias}; }
 template <> FragEpi<Epi2F16<true, true>> make_epi(const Case& c) { return {make_epi<Epi2F16<true, true>>(c)}; }
-template <> FragEpi<Epi2F32Img<true, true, true>> make_epi(const Case& c) { return {make_epi<Epi2F32Img<true, true, true>>(c)}; }
 template <int kG>
 EpiGcSiluImg<kG> make_silu(const Case& c) {
   EpiGcSiluImg<kG> e{};
@@ -381,25 +386,15 @@ template <> EpiGcOut make_epi(const Case& c) {
   e.xout = (float*)c.out; e.xin = c.xin; e.bias = c.bias; e.dstd = c.dstd; e.plane = c.plane; e.nprog = c.nprog;
   return e;
 }
-template <int kRes>
-EpiGcLn<kRes> make_gcln(const Case& c) {
-  EpiGcLn<kRes> e{c.xin, (float*)c.out, (uint8_t*)c.hi, (uint8_t*)c.yimg, c.bias, c.gamma, c.beta, c.eps};
-  e.xin_img = (const uint8_t*)c.xin_img;
-  return e;
-}
-template <> EpiGcLn<0> make_epi(const Case& c) { return make_gcln<0>(c); }
-template <> EpiGcLn<1> make_epi(const Case& c) { return make_gcln<1>(c); }
-template <> EpiGcLn<2> make_epi(const Case& c) { return make_gcln<2>(c); }
 template <> FragEpi<EpiQkvWin> make_epi(const Case& c) {
   return {EpiQkvWin{(uint8_t*)c.hi, c.part_stride, c.bias, probe_geo(c.geo), c.roll, c.geo.C, c.pairs}};
 }
 
 template <int... BNs> struct BnList {};
 
-// launch with the case's BLOCK_N if it is in the list, else refuse
-template <bool kPair, class Epi, class Sched, int... BNs>
-int by_bn(const Case& c, const Sched& sc, cudaStream_t st, BnList<BNs...>) {
-  const Epi e = make_epi<Epi>(c);
+// launch epilogue e with the case's BLOCK_N if it is in the list, else refuse
+template <bool kPair, class Sched, class Epi, int... BNs>
+int launch_bn(const Case& c, const Sched& sc, const Epi& e, cudaStream_t st, BnList<BNs...>) {
   int rc = -1;
   ((c.block_n == BNs ? (rc = run<BNs, kPair>(c, sc, e, st), 0) : 0), ...);
   if (rc == -1) {
@@ -408,17 +403,22 @@ int by_bn(const Case& c, const Sched& sc, cudaStream_t st, BnList<BNs...>) {
   }
   return rc;
 }
+template <bool kPair, class Epi, class Sched, class Bns>
+int by_bn(const Case& c, const Sched& sc, cudaStream_t st, Bns bns) {
+  return launch_bn<kPair>(c, sc, make_epi<Epi>(c), st, bns);
+}
 
 // The (schedule, epilogue, BLOCK_N) lists mirror what the engines instantiate:
 //   SFNO SfnoEngine::gemm_op: SchedW / SchedW<true> x its epilogues x {16, 32, 64, 80, 192, 240, 256};
 //   SFNO SfnoEngine::gemm_tb: SchedTB x {EpiSplitRemap, EpiF32Batched<false>, EpiGeluStatsImg} x {64, 128, 192, 256};
-//   Pangu: SchedW x Epi2F32Img<true, true, *> at 192, and the pair kernel at 192; fc1's Epi2F16<true, true> at 192; the
+//   Pangu: SchedW x Epi2F32Img<true, 1 / 2> at 192, and the pair kernel at 192; fc1's Epi2F16<true, true> at 192; the
 //   fragment path of the QKV projection (FragEpi<EpiQkvWin>, which has no staged form), of the projection / fc2
-//   (FragEpi<Epi2F32Img<true, true, true>>, single CTA and pair) and of fc1 (FragEpi<Epi2F16<true, true>>) at 192.  The
-//   engine no longer launches the staged Epi2F32Img<true, true, true> and Epi2F16<true, true>; the probe keeps them as the
-//   reference of the fragment path;
+//   (FragEpi<Epi2F32Img<true, 2>>, single CTA and pair) and of fc1 (FragEpi<Epi2F16<true, true>>) at 192.  The engine
+//   launches the staged Epi2F32Img<true, 2> only at 256 (GraphCast) and Epi2F16<true, true> not at all; the probe keeps
+//   them at 192 as the reference of the fragment path;
 //   GraphCast: EpiGcSiluImg<0 / 2> and the node tables' Epi2F16<false, false> at 256, EpiGcOut at 128, and the pair kernel
-//   with EpiGcLn<0 / 1 / 2> at 256 (GraphCast never gathers exactly one table: EpiGcSiluImg<1> is not instantiated).
+//   with Epi2F32Img<true, 0 / 1 / 2> at 256 (GraphCast never gathers exactly one table: EpiGcSiluImg<1> is not
+//   instantiated).
 using BnSfno = BnList<16, 32, 64, 80, 192, 240, 256>;
 using BnSfnoMain = BnList<64, 192>;
 using BnTb = BnList<64, 128, 192, 256>;
@@ -444,12 +444,12 @@ int dispatch(const Case& c, cudaStream_t st) {
       const SchedW<false> sc{a, (const uint8_t*)c.w, c.num_kb, c.w_batch_stride, c.w_rep};
       if (c.kernel == SKY_PROBE_PAIR) {
         switch (c.epi) {
-          case SKY_PROBE_EPI_LN: return by_bn<true, Epi2F32Img<true, true, false>>(c, sc, st, BnPair{});
-          case SKY_PROBE_EPI_LN_IMG: return by_bn<true, Epi2F32Img<true, true, true>>(c, sc, st, BnPair{});
-          case SKY_PROBE_EPI_LN_IMG_FRAG: return by_bn<true, FragEpi<Epi2F32Img<true, true, true>>>(c, sc, st, BnPair{});
-          case SKY_PROBE_EPI_GC_LN0: return by_bn<true, EpiGcLn<0>>(c, sc, st, BnList<256>{});
-          case SKY_PROBE_EPI_GC_LN1: return by_bn<true, EpiGcLn<1>>(c, sc, st, BnList<256>{});
-          case SKY_PROBE_EPI_GC_LN2: return by_bn<true, EpiGcLn<2>>(c, sc, st, BnList<256>{});
+          case SKY_PROBE_EPI_LN: return launch_bn<true>(c, sc, make_ln<1>(c), st, BnPair{});
+          case SKY_PROBE_EPI_LN_IMG: return launch_bn<true>(c, sc, make_ln<2>(c), st, BnPair{});
+          case SKY_PROBE_EPI_LN_IMG_FRAG: return launch_bn<true>(c, sc, FragEpi<Epi2F32Img<true, 2>>{make_ln<2>(c)}, st, BnPair{});
+          case SKY_PROBE_EPI_GC_LN0: return launch_bn<true>(c, sc, make_gcln<0>(c), st, BnList<256>{});
+          case SKY_PROBE_EPI_GC_LN1: return launch_bn<true>(c, sc, make_gcln<1>(c), st, BnList<256>{});
+          case SKY_PROBE_EPI_GC_LN2: return launch_bn<true>(c, sc, make_gcln<2>(c), st, BnList<256>{});
           default: break;
         }
       } else if (c.kernel == SKY_PROBE_W) {
@@ -460,10 +460,10 @@ int dispatch(const Case& c, cudaStream_t st) {
           case SKY_PROBE_EPI_SPLIT_GELU: return by_bn<false, EpiSplitImg<true>>(c, sc, st, BnSfnoMain{});
           case SKY_PROBE_EPI_F32_STATS: return by_bn<false, EpiF32ImgStats>(c, sc, st, BnSfnoMain{});
           case SKY_PROBE_EPI_GELU_STATS: return by_bn<false, EpiGeluStatsImg>(c, sc, st, BnSfnoMain{});
-          case SKY_PROBE_EPI_LN: return by_bn<false, Epi2F32Img<true, true, false>>(c, sc, st, BnList<192>{});
-          case SKY_PROBE_EPI_LN_IMG: return by_bn<false, Epi2F32Img<true, true, true>>(c, sc, st, BnList<192>{});
+          case SKY_PROBE_EPI_LN: return launch_bn<false>(c, sc, make_ln<1>(c), st, BnList<192>{});
+          case SKY_PROBE_EPI_LN_IMG: return launch_bn<false>(c, sc, make_ln<2>(c), st, BnList<192>{});
           case SKY_PROBE_EPI_F16_GELU_IMG: return by_bn<false, Epi2F16<true, true>>(c, sc, st, BnList<192>{});
-          case SKY_PROBE_EPI_LN_IMG_FRAG: return by_bn<false, FragEpi<Epi2F32Img<true, true, true>>>(c, sc, st, BnList<192>{});
+          case SKY_PROBE_EPI_LN_IMG_FRAG: return launch_bn<false>(c, sc, FragEpi<Epi2F32Img<true, 2>>{make_ln<2>(c)}, st, BnList<192>{});
           case SKY_PROBE_EPI_F16_GELU_IMG_FRAG: return by_bn<false, FragEpi<Epi2F16<true, true>>>(c, sc, st, BnList<192>{});
           case SKY_PROBE_EPI_F16_ROWS: return by_bn<false, Epi2F16<false, false>>(c, sc, st, BnList<256>{});
           case SKY_PROBE_EPI_GC_SILU0: return by_bn<false, EpiGcSiluImg<0>>(c, sc, st, BnList<256>{});

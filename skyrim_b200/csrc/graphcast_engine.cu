@@ -191,10 +191,8 @@ struct GraphCastEngine : Engine {
     return rc ? rc : range_scan(5, out, (size_t)(M / 128) * GC_NKB * G2_A_BYTES, st);
   }
   template <int kRes>
-  int ln_launch(const uint8_t* hid, const Mlp& m, long long M, const float* xin, float* xout, uint8_t* img, uint8_t* yimg,
-                const uint8_t* xin_img, cudaStream_t st) {
-    EpiGcLn<kRes> epi{xin, xout, img, yimg, m.b2, m.g, m.be, cfg.ln_eps};
-    epi.xin_img = xin_img;
+  int ln_launch(const uint8_t* hid, const Mlp& m, long long M, const void* res, float* xout, uint8_t* img, uint8_t* yimg, cudaStream_t st) {
+    const Epi2F32Img<true, kRes> epi{res, xout, GC_L, img, GC_NKB, yimg, m.b2, m.g, m.be, cfg.ln_eps};
     return launch_gemm2<256, true>(SchedW<>{AOperand(hid, GC_NKB), m.w2s.img, GC_NKB}, epi, M, GC_L, 1, num_sms, st);
   }
   // xin (fp32 rows) or xin_img (fp16 image) is the residual source; at most one of them
@@ -203,9 +201,9 @@ struct GraphCastEngine : Engine {
     prof_begin(tag, st);
     count_launch();
     int rc;
-    if (xin) rc = ln_launch<1>(hid, m, M, xin, xout, img, yimg, nullptr, st);
-    else if (xin_img) rc = ln_launch<2>(hid, m, M, nullptr, xout, img, yimg, xin_img, st);
-    else rc = ln_launch<0>(hid, m, M, nullptr, xout, img, yimg, nullptr, st);
+    if (xin) rc = ln_launch<1>(hid, m, M, xin, xout, img, yimg, st);
+    else if (xin_img) rc = ln_launch<2>(hid, m, M, xin_img, xout, img, yimg, st);
+    else rc = ln_launch<0>(hid, m, M, nullptr, xout, img, yimg, st);
     prof_end(tag, st);
     if (rc) return rc;
     if (img) if (int r2 = range_scan(0, img, (size_t)(M / 128) * GC_NKB * G2_A_BYTES, st)) return r2;

@@ -1,11 +1,12 @@
-// GraphCast step: device pieces that are not GEMM main loops — epilogue functors for k_gemm2 (gemm2.cuh), the feature
-// builder, the CSR aggregation and small set-up kernels.  Latent width is fixed at 512 (GC_L).
+// GraphCast step: device pieces that are not GEMM main loops — the hidden-layer and output-head epilogue functors for
+// k_gemm2 (gemm2.cuh), the feature builder, the CSR aggregation and small set-up kernels.  Latent width is fixed at 512
+// (GC_L).  The LayerNorm layer of every MLP uses gemm2.cuh's Epi2F32Img on the column-split CTA pairs.
 //
 // Data layout (per member): every latent matrix (grid nodes, mesh nodes, the three edge sets) is an fp16 tile image
 // [rows/128][8][128 x 128 B, SWIZZLE_128B] — byte for byte the A operand of the next GEMM.  Of the three residual streams
 // only the mesh nodes keep an fp32 row-major copy; grid nodes and mesh edges are read-modify-written in their images
-// (EpiGcLn<2>).  Per-node first-layer partial products ("tables": v W1_s^T, v W1_r^T) are fp16 row-major and are gathered
-// by edge index inside the hidden GEMM's epilogue.
+// (Epi2F32Img<true, 2>).  Per-node first-layer partial products ("tables": v W1_s^T, v W1_r^T) are fp16 row-major and are
+// gathered by edge index inside the hidden GEMM's epilogue.
 #pragma once
 #include "gemm2.cuh"
 
@@ -122,195 +123,6 @@ struct EpiGcSiluImg {
             stg_hint(ibase + rr * 128 + (((((col & 63) >> 3) + ch) ^ (rr & 7)) << 4), pk, pol_stream);
         }
         __syncwarp();
-      }
-    }
-  }
-};
-
-// y = LayerNorm(acc + bias) * gamma + beta over the full 512-wide row, then any of
-//   xout[row] = residual + y                  fp32 row-major (ld 512); residual = xin (fp32 rows, may equal xout) or
-//                                             xin_img (the fp16 operand image of the stream, may equal img) or nothing
-//   img       = fp16 tile image of that sum   (the A operand of the next GEMM)
-//   yimg      = fp16 tile image of y itself   (what the aggregation sums: the update BEFORE the residual)
-// Grid-node and mesh-edge latents live ONLY as fp16 images (residual read from xin_img, sum formed in fp32, rounded once
-// into img): their consumers round to fp16 anyway, and the measured cost on the oracle is a tendency error of 7.95e-4
-// instead of 7.66e-4 over 16 layers (tests/test_graphcast_cpu.py); it saves 3 KB of HBM traffic per row and launch.
-// Structure follows Epi2F32Img (gemm2.cuh): statistics in the row-owner domain, then 32x32 blocks re-tiled through the
-// warp's patch so that every global access is a 128-bit access on a full 128-byte row segment.
-// kRes: residual source, a compile-time choice (a run-time branch per load serialised the loads and cost 10 - 50 % of the
-// kernel): 0 none, 1 fp32 rows (xin), 2 the stream's fp16 image (xin_img)
-template <int kRes>
-struct EpiGcLn {
-  static constexpr bool kNeedsBias = true;
-  const float* xin; float* xout; uint8_t* img; uint8_t* yimg;
-  const float* bias; const float* gamma; const float* beta; float eps;
-  const uint8_t* xin_img = nullptr;
-  // residual values of the lane's eight (row, 4-column) pieces of the 32-column group at local column c: all eight
-  // loads are issued before any is used
-  __device__ __forceinline__ void residual8(const EpiCtx& e, int c, int rsub4, int c4, size_t rowoff, long long rows_left, bool on,
-                                            float4 (&x)[8]) const {
-    if constexpr (kRes == 1) {
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const int rr = it * 4 + rsub4;
-        x[it] = (on && rr < rows_left) ? *reinterpret_cast<const float4*>(xin + rowoff + (size_t)rr * GC_L + c) : make_float4(0.f, 0.f, 0.f, 0.f);
-      }
-    } else if constexpr (kRes == 2) {
-      const int col = e.n0 + c + c4 * 4;
-      const uint8_t* base = xin_img + ((size_t)(e.row0 >> 7) * GC_NKB + (col >> 6)) * (size_t)G2_A_BYTES + (uint32_t)(e.row0 & 127) * 128 + (c4 & 1) * 8;
-      const uint32_t chunk = (uint32_t)(col & 63) >> 3;
-      uint2 u[8];
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const int rr = it * 4 + rsub4;
-        u[it] = (on && rr < rows_left) ? *reinterpret_cast<const uint2*>(base + rr * 128 + ((chunk ^ (uint32_t)(rr & 7)) << 4)) : make_uint2(0u, 0u);
-      }
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        const float2 a = __half22float2(*reinterpret_cast<const __half2*>(&u[it].x)), b = __half22float2(*reinterpret_cast<const __half2*>(&u[it].y));
-        x[it] = make_float4(a.x, a.y, b.x, b.y);
-      }
-    } else {
-#pragma unroll
-      for (int it = 0; it < 8; ++it) x[it] = make_float4(0.f, 0.f, 0.f, 0.f);
-    }
-  }
-  template <int BN>
-  __device__ void prefetch(const EpiCtx& e) const {
-    if (kRes == 0) return;
-    const long long row = e.row0 + e.lane;
-    if (row >= e.M) return;
-    if (kRes == 2) {
-      const char* p = reinterpret_cast<const char*>(xin_img) + ((size_t)(e.row0 >> 7) * GC_NKB + (e.n0 >> 6)) * (size_t)G2_A_BYTES +
-                      ((uint32_t)(e.row0 & 127) + e.lane) * 128;
-#pragma unroll
-      for (int i = e.part; i < BN / 64; i += e.nparts) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + (size_t)i * G2_A_BYTES));
-      return;
-    }
-    if (!xin) return;
-    const char* p = reinterpret_cast<const char*>(xin + row * GC_L + e.n0);
-#pragma unroll
-    for (int i = e.part; i < BN * 4 / 128; i += e.nparts) asm volatile("prefetch.global.L2 [%0];" ::"l"(p + i * 128));
-  }
-  template <int BN, class Acc>
-  __device__ void run(Acc& acc, const EpiCtx& e) const {
-    static_assert(BN == GC_L || 2 * BN == GC_L, "the tile is the full latent width, or one half of a column-split CTA pair");
-    constexpr int NG = BN / 32;
-    const int rsub4 = e.lane >> 3, c4 = e.lane & 7;
-    const long long rows_left = e.M - e.row0;
-    const size_t rowoff = (size_t)e.row0 * GC_L + e.n0 + c4 * 4;
-    // residual rows of the first column group: requested before the statistics pass (they come from L2: prefetch())
-    float4 xr[8];
-    residual8(e, e.part * 32, rsub4, c4, rowoff, rows_left, true, xr);
-    float s = 0.f, ss = 0.f;
-    for (int g = e.part; g < NG; g += e.nparts) {
-      float v[32];
-      acc.load32(g * 32, v);
-#pragma unroll
-      for (int j = 0; j < 32; j += 4) {
-        const float4 b = lds_f32x4_ro(e.svec_s + (g * 32 + j) * 4);
-        const float y0 = v[j] + b.x, y1 = v[j + 1] + b.y, y2 = v[j + 2] + b.z, y3 = v[j + 3] + b.w;
-        s += (y0 + y1) + (y2 + y3);
-        ss += (y0 * y0 + y1 * y1) + (y2 * y2 + y3 * y3);
-      }
-    }
-    if (e.nparts > 1) {
-      const uint32_t slot = e.patch_s + e.lane * 8;
-      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(slot), "f"(s), "f"(ss) : "memory");
-      const int q = (int)((e.row0 >> 5) & 3);
-      asm volatile("bar.sync %0, %1;" ::"r"(8 + q), "r"(32 * e.nparts) : "memory");
-      for (int p = 0; p < e.nparts; ++p) {
-        if (p == e.part) continue;
-        float ps, pss;
-        asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ps), "=f"(pss) : "r"(slot + (p - e.part) * 4 * e.patch_stride));
-        s += ps; ss += pss;
-      }
-      asm volatile("bar.sync %0, %1;" ::"r"(8 + q), "r"(32 * e.nparts) : "memory");
-    }
-    if (e.x_own_bar) {
-      // column-split pair: the other half of these rows lives in the peer CTA.  Part 0 posts this CTA's sums into the
-      // peer's slot with st.async (the store itself completes the peer's mbarrier transaction: no fence, no release
-      // arrive), then every warp of the lane quarter waits for the peer's sums in its own slot.
-      if (e.part == 0) {
-        if (e.lane == 0) mbar_arrive_expect_tx(e.x_own_bar, 32 * 8);
-        __syncwarp();
-        asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];" ::"r"(e.x_peer_stat + e.lane * 8),
-                     "f"(s), "f"(ss), "r"(e.x_peer_bar)
-                     : "memory");
-      }
-      mbar_wait(e.x_own_bar, e.x_parity);   // CTA-scope acquire: the peer's sums arrive in THIS CTA's shared memory through st.async, whose completion the barrier phase carries (as for bulk copies); the cluster-scope wait added an L1 invalidate (CCTL.IVALL) per tile
-      float ps, pss;
-      asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ps), "=f"(pss) : "r"(e.x_own_stat + e.lane * 8));
-      s += ps; ss += pss;
-    }
-    float rs[8], ns[8];
-    {
-      const float mean = s / GC_L;
-      const float rstd = rsqrtf(fmaxf(ss / GC_L - mean * mean, 0.f) + eps);
-      const float nmr = -mean * rstd;
-#pragma unroll
-      for (int it = 0; it < 8; ++it) {
-        rs[it] = __shfl_sync(0xffffffffu, rstd, it * 4 + rsub4);
-        ns[it] = __shfl_sync(0xffffffffu, nmr, it * 4 + rsub4);
-      }
-    }
-    const uint32_t r0 = (uint32_t)(e.row0 & 127);
-    const int odd = e.lane & 1;
-    for (int g = e.part; g < NG; g += e.nparts) {
-      const int c = g * 32;
-      float4 xn[8];   // next group's residual rows in flight while this group is normalised and stored
-      residual8(e, c + 32 * e.nparts, rsub4, c4, rowoff, rows_left, g + e.nparts < NG, xn);
-      {
-        float v[32];
-        acc.load32(c, v);
-        patch_put_v(e.patch_s, e.lane, v);
-      }
-      __syncwarp();
-      const float4 bs = lds_f32x4_ro(e.svec_s + (c + c4 * 4) * 4);
-      const float4 ga = lds_f32x4_ro(e.svec_s + (e.vstride + c + c4 * 4) * 4);
-      const float4 be = lds_f32x4_ro(e.svec_s + (2 * e.vstride + c + c4 * 4) * 4);
-      const size_t tile_off = ((size_t)(e.row0 >> 7) * GC_NKB + ((e.n0 + c) >> 6)) * (size_t)G2_A_BYTES + r0 * 128;
-      const uint32_t cb = (((uint32_t)c & 63u) >> 3) + (uint32_t)(c4 >> 1);
-#pragma unroll
-      for (int it2 = 0; it2 < 8; it2 += 2) {
-        uint2 hx[2], hy[2];
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const int it = it2 + u;
-          const int rr = it * 4 + rsub4;
-          const float4 t = lds_f32x4(patchv_addr(e.patch_s, rr, c4));
-          float4 y;
-          y.x = fmaf(fmaf(t.x + bs.x, rs[it], ns[it]), ga.x, be.x); y.y = fmaf(fmaf(t.y + bs.y, rs[it], ns[it]), ga.y, be.y);
-          y.z = fmaf(fmaf(t.z + bs.z, rs[it], ns[it]), ga.z, be.z); y.w = fmaf(fmaf(t.w + bs.w, rs[it], ns[it]), ga.w, be.w);
-          hy[u].x = pack_half2(y.x, y.y); hy[u].y = pack_half2(y.z, y.w);
-          if (kRes) { y.x += xr[it].x; y.y += xr[it].y; y.z += xr[it].z; y.w += xr[it].w; }
-          if (xout && rr < rows_left) *reinterpret_cast<float4*>(xout + rowoff + (size_t)rr * GC_L + c) = y;
-          hx[u].x = pack_half2(y.x, y.y); hx[u].y = pack_half2(y.z, y.w);
-        }
-        // even lane assembles the 16-byte chunk of row it2, odd lane the chunk of row it2 + 1
-        const int rr = (it2 + odd) * 4 + rsub4;
-        const uint32_t coff = rr * 128 + ((cb ^ (uint32_t)(rr & 7)) << 4);
-        if (img) {
-          const uint2 send = odd ? hx[0] : hx[1];
-          uint2 recv;
-          recv.x = __shfl_xor_sync(0xffffffffu, send.x, 1);
-          recv.y = __shfl_xor_sync(0xffffffffu, send.y, 1);
-          const uint4 pk = odd ? make_uint4(recv.x, recv.y, hx[1].x, hx[1].y) : make_uint4(hx[0].x, hx[0].y, recv.x, recv.y);
-          if (rr < rows_left) *reinterpret_cast<uint4*>(img + tile_off + coff) = pk;
-        }
-        if (yimg) {
-          const uint2 send = odd ? hy[0] : hy[1];
-          uint2 recv;
-          recv.x = __shfl_xor_sync(0xffffffffu, send.x, 1);
-          recv.y = __shfl_xor_sync(0xffffffffu, send.y, 1);
-          const uint4 pk = odd ? make_uint4(recv.x, recv.y, hy[1].x, hy[1].y) : make_uint4(hy[0].x, hy[0].y, recv.x, recv.y);
-          if (rr < rows_left) *reinterpret_cast<uint4*>(yimg + tile_off + coff) = pk;
-        }
-      }
-      __syncwarp();
-      if (kRes) {
-#pragma unroll
-        for (int it = 0; it < 8; ++it) xr[it] = xn[it];
       }
     }
   }

@@ -575,8 +575,11 @@ struct PanguEngine : Engine {
   }
   template <bool IMG>
   int run_block_t(float* x, uint8_t* xh, const Geo& g, const BlockW& b, int roll, int B, const Ws& ws, cudaStream_t st) {
-    // projection and fc2: the epilogue runs on the accumulator fragments on the fp16 stream (the fp32 rows stay staged)
-    using ELn = std::conditional_t<IMG, FragEpi<Epi2F32Img<true, true, true>>, Epi2F32Img<true, true, false>>;
+    // projection and fc2: the epilogue runs on the accumulator fragments on the fp16 stream (the fp32 rows stay staged).
+    // Both update the stream in place: the residual is what the epilogue overwrites.
+    using ELn = std::conditional_t<IMG, FragEpi<Epi2F32Img<true, 2>>, Epi2F32Img<true, 1>>;
+    const void* res = IMG ? static_cast<const void*>(xh) : x;
+    float* xout = IMG ? nullptr : x;
     const int C = g.C, nkb = C / 64;
     const long long R = (long long)B * g.T;
     int rc;
@@ -607,7 +610,7 @@ struct PanguEngine : Engine {
     {  // projection + LayerNorm + residual.  At C = 384 a 128 x 384 accumulator would take 192 registers per consumer thread:
        // the two CTAs of a cluster take 192 columns each of the same 128 rows, LayerNorm statistics cross through DSMEM
       AOperand A(ws.atth, nkb);
-      ELn e{x, C, xh, nkb, b.proj_b, b.ln1_g, b.ln1_b, cfg.ln_eps};
+      ELn e{res, xout, C, xh, nkb, nullptr, b.proj_b, b.ln1_g, b.ln1_b, cfg.ln_eps};
       rc = C == 192 ? gemm2<192>(KT_PROJ, A, e, b.proj, R, st) : gemm2<192, true>(KT_PROJ, A, e, b.proj, R, st);
       if (rc) return rc;
     }
@@ -616,7 +619,7 @@ struct PanguEngine : Engine {
       FragEpi<Epi2F16<true, true>> e{reinterpret_cast<__half*>(ws.hidh), 0, 4 * nkb, b.fc1_b};
       if ((rc = gemm2<192>(KT_FC1, A, e, b.fc1, R, st))) return rc;
       AOperand A2(ws.hidh, 4 * nkb);
-      ELn e2{x, C, xh, nkb, b.fc2_b, b.ln2_g, b.ln2_b, cfg.ln_eps};
+      ELn e2{res, xout, C, xh, nkb, nullptr, b.fc2_b, b.ln2_g, b.ln2_b, cfg.ln_eps};
       rc = C == 192 ? gemm2<192>(KT_FC2, A2, e2, b.fc2, R, st) : gemm2<192, true>(KT_FC2, A2, e2, b.fc2, R, st);
       if (rc) return rc;
     }
@@ -665,14 +668,8 @@ struct PanguEngine : Engine {
       count_launch();
       SKY_CUDA_OK(cudaGetLastError());
       AOperand A(ws.hidh, 4 * C / 64);
-      if (img_stream) {
-        Epi2F32Img<false, false, true> e{ws.x2, 2 * C, ws.x2h, 2 * C / 64, nullptr, nullptr, nullptr, 0.f};
-        rc = gemm2<192>(KT_DOWN, A, e, down, R2, st);
-      } else {
-        Epi2F32Img<false, false, false> e{ws.x2, 2 * C, ws.x2h, 2 * C / 64, nullptr, nullptr, nullptr, 0.f};
-        rc = gemm2<192>(KT_DOWN, A, e, down, R2, st);
-      }
-      if (rc) return rc;
+      Epi2F32Img<false, 0> e{nullptr, img_stream ? nullptr : ws.x2, 2 * C, ws.x2h, 2 * C / 64, nullptr, nullptr, nullptr, nullptr, 0.f};
+      if ((rc = gemm2<192>(KT_DOWN, A, e, down, R2, st))) return rc;
       if ((rc = range_scan(3, ws.x2h, (size_t)(R2 / 128) * (2 * C / 64) * G2_A_BYTES, st))) return rc;
     }
     if (stop == 2) return 0;
@@ -687,14 +684,8 @@ struct PanguEngine : Engine {
       Epi2UpShuffle e{ws.hidh, C / 64, C, up_g, up_b, cfg.ln_eps, nullptr, g1.H, g1.W, g2.H, g2.W};
       if ((rc = gemm2<192>(KT_UP, A, e, up1, R2, st))) return rc;
       AOperand A2(ws.hidh, C / 64);
-      if (img_stream) {
-        Epi2F32Img<false, false, true> e2{ws.x1, C, ws.x1h, C / 64, nullptr, nullptr, nullptr, 0.f};
-        rc = gemm2<192>(KT_UP, A2, e2, up2, R1, st);
-      } else {
-        Epi2F32Img<false, false, false> e2{ws.x1, C, ws.x1h, C / 64, nullptr, nullptr, nullptr, 0.f};
-        rc = gemm2<192>(KT_UP, A2, e2, up2, R1, st);
-      }
-      if (rc) return rc;
+      Epi2F32Img<false, 0> e2{nullptr, img_stream ? nullptr : ws.x1, C, ws.x1h, C / 64, nullptr, nullptr, nullptr, nullptr, 0.f};
+      if ((rc = gemm2<192>(KT_UP, A2, e2, up2, R1, st))) return rc;
     }
     if (stop == 5) return 0;
     for (size_t i = 0; i < blocks[3].size(); ++i)

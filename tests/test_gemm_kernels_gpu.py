@@ -758,8 +758,9 @@ def test_gc_out(grid):
 @pytest.mark.parametrize("grid", [0, 2])
 @pytest.mark.parametrize("kres", [0, 1, 2])
 def test_gc_layer_norm_pair(kres, grid):
-    """EpiGcLn on the column-split CTA pairs (256-column halves of the 512-wide latent), in place as the engine runs it:
-    kRes 1 with xin == xout (mesh nodes), kRes 2 with xin_img == img (grid nodes, mesh edges), kRes 0 writing y only"""
+    """Epi2F32Img<true, kRes> on the column-split CTA pairs (256-column halves of the 512-wide latent), in place as
+    GraphCast runs it: kRes 1 with xin == xout (mesh nodes), kRes 2 with xin_img == img (grid nodes, mesh edges), kRes 0
+    writing y only"""
     rng = np.random.default_rng(kres + grid + 31)
     M, N, bn, nkb = 128 * 5 + 17, 512, 256, 2
     K = nkb * 64
