@@ -203,6 +203,28 @@ SKY_API int sky_ensemble_stats(const float* x, int32_t members, int64_t member_s
                        const int32_t* event_sel, const float* event_thr, int32_t n_events, float* stats, float* prob,
                        void* stream);
 
+/* The statistics of sky_ensemble_stats over members pooled from several sources (the members of several models on one
+ * device, each model with its own channel layout):
+ *   n_sources      1..4;  host arrays of n_sources entries:
+ *   x[k]           device pointer of source k: its member j, channel c is the plane x[k] + j * member_stride[k] + c * plane;
+ *   members[k]     >= 1, sum over k at most 64;  member_stride[k] >= channel_count[k] * plane;
+ *   channels       host int32 [n_sources][n_sel]: the plane index, in source k, of selected channel s (z500 is a different
+ *                  plane in every model; a GraphCast state's new slice is reached through x[k] itself);
+ *   quantiles, event_sel, event_thr, stats, prob as for sky_ensemble_stats;
+ *   means          device fp32 [n_sources][n_sel][plane] or NULL: the mean of source k's own members.
+ * Members are pooled in source-then-member order, so one source gives sky_ensemble_stats' results bit for bit, and means[k]
+ * is bitwise sky_ensemble_stats' mean over source k alone.  Same arithmetic, NaN rule, reproducibility and independence of
+ * the channel selection as sky_ensemble_stats.  The kernel's parameter block (the per-member pointer table, the channel
+ * tables, quantiles and events) is 3336 bytes, inside the 4 KB launch-parameter limit.  Refused with SKY_ERR_ARG before
+ * any CUDA call: a count, channel, quantile, event index or threshold out of range, a decreasing event_sel, more than 64
+ * members in all; and before any launch: pointers that are not device memory on one device.  Asynchronous and
+ * stream-ordered; launches on the device that owns the sources. */
+SKY_API int sky_ensemble_stats_multi(int32_t n_sources, const float* const* x, const int32_t* members,
+                             const int64_t* member_stride, const int32_t* channel_count, const int32_t* channels,
+                             int32_t n_sel, int64_t plane, const double* quantiles, int32_t n_q, const int32_t* event_sel,
+                             const float* event_thr, int32_t n_events, float* stats, float* prob, float* means,
+                             void* stream);
+
 /* Per-kernel-family device timing (CUDA events recorded on the launching stream around the
  * launches whose family bit is set in tag_mask).  profile_end synchronises on the recorded
  * events and returns the summed milliseconds and launch counts per family.  Used by bench.py

@@ -1,10 +1,19 @@
 """GlobalEnsemblePrediction — the class /root/reference/skyrim/core/models/ensemble.py:131-133 names and leaves empty: the
-per-step statistics of a perturbed-initial-condition ensemble (``GlobalModel.predict_ensemble``), reduced on the GPU."""
+per-step statistics of a perturbed-initial-condition ensemble (``GlobalModel.predict_ensemble``), reduced on the GPU; and
+GlobalEnsemble (ensemble.py:10-128 there): several models side by side on one GPU, reduced on the device every step."""
 from __future__ import annotations
 
-import numpy as np
+import datetime
+from typing import List
 
-from .base import GlobalPrediction
+import numpy as np
+from loguru import logger
+
+from ... import xr_shim as xr
+from ...common import generate_forecast_id, save_forecast
+from ...engine import ENS_MAX_MEMBERS, ENS_MAX_SOURCES
+from .base import GlobalPrediction, SyntheticDataSource
+from .graphcast import GraphcastModel
 
 
 def quantile_name(q: float) -> str:
@@ -75,3 +84,367 @@ class GlobalEnsemblePrediction:
         i, j = int(np.abs(lats - lat).argmin()), int(np.abs(lons - lon).argmin())
         v = np.asarray(self.stats.values)[n_step, self.statistics.index(statistic), self.channels.index(channel), i, j]
         return float(v)
+
+    def model_mean(self, name: str) -> GlobalPrediction:
+        """the mean of one model's own members (statistic "mean:<name>" of a multi-model ensemble)"""
+        return self._statistic(f"mean:{name}")
+
+
+class SourceView:
+    """Channel-selecting view of a data source: ``view[t]`` is ``source[t]`` restricted to ``channel_names``, in that order.
+    ``Skyrim(name, ic_source=SourceView(ensemble.data_source, names))`` starts one model from exactly the initial condition
+    it gets inside a ``GlobalEnsemble``."""
+
+    def __init__(self, source, channel_names):
+        self.source, self.channel_names = source, list(channel_names)
+
+    def __getitem__(self, t):
+        return self.source[t].sel(channel=self.channel_names)
+
+
+class GlobalEnsemble:
+    """Several models side by side on one GPU, reduced on the device every step (the reference's multi-model mean,
+    ensemble.py:10-128, which runs the models one after the other and averages the last step on the host).
+
+    ``Skyrim("pangu", "graphcast", pangu=dict(cfg=...), device=0)``: a keyword named after a model goes to that model only,
+    every other keyword to all of them.  The models must share one grid.  They start from one atmosphere: a data source
+    over the union of their channels (the first model's channels in its order, then each later model's new ones), which
+    every model reads by name through a ``SourceView``.  The shared channels, the ones every model forecasts, are kept in
+    the first model's order; the mean and the statistics are taken over them."""
+
+    def __init__(self, model_names, ic_source="synthetic", **model_kw):
+        from . import MODELS
+        names = list(model_names)
+        if len(set(names)) != len(names):
+            raise ValueError(f"duplicate model names in {names}")
+        missing = [n for n in names if n not in MODELS]
+        if missing:
+            raise ValueError(f"Invalid model name(s): {missing}")
+        if not 1 <= len(names) <= ENS_MAX_SOURCES:
+            raise ValueError(f"{len(names)} models: a multi-model ensemble holds 1 to {ENS_MAX_SOURCES}")
+        common = {k: v for k, v in model_kw.items() if k not in names}
+        self.model_names, self.ic_source = names, ic_source
+        self.models = []
+        try:
+            for n in names:
+                self.models.append(MODELS[n](ic_source=ic_source, **{**common, **dict(model_kw.get(n, {}))}))
+            first = self.models[0].model.grid
+            for n, m in zip(names[1:], self.models[1:]):
+                g = m.model.grid
+                if not (np.array_equal(g.lat, first.lat) and np.array_equal(g.lon, first.lon)):
+                    raise ValueError(f"{n}'s grid ({len(g.lat)}x{len(g.lon)}) differs from {names[0]}'s "
+                                     f"({len(first.lat)}x{len(first.lon)}): the models must share one grid")
+            self.shared_channels = [c for c in self.models[0].out_channel_names
+                                    if all(c in m.out_channel_names for m in self.models[1:])]
+            if not self.shared_channels:
+                raise ValueError(f"{names} share no output channel")
+        except Exception:
+            self.release_model()
+            raise
+        union = list(self.models[0].in_channel_names)
+        for m in self.models[1:]:
+            union += [c for c in m.in_channel_names if c not in union]
+        self.channel_names = union
+        nlat, nlon = len(first.lat), len(first.lon)
+        if ic_source == "synthetic":
+            self.data_source = SyntheticDataSource(union, nlat, nlon)
+        elif hasattr(ic_source, "__getitem__") and not isinstance(ic_source, str):
+            self.data_source = ic_source
+        else:
+            raise NotImplementedError(f"ic_source='{ic_source}': pass 'synthetic' or a data-source object")
+        for m in self.models:
+            m.data_source = SourceView(self.data_source, m.in_channel_names)
+        self.model_predictions, self.model_paths = {}, {}
+
+    def release_model(self):
+        for m in self.models:
+            m.release_model()
+
+    def __repr__(self) -> str:
+        return f"GlobalEnsemble({self.model_names})"
+
+    @property
+    def time_step(self):
+        return self.models[0].time_step
+
+    def time_steps(self, lead_time: int):
+        return self.models[0].time_steps(lead_time)
+
+    @property
+    def in_channel_names(self):
+        return self.channel_names
+
+    @property
+    def out_channel_names(self):
+        return self.shared_channels
+
+    @property
+    def label(self) -> str:
+        """the model name of the files: the reference's "_".join(sorted(names))"""
+        return "_".join(sorted(self.model_names))
+
+    def predict_one_step(self, start_time: datetime.datetime, initial_condition=None):
+        raise NotImplementedError("a multi-model ensemble steps through rollout / forecast (as the reference's)")
+
+    # -- device states ---------------------------------------------------------------------------------------------------
+    def _layout(self, m):
+        """(state channels, offset of the output slice in the state): a GraphCast state holds two time slices"""
+        if isinstance(m, GraphcastModel):
+            ns = m._cfg.n_state
+            return 2 * ns, ns
+        return len(m.in_channel_names), 0
+
+    def _initial_states(self, start_time):
+        """one (1, C_state, H, W) device state per model, assembled as that model's own rollout assembles it"""
+        import torch
+        states = []
+        for m in self.models:
+            if isinstance(m, GraphcastModel):
+                x = m._initial_fields(start_time)
+                m.model.engine.set_clock(start_time)
+            else:
+                vals = np.asarray(m.data_source[start_time].values, dtype=np.float32)
+                x = torch.from_numpy(np.ascontiguousarray(vals[-1] if vals.ndim == 4 else vals))[None].to(m.model.device)
+            states.append(x.reshape(x.shape[0], -1, *x.shape[-2:]).contiguous())
+        return states
+
+    def _step_all(self, states, first: bool = False):
+        """one step of every model, in turn on the current stream (each engine's persistent kernels fill the GPU)"""
+        import torch
+        for k, m in enumerate(self.models):
+            nxt = torch.empty_like(states[k])
+            if first and m.model.guard_first_step:
+                _, m.model.last_ranges = m.model.engine.step_guarded(states[k], nxt)
+            else:
+                m.model.engine.step(states[k], nxt)
+            states[k] = nxt
+
+    def _outputs(self, states):
+        """each model's newest slice, (B, C_out, H, W) views of the states"""
+        return [x[:, self._layout(m)[1]:] for m, x in zip(self.models, states)]
+
+    def _shared_index(self, channels):
+        return [[m.out_channel_names.index(c) for c in channels] for m in self.models]
+
+    def _model_da(self, k, state, prev, times):
+        """model k's (2, C, H, W) DataArray of the step ending at times[1], as its own rollout returns it"""
+        m, (cs, off) = self.models[k], self._layout(self.models[k])
+        if off:
+            vals = state[0].cpu().numpy().reshape(2, off, *state.shape[-2:])
+        else:
+            vals = np.stack([prev, state[0].cpu().numpy()])
+        return xr.DataArray(vals, dims=["time", "channel", "lat", "lon"],
+                            coords=dict(time=np.array([np.datetime64(t, "s") for t in times]),
+                                        channel=np.array(m.out_channel_names), lat=np.array(m.model.grid.lat),
+                                        lon=np.array(m.model.grid.lon)))
+
+    def _mean_da(self, mean_prev, mean_cur, times, channels):
+        g = self.models[0].model.grid
+        return xr.DataArray(np.stack([mean_prev, mean_cur]), dims=["time", "channel", "lat", "lon"],
+                            coords=dict(time=np.array([np.datetime64(t, "s") for t in times]), channel=np.array(channels),
+                                        lat=np.array(g.lat), lon=np.array(g.lon)))
+
+    # -- deterministic: one member per model ------------------------------------------------------------------------------
+    def rollout(self, start_time: datetime.datetime, n_steps: int = 3, save: bool = True, save_config: dict = {}):
+        """Steps every model from the shared initial condition and reduces the K states after each step with one kernel.
+        Returns (DataArray of the model mean over the shared channels with 2 time slices, paths of the per-step mean files,
+        model "<sorted names joined by _>").  With ``save``, every model also writes its own step files as its rollout
+        would; they are in ``model_paths[name]``.  ``model_predictions[name]`` holds each model's last step."""
+        import torch
+        from ... import engine as E
+        if n_steps < 1:
+            raise ValueError(f"n_steps = {n_steps} must be at least 1")
+        save_config = dict(save_config)
+        save_config.setdefault("forecast_id", generate_forecast_id())
+        filt = list(save_config.get("filter_vars", ()))
+        mean_config = dict(save_config, filter_vars=[c for c in filt if c in self.shared_channels])
+        model_config = {n: dict(save_config, filter_vars=[c for c in filt if c in m.out_channel_names])
+                        for n, m in zip(self.model_names, self.models)}
+        source = self.ic_source if isinstance(self.ic_source, str) else "file"
+        chans = self._shared_index(self.shared_channels)
+        states = self._initial_states(start_time)
+        ring = [E.multi_model_statistics(self._outputs(states), chans, source_means=False)]
+        ring.append(tuple(None if t is None else torch.empty_like(t) for t in ring[0]))
+        prev = [o[0].cpu().numpy() for o in self._outputs(states)]
+        paths, model_paths, mean = [], {n: [] for n in self.model_names}, None
+        t_prev = start_time
+        for n in range(1, n_steps + 1):
+            t_cur = t_prev + self.time_step
+            self._step_all(states, first=n == 1)
+            E.multi_model_statistics(self._outputs(states), chans, source_means=False, out=ring[n % 2])
+            if save or n == n_steps:
+                for k, name in enumerate(self.model_names):
+                    da = self._model_da(k, states[k], prev[k], (t_prev, t_cur))
+                    prev[k] = da.values[1]
+                    self.model_predictions[name] = da
+                    if save:
+                        model_paths[name].append(save_forecast(da, name, t_prev, t_cur, source,
+                                                               config=model_config[name]))
+                mean = self._mean_da(ring[(n - 1) % 2][0][0].cpu().numpy(), ring[n % 2][0][0].cpu().numpy(),
+                                     (t_prev, t_cur), self.shared_channels)
+                if save:
+                    paths.append(save_forecast(mean, self.label, t_prev, t_cur, source, config=mean_config))
+            t_prev, source = t_cur, "file"
+            logger.success(f"Multi-model rollout step {n}/{n_steps} completed")
+        self.model_paths = model_paths
+        return mean, paths
+
+    def forecast(self, start_time: datetime.datetime, n_steps: int = 3, channels: List[str] = []):
+        """(n_steps + 1, channel, lat, lon) model mean over the shared channels (or ``channels``, which must be shared),
+        the first slice being the mean of the initial conditions"""
+        from ... import engine as E
+        sel = list(channels) or self.shared_channels
+        unknown = [c for c in sel if c not in self.shared_channels]
+        if unknown:
+            raise ValueError(f"channel(s) {unknown} are not shared by {self.model_names}")
+        chans = self._shared_index(sel)
+        states = self._initial_states(start_time)
+        means = [E.multi_model_statistics(self._outputs(states), chans, source_means=False)[0][0].cpu().numpy()]
+        for n in range(n_steps):
+            self._step_all(states, first=n == 0)
+            means.append(E.multi_model_statistics(self._outputs(states), chans, source_means=False)[0][0].cpu().numpy())
+            logger.success(f"Multi-model forecast step {n + 1}/{n_steps} completed")
+        g = self.models[0].model.grid
+        times = [start_time + i * self.time_step for i in range(n_steps + 1)]
+        return xr.DataArray(np.stack(means), dims=["time", "channel", "lat", "lon"],
+                            coords=dict(time=np.array([np.datetime64(t, "s") for t in times]), channel=np.array(sel),
+                                        lat=np.array(g.lat), lon=np.array(g.lon)))
+
+    # -- perturbed members ------------------------------------------------------------------------------------------------
+    def predict_ensemble(self, start_time: datetime.datetime, n_steps: int, members: int, perturbation: str = "spherical_grf",
+                         amp: float = 0.05, seed: int = 0, quantiles=(), events: dict = {}, channels: List[str] = [],
+                         save: bool = False, save_config: dict = {}, grf: dict | None = None):
+        """``GlobalModel.predict_ensemble`` over K models with ``members`` members each (K members at most 64 in all).
+
+        The perturbation is drawn once, on the (members, union channels, H, W) initial condition, by ``perturb_ic`` /
+        ``perturb_ic_grf`` (channel ids are union indices; GraphCast's forcing channel has sigma 0).  Member m of every
+        model is gathered from member m of that tensor by channel name, so every model sees the same perturbation of the
+        same variable; GraphCast adds it to both history slices and refills the forcing.  The union starts with the first
+        model's channels in its order, so when the first model is Pangu or FourCastNet-v2 its members are bitwise those of
+        its own ``predict_ensemble`` with the same seed, amplitude and perturbation.  Each step the K engines step in turn
+        and one kernel reduces all K x members; only the statistics are copied to the host, each step's copy under the next
+        step.  ``statistic`` is "mean", "spread", the quantiles, then "mean:<model>" for each model
+        (``GlobalEnsemblePrediction.model_mean``).  ``channels`` and ``events`` must be shared channels.  Files are named
+        "<sorted names joined by _>-ens<M>" and "...-prob"."""
+        import torch
+        from ... import engine as E
+        K, names = len(self.models), self.shared_channels
+        if not 1 <= members or K * members > ENS_MAX_MEMBERS:
+            raise ValueError(f"members = {members} per model: {K} models x members must lie in [1, {ENS_MAX_MEMBERS}]")
+        if n_steps < 1:
+            raise ValueError(f"n_steps = {n_steps} must be at least 1")
+        q = [float(v) for v in quantiles]
+        if len(q) > E.ENS_MAX_QUANTILES or not all(0.0 <= v <= 1.0 for v in q):
+            raise ValueError(f"quantiles {q}: at most {E.ENS_MAX_QUANTILES}, each in [0, 1]")
+        ev = {c: [float(t) for t in np.atleast_1d(thr)] for c, thr in dict(events).items()}
+        filt = list(save_config.get("filter_vars", ()))
+        unknown = [c for c in list(channels) + filt + list(ev) if c not in names]
+        if unknown:
+            raise ValueError(f"channel(s) {unknown} are not shared by {self.model_names}")
+        if not all(np.isfinite(t) for ts in ev.values() for t in ts):
+            raise ValueError(f"event thresholds must be finite: {ev}")
+        if save and save_config.get("file_type", "netcdf") == "zarr":
+            raise ValueError("ensemble statistics are written as netCDF only: the zarr writer holds one variable per "
+                             "forecast id")
+        if perturbation not in ("gaussian", "spherical_grf"):
+            raise ValueError(f"unknown perturbation {perturbation!r} (gaussian, spherical_grf)")
+        if grf and perturbation != "spherical_grf":
+            raise ValueError("grf options need perturbation='spherical_grf'")
+        wanted = set(channels or filt or names) | set(ev)
+        sel = [c for c in names if c in wanted]
+        ev_list = [(i, t) for i, c in enumerate(sel) for t in ev.get(c, ())]
+        if len(sel) > E.ENS_MAX_CHANNELS or len(ev_list) > E.ENS_MAX_EVENTS:
+            raise ValueError(f"{len(sel)} channels and {len(ev_list)} events: at most {E.ENS_MAX_CHANNELS} and "
+                             f"{E.ENS_MAX_EVENTS}")
+        g = self.models[0].model.grid
+        if perturbation == "spherical_grf" and grf is None:
+            grf = dict(lmax=min(180, (len(g.lat) - 1) // 2))
+        states = self.ensemble_members(start_time, members, perturbation, amp, seed, grf)
+        chans = self._shared_index(sel)
+        shapes = ((2 + len(q) + K, len(sel)) + tuple(states[0].shape[-2:]), (len(ev_list),) + tuple(states[0].shape[-2:]))
+
+        def reduce(out):
+            stats, prob = out
+            E.multi_model_statistics(self._outputs(states), chans, q, ev_list,
+                                     out=(stats[:2 + len(q)], prob, stats[2 + len(q):]))
+
+        save_config = {k: v for k, v in save_config.items() if k != "filter_vars"}   # selected on the device already
+        save_config.setdefault("forecast_id", generate_forecast_id())
+        label, source = f"{self.label}-ens{members}", self.ic_source if isinstance(self.ic_source, str) else "file"
+        lat, lon = np.array(g.lat), np.array(g.lon)
+        stat_names = np.array(["mean", "spread"] + [quantile_name(v) for v in q] + [f"mean:{n}" for n in self.model_names])
+        ev_names = np.array([event_name(sel[i], t) for i, t in ev_list])
+        result, paths, prev, t_prev = None, [], None, start_time
+        dev = states[0].device
+        main, copy = torch.cuda.current_stream(dev), torch.cuda.Stream(dev)
+        # EnsembleRunner.iter_stats' pattern over K engines: rings of two device and two pinned host buffers
+        ring = [tuple(torch.empty(s, dtype=torch.float32, device=dev) for s in shapes) for _ in range(2)]
+        host = [tuple(torch.empty(s, dtype=torch.float32).pin_memory() for s in shapes) for _ in range(2)]
+        done = [torch.cuda.Event() for _ in range(2)]
+        copied = torch.cuda.Event()
+        reduce(ring[0])
+        done[0].record(main)
+        for n in range(n_steps + 1):
+            if n < n_steps:   # launch step n + 1 and its reduction before waiting for the copy of step n
+                self._step_all(states, first=n == 0)
+                reduce(ring[(n + 1) % 2])
+                done[(n + 1) % 2].record(main)
+            copy.wait_event(done[n % 2])
+            with torch.cuda.stream(copy):
+                for h, d in zip(host[n % 2], ring[n % 2]):
+                    h.copy_(d, non_blocking=True)
+                copied.record(copy)
+            copied.synchronize()   # also orders the next reduction into ring[n % 2] (launched at n + 1) after this copy
+            s, p = host[n % 2]
+            t_cur = start_time + n * self.time_step
+            if n > 0 and (save or n == n_steps):
+                times = np.array([np.datetime64(t_prev, "s"), np.datetime64(t_cur, "s")])
+                stats = xr.DataArray(np.stack([prev[0], s.numpy()]), dims=["time", "statistic", "channel", "lat", "lon"],
+                                     coords=dict(time=times, statistic=stat_names, channel=np.array(sel), lat=lat, lon=lon))
+                prob = None
+                if ev_list:
+                    prob = xr.DataArray(np.stack([prev[1], p.numpy()]), dims=["time", "event", "lat", "lon"],
+                                        coords=dict(time=times, event=ev_names, lat=lat, lon=lon))
+                if save:
+                    paths.append(save_forecast(stats, label, t_prev, t_cur, source, config=save_config))
+                    if prob is not None:
+                        paths.append(save_forecast(prob, f"{label}-prob", t_prev, t_cur, source, config=save_config))
+                result = GlobalEnsemblePrediction(stats, prob, self.label, K * members)
+            if n > 0:
+                source = "file"
+                logger.success(f"Multi-model ensemble step {n}/{n_steps} completed")
+            prev, t_prev = (s.numpy().copy(), p.numpy().copy()), t_cur
+        return result, paths
+
+    def ensemble_members(self, start_time: datetime.datetime, members: int, perturbation: str = "spherical_grf",
+                         amp: float = 0.05, seed: int = 0, grf: dict | None = None):
+        """The perturbed initial states ``predict_ensemble`` steps: one (members, C_state, H, W) device tensor per model
+        (a GraphCast state holds both slices)."""
+        import torch
+        from ...engine import perturb_ic, perturb_ic_grf
+        from ...weights import channel_stats
+        dev = self.models[0].model.device
+        base = torch.from_numpy(np.ascontiguousarray(np.asarray(self.data_source[start_time].values, dtype=np.float32)))
+        base = base.to(dev)
+        sigma = channel_stats(self.channel_names)[1].copy()
+        for m in self.models:
+            if isinstance(m, GraphcastModel):
+                sigma[self.channel_names.index(m.out_channel_names[m._cfg.n_state - 1])] = 0.0   # the toa forcing
+        sigma = torch.as_tensor(sigma, device=dev)
+        x = base[None].repeat(members, 1, 1, 1).contiguous()
+        if perturbation == "gaussian":
+            perturb_ic(x, sigma, amp, seed=seed)
+        else:
+            perturb_ic_grf(x, sigma, amp, seed=seed, **(grf or {}))
+        states = []
+        for m in self.models:
+            idx = torch.tensor([self.channel_names.index(c) for c in m.in_channel_names], device=dev)
+            xm = x.index_select(1, idx)
+            if isinstance(m, GraphcastModel):
+                # the same perturbation on both history slices: slice 0 = source[t - 6 h] + (member - source[t])
+                prev = torch.from_numpy(np.asarray(m.data_source[start_time - m.time_step].values, dtype=np.float32))
+                s0 = prev.to(dev)[None] + (xm - base.index_select(0, idx)[None])
+                xm = m.model.fill_forcing(torch.stack([s0, xm], 1), start_time)
+                m.model.engine.set_clock(start_time)
+            states.append(xm.reshape(members, -1, *xm.shape[-2:]).contiguous())
+        return states

@@ -8,6 +8,7 @@ from loguru import logger
 
 from .models import MODELS
 from .models.base import GlobalModel, GlobalPrediction, adjust_lead_time
+from .models.ensemble import GlobalEnsemble
 
 
 class Skyrim:
@@ -15,13 +16,15 @@ class Skyrim:
         missing_names = [name for name in model_names if name not in MODELS]
         if missing_names:
             raise ValueError(f"Invalid model name(s): {missing_names}")
-        if len(model_names) != 1:
-            # the reference's multi-model mean (ensemble.py:10-133) is broken at HEAD and out of scope;
-            # perturbed-IC ensembles of ONE model live in skyrim_b200.ensemble
-            raise NotImplementedError("exactly one model name is supported; see skyrim_b200.ensemble")
+        if not model_names:
+            raise NotImplementedError("give at least one model name")
         self.model_names = model_names
         self.ic_source = ic_source
-        self.model: GlobalModel = MODELS[model_names[0]](ic_source=ic_source, **model_kw)
+        if len(model_names) > 1:
+            # the reference's GlobalEnsemble (ensemble.py:10-128): every model on this GPU, reduced on the device
+            self.model: GlobalModel | GlobalEnsemble = GlobalEnsemble(model_names, ic_source=ic_source, **model_kw)
+        else:
+            self.model = MODELS[model_names[0]](ic_source=ic_source, **model_kw)
         logger.debug(f"Initialized {self.model} model with initial conditions from {ic_source}")
 
     def __repr__(self) -> str:
@@ -51,7 +54,8 @@ class Skyrim:
     def predict_ensemble(self, date: str, time: str, lead_time: int = 6, members: int = 4, **kw):
         """Perturbed-initial-condition ensemble forecast reduced to per-step statistics on the GPU: the date, time and lead
         time are read as ``predict`` reads them, ``kw`` goes to ``GlobalModel.predict_ensemble`` (perturbation, amp, seed,
-        quantiles, events, channels, save, save_config, grf).  Returns (GlobalEnsemblePrediction, paths)."""
+        quantiles, events, channels, save, save_config, grf); with several models, to ``GlobalEnsemble.predict_ensemble``
+        (``members`` per model).  Returns (GlobalEnsemblePrediction, paths)."""
         start_time = datetime.datetime(int(date[:4]), int(date[4:6]), int(date[6:8]), int(time[:2]), int(time[2:4]))
         n_steps = self.model.time_steps(lead_time)
         logger.debug(f"Ensemble of {members} members, {n_steps} steps")

@@ -13,6 +13,8 @@
 // each member's load is coalesced.  Quantiles come from a fully unrolled bitonic network (min / max on registers only);
 // the QUANT = false instantiation skips it.  No atomics: each output is one thread's fixed-order computation, so results
 // are bitwise reproducible and a channel's outputs do not depend on which other channels are selected.
+// k_ens_stats_multi pools the members of up to four models (sources) with their own channel layouts and also writes
+// each model's own mean; the per-point reduction is the same code.
 #include <algorithm>
 #include <cmath>
 
@@ -38,16 +40,32 @@ struct EnsStatsParams {
   float ev_thr[kMaxEvents];
 };
 
-template <int MP, bool QUANT>
-__global__ void __launch_bounds__(kThreads) k_ens_stats(const __grid_constant__ EnsStatsParams P) {
-  const long long p = (long long)blockIdx.x * kThreads + threadIdx.x;
-  if (p >= P.plane) return;
-  const int s = blockIdx.y, M = P.members;
-  const float* xp = P.x + (long long)P.chan[s] * P.plane + p;
-  float v[MP];
-#pragma unroll
-  for (int m = 0; m < MP; ++m) v[m] = m < M ? xp[m * P.member_stride] : __int_as_float(0x7f800000);
+constexpr int kMaxSources = 4;
 
+// sky_ensemble_stats_multi's block: the fields reduce_point reads carry EnsStatsParams' names
+struct MultiStatsParams {
+  const float* member[kMaxMembers];      // member m's (source base + j member_stride), source-then-member order
+  float* stats;
+  float* prob;
+  float* means;                          // [n_src][n_sel][plane], or null
+  long long plane;
+  int members, n_sel, n_q, n_events, n_src;
+  int src_members[kMaxSources];
+  unsigned char member_src[kMaxMembers];
+  int chan[kMaxSources][kMaxSel];
+  int q_lo[kMaxQ], q_hi[kMaxQ];
+  double q_g[kMaxQ];
+  int ev_sel[kMaxEvents];
+  float ev_thr[kMaxEvents];
+};
+// 3336 bytes: inside the 4 KB every sm_90 launch accepts without the large-parameter path
+static_assert(sizeof(MultiStatsParams) == 3336, "keep the header comment of sky_ensemble_stats_multi in step");
+
+// The statistics of one (selected channel s, point p) from its members v[0, M), padded to MP with +inf.  Shared by both
+// kernels: P is either parameter block (same field names), v is sorted in place when QUANT.
+template <int MP, bool QUANT, class Params>
+__device__ __forceinline__ void reduce_point(float (&v)[MP], const Params& P, int s, long long p) {
+  const int M = P.members;
   double sum = 0.0;
   bool nan = false;
 #pragma unroll
@@ -100,10 +118,77 @@ __global__ void __launch_bounds__(kThreads) k_ens_stats(const __grid_constant__ 
   }
 }
 
+template <int MP, bool QUANT>
+__global__ void __launch_bounds__(kThreads) k_ens_stats(const __grid_constant__ EnsStatsParams P) {
+  const long long p = (long long)blockIdx.x * kThreads + threadIdx.x;
+  if (p >= P.plane) return;
+  const int s = blockIdx.y, M = P.members;
+  const float* xp = P.x + (long long)P.chan[s] * P.plane + p;
+  float v[MP];
+#pragma unroll
+  for (int m = 0; m < MP; ++m) v[m] = m < M ? xp[m * P.member_stride] : __int_as_float(0x7f800000);
+  reduce_point<MP, QUANT>(v, P, s, p);
+}
+
+// Several sources (models) pooled: member m (source-then-member order) starts at member[m], a pointer of the host's table,
+// and its selected channel s is the plane chan[member_src[m]][s] of its own source.  v[] is indexed by unrolled constants
+// only, so it stays in registers.  With means set, the mean of each source's own members, summed in member order (the
+// arithmetic of k_ens_stats over that source alone), goes to means[k][s][p]; it is taken before reduce_point sorts v.
+template <int MP, bool QUANT>
+__global__ void __launch_bounds__(kThreads) k_ens_stats_multi(const __grid_constant__ MultiStatsParams P) {
+  const long long p = (long long)blockIdx.x * kThreads + threadIdx.x;
+  if (p >= P.plane) return;
+  const int s = blockIdx.y, M = P.members;
+  float v[MP];
+#pragma unroll
+  for (int m = 0; m < MP; ++m)
+    v[m] = m < M ? P.member[m][(long long)P.chan[P.member_src[m]][s] * P.plane + p] : __int_as_float(0x7f800000);
+  if (P.means) {
+#pragma unroll
+    for (int k = 0; k < kMaxSources; ++k) {
+      if (k >= P.n_src) break;
+      double sum = 0.0;
+#pragma unroll
+      for (int m = 0; m < MP; ++m)
+        if (m < M && P.member_src[m] == k) sum = __dadd_rn(sum, (double)v[m]);
+      P.means[((long long)k * P.n_sel + s) * P.plane + p] = (float)__ddiv_rn(sum, (double)P.src_members[k]);
+    }
+  }
+  reduce_point<MP, QUANT>(v, P, s, p);
+}
+
 template <int MP>
 void launch(const EnsStatsParams& P, dim3 grid, cudaStream_t st) {
   if (P.n_q > 0) k_ens_stats<MP, true><<<grid, kThreads, 0, st>>>(P);
   else k_ens_stats<MP, false><<<grid, kThreads, 0, st>>>(P);
+}
+
+template <int MP>
+void launch(const MultiStatsParams& P, dim3 grid, cudaStream_t st) {
+  if (P.n_q > 0) k_ens_stats_multi<MP, true><<<grid, kThreads, 0, st>>>(P);
+  else k_ens_stats_multi<MP, false><<<grid, kThreads, 0, st>>>(P);
+}
+
+// quantile positions and events, checked and stored the way both entry points need them
+template <class Params>
+int set_quantiles_events(Params& P, int members, int n_sel, const double* quantiles, int n_q, const int32_t* event_sel,
+                         const float* event_thr, int n_events) {
+  for (int q = 0; q < n_q; ++q) {
+    const double v = quantiles[q];
+    if (!(v >= 0.0 && v <= 1.0)) { set_error("quantile %g is outside [0, 1]", v); return SKY_ERR_ARG; }
+    const double h = (double)(members - 1) * v, lo = std::floor(h);
+    P.q_lo[q] = (int)lo;
+    P.q_hi[q] = std::min((int)lo + 1, members - 1);
+    P.q_g[q] = h - lo;
+  }
+  for (int e = 0; e < n_events; ++e) {
+    if (event_sel[e] < 0 || event_sel[e] >= n_sel) { set_error("event_sel[%d] = %d is outside [0, %d)", e, event_sel[e], n_sel); return SKY_ERR_ARG; }
+    if (e > 0 && event_sel[e] < event_sel[e - 1]) { set_error("event_sel decreases at %d", e); return SKY_ERR_ARG; }
+    if (!std::isfinite(event_thr[e])) { set_error("event threshold %d is not finite", e); return SKY_ERR_ARG; }
+    P.ev_sel[e] = event_sel[e];
+    P.ev_thr[e] = event_thr[e];
+  }
+  return 0;
 }
 
 int device_ptr(const void* p, const char* what, int* dev) {
@@ -149,23 +234,10 @@ int sky_ensemble_stats(const float* x, int32_t members, int64_t member_stride, i
     if (channels[s] < 0 || channels[s] >= channel_count) { set_error("channel %d is outside [0, %d)", channels[s], channel_count); return SKY_ERR_ARG; }
     P.chan[s] = channels[s];
   }
-  for (int q = 0; q < n_q; ++q) {
-    const double v = quantiles[q];
-    if (!(v >= 0.0 && v <= 1.0)) { set_error("quantile %g is outside [0, 1]", v); return SKY_ERR_ARG; }
-    const double h = (double)(members - 1) * v, lo = std::floor(h);
-    P.q_lo[q] = (int)lo;
-    P.q_hi[q] = std::min((int)lo + 1, members - 1);
-    P.q_g[q] = h - lo;
-  }
-  for (int e = 0; e < n_events; ++e) {
-    if (event_sel[e] < 0 || event_sel[e] >= n_sel) { set_error("event_sel[%d] = %d is outside [0, %d)", e, event_sel[e], n_sel); return SKY_ERR_ARG; }
-    if (e > 0 && event_sel[e] < event_sel[e - 1]) { set_error("event_sel decreases at %d", e); return SKY_ERR_ARG; }
-    if (!std::isfinite(event_thr[e])) { set_error("event threshold %d is not finite", e); return SKY_ERR_ARG; }
-    P.ev_sel[e] = event_sel[e];
-    P.ev_thr[e] = event_thr[e];
-  }
+  int rc;
+  if ((rc = set_quantiles_events(P, members, n_sel, quantiles, n_q, event_sel, event_thr, n_events))) return rc;
   if (!x || !stats || (n_events && !prob)) { set_error("x, stats and (with events) prob must not be null"); return SKY_ERR_ARG; }
-  int dev = -1, rc;
+  int dev = -1;
   if ((rc = device_ptr(x, "x", &dev)) || (rc = device_ptr(stats, "stats", &dev)) ||
       (n_events && (rc = device_ptr(prob, "prob", &dev))))
     return rc;
@@ -178,6 +250,79 @@ int sky_ensemble_stats(const float* x, int32_t members, int64_t member_stride, i
   if (members <= 8) launch<8>(P, grid, st);
   else if (members <= 16) launch<16>(P, grid, st);
   else if (members <= 32) launch<32>(P, grid, st);
+  else launch<64>(P, grid, st);
+  count_launch();
+  SKY_CUDA_OK(cudaGetLastError());
+  return SKY_OK;
+}
+
+int sky_ensemble_stats_multi(int32_t n_sources, const float* const* x, const int32_t* members, const int64_t* member_stride,
+                             const int32_t* channel_count, const int32_t* channels, int32_t n_sel, int64_t plane,
+                             const double* quantiles, int32_t n_q, const int32_t* event_sel, const float* event_thr,
+                             int32_t n_events, float* stats, float* prob, float* means, void* stream) {
+  if (n_sources < 1 || n_sources > kMaxSources || !x || !members || !member_stride || !channel_count) {
+    set_error("n_sources = %d must lie in [1, %d], with x, members, member_stride and channel_count given", n_sources, kMaxSources);
+    return SKY_ERR_ARG;
+  }
+  if (plane < 1) { set_error("plane = %lld must be positive", (long long)plane); return SKY_ERR_ARG; }
+  int total = 0;
+  for (int k = 0; k < n_sources; ++k) {
+    if (members[k] < 1 || members[k] > kMaxMembers) { set_error("members[%d] = %d must lie in [1, %d]", k, members[k], kMaxMembers); return SKY_ERR_ARG; }
+    total += members[k];
+    if (channel_count[k] < 1) { set_error("channel_count[%d] = %d must be positive", k, channel_count[k]); return SKY_ERR_ARG; }
+    if (member_stride[k] < (int64_t)channel_count[k] * plane) {
+      set_error("member_stride[%d] = %lld is below channel_count x plane = %lld", k, (long long)member_stride[k],
+                (long long)channel_count[k] * plane);
+      return SKY_ERR_ARG;
+    }
+  }
+  if (total > kMaxMembers) { set_error("total members = %d exceed %d", total, kMaxMembers); return SKY_ERR_ARG; }
+  if (n_sel < 1 || n_sel > kMaxSel || !channels) { set_error("n_sel = %d channels must lie in [1, %d]", n_sel, kMaxSel); return SKY_ERR_ARG; }
+  if (n_q < 0 || n_q > kMaxQ || (n_q && !quantiles)) { set_error("n_q = %d quantiles must lie in [0, %d]", n_q, kMaxQ); return SKY_ERR_ARG; }
+  if (n_events < 0 || n_events > kMaxEvents || (n_events && (!event_sel || !event_thr))) {
+    set_error("n_events = %d events must lie in [0, %d]", n_events, kMaxEvents);
+    return SKY_ERR_ARG;
+  }
+  MultiStatsParams P{};
+  P.plane = plane;
+  P.members = total;
+  P.n_sel = n_sel;
+  P.n_q = n_q;
+  P.n_events = n_events;
+  P.n_src = n_sources;
+  for (int k = 0; k < n_sources; ++k) {
+    P.src_members[k] = members[k];
+    for (int s = 0; s < n_sel; ++s) {
+      const int c = channels[k * n_sel + s];
+      if (c < 0 || c >= channel_count[k]) { set_error("channel %d of source %d is outside [0, %d)", c, k, channel_count[k]); return SKY_ERR_ARG; }
+      P.chan[k][s] = c;
+    }
+  }
+  int rc;
+  if ((rc = set_quantiles_events(P, total, n_sel, quantiles, n_q, event_sel, event_thr, n_events))) return rc;
+  for (int k = 0; k < n_sources; ++k)
+    if (!x[k]) { set_error("x[%d] must not be null", k); return SKY_ERR_ARG; }
+  if (!stats || (n_events && !prob)) { set_error("stats and (with events) prob must not be null"); return SKY_ERR_ARG; }
+  int dev = -1;
+  for (int k = 0; k < n_sources; ++k)
+    if ((rc = device_ptr(x[k], "x[k]", &dev))) return rc;
+  if ((rc = device_ptr(stats, "stats", &dev)) || (n_events && (rc = device_ptr(prob, "prob", &dev))) ||
+      (means && (rc = device_ptr(means, "means", &dev))))
+    return rc;
+  for (int k = 0, m = 0; k < n_sources; ++k)
+    for (int j = 0; j < members[k]; ++j, ++m) {
+      P.member[m] = x[k] + j * member_stride[k];
+      P.member_src[m] = (unsigned char)k;
+    }
+  P.stats = stats;
+  P.prob = prob;
+  P.means = means;
+  DeviceGuard guard(dev);
+  const dim3 grid((unsigned)((plane + kThreads - 1) / kThreads), (unsigned)n_sel);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (total <= 8) launch<8>(P, grid, st);
+  else if (total <= 16) launch<16>(P, grid, st);
+  else if (total <= 32) launch<32>(P, grid, st);
   else launch<64>(P, grid, st);
   count_launch();
   SKY_CUDA_OK(cudaGetLastError());

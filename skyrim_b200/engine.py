@@ -309,6 +309,7 @@ def perturb_ic_grf(x, sigma_c, amp: float, seed: int, member0: int = 0, alpha: f
 
 
 ENS_MAX_MEMBERS, ENS_MAX_CHANNELS, ENS_MAX_QUANTILES, ENS_MAX_EVENTS = 64, 128, 8, 64
+ENS_MAX_SOURCES = 4
 
 
 def ensemble_statistics(x, channels=None, quantiles=(), events=(), channel_offset: int = 0, out=None):
@@ -347,6 +348,56 @@ def ensemble_statistics(x, channels=None, quantiles=(), events=(), channel_offse
                                     arr(C.c_float, ev_thr), len(ev_sel), stats.data_ptr(),
                                     prob.data_ptr() if prob.numel() else None, st), "sky_ensemble_stats", L)
     return stats, prob
+
+
+def multi_model_statistics(sources, channels_per_source, quantiles=(), events=(), source_means: bool = True, out=None):
+    """``ensemble_statistics`` over the members of up to four sources pooled in source-then-member order
+    (include/skyrim_b200.h sky_ensemble_stats_multi).  ``sources``: CUDA fp32 (M_k, C_k, H, W) tensors or views whose
+    members each hold contiguous (C_k, H, W) planes, sum of M_k at most 64 (a GraphCast state's new slice is the view
+    ``state.view(M, 166, H, W)[:, 83:]``); ``channels_per_source[k]`` lists, for every selected channel, its index in
+    source k; ``events`` as for ``ensemble_statistics``.  Returns (stats (2 + n_q, n_sel, H, W), prob (n_events, H, W),
+    means (K, n_sel, H, W): the mean of each source's own members, or None without ``source_means``), into ``out`` =
+    (stats, prob, means) when given.  Asynchronous on the current stream."""
+    import torch
+    K = len(sources)
+    if not 1 <= K <= ENS_MAX_SOURCES or len(channels_per_source) != K:
+        raise ValueError(f"{K} sources with {len(channels_per_source)} channel lists: 1 to {ENS_MAX_SOURCES} sources, one "
+                         "list each")
+    H, W = sources[0].shape[2:]
+    plane = H * W
+    for x in sources:
+        if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and tuple(x.shape[2:]) == (H, W)):
+            raise ValueError("each source must be a CUDA fp32 (members, channels, nlat, nlon) tensor on one grid")
+        if x.stride(3) != 1 or x.stride(2) != W or x.stride(1) != plane:
+            raise ValueError(f"each member of a source must hold contiguous (C, H, W) planes (strides {x.stride()})")
+    sel = [[int(c) for c in chans] for chans in channels_per_source]
+    n_sel = len(sel[0])
+    if any(len(c) != n_sel for c in sel):
+        raise ValueError("every source must list the same number of channels")
+    q = [float(v) for v in quantiles]
+    ev_sel, ev_thr = [int(i) for i, _ in events], [float(t) for _, t in events]
+    shapes = ((2 + len(q), n_sel, H, W), (len(ev_sel), H, W), (K, n_sel, H, W))
+    if out is None:
+        out = tuple(torch.empty(s, dtype=torch.float32, device=sources[0].device) for s in shapes)
+        if not source_means:
+            out = out[:2] + (None,)
+    stats, prob, means = out
+    for t, s in zip(out, shapes):
+        if t is not None and (tuple(t.shape) != s or t.dtype != torch.float32 or not t.is_contiguous()):
+            raise ValueError(f"output of shape {tuple(t.shape)} {t.dtype}: contiguous fp32 {s} needed")
+    arr = lambda ct, v: (ct * max(len(v), 1))(*v)  # noqa: E731
+    members = [x.shape[0] for x in sources]
+    strides = [x.stride(0) if x.shape[0] > 1 else max(x.stride(0), x.shape[1] * plane) for x in sources]
+    L = _ffi.lib()
+    st = torch.cuda.current_stream(sources[0].device).cuda_stream
+    _ffi.check(L.sky_ensemble_stats_multi(K, arr(C.c_void_p, [x.data_ptr() for x in sources]), arr(C.c_int32, members),
+                                          arr(C.c_int64, strides), arr(C.c_int32, [x.shape[1] for x in sources]),
+                                          arr(C.c_int32, [c for chans in sel for c in chans]), n_sel, plane,
+                                          arr(C.c_double, q), len(q), arr(C.c_int32, ev_sel), arr(C.c_float, ev_thr),
+                                          len(ev_sel), stats.data_ptr(), prob.data_ptr() if prob.numel() else None,
+                                          means.data_ptr() if means is not None else None, st),
+               "sky_ensemble_stats_multi", L)
+    return stats, prob, means
 
 
 def unix_seconds(when) -> float:

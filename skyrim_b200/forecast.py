@@ -3,9 +3,11 @@ defaults; same `run_forecast` signature and return value) on top of the H100 eng
 
     python -m skyrim_b200.forecast -m pangu -d 20240507 -t 0000 -l 24 -o outputs
     python -m skyrim_b200.forecast -m pangu -l 24 --members 8 --quantiles 0.1,0.5,0.9 --exceed t2m:273.15 -o outputs
+    python -m skyrim_b200.forecast --models pangu,fourcastnet_v2,graphcast -l 24 --members 4 -o outputs
 
 The second form runs a perturbed-initial-condition ensemble and saves its per-step statistics (mean, spread, quantiles)
-and exceedance probabilities instead of the members.
+and exceedance probabilities instead of the members.  The third runs several models side by side on one GPU
+(``GlobalEnsemble``): with ``--members 1`` it saves every model's steps and their mean, above 1 the pooled statistics.
 
 Differences, all forced by the scope of this build (SURVEY.md section 2): `--initial_conditions` accepts `synthetic`
 (the default here: the network IC providers cds / ifs / gfs are the reference's `libs/ic`, out of scope, and raise a clear
@@ -32,7 +34,8 @@ def run_forecast(model_name: str, date: str, time: str, lead_time: int, list_mod
         return []
     logger.debug(f"Starting forecast run with model_name={model_name}, date={date}, time={time}, lead_time={lead_time}, "
                  f"initial_conditions={initial_conditions}, output_dir={output_dir}, filter_vars={filter_vars}")
-    model = Skyrim(model_name, ic_source=initial_conditions, **model_kw)
+    names = [model_name] if isinstance(model_name, str) else list(model_name)
+    model = Skyrim(*names, ic_source=initial_conditions, **model_kw)
     pred, output_paths = model.predict(
         date=date, time=time, lead_time=lead_time, save=True,
         save_config={"output_dir": output_dir or str(Path.cwd() / "outputs"),
@@ -45,7 +48,8 @@ def run_ensemble_forecast(model_name: str, date: str, time: str, lead_time: int,
                           events: dict = {}, **model_kw):
     """``--members`` > 1: ``Skyrim.predict_ensemble(save=True)``; returns the statistics and probability file paths"""
     from .core import Skyrim
-    model = Skyrim(model_name, ic_source=initial_conditions, **model_kw)
+    names = [model_name] if isinstance(model_name, str) else list(model_name)
+    model = Skyrim(*names, ic_source=initial_conditions, **model_kw)
     _, paths = model.predict_ensemble(
         date=date, time=time, lead_time=lead_time, members=members, perturbation=perturbation, amp=amp, seed=seed,
         quantiles=quantiles, events=events, save=True,
@@ -93,8 +97,10 @@ def parse_exceed(text: str):
 @click.option("--seed", type=int, default=0, help="Perturbation seed")
 @click.option("--quantiles", type=str, default="", help="Ensemble quantiles such as 0.1,0.5,0.9")
 @click.option("--exceed", type=str, default="", help="Exceedance events channel:threshold such as t2m:273.15,u10m:15")
+@click.option("--models", type=str, default="",
+              help="Several models side by side on one GPU, such as pangu,graphcast (replaces -m); --members counts per model")
 def main(model_name, date, time, lead_time, list_models, initial_conditions, output_dir, filter_vars, modal, weight_seed, device, grid,
-         members, perturbation, amp, seed, quantiles, exceed):
+         members, perturbation, amp, seed, quantiles, exceed, models):
     if modal:
         raise click.UsageError("--modal: remote execution through Modal is outside this build (SURVEY.md section 2); run locally")
     if not 1 <= members <= 64:
@@ -106,11 +112,22 @@ def main(model_name, date, time, lead_time, list_models, initial_conditions, out
     if members == 1 and (q or events):
         raise click.UsageError("--quantiles and --exceed describe an ensemble: give --members > 1")
     kw = {"weight_seed": weight_seed, "device": device}
+    names = [v.strip() for v in models.split(",") if v.strip()]
+    unknown = [n for n in names if n not in AVAILABLE_MODELS]
+    if unknown or len(set(names)) != len(names) or len(names) == 1 or len(names) * members > 64:
+        raise click.UsageError(f"--models {models}: two to four distinct models of {AVAILABLE_MODELS}, at most 64 members "
+                               "in all")
     if grid:
         from .config import graphcast_small, pangu_small, sfno_small
         nlat, nlon = (int(v) for v in grid.lower().split("x"))
-        kw["cfg"] = (pangu_small(nlat, nlon) if model_name == "pangu" else graphcast_small(nlat, nlon) if model_name == "graphcast"
-                     else sfno_small(nlat, nlon))
+        small = lambda n: (pangu_small(nlat, nlon) if n == "pangu" else graphcast_small(nlat, nlon) if n == "graphcast"  # noqa: E731
+                           else sfno_small(nlat, nlon))
+        if names:
+            kw.update({n: dict(cfg=small(n)) for n in names})
+        else:
+            kw["cfg"] = small(model_name)
+    if names:
+        model_name = names
     if members > 1 and not list_models:
         paths = run_ensemble_forecast(model_name, date, time, lead_time, initial_conditions, output_dir, filter_vars, members,
                                       perturbation, amp, seed, q, events, **kw)
