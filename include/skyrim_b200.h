@@ -143,8 +143,8 @@ SKY_API int sky_model_debug_copy(sky_model_t* m, const char* what, float* dst, u
 /* Switches of a handle (never read from the environment).  "fp32_stream" = 1 (Pangu) keeps the token stream as fp32 rows beside
  * its fp16 operand image instead of the default image-only stream: 1.1 ms per step slower, one rounding per residual add less
  * (DESIGN.md section 3).  Test taps: "stop_after" = n makes step() return after
- * stage n (0 embed, 1 layer0, 2 down, 3 layer1, 4 layer2, 5 up, 6 layer3; 99 = run the whole step) so that
- * sky_model_debug_copy can read the intermediate token buffers. */
+ * stage n (Pangu: 0 embed, 1 layer0, 2 down, 3 layer1, 4 layer2, 5 up, 6 layer3; SFNO: 0 encoder, 1 + i block i;
+ * 99 = run the whole step) so that sky_model_debug_copy can read the intermediate buffers. */
 SKY_API int sky_model_debug_set(sky_model_t* m, const char* key, int64_t value);
 
 /* x[m, c, :, :] += amp * sigma[c] * N(0,1), Philox4x32-10 keyed by (seed, member0 + m):

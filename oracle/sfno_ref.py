@@ -65,7 +65,14 @@ class SFNORef:
     def _inorm(self, x, g, b):
         return F.instance_norm(x[None], weight=g, bias=b, eps=self.cfg.eps)[0]
 
-    def block(self, x, i):
+    def _inorm_affine(self, x, g, b):
+        """(scale, shift) of the instance norm with affine: norm(x) = scale * x + shift per channel (biased variance)"""
+        mean = x.mean(dim=(1, 2))
+        var = ((x - mean[:, None, None]) ** 2).mean(dim=(1, 2))
+        sc = g / torch.sqrt(var + self.cfg.eps)
+        return sc, b - mean * sc
+
+    def block(self, x, i, taps=None):
         cfg, w = self.cfg, self.w
         p = f"blk{i}."
         tin = "big" if i == 0 else "int"
@@ -78,22 +85,71 @@ class SFNORef:
         y = self.isht(Xo, tout)
         y = y + self._conv1x1(residual, w[p + "inner.w"], w[p + "inner.b"])
         y = F.gelu(y)
+        g = y
         y = self._inorm(y, w[p + "norm1.g"], w[p + "norm1.b"])
         hdn = F.gelu(self._conv1x1(y, w[p + "fc1.w"], w[p + "fc1.b"]))
         y = self._conv1x1(hdn, w[p + "fc2.w"], w[p + "fc2.b"])
-        return y + residual
+        out = y + residual
+        if taps is not None:
+            self._block_taps(taps, f"b{i}.", x, X, Xo, g, hdn, out, i, tin, tout)
+        return out
+
+    def _block_taps(self, taps, k, x, X, Xo, g, hdn, out, i, tin, tout):
+        """the block's intermediates in the engine's layouts (skyrim_b200/csrc/sfno_engine.cu header): pixel-major fields
+        [pixel][channel], spectra [l][m][(ri, c)] / [m][l][(ro, o)], DFT rows [m][lat][(ri, c)], [lat][(m, ro)][o]"""
+        w, p = self.w, f"blk{i}."
+        ri = lambda z, dim: torch.cat([z.real, z.imag], dim=dim)
+        pm = lambda f: f.reshape(f.shape[0], -1).T.contiguous()
+        sc, sh = self._inorm_affine(x, w[p + "norm0.g"], w[p + "norm0.b"])
+        taps[k + "norm0"] = torch.cat([sc, sh])
+        xn = x * sc[:, None, None] + sh[:, None, None]
+        f = 2.0 * np.pi * torch.fft.rfft(xn, dim=-1, norm="forward")[..., : self.cfg.mmax]      # (c, lat, m)
+        taps[k + "li"] = ri(f.permute(2, 1, 0), 2)                                               # [m][lat][(ri, c)]
+        taps[k + "si"] = ri(X.permute(1, 2, 0), 2)                                               # [l][m][(ri, c)]
+        if tin == tout:
+            taps[k + "mi"] = ri(Xo.permute(2, 1, 0), 2)                                          # [m][l][(ro, o)]
+            taps[k + "inner_bias"] = w[p + "inner.b"] + w[p + "inner.w"] @ sh
+            taps[k + "f1"] = pm(self.isht(Xo, tout))
+        else:   # the engine folds the inner skip into the mixing matrices: its mixing output is (W_l + V) X
+            taps[k + "mi"] = ri((Xo + torch.einsum("oi,ilm->olm", w[p + "inner.w"].to(X.dtype), X)).permute(2, 1, 0), 2)
+            taps[k + "mi2"] = ri(X.permute(2, 1, 0), 2)
+            taps[k + "rpm"] = pm(self.isht(X, tout))
+            Xo = Xo + torch.einsum("oi,ilm->olm", w[p + "inner.w"].to(X.dtype), X)
+        t = self.tabs[tout]
+        d = torch.einsum("mkl,clm->ckm", t["inv"].to(self.cd), Xo)                               # (o, lat, m)
+        taps[k + "di"] = ri(d.permute(1, 2, 0)[:, :, None, :], 2).reshape(d.shape[1], -1, d.shape[0])  # [lat][(m, ro)][o]
+        taps[k + "g"] = pm(g)
+        taps[k + "sums"] = torch.cat([pm(g).sum(0), (pm(g) ** 2).sum(0)])
+        n1sc, n1sh = self._inorm_affine(g, w[p + "norm1.g"], w[p + "norm1.b"])
+        taps[k + "norm1"] = torch.cat([n1sc, n1sh])
+        taps[k + "fc1_bias"] = w[p + "fc1.b"] + w[p + "fc1.w"] @ n1sh
+        taps[k + "hidden"] = pm(hdn)
+        taps[k + "x"] = pm(out)
+        d = pm(out) - w[p + "fc2.b"]    # the engine gathers the statistics about the bias of the epilogue that writes x
+        taps[k + "sums0"] = torch.cat([d.sum(0), (d ** 2).sum(0)])
 
     @torch.no_grad()
-    def step(self, state):
-        """(73, nlat, nlon) de-normalised -> (73, nlat, nlon) de-normalised."""
+    def step(self, state, taps=None):
+        """(73, nlat, nlon) de-normalised -> (73, nlat, nlon) de-normalised.  ``taps``: a dict that receives every
+        intermediate the engine exposes through debug_copy, in its layouts (``_block_taps``): "in" (normalised input),
+        "enc.hidden", "enc.x", "enc.sums0", "b{i}.*" per block, "dec.hidden"."""
         w = self.w
         x = torch.as_tensor(state).to(self.dtype)
         xh = (x - w["norm.mean"][:, None, None]) / w["norm.std"][:, None, None]
         y = F.gelu(self._conv1x1(xh, w["enc.fc1.w"], w["enc.fc1.b"]))
+        if taps is not None:
+            pm = lambda f: f.reshape(f.shape[0], -1).T.contiguous()
+            taps["in"], taps["enc.hidden"] = pm(xh), pm(y)
         y = self._conv1x1(y, w["enc.fc2.w"], w["enc.fc2.b"]) + w["pos_embed"]
+        if taps is not None:
+            taps["enc.x"] = pm(y)
+            d = pm(y) - w["enc.fc2.b"]
+            taps["enc.sums0"] = torch.cat([d.sum(0), (d ** 2).sum(0)])
         for i in range(self.cfg.layers):
-            y = self.block(y, i)
+            y = self.block(y, i, taps)
         y = torch.cat([y, xh], 0)
         y = F.gelu(self._conv1x1(y, w["dec.fc1.w"], w["dec.fc1.b"]))
+        if taps is not None:
+            taps["dec.hidden"] = pm(y)
         y = self._conv1x1(y, w["dec.fc2.w"], w["dec.fc2.b"])
         return y * w["norm.std"][:, None, None] + w["norm.mean"][:, None, None]

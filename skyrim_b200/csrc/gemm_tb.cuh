@@ -227,7 +227,10 @@ struct EpiGeluStatsImg {
 // x_out = acc + bias[col] + addend, where addend = asc[col] * add[pixel][col] + ash[col] (the outer skip: norm0 of the block
 // input, evaluated on the fly) or plain add[pixel][col] (positional embedding, resampled residual).  Writes the fp32 state
 // (the next block's skip source), its hi / lo pixel image (the next block's transform data and inner-skip operand, or the
-// decoder's input) and per-channel sum / sum of squares (the next block's norm0) in one pass.
+// decoder's input) and per-channel sum / sum of squares (the next block's norm0) in one pass.  With stat_shift set, the
+// statistics are those of x_out - stat_shift[col]: the variance comes from E[d^2] - E[d]^2, which cancels catastrophically
+// when |mean| >> std, so the engine passes the bias, which carries a channel's constant offset (k_finalize_norm adds the
+// shift back to the mean).
 struct EpiF32ImgStats {
   static constexpr bool kNeedsBias = false;
   static constexpr bool kCtaStats = true;   // n_valid <= CTA_STATS_MAX
@@ -237,6 +240,7 @@ struct EpiF32ImgStats {
   const float* add; const float* asc; const float* ash;   // add may be null; asc / ash null = plain addend
   double* sums;                                           // may be null (last block: no norm follows)
   int n_valid;
+  const float* stat_shift = nullptr;                      // per column, may be null: the statistics are of x_out - shift
   template <int BN, class Acc>
   __device__ void run(Acc& acc, const EpiCtx& x) const {
     const int rsub = x.lane >> 2, ch = x.lane & 3;
@@ -254,12 +258,16 @@ struct EpiF32ImgStats {
           a1[it] = __ldg(reinterpret_cast<const float4*>(ap + 4));
         }
       }
-      float bb[8], sc[8];
+      float bb[8], sc[8], sb[8];   // sb: the statistics' shift
 #pragma unroll
-      for (int e = 0; e < 8; ++e) { bb[e] = 0.f; sc[e] = 1.f; }
+      for (int e = 0; e < 8; ++e) { bb[e] = 0.f; sc[e] = 1.f; sb[e] = 0.f; }
       if (cols_ok) {
         const float4 b0 = __ldg(reinterpret_cast<const float4*>(bias + col)), b1 = __ldg(reinterpret_cast<const float4*>(bias + col + 4));
         bb[0] = b0.x; bb[1] = b0.y; bb[2] = b0.z; bb[3] = b0.w; bb[4] = b1.x; bb[5] = b1.y; bb[6] = b1.z; bb[7] = b1.w;
+        if (stat_shift) {
+          const float4 t0 = __ldg(reinterpret_cast<const float4*>(stat_shift + col)), t1 = __ldg(reinterpret_cast<const float4*>(stat_shift + col + 4));
+          sb[0] = t0.x; sb[1] = t0.y; sb[2] = t0.z; sb[3] = t0.w; sb[4] = t1.x; sb[5] = t1.y; sb[6] = t1.z; sb[7] = t1.w;
+        }
         if (asc) {
           const float4 s0 = __ldg(reinterpret_cast<const float4*>(asc + col)), s1 = __ldg(reinterpret_cast<const float4*>(asc + col + 4));
           const float4 h0 = __ldg(reinterpret_cast<const float4*>(ash + col)), h1 = __ldg(reinterpret_cast<const float4*>(ash + col + 4));
@@ -290,7 +298,8 @@ struct EpiF32ImgStats {
           for (int e = 0; e < 8; ++e) {
             f[e] = f[e] + fmaf(av[e], sc[e], bb[e]);
             h[e] = __float2half_rn(f[e]); l[e] = __float2half_rn(f[e] - __half2float(h[e]));
-            s[e] += f[e]; q[e] = fmaf(f[e], f[e], q[e]);
+            const float d = f[e] - sb[e];
+            s[e] += d; q[e] = fmaf(d, d, q[e]);
           }
           if (out) {
             float* op = out + (size_t)p * ld + col;

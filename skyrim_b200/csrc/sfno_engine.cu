@@ -27,13 +27,14 @@ namespace sky {
 static inline int pad_to(int x, int m) { return (x + m - 1) / m * m; }
 
 // ======================================================================================
-// generic re-indexing pack: fp32 tensor -> hi / lo fp16 tile images (+ optional fp32 copy)
-//   dest element (batch b, row r = r1*R0 + r0, col k), rows < rows_valid, k < k_valid
-//   source offset = b*s_b + r1*s_r1 + r0*s_r0 + (k>>1)*s_kh + (k&1)*s_kl
+// transposing pack: fp32 tensor -> hi / lo fp16 tile images
+//   dest element (batch b, row r = r1*R0 + r0, col k), r0 < R0, k < k_valid (columns up to Kp are zero)
+//   source offset = b*s_b + r1*s_r1 + r0*s_r0 + (k>>1)*s_kh + (k&1)*s_kl, contiguous along r0 (s_r0 == 1)
 //   value = affine(act(v)):  act: 0 none, 1 GELU ;  affine: y*sc[i] + sh[i], i by aff_mode
 //           (0 none, 1 r1, 2 k)
-// thread order: digits (chunk, r0, r1, batch) peeled from the linear thread id in the order
-// given by `ord` (fastest first) so that the SOURCE side is read coalesced.
+// A block moves a 32 (r0) x 64 (k) tile through shared memory, so the reads are 128-byte coalesced along r0 and every
+// image row receives its 64 k-values as one 128-byte run (hi) + one (lo).  Used for the state input (channel-major
+// (C, lat, lon) -> pixel image with the input normalisation).
 // ======================================================================================
 struct PackDesc {
   const float* src;
@@ -43,73 +44,15 @@ struct PackDesc {
   int rows_pad;                  // rows per batch in the image (multiple of 128)
   const float* sc; const float* sh; int aff_mode; int act;
   uint8_t* hi; uint8_t* lo;      // images [batch][rows_pad/128][Kp/64][16 KB]
-  float* f32; long long f32_ld;  // optional fp32 row-major copy of the transformed values (batch 0 only)
-  int ord[4];                    // permutation of {0: chunk, 1: r0, 2: r1, 3: batch}
 };
 
-__global__ void __launch_bounds__(256) k_pack_img(PackDesc d, long long total) {
-  long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= total) return;
-  const int ext[4] = {d.Kp / 8, d.R0, d.R1, d.batches};
-  int dig[4];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const int w = d.ord[i];
-    dig[w] = (int)(t % ext[w]);
-    t /= ext[w];
-  }
-  const int chunk = dig[0], r0 = dig[1], r1 = dig[2], b = dig[3];
-  const long long r = (long long)r1 * d.R0 + r0;
-  const long long base = (long long)b * d.s_b + (long long)r1 * d.s_r1 + (long long)r0 * d.s_r0;
-  float v[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    const int k = chunk * 8 + e;
-    float x = 0.f;
-    if (k < d.k_valid) {
-      x = d.src[base + (long long)(k >> 1) * d.s_kh + (long long)(k & 1) * d.s_kl];
-      if (d.act == 1) x = gelu_erf(x);
-      if (d.aff_mode == 1) x = x * d.sc[r1] + d.sh[r1];
-      else if (d.aff_mode == 2) x = x * d.sc[k] + d.sh[k];
-    }
-    v[e] = x;
-  }
-  if (d.f32 && b == 0) {
-#pragma unroll
-    for (int e = 0; e < 8; ++e)
-      if (chunk * 8 + e < d.k_valid) d.f32[r * d.f32_ld + chunk * 8 + e] = v[e];
-  }
-  __half h[8], l[8];
-#pragma unroll
-  for (int e = 0; e < 8; ++e) {
-    h[e] = __float2half_rn(v[e]);
-    l[e] = __float2half_rn(v[e] - __half2float(h[e]));
-  }
-  const int nkb = d.Kp / 64;
-  const size_t off = (size_t)b * (d.rows_pad / 128) * nkb * G2_A_BYTES + ((size_t)(r >> 7) * nkb + (chunk >> 3)) * G2_A_BYTES +
-                     sw128_offset((uint32_t)(r & 127), chunk & 7);
-  *reinterpret_cast<uint4*>(d.hi + off) = *reinterpret_cast<uint4*>(h);
-  *reinterpret_cast<uint4*>(d.lo + off) = *reinterpret_cast<uint4*>(l);
-}
-
-// Tiled variant for the packs that TRANSPOSE (the source is contiguous along a row index, not along k): a block moves a
-// 32 (source-contiguous index d) x 64 (k) tile through shared memory, so the reads are 128-byte coalesced along d and
-// every image row receives its 64 k-values as one 128-byte run (hi) + one (lo).  FAST selects which index is d:
-//   1 = r0, 2 = r1, 3 = batch, 4 = (batch, r0) combined (r0 fastest; s_b == R0 * s_r0, e.g. (m, re/im))
-// The generic kernel above wrote 16-byte chunks 128..2048 bytes apart and ran at ~1.8 TB/s (profiles/r2_sfno.md).
-template <int FAST>
 __global__ void __launch_bounds__(256) k_pack_tile(PackDesc d, int ext_d, int n_kb) {
   __shared__ float tile[32][65];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;
   const int dt = blockIdx.x / n_kb, kb = blockIdx.x % n_kb;
   const int y = blockIdx.y;
   // decode (b, r1, r0) of element dd of this tile
-  auto coords = [&](int dd, int& b, int& r1, int& r0) {
-    if (FAST == 1) { r0 = dd; r1 = y % d.R1; b = y / d.R1; }
-    else if (FAST == 2) { r1 = dd; r0 = y % d.R0; b = y / d.R0; }
-    else if (FAST == 3) { b = dd; r0 = y % d.R0; r1 = y / d.R0; }
-    else { b = dd / d.R0; r0 = dd % d.R0; r1 = y; }
-  };
+  auto coords = [&](int dd, int& b, int& r1, int& r0) { r0 = dd; r1 = y % d.R1; b = y / d.R1; };
   {
     const int dd = dt * 32 + tx;
     int b, r1, r0;
@@ -199,10 +142,6 @@ __global__ void __launch_bounds__(256) k_pack_w3(WPackDesc d, long long total) {
   *reinterpret_cast<uint4*>(base + (size_t)(nkb + kb) * tile_bytes + o) = *reinterpret_cast<uint4*>(l);
 }
 
-// per-column sums of (optionally GELU'd) fp32 [P, E]:  sums[c], sums[E + c]  (instance norm).
-// Block = 32 lanes x 8 row-lanes; a lane owns FOUR consecutive columns (128-bit loads: a warp reads 512 contiguous
-// bytes of a row), strides over its rows, the 8 partials of a column meet in shared memory, one fp64 atomic per
-// (block, column).  E % 4 == 0.
 // Grid-changing blocks (first: 721x1440 -> 240x480, last: back): the inner skip acts on residual = iSHT(X), X the block's
 // own forward spectrum, and a 1x1 convolution commutes with the (linear, per-channel) inverse transform:
 //   iSHT(W_l X) + V iSHT(X) = iSHT((W_l + V) X)
@@ -213,45 +152,16 @@ __global__ void k_fold_inner_into_spec(float* __restrict__ spec, const float* __
   if (i < total) spec[2 * i] += inner[i % EE];
 }
 
-__global__ void __launch_bounds__(256) k_colstats(const float* __restrict__ x, long long P, int E, int act,
-                                                  double* __restrict__ sums, int rows_per_block) {
-  __shared__ float4 red[2][8][33];
-  const int cx = threadIdx.x & 31, ry = threadIdx.x >> 5;
-  const long long r0 = (long long)blockIdx.y * rows_per_block;
-  const int c = (blockIdx.x * 32 + cx) * 4;
-  float4 s = make_float4(0.f, 0.f, 0.f, 0.f), ss = s;
-  if (c < E) {
-    long long rend = r0 + rows_per_block;
-    if (rend > P) rend = P;
-#pragma unroll 4
-    for (long long r = r0 + ry; r < rend; r += 8) {
-      float4 v = __ldg(reinterpret_cast<const float4*>(x + r * E + c));
-      if (act) { v.x = gelu_erf(v.x); v.y = gelu_erf(v.y); v.z = gelu_erf(v.z); v.w = gelu_erf(v.w); }
-      s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
-      ss.x += v.x * v.x; ss.y += v.y * v.y; ss.z += v.z * v.z; ss.w += v.w * v.w;
-    }
-  }
-  red[0][ry][cx] = s; red[1][ry][cx] = ss;
-  __syncthreads();
-  if (ry == 0 && c < E) {
-    float4 a = make_float4(0.f, 0.f, 0.f, 0.f), b = a;
-#pragma unroll
-    for (int i = 0; i < 8; ++i) {
-      const float4 u = red[0][i][cx], w = red[1][i][cx];
-      a.x += u.x; a.y += u.y; a.z += u.z; a.w += u.w; b.x += w.x; b.y += w.y; b.z += w.z; b.w += w.w;
-    }
-    atomicAdd(&sums[c], (double)a.x); atomicAdd(&sums[c + 1], (double)a.y); atomicAdd(&sums[c + 2], (double)a.z); atomicAdd(&sums[c + 3], (double)a.w);
-    atomicAdd(&sums[E + c], (double)b.x); atomicAdd(&sums[E + c + 1], (double)b.y); atomicAdd(&sums[E + c + 2], (double)b.z); atomicAdd(&sums[E + c + 3], (double)b.w);
-  }
-}
-// sc = gamma * rstd, sh = beta - mean * sc
-__global__ void k_finalize_norm(const double* __restrict__ sums, const float* __restrict__ g,
+// sc = gamma * rstd, sh = beta - mean * sc.  sums: per-channel sum and sum of squares of x - shift[c] (shift may be null:
+// the statistics of x itself); the variance does not depend on the shift, the mean gets it back.
+__global__ void k_finalize_norm(const double* __restrict__ sums, const float* __restrict__ shift, const float* __restrict__ g,
                                 const float* __restrict__ b, float eps, long long P, int E, float* __restrict__ sc,
                                 float* __restrict__ sh) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= E) return;
-  const double mean = sums[c] / (double)P;
-  const double var = fmax(sums[E + c] / (double)P - mean * mean, 0.0);
+  const double md = sums[c] / (double)P;
+  const double var = fmax(sums[E + c] / (double)P - md * md, 0.0);
+  const double mean = shift ? (double)shift[c] + md : md;
   const float s = g[c] * (float)(1.0 / sqrt(var + (double)eps));
   sc[c] = s;
   sh[c] = b[c] - (float)mean * s;
@@ -351,6 +261,7 @@ struct SfnoEngine : Engine {
   float *n0_sc = nullptr, *n0_sh = nullptr;       // norm0 scale / shift of the current block (n_sc / n_sh: norm1)
   float *t1_big = nullptr, *t1_int = nullptr;     // row sums of the forward DFT tables
   double* sums0 = nullptr;                        // statistics of the NEXT block's input, gathered by the epilogue that writes it
+  const float* sums0_shift = nullptr;             // ... about that epilogue's bias (EpiF32ImgStats)
   std::vector<Blk> blk;
   const float *mean, *stdv, *enc1_b, *enc2_b, *dec1_b, *dec2_b;
   float* pos_pm = nullptr;  // [P1, E]
@@ -362,6 +273,7 @@ struct SfnoEngine : Engine {
   // spectral-chain data images: LI [m][lat][(ri,c)], SI [l][m][(ri,c)], MI / MI2 [m][l][(ro,o)], DI [lat][(m,ro)][o]
   Img2 LI, SI, MI, MI2, DI;
   bool scratch_ready = false;
+  const float* x_tap = nullptr;   // fp32 state of the last stage run (debug_copy "x"); null where only the image is kept
 
   SfnoEngine(const sky_sfno_config_t& c, int dev) : cfg(c) {
     device = dev;
@@ -540,39 +452,19 @@ struct SfnoEngine : Engine {
   // ---- helpers -------------------------------------------------------------------------
   int pack(int tag, const float* src, Img2& im, int batches, int R1, int R0, int k_valid, long long s_b, long long s_r1,
            long long s_r0, long long s_kh, long long s_kl, int aff_mode, const float* sc, const float* sh, int act,
-           int o0, int o1, int o2, int o3, cudaStream_t st, float* f32 = nullptr, long long f32_ld = 0) {
+           cudaStream_t st) {
     PackDesc d;
     d.src = src; d.s_b = s_b; d.s_r1 = s_r1; d.s_r0 = s_r0; d.s_kh = s_kh; d.s_kl = s_kl;
     d.R0 = R0; d.R1 = R1; d.batches = batches; d.k_valid = k_valid; d.Kp = pad_to(k_valid, 64);
     d.rows_pad = pad_to(R1 * R0, 128);
-    d.sc = sc; d.sh = sh; d.aff_mode = aff_mode; d.act = act; d.hi = im.hi; d.lo = im.lo; d.f32 = f32; d.f32_ld = f32_ld;
-    d.ord[0] = o0; d.ord[1] = o1; d.ord[2] = o2; d.ord[3] = o3;
+    d.sc = sc; d.sh = sh; d.aff_mode = aff_mode; d.act = act; d.hi = im.hi; d.lo = im.lo;
     const size_t need = (size_t)batches * (d.rows_pad / 128) * (d.Kp / 64) * G2_A_BYTES;
     if (need > im.bytes) { set_error("internal: image buffer too small (%zu > %zu)", need, im.bytes); return SKY_ERR_STATE; }
-    const long long total = (long long)batches * R1 * R0 * (d.Kp / 8);
-    prof_begin(tag, st);
-    // choose the tiled (transposing) kernel when the source is contiguous along a row index rather than along k
+    const long long ny = (long long)batches * R1;
+    if (s_r0 != 1 || ny > 65535) { set_error("internal: pack source must be contiguous along r0 (s_r0 %lld, %lld row groups)", s_r0, ny); return SKY_ERR_STATE; }
     const int n_kb = d.Kp / 64;
-    const bool k_contig = s_kh == 2 && s_kl == 1;
-    int fast = 0, ext = 0; long long ny = 0;
-    if (!k_contig && !f32) {
-      if (s_r0 == 1 && R0 >= 32) { fast = 1; ext = R0; ny = (long long)batches * R1; }
-      else if (s_r1 == 1 && R1 >= 32) { fast = 2; ext = R1; ny = (long long)batches * R0; }
-      else if (s_b == 1 && batches >= 32) { fast = 3; ext = batches; ny = (long long)R1 * R0; }
-      else if (s_r0 == 1 && s_b == R0 && batches * R0 >= 32) { fast = 4; ext = batches * R0; ny = R1; }
-      if (ny > 65535) fast = 0;
-    }
-    if (fast) {
-      dim3 grid((unsigned)(((ext + 31) / 32) * n_kb), (unsigned)ny);
-      switch (fast) {
-        case 1: k_pack_tile<1><<<grid, 256, 0, st>>>(d, ext, n_kb); break;
-        case 2: k_pack_tile<2><<<grid, 256, 0, st>>>(d, ext, n_kb); break;
-        case 3: k_pack_tile<3><<<grid, 256, 0, st>>>(d, ext, n_kb); break;
-        default: k_pack_tile<4><<<grid, 256, 0, st>>>(d, ext, n_kb); break;
-      }
-    } else {
-      k_pack_img<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(d, total);
-    }
+    prof_begin(tag, st);
+    k_pack_tile<<<dim3((unsigned)(((R0 + 31) / 32) * n_kb), (unsigned)ny), 256, 0, st>>>(d, R0, n_kb);
     prof_end(tag, st);
     count_launch();
     SKY_CUDA_OK(cudaGetLastError());
@@ -624,19 +516,6 @@ struct SfnoEngine : Engine {
     if (gelu) { EpiSplitImg<true> e{out.hi, out.lo, Nout / 64, bias, w.N}; return gemm_epi(tag, A, nkb, 0, e, w, rows, st); }
     EpiSplitImg<false> e{out.hi, out.lo, Nout / 64, bias, w.N};
     return gemm_epi(tag, A, nkb, 0, e, w, rows, st);
-  }
-
-  int norm_stats(const float* x, long long P, int act, const float* g, const float* b, cudaStream_t st) {
-    prof_begin(KT_SFNO_MISC, st);
-    SKY_CUDA_OK(cudaMemsetAsync(sums, 0, 2 * E * sizeof(double), st));
-    const int rpb = 256;
-    dim3 grid((unsigned)((E / 4 + 31) / 32), (unsigned)((P + rpb - 1) / rpb));
-    k_colstats<<<grid, 256, 0, st>>>(x, P, E, act, sums, rpb);
-    k_finalize_norm<<<(E + 127) / 128, 128, 0, st>>>(sums, g, b, cfg.eps, P, E, n_sc, n_sh);
-    prof_end(KT_SFNO_MISC, st);
-    count_launch(2);
-    SKY_CUDA_OK(cudaGetLastError());
-    return 0;
   }
 
   // ---- spherical transforms: table x data GEMMs (gemm_tb.cuh) ----
@@ -716,7 +595,7 @@ struct SfnoEngine : Engine {
     // norm0 of the block input: its statistics were gathered by the epilogue that wrote xin (encoder fc2 / previous fc2);
     // the affine is applied behind the forward DFT, inside the inner skip's weights and inside the outer skip's addend
     prof_begin(KT_SFNO_MISC, st);
-    k_finalize_norm<<<(E + 127) / 128, 128, 0, st>>>(sums0, b.n0g, b.n0b, cfg.eps, Pi, E, n0_sc, n0_sh);
+    k_finalize_norm<<<(E + 127) / 128, 128, 0, st>>>(sums0, sums0_shift, b.n0g, b.n0b, cfg.eps, Pi, E, n0_sc, n0_sh);
     count_launch();
     prof_end(KT_SFNO_MISC, st);
     if (Hi == Ho) {
@@ -750,7 +629,7 @@ struct SfnoEngine : Engine {
     }
     // norm1 folded into fc1:  fc1(norm1(g)) = (W1 diag(sc)) g + (W1 sh + b1)
     prof_begin(KT_SFNO_MISC, st);
-    k_finalize_norm<<<(E + 127) / 128, 128, 0, st>>>(sums, b.n1g, b.n1b, cfg.eps, Po, E, n_sc, n_sh);
+    k_finalize_norm<<<(E + 127) / 128, 128, 0, st>>>(sums, nullptr, b.n1g, b.n1b, cfg.eps, Po, E, n_sc, n_sh);
     count_launch();
     if ((rc = fold_norm(b.fc1, fc1_bs, b.fc1_w, b.fc1_b, Hd, E, n_sc, n_sh, st))) return rc;
     prof_end(KT_SFNO_MISC, st);
@@ -763,8 +642,9 @@ struct SfnoEngine : Engine {
     {
       const bool same = Hi == Ho;
       EpiF32ImgStats e{i + 1 < L ? xout : nullptr, E, I_x.hi, I_x.lo, E / 64, b.fc2_b, same ? xin : Rpm, same ? n0_sc : nullptr, same ? n0_sh : nullptr,
-                       i + 1 < L ? sums0 : nullptr, E};
+                       i + 1 < L ? sums0 : nullptr, E, b.fc2_b};
       if ((rc = gemm_epi(KT_SFNO_MLP, I_a, Hd / 64, 0, e, b.fc2, Po, st))) return rc;
+      sums0_shift = b.fc2_b;
     }
     if (range_guard) {   // fp16 (hi) operand images this block produced: pixel images, hidden image, spectral images
       if ((rc = range_scan(4, I_x.hi, (size_t)(Po / 128) * (E / 64) * G2_A_BYTES, st))) return rc;
@@ -782,17 +662,25 @@ struct SfnoEngine : Engine {
   int step_one(const float* x_in, float* x_out, cudaStream_t st) {
     int rc;
     // encoder
-    if ((rc = pack(KT_SFNO_ENC, x_in, I_in, 1, 1, (int)P1, Cin, 0, 0, 1, 2LL * P1, P1, 2, in_sc, in_sh, 0, 1, 0, 2, 3, st))) return rc;
+    if ((rc = pack(KT_SFNO_ENC, x_in, I_in, 1, 1, (int)P1, Cin, 0, 0, 1, 2LL * P1, P1, 2, in_sc, in_sh, 0, st))) return rc;
     if ((rc = gemm_to_img(KT_SFNO_ENC, I_in, Cin, P1, I_a, E, enc1_b, true, enc1, st))) return rc;   // GELU(fc1) -> split images
     SKY_CUDA_OK(cudaMemsetAsync(sums0, 0, 2 * E * sizeof(double), st));
     {   // + positional embedding; fp32 state, pixel image and the first block's norm0 statistics from one epilogue
       // (the fp32 copy is only read by an unchanged-grid first block's outer skip, i.e. when there is a single block)
-      EpiF32ImgStats e{L > 1 ? nullptr : X, E, I_x.hi, I_x.lo, E / 64, enc2_b, pos_pm, nullptr, nullptr, sums0, E};
+      EpiF32ImgStats e{L > 1 ? nullptr : X, E, I_x.hi, I_x.lo, E / 64, enc2_b, pos_pm, nullptr, nullptr, sums0, E, enc2_b};
       if ((rc = gemm_epi(KT_SFNO_ENC, I_a, E / 64, 0, e, enc2, P1, st))) return rc;
+      sums0_shift = enc2_b;
     }
+    // test tap (sky_model_debug_set "stop_after"): 0 returns after the encoder, 1 + i after block i, so that debug_copy
+    // reads that stage's buffers
+    x_tap = L > 1 ? nullptr : X;
+    if (stop_after == 0) return 0;
     float *a = X, *b = Xn;
-    for (int i = 0; i < L; ++i)
+    for (int i = 0; i < L; ++i) {
       if ((rc = run_block(i, a, b, st))) return rc;
+      x_tap = i + 1 < L ? a : nullptr;   // run_block swapped: a is the block output
+      if (stop_after == 1 + i) return 0;
+    }
     // decoder on concat(x, normalised input): x is already there as the last fc2's pixel image
     {
       const int kx = E / 64, ki = pad_to(Cin, 64) / 64;
@@ -822,8 +710,45 @@ struct SfnoEngine : Engine {
       SKY_CUDA_OK(cudaMemcpyAsync(dst, range_dev, 8 * sizeof(float), cudaMemcpyDeviceToDevice, st));
       return 0;
     }
-    set_error("unknown debug buffer '%s'", what);
-    return SKY_ERR_ARG;
+    // stage taps (after a step with debug_set "stop_after"; they show the last member stepped).  Operand images are copied
+    // as raw bytes, hi image then lo image (whole allocations: the tile layouts are in the header comment); fp32 buffers as
+    // they are; the fp64 statistics (sums, then sums of squares) as bytes.
+    struct Part { const void* p; size_t bytes; };
+    Part parts[2] = {{nullptr, 0}, {nullptr, 0}};
+    const Img2* im = nullptr;
+    const size_t pe = (size_t)P1 * E * sizeof(float);
+    if (!strcmp(what, "in_img")) im = &I_in;
+    else if (!strcmp(what, "x_img")) im = &I_x;
+    else if (!strcmp(what, "g_img")) im = &I_b;
+    else if (!strcmp(what, "hidden_img")) im = &I_a;
+    else if (!strcmp(what, "li")) im = &LI;
+    else if (!strcmp(what, "si")) im = &SI;
+    else if (!strcmp(what, "mi")) im = &MI;
+    else if (!strcmp(what, "mi2")) im = &MI2;
+    else if (!strcmp(what, "di")) im = &DI;
+    else if (!strcmp(what, "x")) {
+      if (!x_tap) { set_error("no fp32 state is kept after this stage (the last block and a multi-block encoder write the image only)"); return SKY_ERR_STATE; }
+      parts[0] = {x_tap, pe};
+    }
+    else if (!strcmp(what, "rpm")) parts[0] = {Rpm, pe};
+    else if (!strcmp(what, "f1")) parts[0] = {F1, pe};
+    else if (!strcmp(what, "norm0")) { parts[0] = {n0_sc, E * sizeof(float)}; parts[1] = {n0_sh, E * sizeof(float)}; }
+    else if (!strcmp(what, "norm1")) { parts[0] = {n_sc, E * sizeof(float)}; parts[1] = {n_sh, E * sizeof(float)}; }
+    else if (!strcmp(what, "fc1_bias")) parts[0] = {fc1_bs, (size_t)cfg.mlp_ratio * E * sizeof(float)};
+    else if (!strcmp(what, "inner_bias")) parts[0] = {inner_bs, E * sizeof(float)};
+    else if (!strcmp(what, "sums0")) parts[0] = {sums0, 2 * E * sizeof(double)};
+    else if (!strcmp(what, "sums")) parts[0] = {sums, 2 * E * sizeof(double)};
+    else { set_error("unknown debug buffer '%s'", what); return SKY_ERR_ARG; }
+    if (im) { parts[0] = {im->hi, im->bytes}; parts[1] = {im->lo, im->bytes}; }
+    const size_t total = parts[0].bytes + parts[1].bytes;
+    if (total != max_floats * sizeof(float)) {
+      set_error("debug buffer '%s' is %zu floats, destination %llu", what, total / sizeof(float), (unsigned long long)max_floats);
+      return SKY_ERR_ARG;
+    }
+    SKY_CUDA_OK(cudaMemcpyAsync(dst, parts[0].p, parts[0].bytes, cudaMemcpyDeviceToDevice, st));
+    if (parts[1].p)
+      SKY_CUDA_OK(cudaMemcpyAsync(reinterpret_cast<uint8_t*>(dst) + parts[0].bytes, parts[1].p, parts[1].bytes, cudaMemcpyDeviceToDevice, st));
+    return 0;
   }
 };
 
