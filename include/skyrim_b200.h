@@ -144,7 +144,12 @@ SKY_API int sky_model_debug_copy(sky_model_t* m, const char* what, float* dst, u
  * its fp16 operand image instead of the default image-only stream: 1.1 ms per step slower, one rounding per residual add less
  * (DESIGN.md section 3).  Test taps: "stop_after" = n makes step() return after
  * stage n (Pangu: 0 embed, 1 layer0, 2 down, 3 layer1, 4 layer2, 5 up, 6 layer3; SFNO: 0 encoder, 1 + i block i;
- * 99 = run the whole step) so that sky_model_debug_copy can read the intermediate buffers. */
+ * 99 = run the whole step) so that sky_model_debug_copy can read the intermediate buffers.  GraphCast also takes
+ * "stop_launch" = n: a member's step returns after its n-th unit in program order (the feature kernel, every hidden GEMM,
+ * LayerNorm GEMM, per-node table and aggregation), because its workspace buffers are reused within a step; -1 = never.
+ * Its debug_copy names "feat", "hid", "hid_m", "vg_img", "tg", "tm", "yimg", "ym_img", "em_img", "agg_img", "vm_img",
+ * "vm0_img", "e_g2m_img", "e_m2g_img", "e_mesh_img" and "g2m_tr" copy the whole buffer as raw bytes (fp16 tile images,
+ * fp16 row-major tables); max_floats must be its exact size. */
 SKY_API int sky_model_debug_set(sky_model_t* m, const char* key, int64_t value);
 
 /* x[m, c, :, :] += amp * sigma[c] * N(0,1), Philox4x32-10 keyed by (seed, member0 + m):

@@ -148,12 +148,15 @@ class GraphCastRef:
         tap = (lambda k, v: taps.__setitem__(k, v.clone())) if taps is not None else (lambda k, v: None)
         qs = (lambda t: t.half().to(self.dtype)) if self.emulate == "fp16s" else (lambda t: t)   # fp16-only residual streams
         # encoder
-        vg = qs(self.mlp("enc.grid_embed", [self.features(x, t_seconds)]))
+        feat = self.features(x, t_seconds)
+        tap("feat", feat)
+        vg = qs(self.mlp("enc.grid_embed", [feat]))
         tap("grid_embed", vg)
         vm = st["vm"]
         s, r = ix["g2m.senders"], ix["g2m.receivers"]
         e = self.mlp("enc.g2m_edge", [st["e_g2m"], vg[s], vm[r]], table_parts=(1, 2))
         agg = torch.zeros(nm, cfg.latent, dtype=self.dtype).index_add_(0, r, e)
+        tap("g2m_update", e); tap("g2m_agg", agg)
         vm = vm + self.mlp("enc.g2m_mesh", [vm, agg])
         vg = qs(vg + self.mlp("enc.g2m_grid", [vg]))
         tap("enc_mesh", vm); tap("enc_grid", vg)
@@ -166,15 +169,17 @@ class GraphCastRef:
             vm_new = vm + self.mlp(f"proc{i}.node", [vm, agg])
             em = qs(em + e)
             vm = vm_new
-            tap(f"proc{i}_mesh", vm)
+            tap(f"proc{i}_mesh", vm); tap(f"proc{i}_update", e); tap(f"proc{i}_agg", agg); tap(f"proc{i}_edges", em)
         # decoder
         s, r = ix["m2g.senders"], ix["m2g.receivers"]
         e = self.mlp("dec.m2g_edge", [st["e_m2g"], vm[s], vg[r]], table_parts=(1, 2))
         agg = torch.zeros(cfg.n_grid, cfg.latent, dtype=self.dtype).index_add_(0, r, e)
+        tap("m2g_update", e)
         del e
         vg = qs(vg + self.mlp("dec.m2g_grid", [vg, agg]))
         tap("dec_grid", vg)
         out = self.mlp("dec.out", [vg], ln=False)
+        tap("out", out[:, :cfg.n_prog])
         return out[:, :cfg.n_prog]
 
     @torch.no_grad()

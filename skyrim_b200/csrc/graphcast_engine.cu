@@ -176,6 +176,30 @@ struct GraphCastEngine : Engine {
     return 0;
   }
 
+  // ---- test tap: stop inside a member's step ---------------------------------------------------------------------
+  // debug_set "stop_launch" n: a member's step returns after its n-th unit, counted in program order over the feature
+  // kernel and the hidden / ln_gemm / table / segsum calls (segsum's two kernels are one unit), so that debug_copy reads a
+  // reused workspace buffer right after its producer.  -1 (the default) never stops.  A stopped step is never captured
+  // (Engine::step_cached), and the counter is host state only: the launch sequence of an unstopped step is unchanged.
+  static constexpr int GC_STOPPED = 1 << 20;   // not an error code: step() swallows it
+  int units_done = 0;
+  int unit_done() { return stop_launch >= 0 && loaded && ++units_done >= stop_launch ? GC_STOPPED : 0; }
+  int debug_set(const char* key, long long value) override {
+    if (!strcmp(key, "stop_launch")) { stop_launch = (int)value; return 0; }
+    return Engine::debug_set(key, value);
+  }
+  // fp16-range guard over the VALID rows of an M-row image: the whole tiles, then rows [0, M % 128) of each k-block of the
+  // partial last tile (a row's 128 bytes stay inside the row under the swizzle; the rows past M hold whatever the workspace
+  // held and are not scanned)
+  int scan_img(int slot, const uint8_t* img, long long M, cudaStream_t st) {
+    if (!range_guard) return 0;
+    const size_t full = (size_t)(M / 128) * GC_NKB * G2_A_BYTES;
+    if (int rc = range_scan(slot, img, full, st)) return rc;
+    for (int kb = 0; kb < GC_NKB && M % 128; ++kb)
+      if (int rc = range_scan(slot, img + full + (size_t)kb * G2_A_BYTES, (size_t)(M % 128) * 128, st)) return rc;
+    return 0;
+  }
+
   // ---- GEMM wrappers --------------------------------------------------------------------------------------------
   template <int kG>
   int hidden(int tag, const AOperand& A, int Kp, const WImg& w, const float* b1, long long M, uint8_t* out, const __half* ta, int lda,
@@ -188,7 +212,9 @@ struct GraphCastEngine : Engine {
     const int rc = launch_gemm2<256>(SchedW<>{A, w.img, Kp / 64}, epi, M, GC_L, 1, num_sms, st);
     prof_end(tag, st);
     // fp16-range guard (engine.h; a no-op unless enabled): class 5 hidden images, 0 latent / update images, 6 per-node tables
-    return rc ? rc : range_scan(5, out, (size_t)(M / 128) * GC_NKB * G2_A_BYTES, st);
+    if (rc) return rc;
+    if (int r2 = scan_img(5, out, M, st)) return r2;
+    return unit_done();
   }
   template <int kRes>
   int ln_launch(const uint8_t* hid, const Mlp& m, long long M, const void* res, float* xout, uint8_t* img, uint8_t* yimg, cudaStream_t st) {
@@ -206,8 +232,9 @@ struct GraphCastEngine : Engine {
     else rc = ln_launch<0>(hid, m, M, nullptr, xout, img, yimg, st);
     prof_end(tag, st);
     if (rc) return rc;
-    if (img) if (int r2 = range_scan(0, img, (size_t)(M / 128) * GC_NKB * G2_A_BYTES, st)) return r2;
-    return yimg ? range_scan(0, yimg, (size_t)(M / 128) * GC_NKB * G2_A_BYTES, st) : 0;
+    if (img) if (int r2 = scan_img(0, img, M, st)) return r2;
+    if (yimg) if (int r2 = scan_img(0, yimg, M, st)) return r2;
+    return unit_done();
   }
   // per-node table: T (M, N) fp16 row-major = A W^T
   int table(int tag, const uint8_t* aimg, const WImg& w, long long M, __half* out, cudaStream_t st) {
@@ -217,7 +244,9 @@ struct GraphCastEngine : Engine {
     count_launch();
     const int rc = launch_gemm2<256>(SchedW<>{AOperand(aimg, GC_NKB), w.img, GC_NKB}, epi, M, w.N, 1, num_sms, st);
     prof_end(tag, st);
-    return rc ? rc : range_scan(6, out, (size_t)M * w.N * 2, st);
+    if (rc) return rc;
+    if (int r2 = range_scan(6, out, (size_t)M * w.N * 2, st)) return r2;
+    return unit_done();
   }
   int segsum(int tag, const uint8_t* yimg, const SegPlan& sp, uint8_t* out, cudaStream_t st) {
     prof_begin(tag, st);
@@ -231,7 +260,7 @@ struct GraphCastEngine : Engine {
       prof_end(tag, st);
     }
     SKY_CUDA_OK(cudaGetLastError());
-    return 0;
+    return unit_done();
   }
 
   // ---- load: parameters, graph tables, input-independent embeddings ------------------------------------------
@@ -255,7 +284,12 @@ struct GraphCastEngine : Engine {
   int prepare(cudaStream_t st) override {
     prep_stream = st;
     if (cfg.latent != GC_L) { set_error("GraphCast engine is built for latent %d", GC_L); return SKY_ERR_ARG; }
-    if (nfeat > GC_FEAT_KP || cfg.n_state != cfg.n_prog + 1) { set_error("unsupported GraphCast channel layout"); return SKY_ERR_ARG; }
+    if (cfg.n_state != cfg.n_prog + 1) { set_error("unsupported GraphCast channel layout"); return SKY_ERR_ARG; }
+    if (nfeat > GC_FEAT_TS) {   // k_gc_features stages one row of GC_FEAT_TS halves per grid point in shared memory
+      set_error("GraphCast: %d grid-node features (n_static = %d) exceed the %d columns the feature kernel stages per grid point",
+                nfeat, cfg.n_static, GC_FEAT_TS);
+      return SKY_ERR_ARG;
+    }
     const int L = GC_L;
     int rc;
 #define P(dst, name, cnt) if (!((dst) = keep(name, (uint64_t)(cnt), st))) return SKY_ERR_ARG;
@@ -395,9 +429,8 @@ struct GraphCastEngine : Engine {
     count_launch();
     k_gc_clock<<<1, 32, 0, st>>>(clock_dev, clk_dev, 3600.0 * cfg.dt_hours, 1);
     prof_end(KT_GC_FEAT, st);
-    for (int b = 0; b < batch; ++b) {
-      const float* xi = x_in + (size_t)b * 2 * cfg.n_state * plane;
-      float* xo = x_out + (size_t)b * 2 * cfg.n_state * plane;
+    // one member: encoder, processor, decoder, output head (returns early at a test tap's stop point)
+    auto member = [&](const float* xi, float* xo) -> int {
       // ---------------- encoder
       prof_begin(KT_GC_FEAT, st);
       count_launch();
@@ -405,10 +438,11 @@ struct GraphCastEngine : Engine {
                                                             cfg.n_state, cfg.n_prog, cfg.n_static);
       prof_end(KT_GC_FEAT, st);
       SKY_CUDA_OK(cudaGetLastError());
+      if ((rc = unit_done())) return rc;
       if ((rc = hidden<0>(KT_GC_HIDDEN, AOperand(w.feat, GC_FEAT_KP / 64), GC_FEAT_KP, grid_embed.w1, grid_embed.b1, Ng, w.hid, nullptr, 0, nullptr,
                           nullptr, 0, nullptr, st))) return rc;
       if ((rc = ln_gemm(KT_GC_LN, w.hid, grid_embed, Ng, nullptr, nullptr, w.vg_img, nullptr, st))) return rc;
-      if (stop_after == 0) continue;
+      if (stop_after == 0) return 0;
       if ((rc = table(KT_GC_TABLE, w.vg_img, g2m_ws, Ng, w.tg, st))) return rc;
       if ((rc = hidden<2>(KT_GC_HIDDEN, AOperand(e_g2m_img, GC_NKB), L, g2m_edge.w1, g2m_edge.b1, Eg, w.hid, w.tg, L, g2m_s, g2m_tr, L, g2m_r, st))) return rc;
       if ((rc = ln_gemm(KT_GC_LN, w.hid, g2m_edge, Eg, nullptr, nullptr, nullptr, w.yimg, st))) return rc;
@@ -417,9 +451,8 @@ struct GraphCastEngine : Engine {
       if ((rc = ln_gemm(KT_GC_LN, w.hid_m, g2m_mesh, Nm, vm0_f32, w.vm, w.vm_img, nullptr, st))) return rc;
       if ((rc = hidden<0>(KT_GC_HIDDEN, AOperand(w.vg_img, GC_NKB), L, g2m_grid.w1, g2m_grid.b1, Ng, w.hid, nullptr, 0, nullptr, nullptr, 0, nullptr, st))) return rc;
       if ((rc = ln_gemm(KT_GC_LN, w.hid, g2m_grid, Ng, nullptr, nullptr, w.vg_img, nullptr, st, w.vg_img))) return rc;
-      if (stop_after == 1) continue;
+      if (stop_after == 1) return 0;
       // ---------------- processor
-      bool stopped = false;
       for (int i = 0; i < cfg.layers; ++i) {
         const uint8_t* em_in_img = i ? w.em_img : e_mesh_img;
         if ((rc = table(KT_GC_TABLE, w.vm_img, proc_wsr[i], Nm, w.tm, st))) return rc;
@@ -433,9 +466,8 @@ struct GraphCastEngine : Engine {
         if ((rc = hidden<0>(KT_GC_HIDDEN, AOperand(w.vm_img, GC_NKB).add(w.agg_img, GC_NKB), 2 * L, proc_node[i].w1, proc_node[i].b1, Nm, w.hid_m, nullptr, 0, nullptr, nullptr, 0,
                             nullptr, st))) return rc;
         if ((rc = ln_gemm(KT_GC_LN, w.hid_m, proc_node[i], Nm, w.vm, w.vm, w.vm_img, nullptr, st))) return rc;
-        if (stop_after == 2 + i) { stopped = true; break; }
+        if (stop_after == 2 + i) return 0;
       }
-      if (stopped) continue;
       // ---------------- decoder
       if ((rc = table(KT_GC_TABLE, w.vm_img, m2g_ws, Nm, w.tm, st))) return rc;
       if ((rc = table(KT_GC_TABLE, w.vg_img, m2g_wr, Ng, w.tg, st))) return rc;
@@ -448,7 +480,7 @@ struct GraphCastEngine : Engine {
       }
       if ((rc = ln_gemm(KT_GC_LN, w.hid, m2g_grid, Ng, nullptr, nullptr, w.vg_img, nullptr, st, w.vg_img))) return rc;
       if ((rc = range_scan(0, w.feat, img_bytes(Ng, GC_FEAT_KP / 64), st))) return rc;
-      if (stop_after == 100) continue;
+      if (stop_after == 100) return 0;
       if ((rc = hidden<0>(KT_GC_HIDDEN, AOperand(w.vg_img, GC_NKB), L, out_mlp.w1, out_mlp.b1, Ng, w.hid, nullptr, 0, nullptr, nullptr, 0, nullptr, st))) return rc;
       {
         EpiGcOut epi{};
@@ -460,6 +492,12 @@ struct GraphCastEngine : Engine {
         prof_end(KT_GC_OUT, st);
         if (rc) return rc;
       }
+      return unit_done();
+    };
+    for (int b = 0; b < batch; ++b) {
+      units_done = 0;
+      rc = member(x_in + (size_t)b * 2 * cfg.n_state * plane, x_out + (size_t)b * 2 * cfg.n_state * plane);
+      if (rc && rc != GC_STOPPED) return rc;
     }
     SKY_CUDA_OK(cudaGetLastError());
     return 0;
@@ -467,6 +505,29 @@ struct GraphCastEngine : Engine {
 
   int debug_copy(const char* what, float* dst, uint64_t max_floats, void* ws_base, int, cudaStream_t st) override {
     const Ws w = carve(ws_base);
+    {   // raw taps: a buffer as it lies in memory (fp16 tile images, fp16 row-major tables), decoded on the host.  The
+        // workspace is reused, so a tap is meaningful right after its producer (debug_set "stop_launch").
+      const long long Emax = E3 > pad128(Eg) ? E3 : pad128(Eg);
+      const size_t nm_rows = (size_t)pad128(Nm) * GC_L * 2;
+      const struct { const char* name; const void* p; size_t bytes; } raw[] = {
+          {"feat", w.feat, img_bytes(Ng, GC_FEAT_KP / 64)}, {"hid", w.hid, img_bytes(Emax, GC_NKB)},
+          {"hid_m", w.hid_m, img_bytes(Em, GC_NKB)},        {"vg_img", w.vg_img, img_bytes(Ng, GC_NKB)},
+          {"tg", w.tg, (size_t)Ngp * GC_L * 2},             {"yimg", w.yimg, img_bytes(Emax, GC_NKB)},
+          {"vm_img", w.vm_img, img_bytes(Nm, GC_NKB)},      {"tm", w.tm, 2 * nm_rows},
+          {"em_img", w.em_img, img_bytes(Em, GC_NKB)},      {"ym_img", w.ym_img, img_bytes(Em, GC_NKB)},
+          {"agg_img", w.agg_img, img_bytes(Nm, GC_NKB)},    {"vm0_img", vm0_img, img_bytes(Nm, GC_NKB)},
+          {"e_g2m_img", e_g2m_img, img_bytes(Eg, GC_NKB)},  {"e_m2g_img", e_m2g_img, img_bytes(E3, GC_NKB)},
+          {"e_mesh_img", e_mesh_img, img_bytes(Em, GC_NKB)}, {"g2m_tr", g2m_tr, nm_rows}};
+      for (const auto& r : raw)
+        if (!strcmp(what, r.name)) {
+          if (r.bytes != max_floats * sizeof(float)) {
+            set_error("debug buffer '%s' is %zu floats, destination %llu", what, r.bytes / sizeof(float), (unsigned long long)max_floats);
+            return SKY_ERR_ARG;
+          }
+          SKY_CUDA_OK(cudaMemcpyAsync(dst, r.p, r.bytes, cudaMemcpyDeviceToDevice, st));
+          return 0;
+        }
+    }
     const float* src = nullptr; uint64_t n = 0;
     if (!strcmp(what, "range")) { src = range_dev; n = 8; if (!src) { set_error("range guard was never enabled"); return SKY_ERR_STATE; } }
     else if (!strcmp(what, "vm")) { src = w.vm; n = (uint64_t)Nm * GC_L; }

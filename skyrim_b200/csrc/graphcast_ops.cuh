@@ -278,6 +278,7 @@ __global__ void k_gc_toa(float* __restrict__ out, int nlat, int nlon, double t) 
 }
 
 constexpr int GC_FEAT_KP = 192;   // 184 features padded to three k-blocks
+constexpr int GC_FEAT_TS = 186;   // halves k_gc_features stages per grid point: the most features a configuration may have
 
 // state (2 x n_state planes at t-6h, t) -> grid-node feature image [n_grid/128][3][128 x 128 B]; also writes the two
 // slices of the next state that do not depend on the network: x_out[slice 0] = x_in[slice 1], x_out[slice 1][forcing]
@@ -287,7 +288,7 @@ __global__ void __launch_bounds__(128) k_gc_features(const float* __restrict__ x
                                                      const float* __restrict__ mean, const float* __restrict__ stdv,
                                                      const float* __restrict__ statics, const GcClock* __restrict__ clk,
                                                      int nlat, int nlon, int nstate, int nprog, int nstatic) {
-  constexpr int TS = 186;   // row stride in halves: 93 words (odd) -> conflict-free row-owner writes; 47.6 KB static
+  constexpr int TS = GC_FEAT_TS;   // row stride in halves: 93 words (odd) -> conflict-free row-owner writes; 47.6 KB static
   __shared__ __half tile[128][TS];
   __shared__ GcClock c;
   const long long plane = (long long)nlat * nlon;

@@ -27,7 +27,7 @@ void Engine::drop_graphs() {
 
 int Engine::step_cached(const float* x_in, float* x_out, int batch, void* ws, size_t ws_bytes, cudaStream_t st) {
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-  if (!use_graphs || prof_mask != 0 || stop_after != 99 || range_guard || cudaStreamIsCapturing(st, &cs) != cudaSuccess ||
+  if (!use_graphs || prof_mask != 0 || stop_after != 99 || stop_launch >= 0 || range_guard || cudaStreamIsCapturing(st, &cs) != cudaSuccess ||
       cs != cudaStreamCaptureStatusNone)
     return step(x_in, x_out, batch, ws, ws_bytes, st);
   GraphEntry* e = nullptr;
