@@ -29,6 +29,7 @@
 #include <cstring>
 
 #include "gemm2.cuh"
+#include "pangu_ops.cuh"
 
 namespace sky {
 

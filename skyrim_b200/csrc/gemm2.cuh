@@ -9,9 +9,10 @@
 //   W image  [N/BLOCK_N][K/64][BLOCK_N rows x 128 B]  packed once at weight load
 // so no warp ever touches the operands with ld/st.  A schedule (SchedW here, SchedTB in gemm_tb.cuh) decides which
 // images a tile's k-blocks come from; the pipeline is the same for all.  Warp roles: 0..7 = two consumer warpgroups,
-// 8 = loader.  Warpgroup g issues the wgmma products of rows 64g .. 64g+63 of the 128-row tile
-// over all BLOCK_N columns (fp32 accumulators in registers, BLOCK_N / 2 per thread).  At the end of
-// a tile both warpgroups stage their accumulators in shared memory — over the operand ring, which
+// 8 = loader.  One schedule has no A image: under SchedProd four more warps (9..12) gather and convert A straight into
+// the ring (Pangu's patch embedding) and the loader fetches only W.  Warpgroup g issues the wgmma products of rows
+// 64g .. 64g+63 of the 128-row tile over all BLOCK_N columns (fp32 accumulators in registers, BLOCK_N / 2 per thread).
+// At the end of a tile both warpgroups stage their accumulators in shared memory — over the operand ring, which
 // is drained by then — and the same eight warps run the row-owner epilogue on the staged tile
 // (warp%4 selects the 32-row quarter, warp/4 the column partition).  Epilogues re-tile their 32x32
 // accumulator blocks through a padded smem patch so that every global access is a full
@@ -23,7 +24,7 @@
 #include <type_traits>
 
 #include "../../include/skyrim_b200.h"
-#include "pangu_ops.cuh"
+#include "sky_common.cuh"
 #include "wgmma_ops.cuh"
 
 namespace sky {
@@ -76,8 +77,9 @@ struct AOperand {
 };
 
 // kFrag: the epilogue runs on the accumulator fragments (FragEpi below); the patches give way to the output tile,
-// BLOCK_N / 64 blocks of 128 rows x 128 B laid out as the destination image's blocks
-template <int BLOCK_N, int EPI_WARPS, bool kFrag = false>
+// BLOCK_N / 64 blocks of 128 rows x 128 B laid out as the destination image's blocks.  PROD_WARPS: the A producer warps
+// of the schedule (SchedProd), 0 for image-fed A.
+template <int BLOCK_N, int EPI_WARPS, bool kFrag = false, int PROD_WARPS = 0>
 struct G2Cfg {
   static constexpr int B_BYTES = BLOCK_N * 128;
   static constexpr int STAGE_BYTES = G2_A_BYTES + B_BYTES;
@@ -91,7 +93,7 @@ struct G2Cfg {
   // accumulator staging over the drained ring: all 128 rows at once
   static constexpr int STG_LD = (BLOCK_N + 31) / 32 * 32 + 4;
   static constexpr int SMEM_BYTES = RING_BYTES + FIXED;
-  static constexpr int THREADS = (EPI_WARPS + 1) * 32;
+  static constexpr int THREADS = (EPI_WARPS + 1 + PROD_WARPS) * 32;   // consumers, loader, A producers
   static_assert(BLOCK_N % 8 == 0 && BLOCK_N <= 256, "wgmma N, accumulator registers");
   static_assert(STAGE_BYTES % 1024 == 0, "stage alignment");
   static_assert(STAGES >= 2, "pipeline depth");
@@ -350,10 +352,37 @@ struct SchedW {
   }
 };
 
+// Producer-fed A: the A tile of every k-block is written into the ring by kProdWarps producer warps, one tile row per
+// thread, through prod.prep(row) (once per tile) and prod.load8(info, k) (the 8 halves at columns k .. k + 7, zeros past
+// M and past the valid K).  Only W, packed as for SchedW, is bulk-copied.  Staged epilogues only.
+template <class Prod>
+struct SchedProd {
+  static constexpr bool kBMN = false;
+  static constexpr int kProdWarps = 4;
+  Prod prod;
+  const uint8_t* W;
+  int num_kb;
+  bool valid() const { return true; }
+  template <int BN>
+  __device__ G2Tile tile(const G2Grid& g, int i) const { return G2Tile::at(g, i); }
+  template <int BN>
+  __device__ __forceinline__ void issue(uint8_t* dst, uint64_t* full, const G2Tile& t, int kb, int lane) const {
+    constexpr int B_BYTES = BN * 128;
+    if (lane == 0) {
+      mbar_arrive_expect_tx(full, B_BYTES);
+      bulk_g2s(dst + G2_A_BYTES, W + ((size_t)t.nt * num_kb + kb) * B_BYTES, B_BYTES, full);
+    }
+  }
+};
+// producer warps of a schedule: S::kProdWarps, none for the image-fed schedules
+template <class S, class = void> struct sched_prod_warps : std::integral_constant<int, 0> {};
+template <class S> struct sched_prod_warps<S, std::void_t<decltype(S::kProdWarps)>> : std::integral_constant<int, S::kProdWarps> {};
+
 // ---------------------------------------------------------------------------------------------------------------
 // The TMA-fed persistent GEMM.  One loader warp fills the stage ring (stage = A tile | B tile) through the schedule; two
 // consumer warpgroups run the main loop and the epilogue of each tile.  The loader starts the next tile's copies once the
-// previous tile's epilogue has left the ring (stg_free); a tile the schedule skips counts for no role.
+// previous tile's epilogue has left the ring (stg_free); a tile the schedule skips counts for no role.  Under a producer
+// schedule the producer warps fill the A half of each stage on the same protocol, and full[s] also counts their arrivals.
 // kPair (k_gemm2_pair): the two CTAs of a cluster take the same m-tile and n-tiles 0 / 1 (N = 2 BLOCK_N; the persistent
 // walk over 2 n-tiles with an even grid gives CTA rank r exactly the tiles (mt, r)), and exchange LayerNorm row statistics
 // through distributed shared memory (PairStats).  A 128 x 512 fp32 accumulator is the whole register file of an SM;
@@ -362,6 +391,8 @@ struct SchedW {
 // ---------------------------------------------------------------------------------------------------------------
 constexpr int G2_EPI_WARPS = 8;
 constexpr int G2_PAIR_SMEM = 2048;   // the pair's exchange slots, behind the barrier block
+template <class Sched, class Epi, int BLOCK_N>
+using G2CfgOf = G2Cfg<BLOCK_N, G2_EPI_WARPS, is_fragment_epi<Epi>::value, sched_prod_warps<Sched>::value>;
 
 // Fragment epilogues (FragEpi): the loader warp stores the output tile of tile `t` (a finished tile) to the destination
 // image.  The three 16 KB blocks of a tile are contiguous there (n0 is a multiple of BLOCK_N); a partial last m-tile is
@@ -388,7 +419,10 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
   constexpr bool kFrag = is_fragment_epi<Epi>::value;
   constexpr bool kScatter = is_scatter_epi<Epi>::value;
   if constexpr (kScatter) static_assert(kFrag && !Epi::kNeedsBias && !Epi::kLoadsTile, "scatter: fragment path, map over the bias region");
-  using Cfg = G2Cfg<BLOCK_N, EPI_WARPS, kFrag>;
+  constexpr int PROD_WARPS = sched_prod_warps<Sched>::value;
+  static_assert(PROD_WARPS == 0 || (!kFrag && !kPair && PROD_WARPS * 32 == G2_BLOCK_M),
+                "producer schedules: staged epilogue, one CTA, one tile row per producer thread");
+  using Cfg = G2CfgOf<Sched, Epi, BLOCK_N>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   float* patches = reinterpret_cast<float*>(smem + Cfg::RING_BYTES);
@@ -412,7 +446,7 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
   constexpr int LOADER = EPI_WARPS;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], EPI_WARPS); }
+    for (int s = 0; s < Cfg::STAGES; ++s) { mbar_init(&full[s], 1 + PROD_WARPS * 32); mbar_init(&empty[s], EPI_WARPS); }
     mbar_init(stg_free, EPI_WARPS);
     if (kPair) for (int i = 0; i < 8; ++i) mbar_init(&xbar[i], 1);
     if constexpr (kFrag) mbar_init(out_ready, 1);
@@ -524,6 +558,34 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
         if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
       }
     }
+  } else if (PROD_WARPS > 0 && warp > LOADER) {
+    // ---------------- A producers (SchedProd) ----------------
+    // thread = tile row, the 8 chunks of a k-block in sequence: for one chunk the 32 lanes of a warp are 32 consecutive
+    // rows (for the patch embedding 32 consecutive tokens, i.e. one contiguous 512-byte run of the source field per load
+    // instruction), and the 16-byte shared-memory stores of a quarter warp fall into 8 different swizzled chunk slots
+    if constexpr (PROD_WARPS > 0) {
+      const int row = threadIdx.x - (LOADER + 1) * 32;
+      int s = 0; uint32_t ph = 0; int it = 0;
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+        const auto t = sc.template tile<BLOCK_N>(g, tile);
+        if (t.skip) continue;
+        const auto ri = sc.prod.prep((long long)t.mt * G2_BLOCK_M + row);
+        if (it > 0) mbar_wait(stg_free, (uint32_t)(it - 1) & 1);
+        ++it;
+        for (int kb = 0; kb < sc.num_kb; ++kb) {
+          mbar_wait(&empty[s], ph ^ 1);
+          uint8_t* a_s = smem + s * Cfg::STAGE_BYTES;
+          uint4 v[8];
+#pragma unroll
+          for (int i = 0; i < 8; ++i) v[i] = sc.prod.load8(ri, kb * 64 + i * 8);
+#pragma unroll
+          for (int i = 0; i < 8; ++i) *reinterpret_cast<uint4*>(a_s + sw128_offset(row, i)) = v[i];
+          fence_proxy_async_smem();
+          mbar_arrive(&full[s]);
+          if (++s == Cfg::STAGES) { s = 0; ph ^= 1; }
+        }
+      }
+    }
   } else {
     // ---------------- consumer warpgroups: MMA, then epilogue ----------------
     const int q = warp & 3, part = warp >> 2, wg = warp >> 2;
@@ -560,11 +622,11 @@ __device__ __forceinline__ void gemm2_body(const Sched& sc, const Epi& epi, cons
 }
 
 template <class Sched, class Epi, int BLOCK_N>
-__global__ void __launch_bounds__((G2_EPI_WARPS + 1) * 32, 1) k_gemm2(const Sched sc, const Epi epi, const G2Grid g) {
+__global__ void __launch_bounds__(G2CfgOf<Sched, Epi, BLOCK_N>::THREADS, 1) k_gemm2(const Sched sc, const Epi epi, const G2Grid g) {
   gemm2_body<Sched, Epi, BLOCK_N, false>(sc, epi, g);
 }
 template <class Sched, class Epi, int BLOCK_N>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__((G2_EPI_WARPS + 1) * 32, 1)
+__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(G2CfgOf<Sched, Epi, BLOCK_N>::THREADS, 1)
 k_gemm2_pair(const Sched sc, const Epi epi, const G2Grid g) {
   gemm2_body<Sched, Epi, BLOCK_N, true>(sc, epi, g);
 }
@@ -573,7 +635,7 @@ k_gemm2_pair(const Sched sc, const Epi epi, const G2Grid g) {
 // halves: 256 for GraphCast's 512-wide latents, 192 for Pangu's C = 384 projection and fc2).
 template <int BLOCK_N, bool kPair = false, class Sched, class Epi>
 int launch_gemm2(const Sched& sc, const Epi& epi, long long M, int N, int batches, int num_sms, cudaStream_t st) {
-  using Cfg = G2Cfg<BLOCK_N, G2_EPI_WARPS, is_fragment_epi<Epi>::value>;
+  using Cfg = G2CfgOf<Sched, Epi, BLOCK_N>;
   constexpr int SMEM = Cfg::SMEM_BYTES + (kPair ? G2_PAIR_SMEM : 0);
   static_assert(SMEM <= 232448, "smem budget");
   auto kern = [] {   // instantiates only the entry that is launched

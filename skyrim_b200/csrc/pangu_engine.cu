@@ -15,7 +15,7 @@
 #include "attention_tc.cuh"
 #include "engine.h"
 #include "gemm2.cuh"
-#include "gemm_tc.cuh"
+#include "pangu_ops.cuh"
 
 namespace sky {
 
@@ -548,24 +548,19 @@ struct PanguEngine : Engine {
   size_t workspace_bytes(int batch) const override { return carve(nullptr, batch).total; }
 
   // ---- GEMM dispatch -----------------------------------------------------------------------
-  // kPair: N = 2 BN on the column-split CTA pairs (k_gemm2_pair)
-  template <int BN, bool kPair = false, class Epi>
-  int gemm2(int tag, const AOperand& A, const Epi& epi, const GemmW& w, long long M, cudaStream_t st) {
+  // kPair: N = 2 BN on the column-split CTA pairs (k_gemm2_pair).  sc reads the weight w.
+  template <int BN, bool kPair = false, class Sched, class Epi>
+  int gemm2(int tag, const Sched& sc, const Epi& epi, const GemmW& w, long long M, cudaStream_t st) {
     if (w.BN != BN) { set_error("internal: weight packed for BLOCK_N=%d used with %d", w.BN, BN); return SKY_ERR_STATE; }
     prof_begin(tag, st);
     count_launch();
-    const int rc = launch_gemm2<BN, kPair>(SchedW<>{A, w.img, w.Kp / 64}, epi, M, w.N, 1, num_sms, st);
+    const int rc = launch_gemm2<BN, kPair>(sc, epi, M, w.N, 1, num_sms, st);
     prof_end(tag, st);
     return rc;
   }
-  // patch embedding keeps warp producers (im2col + normalisation of the fp32 state)
-  template <int BN, class Prod, class Epi>
-  int gemm_prod(int tag, const Prod& prod, const Epi& epi, const GemmW& w, long long M, cudaStream_t st) {
-    prof_begin(tag, st);
-    count_launch();
-    const int rc = launch_gemm_tc<Prod, Epi, BN>(prod, epi, w.img, M, w.N, w.Kp, num_sms, st);
-    prof_end(tag, st);
-    return rc;
+  template <int BN, bool kPair = false, class Epi>
+  int gemm2(int tag, const AOperand& A, const Epi& epi, const GemmW& w, long long M, cudaStream_t st) {
+    return gemm2<BN, kPair>(tag, SchedW<>{A, w.img, w.Kp / 64}, epi, w, M, st);
   }
 
   // IMG: the token stream of this handle lives only as its fp16 operand image (img_stream) — the LayerNorm epilogues then read
@@ -642,16 +637,16 @@ struct PanguEngine : Engine {
     // test tap (sky_model_debug_set "stop_after"): return early so that debug_copy can read the token buffers
     // (0 embed, 1 layer0, 2 down, 3 layer1, 4 layer2, 5 up, 6 layer3; default 99 = whole step)
     const int stop = stop_after;
-    // ---- patch embedding ----
+    // ---- patch embedding: producer warps gather and normalise the fp32 state into the A tiles (im2col) ----
     {
       long long M = (long long)B * nzt * HW;
       ProdEmbedUpper p{x_in, mean, stdv, cfg.nlat, cfg.nlon, cfg.n_levels, 5, nch, g1.H, g1.W, nzt, M};
-      EpiStoreF32 e{img_stream ? nullptr : ws.x1, C, embed_u_b, M, g1.T, HW, 1, (long long)nzt * HW, ws.skiph, C / 64};
-      if ((rc = gemm_prod<192>(KT_EMBED, p, e, embed_u, M, st))) return rc;
+      EpiStoreF32 e{img_stream ? nullptr : ws.x1, C, embed_u_b, g1.T, HW, 1, (long long)nzt * HW, ws.skiph, C / 64};
+      if ((rc = gemm2<192>(KT_EMBED, SchedProd<ProdEmbedUpper>{p, embed_u.img, embed_u.Kp / 64}, e, embed_u, M, st))) return rc;
       long long Ms = (long long)B * HW;
       ProdEmbedSurf ps{x_in, masks, mean, stdv, cfg.nlat, cfg.nlon, nch, nup, 4, 3, g1.H, g1.W, Ms};
-      EpiStoreF32 es{img_stream ? nullptr : ws.x1, C, embed_s_b, Ms, g1.T, HW, 0, (long long)HW, ws.skiph, C / 64};
-      if ((rc = gemm_prod<192>(KT_EMBED, ps, es, embed_s, Ms, st))) return rc;
+      EpiStoreF32 es{img_stream ? nullptr : ws.x1, C, embed_s_b, g1.T, HW, 0, (long long)HW, ws.skiph, C / 64};
+      if ((rc = gemm2<192>(KT_EMBED, SchedProd<ProdEmbedSurf>{ps, embed_s.img, embed_s.Kp / 64}, es, embed_s, Ms, st))) return rc;
     }
     if (stop == 0) return 0;
     for (size_t i = 0; i < blocks[0].size(); ++i)

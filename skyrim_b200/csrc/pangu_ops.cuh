@@ -1,12 +1,11 @@
 // Pangu-Weather step: the token geometry, and the patch embedding's A-operand producers
-// (gather + normalise + fp32->fp16) and epilogue, on which the producer-fed wgmma GEMM
-// (gemm_tc.cuh) is templated.  The epilogues of the TMA-fed GEMM are in gemm2.cuh and
-// attention_tc.cuh.
+// (gather + normalise + fp32->fp16) and epilogue, which run on k_gemm2 under SchedProd
+// (gemm2.cuh).  The other epilogues of the wgmma GEMM are in gemm2.cuh and attention_tc.cuh.
 //
 // Architecture restated from SURVEY.md Appendix A; the reference reaches it through
 // /root/reference/skyrim/core/models/pangu.py:45-46.
 #pragma once
-#include "sky_common.cuh"
+#include "gemm2.cuh"
 
 namespace sky {
 
@@ -110,42 +109,40 @@ struct ProdEmbedSurf {
 };
 
 // ======================================================================================
-// Epilogues.  Model: one lane owns one accumulator row; `acc.load32(col, v)` is a
-// warp-collective read of 32 consecutive columns of the lane's row (staged accumulator or scratch).
-// `row` may be >= M (tail tile): loads still execute, stores are predicated off.
-// n0 = first column of this tile in the full N, BN = tile width.
+// epilogue of the patch embedding
 // ======================================================================================
-
-// out_f32[dstrow, n0+col] = acc + bias  (+ the fp16 tile image of the same rows)   (patch embedding)
+// out_f32[dstrow, n0+col] = acc + bias  (+ the fp16 tile image of the same rows).  The lane owns tile row row0 + lane;
+// its 32-column groups are split over the warps of its lane quarter.
 struct EpiStoreF32 {
+  static constexpr bool kNeedsBias = false;   // the bias is read from global memory
   float* out; int ldo; const float* bias;  // bias may be null
-  long long M;
   // dst row = member*T + zoff*HW + (row % rows_per_member); identity when rows_per_member==0
   int T; int HW; int zoff; long long rows_per_member;
   uint8_t* img; int nkb;  // optional fp16 image (SWIZZLE_128B tiles of 128 rows x 64 cols)
-  template <class Acc>
-  __device__ void run(Acc& acc, long long row, int n0, int BN) const {
+  template <int BN, class Acc>
+  __device__ void run(Acc& acc, const EpiCtx& x) const {
+    const long long row = x.row0 + x.lane;
     long long dst = row;
     if (rows_per_member > 0) dst = (row / rows_per_member) * T + (long long)zoff * HW + row % rows_per_member;
-    for (int c = 0; c < BN; c += 32) {
+    for (int c = x.part * 32; c < BN; c += 32 * x.nparts) {
       float v[32];
       acc.load32(c, v);
-      if (row < M) {
+      if (row < x.M) {
         if (bias) {
 #pragma unroll
           for (int j = 0; j < 8; ++j) {
-            const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + n0 + c) + j);
+            const float4 bb = __ldg(reinterpret_cast<const float4*>(bias + x.n0 + c) + j);
             v[4 * j] += bb.x; v[4 * j + 1] += bb.y; v[4 * j + 2] += bb.z; v[4 * j + 3] += bb.w;
           }
         }
         // the lane owns its row: 256-bit stores, one full 32-byte sector per lane and instruction
         if (out) {   // null with the image-only token stream: nothing reads the fp32 rows
-          float* o = out + dst * ldo + n0 + c;
+          float* o = out + dst * ldo + x.n0 + c;
 #pragma unroll
           for (int j = 0; j < 4; ++j) stg_f32x8(o + 8 * j, v + 8 * j);
         }
         if (img) {
-          const int col = n0 + c;
+          const int col = x.n0 + c;
           uint8_t* base = img + ((size_t)(dst >> 7) * nkb + (col >> 6)) * 16384 + (size_t)(dst & 127) * 128;
           const uint32_t r7 = (uint32_t)dst & 7u, cb = ((uint32_t)col & 63u) >> 3;   // cb = 0 or 4
           // SWIZZLE_128B permutes 16-byte chunks by XOR with (row & 7): an aligned chunk pair stays an aligned pair
