@@ -4,6 +4,7 @@ GlobalPredictionRollout :277-303), with the back-end replaced by the CUDA step e
 from __future__ import annotations
 
 import datetime
+import functools
 import time
 from pathlib import Path
 from typing import List
@@ -111,6 +112,18 @@ class GlobalModel:
         vals = np.asarray(ic.values, dtype=np.float32)
         vals = vals[-1] if vals.ndim == 4 else vals
         x = torch.from_numpy(np.ascontiguousarray(vals))[None, None]
+
+        def pair(t0, a0, t1, a1):
+            return xr.DataArray(np.stack([a0, a1]), dims=["time", "channel", "lat", "lon"],
+                                coords=dict(time=np.array([np.datetime64(t0, "s"), np.datetime64(t1, "s")]),
+                                            channel=np.array(self.out_channel_names),
+                                            lat=np.array(self.model.grid.lat), lon=np.array(self.model.grid.lon)))
+
+        if not save and n_steps > 0 and hasattr(self.model, "last_slices"):
+            # a schedule that can skip slices (Pangu's hierarchical one) computes only the two returned ones
+            (t_prev, prev), (t_cur, cur) = self.model.last_slices(start_time, x, n_steps)
+            logger.success(f"Rollout to step {n_steps} completed")
+            return pair(t_prev, prev.cpu().numpy()[0], t_cur, cur.cpu().numpy()[0]), output_paths
         if save and hasattr(self.model, "iter_host"):
             # every state is needed on the host: device->host copy of step n overlaps step n+1 (timeloop.iter_host)
             gen = ((t, h[0].numpy(), None) for t, h in self.model.iter_host(start_time, x, n_steps))
@@ -124,11 +137,7 @@ class GlobalModel:
             t_cur, cur, _ = next(gen)
             need_host = save or n == n_steps - 1
             if need_host:
-                cur_host = to_host(cur)
-                pred = xr.DataArray(np.stack([prev_host, cur_host]), dims=["time", "channel", "lat", "lon"],
-                                    coords=dict(time=np.array([np.datetime64(t_prev, "s"), np.datetime64(t_cur, "s")]),
-                                                channel=np.array(self.out_channel_names),
-                                                lat=np.array(self.model.grid.lat), lon=np.array(self.model.grid.lon)))
+                pred = pair(t_prev, prev_host, t_cur, to_host(cur))
                 if save:
                     output_paths.append(save_forecast(pred, self.model_name, t_prev, t_cur, source, config=save_config))
                 prev_host = pred.values[1]
@@ -179,12 +188,15 @@ class GlobalModel:
         if len(sel) > E.ENS_MAX_CHANNELS or len(ev_list) > E.ENS_MAX_EVENTS:
             raise ValueError(f"{len(sel)} channels and {len(ev_list)} events: at most {E.ENS_MAX_CHANNELS} and "
                              f"{E.ENS_MAX_EVENTS}")
-        from ...ensemble import EnsembleRunner
+        from ...ensemble import EnsembleRunner, HierarchicalEnsembleRunner
         if perturbation == "spherical_grf" and grf is None:
             grf = dict(lmax=min(180, (len(self.model.grid.lat) - 1) // 2))
         base, sigma, offset = self._ensemble_initial_state(start_time)
-        runner = EnsembleRunner(self.model.engine, base, sigma, members_per_gpu=members, rank=0, amp=amp, seed=seed,
-                                perturbation=perturbation, grf=grf)
+        make = EnsembleRunner
+        if hasattr(self.model, "engine_24"):   # Pangu's hierarchical schedule: without save, the last two steps only
+            make = functools.partial(HierarchicalEnsembleRunner, engine_24=self.model.engine_24, every_slice=save)
+        runner = make(self.model.engine, base, sigma, members_per_gpu=members, rank=0, amp=amp, seed=seed,
+                      perturbation=perturbation, grf=grf)
         save_config = {k: v for k, v in save_config.items() if k != "filter_vars"}   # selected on the device already
         save_config.setdefault("forecast_id", generate_forecast_id())
         label, source = f"{self.model_name}-ens{members}", self.ic_source if isinstance(self.ic_source, str) else "file"

@@ -123,6 +123,10 @@ class GlobalEnsemble:
         if not 1 <= len(names) <= ENS_MAX_SOURCES:
             raise ValueError(f"{len(names)} models: a multi-model ensemble holds 1 to {ENS_MAX_SOURCES}")
         common = {k: v for k, v in model_kw.items() if k not in names}
+        if "pangu" in names and {**common, **dict(model_kw.get("pangu", {}))}.get("schedule", "6h") != "6h":
+            # the models step in lockstep (_step_all): a schedule that skips or re-anchors steps is not built here
+            raise ValueError("a multi-model run steps Pangu on its 6-h schedule only; the hierarchical schedule runs "
+                             "with Pangu alone")
         self.model_names, self.ic_source = names, ic_source
         self.models = []
         try:

@@ -102,6 +102,56 @@ class EnsembleRunner:
             yield (n,) + host[n % 2]
 
 
+class HierarchicalEnsembleRunner(EnsembleRunner):
+    """``EnsembleRunner`` on Pangu's hierarchical schedule (schedule.py): ``engine`` is the 6-h handle, ``engine_24`` the
+    24-h one on its workspace, both batched over the M members, whose anchor states sit beside their chain states in the
+    plan's four buffers.  Without ``every_slice``, ``iter_stats`` yields only steps n_steps - 1 and n_steps, reached with
+    the fewest forwards.  The members are perturbed exactly as ``EnsembleRunner`` perturbs them."""
+
+    def __init__(self, engine, *args, engine_24, every_slice: bool = True, **kw):
+        super().__init__(engine, *args, **kw)
+        self.engine_24, self.every_slice = engine_24, every_slice
+
+    def step(self, n: int = 1):
+        raise NotImplementedError("a hierarchical ensemble steps through iter_stats, which follows the schedule")
+
+    def iter_stats(self, n_steps: int, channels=None, quantiles=(), events=(), channel_offset: int = 0):
+        import torch
+        from . import schedule
+        from .engine import ensemble_statistics
+        p = schedule.plan("hierarchical", n_steps, self.every_slice)
+        bufs = [self.x, self.y] + [torch.empty_like(self.x) for _ in range(schedule.N_BUFFERS - 2)]
+        engines = {"6h": self.engine, "24h": self.engine_24}
+        dev = self.x.device
+        main = torch.cuda.current_stream(dev)
+        copy = torch.cuda.Stream(dev)
+        for op, src, dst in p.forwards[:p.slices[0][2]]:   # none for slice 0; a last-slices plan may need many
+            engines[op].step(bufs[src], bufs[dst])
+        ring = [ensemble_statistics(bufs[p.slices[0][1]], channels, quantiles, events, channel_offset)]
+        ring.append(tuple(torch.empty_like(t) for t in ring[0]))
+        host = [tuple(torch.empty(t.shape, dtype=t.dtype).pin_memory() for t in ring[0]) for _ in range(2)]
+        done = [torch.cuda.Event() for _ in range(2)]    # statistics i % 2 are complete on the main stream
+        copied = torch.cuda.Event()
+        done[0].record(main)
+        for i, (n, _, _) in enumerate(p.slices):
+            if i + 1 < len(p.slices):   # the forwards and the reduction of slice i + 1 before waiting for the copy of i
+                _, buf, after = p.slices[i + 1]
+                for op, src, dst in p.forwards[p.slices[i][2]:after]:
+                    engines[op].step(bufs[src], bufs[dst])
+                ensemble_statistics(bufs[buf], channels, quantiles, events, channel_offset, out=ring[(i + 1) % 2])
+                done[(i + 1) % 2].record(main)
+            copy.wait_event(done[i % 2])
+            with torch.cuda.stream(copy):
+                for h, d in zip(host[i % 2], ring[i % 2]):
+                    h.copy_(d, non_blocking=True)
+                copied.record(copy)
+            copied.synchronize()
+            yield (n,) + host[i % 2]
+        last = p.slices[-1][1]
+        self.x, self.y = bufs[last], bufs[schedule.A1 if last == schedule.A0 else schedule.A0]
+        self.steps += n_steps
+
+
 def mean_and_spread(x, world: int = 1):
     """x: this rank's members (M, C, H, W).  Two-pass: the mean is reduced first, then the sum of squared DEVIATIONS —
     E[x^2] - mean^2 in fp32 cancels catastrophically on de-normalised fields (z ~ 5e4, t ~ 280 with a spread of a few

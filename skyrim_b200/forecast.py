@@ -4,6 +4,7 @@ defaults; same `run_forecast` signature and return value) on top of the H100 eng
     python -m skyrim_b200.forecast -m pangu -d 20240507 -t 0000 -l 24 -o outputs
     python -m skyrim_b200.forecast -m pangu -l 24 --members 8 --quantiles 0.1,0.5,0.9 --exceed t2m:273.15 -o outputs
     python -m skyrim_b200.forecast --models pangu,fourcastnet_v2,graphcast -l 24 --members 4 -o outputs
+    python -m skyrim_b200.forecast -m pangu -l 168 --pangu_schedule hierarchical -o outputs
 
 The second form runs a perturbed-initial-condition ensemble and saves its per-step statistics (mean, spread, quantiles)
 and exceedance probabilities instead of the members.  The third runs several models side by side on one GPU
@@ -22,6 +23,7 @@ import click
 from loguru import logger
 
 from .common import AVAILABLE_MODELS
+from .schedule import SCHEDULES
 
 yesterday = (datetime.now() - timedelta(days=1)).date().isoformat().replace("-", "")
 
@@ -99,8 +101,11 @@ def parse_exceed(text: str):
 @click.option("--exceed", type=str, default="", help="Exceedance events channel:threshold such as t2m:273.15,u10m:15")
 @click.option("--models", type=str, default="",
               help="Several models side by side on one GPU, such as pangu,graphcast (replaces -m); --members counts per model")
+@click.option("--pangu_schedule", type=click.Choice(SCHEDULES), default=None,
+              help="Pangu alone: '6h' (default) chains the 6-h model; 'hierarchical' interleaves the 6-h and 24-h models "
+                   "as earth2mip's PanguInference does")
 def main(model_name, date, time, lead_time, list_models, initial_conditions, output_dir, filter_vars, modal, weight_seed, device, grid,
-         members, perturbation, amp, seed, quantiles, exceed, models):
+         members, perturbation, amp, seed, quantiles, exceed, models, pangu_schedule):
     if modal:
         raise click.UsageError("--modal: remote execution through Modal is outside this build (SURVEY.md section 2); run locally")
     if not 1 <= members <= 64:
@@ -117,6 +122,10 @@ def main(model_name, date, time, lead_time, list_models, initial_conditions, out
     if unknown or len(set(names)) != len(names) or len(names) == 1 or len(names) * members > 64:
         raise click.UsageError(f"--models {models}: two to four distinct models of {AVAILABLE_MODELS}, at most 64 members "
                                "in all")
+    if pangu_schedule is not None:
+        if names or model_name != "pangu":
+            raise click.UsageError("--pangu_schedule applies to -m pangu alone, not to --models or another model")
+        kw["schedule"] = pangu_schedule
     if grid:
         from .config import graphcast_small, pangu_small, sfno_small
         nlat, nlon = (int(v) for v in grid.lower().split("x"))

@@ -10,7 +10,8 @@ ONNXRuntime sessions over pangu_weather_{6,24}.onnx) and fourcastnet_v2.py:36-37
                                 ((n_type, heads, 144, 144), ~1 GB); the engine wants the compact (3312, n_type, heads) table;
   * ``pangu_from_onnx``         shape-and-order driven mapping of the initialisers onto the Pangu parameter names;
   * ``sfno_from_checkpoint``    key-pattern mapping of an fcnv2_sm ``model_state`` dict; hyper-parameters from shapes;
-  * ``check_fp16_range``        guard for real weights: the engine feeds fp16 operands to the tensor cores.
+  * ``check_fp16_range``        guard for real weights: the engine feeds fp16 operands to the tensor cores;
+  * ``load_pangu_pair``         both Pangu operators from one directory, for the hierarchical schedule.
 
 No such file exists in the build environment (no network), so the mappings are exercised on files the unit tests
 write with the same wire format (tests/test_importers_cpu.py).  Free choices that can only be confirmed against
@@ -391,3 +392,21 @@ def load_real_weights(model: str, path: str):
     cfg, w = sfno_from_checkpoint(wp, mp if os.path.exists(mp) else None, sp if os.path.exists(sp) else None)
     check_fp16_range(w)
     return cfg, w
+
+
+def load_pangu_pair(path: str, cfg=None):
+    """Both Pangu operators for the hierarchical schedule: ``path`` is a directory holding pangu_weather_6.onnx and
+    pangu_weather_24.onnx (the two files ``pangu.load(registry.get_model("e2mip://pangu"))`` opens).  Each goes through
+    ``pangu_from_onnx`` and ``check_fp16_range``.  Returns (6-h parameters, 24-h parameters)."""
+    if not os.path.isdir(path):
+        raise ValueError(f"{path} is one file: the hierarchical Pangu schedule also needs pangu_weather_24.onnx; point "
+                         "SKYRIM_B200_WEIGHTS at the directory holding pangu_weather_6.onnx and pangu_weather_24.onnx")
+    out = []
+    for hours in (6, 24):
+        p = os.path.join(path, f"pangu_weather_{hours}.onnx")
+        if not os.path.isfile(p):
+            raise FileNotFoundError(f"{p} is missing: the hierarchical Pangu schedule needs both operators")
+        w = pangu_from_onnx(p, cfg)
+        check_fp16_range(w)
+        out.append(w)
+    return tuple(out)

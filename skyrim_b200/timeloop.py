@@ -16,6 +16,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
+from . import schedule
 from .config import FCNV2_CHANNELS, GRAPHCAST_CHANNELS, PANGU_CHANNELS
 
 
@@ -137,6 +138,95 @@ class _EngineTimeLoop:
 
 class PanguTimeLoop(_EngineTimeLoop):
     channel_names = PANGU_CHANNELS
+
+
+class PanguHierarchicalTimeLoop(PanguTimeLoop):
+    """Pangu's 6-h and 24-h operators interleaved as earth2mip's ``PanguInference`` runs them (``schedule.py``): still one
+    slice every 6 h, but the slice at 24 d + 6 k hours is P6^k(P24^d(x0)).  ``engine`` is the 6-h handle, ``engine_24``
+    the 24-h one; both step in order on the current stream on the 6-h handle's workspace, over four fixed state buffers.
+    With ``guard_first_step``, each handle's first forward of a rollout runs under ``step_guarded`` (its ranges land in
+    ``last_ranges`` and ``last_ranges_24``)."""
+
+    def __init__(self, engine, engine_24):
+        super().__init__(engine)
+        engine_24.share_workspace(engine)
+        self.engine_24 = engine_24
+        self.last_ranges_24 = None
+        self._bufs = None
+
+    def _load(self, x):
+        """the four state buffers of schedule.py, the initial condition in A0"""
+        torch = self.torch
+        assert x.dim() == 5 and x.shape[1] == self.n_history_levels, x.shape
+        shape = (x.shape[0],) + tuple(x.shape[2:])
+        if self._bufs is None or tuple(self._bufs[0].shape) != shape:
+            self._bufs = [torch.empty(shape, dtype=torch.float32, device=self.device) for _ in range(schedule.N_BUFFERS)]
+        self._bufs[schedule.A0].copy_(x[:, -1].to(dtype=torch.float32), non_blocking=True)
+        self._guarded = set()
+        return self._bufs
+
+    def _forward(self, fwd):
+        op, src, dst = fwd
+        eng = self.engine if op == "6h" else self.engine_24
+        if self.guard_first_step and op not in self._guarded:
+            self._guarded.add(op)
+            _, ranges = eng.step_guarded(self._bufs[src], self._bufs[dst])
+            if op == "6h":
+                self.last_ranges = ranges
+            else:
+                self.last_ranges_24 = ranges
+        else:
+            eng.step(self._bufs[src], self._bufs[dst])
+
+    def __call__(self, time, x, restart=None):
+        """the TimeLoop protocol: the initial condition, then one slice per 6 h; each yielded tensor is a copy of its
+        buffer, so it stays valid"""
+        bufs = self._load(x)
+        yield time, bufs[schedule.A0].clone(), None
+        for _, buf, forwards in schedule.iter_slices("hierarchical"):
+            for f in forwards:
+                self._forward(f)
+            time = time + self.time_step
+            yield time, bufs[buf].clone(), None
+
+    def iter_host(self, time, x, n_steps: int):
+        """``_EngineTimeLoop.iter_host`` under the schedule: the copy of slice n runs on a copy stream under the forwards
+        of slice n + 1, which never write slice n's buffer (schedule.py).  Host tensors: a ring of two."""
+        torch = self.torch
+        p = schedule.plan("hierarchical", n_steps)
+        main = torch.cuda.current_stream(self.device)
+        if getattr(self, "_copy_stream", None) is None:
+            self._copy_stream = torch.cuda.Stream(self.device)
+        bufs = self._load(x)
+        if getattr(self, "_host_ring", None) is None or self._host_ring[0].shape != bufs[0].shape:
+            self._host_ring = [torch.empty(bufs[0].shape, dtype=torch.float32).pin_memory() for _ in range(2)]
+        host = self._host_ring
+        done = [torch.cuda.Event() for _ in range(2)]   # slice i is complete on the main stream
+        copied = torch.cuda.Event()
+        issued = 0
+        for i, (n, buf, _) in enumerate(p.slices):
+            if i == 0:
+                done[0].record(main)
+            if i + 1 < len(p.slices):   # launch the forwards of slice i + 1 before waiting for the copy of slice i
+                for f in p.forwards[issued:p.slices[i + 1][2]]:
+                    self._forward(f)
+                issued = p.slices[i + 1][2]
+                done[(i + 1) % 2].record(main)
+            self._copy_stream.wait_event(done[i % 2])
+            with torch.cuda.stream(self._copy_stream):
+                host[i % 2].copy_(bufs[buf], non_blocking=True)
+                copied.record(self._copy_stream)
+            copied.synchronize()
+            yield time + n * self.time_step, host[i % 2]
+
+    def last_slices(self, time, x, n_steps: int):
+        """Slices n_steps - 1 and n_steps (only slice 0 for n_steps = 0) with the fewest forwards: [(time, device
+        tensor)], each tensor a copy of its buffer."""
+        p = schedule.plan("hierarchical", n_steps, every_slice=False)
+        bufs = self._load(x)
+        for f in p.forwards:
+            self._forward(f)
+        return [(time + n * self.time_step, bufs[buf].clone()) for n, buf, _ in p.slices]
 
 
 class SFNOTimeLoop(_EngineTimeLoop):
