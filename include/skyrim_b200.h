@@ -230,6 +230,36 @@ SKY_API int sky_ensemble_stats_multi(int32_t n_sources, const float* const* x, c
                              const float* event_thr, int32_t n_events, float* stats, float* prob, float* means,
                              void* stream);
 
+/* Forecast verification sums of `members` states on one device against an analysis (and optionally a climatology), per
+ * latitude-band region and selected channel, into caller-owned device buffers (skyrim_b200/scores.py forms the metrics):
+ *   member m, channel c is the plane x + m * member_stride + c * plane (plane = nlat * nlon floats, rows of nlon points
+ *              from the northernmost latitude), c < channel_count; members 1..64;
+ *   channels     host int32 [n_sel], 1 <= n_sel <= 128, each in [0, channel_count); the order of the outputs;
+ *   truth        device fp32 [n_sel][plane]: the analysis of each selected channel (only the selected planes);
+ *   clim         device fp32 [n_sel][plane], or NULL: the climatology of each selected channel;
+ *   row_weights  device fp64 [n_regions][nlat], 1 <= n_regions <= 4: the weight of every point of row i in region r,
+ *                unnormalised, 0 outside the region's band (skyrim_b200.scores.region_weights: cos latitude, poles 0);
+ *   partial      device fp64 workspace of at least partial_bytes = 8 * SKY_SCORES_BLOCKS * 9 * n_regions * n_sel bytes;
+ *   sums         device fp64 [n_regions][n_sel][9].
+ * With M members, x_bar their mean summed in member order in fp64 (the unrounded mean of sky_ensemble_stats), y the truth,
+ * k the climatology and w the row weight of a point, the nine sums over the points with w > 0 are
+ *   sum w,  sum w e,  sum w e^2  (e = x_bar - y),  sum w sum_m (x_m - x_bar)^2,  sum w (1/M) sum_m |x_m - y|,
+ *   sum w G  (G = sum_{m<k} |x_m - x_k|, from the sorted members),  sum w f'o',  sum w f'^2,  sum w o'^2
+ *   (f' = x_bar - k, o' = y - k; these three are NaN when clim is NULL).
+ * All per-point arithmetic is fp64.  A NaN member, truth or climatology value at a point with w > 0 in a region makes that
+ * region's sums 1..8 of that channel NaN; points with w = 0 in a region are not read into its sums.  Two launches, no
+ * atomics: each of SKY_SCORES_BLOCKS blocks per channel writes one partial per (region, channel, sum), then the partials
+ * are summed in block order, so the sums are bitwise reproducible and a channel's or a region's sums do not depend on the
+ * rest of the request.  Refused with SKY_ERR_ARG before any CUDA call: members, nlat, nlon, channel_count, member_stride
+ * (< channel_count * plane), a channel, n_sel, n_regions or partial_bytes out of range, null pointers; and before any
+ * launch: x, truth, clim, row_weights, partial or sums not device memory on one device.  Asynchronous and stream-ordered;
+ * launches on the device that owns x. */
+#define SKY_SCORES_BLOCKS 128
+SKY_API int sky_forecast_scores(const float* x, int32_t members, int64_t member_stride, int32_t nlat, int32_t nlon,
+                                int32_t channel_count, const int32_t* channels, int32_t n_sel, const float* truth,
+                                const float* clim, const double* row_weights, int32_t n_regions, double* partial,
+                                uint64_t partial_bytes, double* sums, void* stream);
+
 /* Per-kernel-family device timing (CUDA events recorded on the launching stream around the
  * launches whose family bit is set in tag_mask).  profile_end synchronises on the recorded
  * events and returns the summed milliseconds and launch counts per family.  Used by bench.py

@@ -40,6 +40,9 @@ class SyntheticDataSource:
 
 
 class GlobalModel:
+    # channels that are forcings rather than forecasts (GraphCast's toa radiation): never scored
+    forcing_channels: tuple = ()
+
     def __init__(self, model_name: str, ic_source: str = "synthetic", **engine_kw):
         clock = time.time()
         self.model_name = model_name
@@ -225,6 +228,77 @@ class GlobalModel:
                 logger.success(f"Ensemble step {n}/{n_steps} completed")
             prev, t_prev = (s, p), t_cur
         return result, paths
+
+    def score(self, start_time: datetime.datetime, n_steps: int, truth=None, climatology=None, members: int = 1,
+              perturbation: str | None = None, amp: float = 0.05, seed: int = 0, grf: dict | None = None,
+              channels: List[str] = [], regions: dict | None = None, save: bool = False, save_config: dict = {}):
+        """Verifies the forecast from ``start_time`` at every lead 0, 6, .., 6 ``n_steps`` h against ``truth`` and returns
+        (scorecard, paths): a DataArray (lead_time, metric, region, channel) of the latitude-weighted scores of
+        ``skyrim_b200/scores.py`` (bias, rmse, acc, spread, ssr, crps, crps_fair) in fp64, lead_time in hours (0: the
+        initial condition), attrs model / members / start_time.  ``truth`` is a data source (``source[time] ->
+        DataArray(channel, lat, lon)``) or a DataArray (time, channel, lat, lon) on the model's grid; it defaults to the
+        model's own data source, as earth2mip verifies against its IC source.  ``climatology``: DataArray (channel, lat,
+        lon), needed for acc.  ``members = 1`` scores the model's own unperturbed trajectory; above 1, ``perturbation``
+        defaults to "spherical_grf" (as ``predict_ensemble``, with the same ``amp``, ``seed`` and ``grf``).  ``channels``
+        default to the forecast channels (forcings excluded), ``regions`` to ``{"global": (-90, 90)}`` (at most 4 latitude
+        bands).  The scores are formed on the device and the sums of all leads cross to the host once.  ``save`` writes
+        the scorecard as one netCDF file, model "<model>-score<M>", under the forecast id."""
+        from ... import engine as E
+        from ... import scores as S
+        names = list(self.out_channel_names)
+        if not 1 <= members <= E.ENS_MAX_MEMBERS:
+            raise ValueError(f"members = {members} must lie in [1, {E.ENS_MAX_MEMBERS}]")
+        if n_steps < 0:
+            raise ValueError(f"n_steps = {n_steps} must not be negative")
+        if perturbation is None:
+            perturbation = "none" if members == 1 else "spherical_grf"
+        if perturbation not in ("none", "gaussian", "spherical_grf"):
+            raise ValueError(f"unknown perturbation {perturbation!r} (none, gaussian, spherical_grf)")
+        if save and save_config.get("file_type", "netcdf") == "zarr":
+            raise ValueError("a scorecard is written as netCDF only: the zarr writer appends along time")
+        filt = list(save_config.get("filter_vars", ()))
+        wanted = list(channels) or filt
+        unknown = [c for c in wanted if c not in names]
+        if unknown:
+            raise ValueError(f"unknown channel(s) {unknown} for {self.model_name}")
+        forcing = [c for c in wanted if c in self.forcing_channels]
+        if forcing:
+            raise ValueError(f"{forcing} are forcings, not forecasts, and are not scored")
+        sel = [c for c in names if (c in wanted if wanted else c not in self.forcing_channels)]
+        if len(sel) > E.ENS_MAX_CHANNELS:
+            raise ValueError(f"{len(sel)} channels: at most {E.ENS_MAX_CHANNELS}")
+        lat, lon = np.array(self.model.grid.lat), np.array(self.model.grid.lon)
+        region_names, row_weights = S.region_weights(lat, regions)
+        if truth is None:
+            truth = self.data_source
+            if truth is None:
+                raise ValueError(f"{self.model_name} has no data source to verify against (synthetic initial conditions): "
+                                 "pass truth=")
+        times = [start_time + n * self.time_step for n in range(n_steps + 1)]
+        truth_at = S.truth_fetcher(truth, sel, lat, lon, times)
+        clim = S.climatology_fields(climatology, sel, lat, lon)
+        from ...ensemble import EnsembleRunner, HierarchicalEnsembleRunner
+        if perturbation == "spherical_grf" and grf is None:
+            grf = dict(lmax=min(180, (len(lat) - 1) // 2))
+        base, sigma, offset = self._ensemble_initial_state(start_time)
+        make = EnsembleRunner
+        if hasattr(self.model, "engine_24"):   # Pangu's hierarchical schedule: every slice is scored
+            make = functools.partial(HierarchicalEnsembleRunner, engine_24=self.model.engine_24, every_slice=True)
+        runner = make(self.model.engine, base, sigma, members_per_gpu=members, rank=0, amp=amp, seed=seed,
+                      perturbation=perturbation, grf=grf)
+        leads, sums = runner.iter_scores(n_steps, lambda n: truth_at(times[n]), clim,
+                                         [names.index(c) for c in sel], row_weights, offset)
+        hours = [n * self.time_step.total_seconds() / 3600 for n in leads]
+        card = S.scorecard(np.asarray(sums), members, hours, region_names, sel, self.model_name, start_time)
+        logger.success(f"Scored {len(leads)} leads of {members} member(s) on {len(sel)} channels")
+        paths = []
+        if save:
+            save_config = {k: v for k, v in save_config.items() if k != "filter_vars"}   # selected on the device already
+            save_config.setdefault("forecast_id", generate_forecast_id())
+            source = self.ic_source if isinstance(self.ic_source, str) else "file"
+            paths.append(save_forecast(card, f"{self.model_name}-score{members}", start_time,
+                                       start_time + n_steps * self.time_step, source, config=save_config))
+        return card, paths
 
 
 class GlobalPrediction:

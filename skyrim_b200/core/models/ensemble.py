@@ -190,6 +190,10 @@ class GlobalEnsemble:
     def predict_one_step(self, start_time: datetime.datetime, initial_condition=None):
         raise NotImplementedError("a multi-model ensemble steps through rollout / forecast (as the reference's)")
 
+    def score(self, *args, **kw):
+        raise NotImplementedError("forecast scores are computed per model: score each model with Skyrim(name).score; "
+                                  "multi-model scoring is not built")
+
     # -- device states ---------------------------------------------------------------------------------------------------
     def _layout(self, m):
         """(state channels, offset of the output slice in the state): a GraphCast state holds two time slices"""

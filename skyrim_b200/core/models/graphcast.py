@@ -21,6 +21,7 @@ CHANNELS = GRAPHCAST_CHANNELS
 
 class GraphcastModel(GlobalModel):
     model_name = "graphcast"
+    forcing_channels = (CHANNELS[-1],)   # "tp06", the toa radiation the engine recomputes every step
 
     def __init__(self, *args, cfg: GraphCastConfig | None = None, weights=None, weight_seed: int = 0, device: int = 0,
                  graph=None, **kwargs):

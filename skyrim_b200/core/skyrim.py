@@ -60,3 +60,12 @@ class Skyrim:
         n_steps = self.model.time_steps(lead_time)
         logger.debug(f"Ensemble of {members} members, {n_steps} steps")
         return self.model.predict_ensemble(start_time=start_time, n_steps=n_steps, members=members, **kw)
+
+    def score(self, date: str, time: str, lead_time: int = 6, **kw):
+        """Forecast verification (``GlobalModel.score``): the date, time and lead time are read as ``predict`` reads them,
+        ``kw`` goes to ``GlobalModel.score`` (truth, climatology, members, perturbation, amp, seed, grf, channels, regions,
+        save, save_config).  Returns (scorecard DataArray (lead_time, metric, region, channel), paths)."""
+        start_time = datetime.datetime(int(date[:4]), int(date[4:6]), int(date[6:8]), int(time[:2]), int(time[2:4]))
+        n_steps = self.model.time_steps(lead_time)
+        logger.debug(f"Scoring {n_steps} steps")
+        return self.model.score(start_time=start_time, n_steps=n_steps, **kw)

@@ -10,8 +10,8 @@
 //
 // One thread owns one (channel, point) and holds its M values in registers, padded to MP (8, 16, 32, 64) with +inf; the
 // padding is excluded from every statistic and sorts behind the members.  Consecutive threads take consecutive points, so
-// each member's load is coalesced.  Quantiles come from a fully unrolled bitonic network (min / max on registers only);
-// the QUANT = false instantiation skips it.  No atomics: each output is one thread's fixed-order computation, so results
+// each member's load is coalesced.  Quantiles come from a fully unrolled bitonic network (min / max on registers only,
+// sort_net.cuh); the QUANT = false instantiation skips it.  No atomics: each output is one thread's fixed-order computation, so results
 // are bitwise reproducible and a channel's outputs do not depend on which other channels are selected.
 // k_ens_stats_multi pools the members of up to four models (sources) with their own channel layouts and also writes
 // each model's own mean; the per-point reduction is the same code.
@@ -20,6 +20,7 @@
 
 #include "engine.h"
 #include "sky_common.cuh"
+#include "sort_net.cuh"
 
 namespace sky {
 namespace {
@@ -92,20 +93,7 @@ __device__ __forceinline__ void reduce_point(float (&v)[MP], const Params& P, in
   }
 
   if constexpr (QUANT) {
-#pragma unroll
-    for (int k = 2; k <= MP; k <<= 1)
-#pragma unroll
-      for (int j = k >> 1; j > 0; j >>= 1)
-#pragma unroll
-        for (int i = 0; i < MP; ++i) {
-          const int l = i ^ j;
-          if (l > i) {
-            const float a = v[i], b = v[l];
-            const bool up = (i & k) == 0;
-            v[i] = up ? fminf(a, b) : fmaxf(a, b);
-            v[l] = up ? fmaxf(a, b) : fminf(a, b);
-          }
-        }
+    bitonic_sort(v);
     for (int q = 0; q < P.n_q; ++q) {
       const int lo = P.q_lo[q], hi = P.q_hi[q];
       float a = 0.f, b = 0.f;

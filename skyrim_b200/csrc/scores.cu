@@ -1,0 +1,238 @@
+// Forecast verification sums on the device (DESIGN.md section 5; the metrics are formed in skyrim_b200/scores.py).
+//
+// For members x_1..x_M of one selected channel, truth y, optional climatology k, ensemble mean xb (fp64, summed in member
+// order: the unrounded mean of k_ens_stats) and latitude-band regions r with row weights w_r[i], this writes per
+// (region, selected channel) the nine fp64 sums over the points p of the plane (row i = p / nlon) with w_r[i] > 0:
+//     0  sum w                           1  sum w e,  e = xb - y          2  sum w e^2
+//     3  sum w sum_m (x_m - xb)^2        4  sum w (1/M) sum_m |x_m - y|
+//     5  sum w G,  G = sum_{m<k} |x_m - x_k| = sum_i (2i - M + 1) (x_(i) - x_(0)) over the sorted values (i from 0)
+//     6  sum w f'o'   7  sum w f'^2   8  sum w o'^2,  f' = xb - k, o' = y - k  (NaN without a climatology)
+// A NaN member, truth or climatology value at a point makes its terms 1..8 NaN; a region reads no point whose weight in it
+// is 0 (a point with weight 0 in every region is not loaded at all).
+//
+// One thread owns one (channel, point) at a time (U of them per pass, loaded together) and holds its M values in
+// registers, padded to MP (8, 16, 32, 64) with +inf, as k_ens_stats does; G takes the bitonic network of sort_net.cuh (the
+// M = 1 instantiation does no sort).  No atomics.  Launch 1: a fixed grid of kBlocks x n_sel blocks; block b takes rows
+// b, b + kBlocks, ... in order, thread j sums the terms of points j, j + kThreads, ... of a row, then adds the row's sums,
+// weighted per region, to its running sums; the block adds its threads' sums in thread order and writes one partial per
+// (region, channel, term, block).  Launch 2 sums the kBlocks partials of each (region, channel, term) in block order.  The
+// partial layout does not depend on the SM count, so the sums are bitwise reproducible and a channel's or a region's sums
+// do not depend on the rest of the request.
+#include <cmath>
+
+#include "engine.h"
+#include "sky_common.cuh"
+#include "sort_net.cuh"
+
+namespace sky {
+namespace {
+
+constexpr int kMaxMembers = 64, kMaxSel = 128, kMaxRegions = 4, kTerms = 9, kThreads = 128, kBlocks = SKY_SCORES_BLOCKS;
+
+struct ScoresParams {
+  const float* x;              // member m, selected channel s at x + m member_stride + chan[s] plane
+  const float* truth;          // [n_sel][plane]
+  const float* clim;           // [n_sel][plane] or null
+  const double* roww;          // [n_reg][nlat]
+  double* partial;             // [n_reg][n_sel][kTerms][kBlocks]
+  double* sums;                // [n_reg][n_sel][kTerms]
+  long long member_stride;
+  int plane, nlat, nlon, members, n_sel, n_reg;
+  int chan[kMaxSel];
+};
+
+template <int MP, int U>
+__global__ void __launch_bounds__(kThreads) k_scores_partial(const __grid_constant__ ScoresParams P) {
+  const int s = blockIdx.y, b = blockIdx.x, M = P.members, R = P.n_reg, tid = threadIdx.x;
+  const double invM = 1.0 / M;
+  const float* xs = P.x + (long long)P.chan[s] * P.plane;
+  const float* ys = P.truth + (long long)s * P.plane;
+  const float* ks = P.clim ? P.clim + (long long)s * P.plane : nullptr;
+  const double qnan = __longlong_as_double(0x7ff8000000000000ll);
+  // each thread's running sums per (region, term) live in its own shared-memory column: registers hold the members
+  __shared__ double acc[kMaxRegions * kTerms][kThreads];
+  for (int i = 0; i < R * kTerms; ++i) acc[i][tid] = 0.0;
+
+  for (int row = b; row < P.nlat; row += kBlocks) {
+    double w[kMaxRegions];
+    bool any = false;
+#pragma unroll
+    for (int r = 0; r < kMaxRegions; ++r) {
+      w[r] = r < R ? P.roww[r * P.nlat + row] : 0.0;
+      any |= w[r] > 0.0;
+    }
+    if (!any) continue;   // a row outside every region is not read
+    double ra[kTerms];
+#pragma unroll
+    for (int t = 0; t < kTerms; ++t) ra[t] = 0.0;
+    for (int j0 = tid; j0 < P.nlon; j0 += U * kThreads) {
+      // U points per thread per pass: all their loads are issued before the arithmetic of the first one
+      float v[U][MP], yf[U], kf[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int j = j0 + u * kThreads;
+        const bool in = j < P.nlon;
+        const long long p = (long long)row * P.nlon + (in ? j : 0);
+#pragma unroll
+        for (int m = 0; m < MP; ++m) v[u][m] = m < M && in ? xs[m * P.member_stride + p] : __int_as_float(0x7f800000);
+        yf[u] = in ? ys[p] : 0.f;
+        kf[u] = in && ks ? ks[p] : 0.f;
+      }
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        if (j0 + u * kThreads >= P.nlon) break;
+        const double y = yf[u];
+        bool nan = yf[u] != yf[u] || kf[u] != kf[u];
+        double sum = 0.0;
+#pragma unroll
+        for (int m = 0; m < MP; ++m)
+          if (m < M) { sum = __dadd_rn(sum, (double)v[u][m]); nan |= v[u][m] != v[u][m]; }
+        const double xb = __ddiv_rn(sum, (double)M);
+        // the remaining terms do not depend on the member order: take them from the sorted values
+        if constexpr (MP > 1) bitonic_sort(v[u]);
+        const double lo = v[u][0];
+        double var = 0.0, mae = 0.0, g = 0.0, c = 1.0 - M;
+#pragma unroll
+        for (int m = 0; m < MP; ++m)
+          if (m < M) {
+            const double xm = v[u][m], d = xm - xb;
+            var += d * d;
+            mae += fabs(xm - y);
+            g += c * (xm - lo);   // G = sum_i (2i - M + 1) x_(i), shifted by x_(0): no cancellation
+            c += 2.0;
+          }
+        const double e = xb - y;
+        double term[kTerms];
+        term[0] = 1.0;
+        term[1] = e;
+        term[2] = e * e;
+        term[3] = var;
+        term[4] = mae * invM;
+        term[5] = g;
+        if (ks) {
+          const double k = kf[u], f = xb - k, o = y - k;
+          term[6] = f * o;
+          term[7] = f * f;
+          term[8] = o * o;
+        } else {
+          term[6] = term[7] = term[8] = qnan;
+        }
+#pragma unroll
+        for (int t = 0; t < kTerms; ++t) ra[t] += (nan && t > 0) ? qnan : term[t];
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < kMaxRegions; ++r)
+      if (w[r] > 0.0) {
+#pragma unroll
+        for (int t = 0; t < kTerms; ++t) acc[r * kTerms + t][tid] += w[r] * ra[t];
+      }
+  }
+  __syncthreads();
+  // fixed order: thread i sums column i of every thread in thread order
+  if (tid < R * kTerms) {
+    double a = 0.0;
+    for (int k = 0; k < kThreads; ++k) a += acc[tid][k];
+    const int r = tid / kTerms, t = tid % kTerms;
+    P.partial[(((long long)r * P.n_sel + s) * kTerms + t) * kBlocks + b] = a;
+  }
+}
+
+__global__ void __launch_bounds__(kThreads) k_scores_final(const __grid_constant__ ScoresParams P) {
+  const int i = blockIdx.x * kThreads + threadIdx.x;
+  if (i >= P.n_reg * P.n_sel * kTerms) return;
+  const double* src = P.partial + (long long)i * kBlocks;
+  double a = 0.0;
+  for (int b = 0; b < kBlocks; ++b) a += src[b];
+  P.sums[i] = a;
+}
+
+// points per thread per pass: enough loads in flight at the occupancy each padding allows
+template <int MP>
+void launch(const ScoresParams& P, cudaStream_t st) {
+  constexpr int U = MP <= 8 ? 4 : MP == 16 ? 2 : 1;
+  k_scores_partial<MP, U><<<dim3(kBlocks, P.n_sel), kThreads, 0, st>>>(P);
+}
+
+int device_ptr(const void* p, const char* what, int* dev) {
+  cudaPointerAttributes attr;
+  SKY_CUDA_OK(cudaPointerGetAttributes(&attr, p));
+  if (attr.type != cudaMemoryTypeDevice) { set_error("%s must be device memory", what); return SKY_ERR_ARG; }
+  if (*dev >= 0 && attr.device != *dev) { set_error("%s is on device %d, x on device %d", what, attr.device, *dev); return SKY_ERR_ARG; }
+  *dev = attr.device;
+  return 0;
+}
+
+}  // namespace
+}  // namespace sky
+
+using namespace sky;
+
+extern "C" {
+
+int sky_forecast_scores(const float* x, int32_t members, int64_t member_stride, int32_t nlat, int32_t nlon,
+                        int32_t channel_count, const int32_t* channels, int32_t n_sel, const float* truth, const float* clim,
+                        const double* row_weights, int32_t n_regions, double* partial, uint64_t partial_bytes, double* sums,
+                        void* stream) {
+  if (members < 1 || members > kMaxMembers) { set_error("members = %d must lie in [1, %d]", members, kMaxMembers); return SKY_ERR_ARG; }
+  if (nlat < 1 || nlon < 1 || (int64_t)nlat * nlon > INT32_MAX) {
+    set_error("nlat = %d and nlon = %d must be positive with nlat x nlon < 2^31", nlat, nlon);
+    return SKY_ERR_ARG;
+  }
+  const int64_t plane = (int64_t)nlat * nlon;
+  if (channel_count < 1) { set_error("channel_count = %d must be positive", channel_count); return SKY_ERR_ARG; }
+  if (member_stride < (int64_t)channel_count * plane) {
+    set_error("member_stride = %lld is below channel_count x plane = %lld", (long long)member_stride, (long long)channel_count * plane);
+    return SKY_ERR_ARG;
+  }
+  if (n_sel < 1 || n_sel > kMaxSel || !channels) { set_error("n_sel = %d channels must lie in [1, %d]", n_sel, kMaxSel); return SKY_ERR_ARG; }
+  if (n_regions < 1 || n_regions > kMaxRegions) { set_error("n_regions = %d must lie in [1, %d]", n_regions, kMaxRegions); return SKY_ERR_ARG; }
+  ScoresParams P{};
+  for (int s = 0; s < n_sel; ++s) {
+    if (channels[s] < 0 || channels[s] >= channel_count) { set_error("channel %d is outside [0, %d)", channels[s], channel_count); return SKY_ERR_ARG; }
+    P.chan[s] = channels[s];
+  }
+  const uint64_t need = (uint64_t)n_regions * n_sel * kTerms * kBlocks * sizeof(double);
+  if (partial_bytes < need) {
+    set_error("partial_bytes = %llu is below %llu (n_regions x n_sel x 9 x %d doubles)", (unsigned long long)partial_bytes,
+              (unsigned long long)need, kBlocks);
+    return SKY_ERR_ARG;
+  }
+  if (!x || !truth || !row_weights || !partial || !sums) {
+    set_error("x, truth, row_weights, partial and sums must not be null");
+    return SKY_ERR_ARG;
+  }
+  int dev = -1, rc;
+  if ((rc = device_ptr(x, "x", &dev)) || (rc = device_ptr(truth, "truth", &dev)) || (clim && (rc = device_ptr(clim, "clim", &dev))) ||
+      (rc = device_ptr(row_weights, "row_weights", &dev)) || (rc = device_ptr(partial, "partial", &dev)) ||
+      (rc = device_ptr(sums, "sums", &dev)))
+    return rc;
+  P.x = x;
+  P.truth = truth;
+  P.clim = clim;
+  P.roww = row_weights;
+  P.partial = partial;
+  P.sums = sums;
+  P.member_stride = member_stride;
+  P.plane = (int)plane;
+  P.nlat = nlat;
+  P.nlon = nlon;
+  P.members = members;
+  P.n_sel = n_sel;
+  P.n_reg = n_regions;
+  DeviceGuard guard(dev);   // launch on the device that owns the members, whatever the caller's current device is
+  cudaStream_t st = (cudaStream_t)stream;
+  if (members == 1) launch<1>(P, st);
+  else if (members <= 8) launch<8>(P, st);
+  else if (members <= 16) launch<16>(P, st);
+  else if (members <= 32) launch<32>(P, st);
+  else launch<64>(P, st);
+  count_launch();
+  SKY_CUDA_OK(cudaGetLastError());
+  k_scores_final<<<(n_regions * n_sel * kTerms + kThreads - 1) / kThreads, kThreads, 0, st>>>(P);
+  count_launch();
+  SKY_CUDA_OK(cudaGetLastError());
+  return SKY_OK;
+}
+
+}  // extern "C"

@@ -416,6 +416,52 @@ def multi_model_statistics(sources, channels_per_source, quantiles=(), events=()
     return stats, prob, means
 
 
+SCORES_MAX_REGIONS, SCORES_TERMS, SCORES_BLOCKS = 4, 9, 128
+
+
+def forecast_scores(x, truth, row_weights, channels=None, clim=None, channel_offset: int = 0, out=None):
+    """Verification sums of the members of a CUDA fp32 (M, C, H, W) tensor, or a view of one whose members each hold
+    contiguous (C, H, W) planes, against ``truth`` (CUDA fp32 (n_sel, H, W)) and optionally ``clim`` (same shape), per
+    region of ``row_weights`` (CUDA fp64 (n_regions, H), ``scores.region_weights``) (include/skyrim_b200.h
+    sky_forecast_scores).  Channels are counted from ``channel_offset`` (a GraphCast state scores its new time slice with
+    offset 83); ``channels`` lists the scored ones (default: all), in the order of the truth's planes.  Returns the CUDA
+    fp64 sums (n_regions, n_sel, 9) (``scores.SUMS`` names them; ``scores.metrics_from_sums`` forms the metrics), into
+    ``out`` when given.  Asynchronous on the current stream."""
+    import torch
+    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4):
+        raise ValueError("x must be a CUDA fp32 (members, channels, nlat, nlon) tensor")
+    M, Cn, H, W = x.shape
+    plane = H * W
+    if x.stride(3) != 1 or x.stride(2) != W or x.stride(1) != plane:
+        raise ValueError(f"each member of x must hold contiguous (C, H, W) planes (strides {x.stride()})")
+    if not 0 <= channel_offset < Cn:
+        raise ValueError(f"channel_offset = {channel_offset} is outside [0, {Cn})")
+    count = Cn - channel_offset
+    member_stride = x.stride(0) if M > 1 else max(x.stride(0), Cn * plane)
+    sel = list(range(count)) if channels is None else [int(c) for c in channels]
+    for name, t in (("truth", truth), ("clim", clim)):
+        if t is not None and (not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous()
+                              or tuple(t.shape) != (len(sel), H, W)):
+            raise ValueError(f"{name} must be a contiguous CUDA fp32 {(len(sel), H, W)} tensor (got {tuple(t.shape)})")
+    if not (row_weights.is_cuda and row_weights.dtype == torch.float64 and row_weights.is_contiguous()
+            and row_weights.dim() == 2 and row_weights.shape[1] == H):
+        raise ValueError(f"row_weights must be a contiguous CUDA fp64 (n_regions, {H}) tensor")
+    R = row_weights.shape[0]
+    shape = (R, len(sel), SCORES_TERMS)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float64, device=x.device)
+    if tuple(out.shape) != shape or out.dtype != torch.float64 or not out.is_contiguous():
+        raise ValueError(f"output of shape {tuple(out.shape)} {out.dtype}: contiguous fp64 {shape} needed")
+    ws = torch.empty(max(R * len(sel) * SCORES_TERMS * SCORES_BLOCKS, 1), dtype=torch.float64, device=x.device)
+    L = _ffi.lib()
+    st = torch.cuda.current_stream(x.device).cuda_stream
+    _ffi.check(L.sky_forecast_scores(x.data_ptr() + 4 * channel_offset * plane, M, member_stride, H, W, count,
+                                     (C.c_int32 * max(len(sel), 1))(*sel), len(sel), truth.data_ptr(),
+                                     None if clim is None else clim.data_ptr(), row_weights.data_ptr(), R, ws.data_ptr(),
+                                     8 * ws.numel(), out.data_ptr(), st), "sky_forecast_scores", L)
+    return out
+
+
 def unix_seconds(when) -> float:
     """datetime (naive = UTC) / numpy datetime64 / number -> unix seconds"""
     import datetime as _dt

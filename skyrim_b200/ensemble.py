@@ -41,11 +41,12 @@ class EnsembleRunner:
                  seed: int = 0, perturbation: str = "gaussian", grf: dict | None = None):
         """``perturbation``: "gaussian" adds independent N(0, 1) amp sigma_c noise at every grid point (K11);
         "spherical_grf" adds amp sigma_c times a spherical Gaussian random field of unit pointwise variance,
-        ``grf`` = keyword arguments of ``engine.perturb_ic_grf`` (alpha, tau, lmax)."""
+        ``grf`` = keyword arguments of ``engine.perturb_ic_grf`` (alpha, tau, lmax); "none" leaves every member equal to
+        ``base_state`` (one member is then the model's own unperturbed trajectory)."""
         import torch
         from .engine import perturb_ic, perturb_ic_grf
-        if perturbation not in ("gaussian", "spherical_grf"):
-            raise ValueError(f"unknown perturbation {perturbation!r} (gaussian, spherical_grf)")
+        if perturbation not in ("gaussian", "spherical_grf", "none"):
+            raise ValueError(f"unknown perturbation {perturbation!r} (gaussian, spherical_grf, none)")
         if grf and perturbation != "spherical_grf":
             raise ValueError("grf options need perturbation='spherical_grf'")
         self.engine, self.M, self.rank = engine, members_per_gpu, rank
@@ -55,7 +56,7 @@ class EnsembleRunner:
         # Philox keyed by the GLOBAL member id
         if perturbation == "gaussian":
             perturb_ic(x, self.sigma, amp, seed=seed, member0=rank * self.M)
-        else:
+        elif perturbation == "spherical_grf":
             perturb_ic_grf(x, self.sigma, amp, seed=seed, member0=rank * self.M, **(grf or {}))
         self.x, self.y = x, torch.empty_like(x)
         self.steps = 0
@@ -71,6 +72,14 @@ class EnsembleRunner:
         """ensemble mean / standard deviation over ALL members (two all-reduces, outside the step loop)"""
         return mean_and_spread(self.x, world)
 
+    def _walk(self, n_steps: int, every_slice: bool = True):
+        """Yields (n, members) for the current state (n = 0) and after each of ``n_steps`` steps; the forwards of lead n
+        are launched when the walk is asked for it.  ``members`` stays valid until the second next() after it.  The plain
+        chain has every slice; only the hierarchical schedule reads ``every_slice``."""
+        yield 0, self.x
+        for n in range(1, n_steps + 1):
+            yield n, self.step()
+
     def iter_stats(self, n_steps: int, channels=None, quantiles=(), events=(), channel_offset: int = 0):
         """Steps ``n_steps`` times and yields (n, stats, prob) for the current state (n = 0) and after each step:
         ``engine.ensemble_statistics`` of this rank's members, as pinned host tensors.  Only the statistics leave the
@@ -82,71 +91,95 @@ class EnsembleRunner:
         dev = self.x.device
         main = torch.cuda.current_stream(dev)
         copy = torch.cuda.Stream(dev)
-        ring = [ensemble_statistics(self.x, channels, quantiles, events, channel_offset)]
+        walk = self._walk(n_steps)
+        cur = next(walk)
+        ring = [ensemble_statistics(cur[1], channels, quantiles, events, channel_offset)]
         ring.append(tuple(torch.empty_like(t) for t in ring[0]))
         host = [tuple(torch.empty(t.shape, dtype=t.dtype).pin_memory() for t in ring[0]) for _ in range(2)]
         done = [torch.cuda.Event() for _ in range(2)]    # statistics i % 2 are complete on the main stream
         copied = torch.cuda.Event()
         done[0].record(main)
-        for n in range(n_steps + 1):
-            if n < n_steps:   # launch step n + 1 and its reduction before waiting for the copy of step n
-                self.step()
-                ensemble_statistics(self.x, channels, quantiles, events, channel_offset, out=ring[(n + 1) % 2])
-                done[(n + 1) % 2].record(main)
-            copy.wait_event(done[n % 2])
-            with torch.cuda.stream(copy):
-                for h, d in zip(host[n % 2], ring[n % 2]):
-                    h.copy_(d, non_blocking=True)
-                copied.record(copy)
-            copied.synchronize()   # also orders the next reduction into ring[n % 2] (launched at n + 1) after this copy
-            yield (n,) + host[n % 2]
-
-
-class HierarchicalEnsembleRunner(EnsembleRunner):
-    """``EnsembleRunner`` on Pangu's hierarchical schedule (schedule.py): ``engine`` is the 6-h handle, ``engine_24`` the
-    24-h one on its workspace, both batched over the M members, whose anchor states sit beside their chain states in the
-    plan's four buffers.  Without ``every_slice``, ``iter_stats`` yields only steps n_steps - 1 and n_steps, reached with
-    the fewest forwards.  The members are perturbed exactly as ``EnsembleRunner`` perturbs them."""
-
-    def __init__(self, engine, *args, engine_24, every_slice: bool = True, **kw):
-        super().__init__(engine, *args, **kw)
-        self.engine_24, self.every_slice = engine_24, every_slice
-
-    def step(self, n: int = 1):
-        raise NotImplementedError("a hierarchical ensemble steps through iter_stats, which follows the schedule")
-
-    def iter_stats(self, n_steps: int, channels=None, quantiles=(), events=(), channel_offset: int = 0):
-        import torch
-        from . import schedule
-        from .engine import ensemble_statistics
-        p = schedule.plan("hierarchical", n_steps, self.every_slice)
-        bufs = [self.x, self.y] + [torch.empty_like(self.x) for _ in range(schedule.N_BUFFERS - 2)]
-        engines = {"6h": self.engine, "24h": self.engine_24}
-        dev = self.x.device
-        main = torch.cuda.current_stream(dev)
-        copy = torch.cuda.Stream(dev)
-        for op, src, dst in p.forwards[:p.slices[0][2]]:   # none for slice 0; a last-slices plan may need many
-            engines[op].step(bufs[src], bufs[dst])
-        ring = [ensemble_statistics(bufs[p.slices[0][1]], channels, quantiles, events, channel_offset)]
-        ring.append(tuple(torch.empty_like(t) for t in ring[0]))
-        host = [tuple(torch.empty(t.shape, dtype=t.dtype).pin_memory() for t in ring[0]) for _ in range(2)]
-        done = [torch.cuda.Event() for _ in range(2)]    # statistics i % 2 are complete on the main stream
-        copied = torch.cuda.Event()
-        done[0].record(main)
-        for i, (n, _, _) in enumerate(p.slices):
-            if i + 1 < len(p.slices):   # the forwards and the reduction of slice i + 1 before waiting for the copy of i
-                _, buf, after = p.slices[i + 1]
-                for op, src, dst in p.forwards[p.slices[i][2]:after]:
-                    engines[op].step(bufs[src], bufs[dst])
-                ensemble_statistics(bufs[buf], channels, quantiles, events, channel_offset, out=ring[(i + 1) % 2])
+        i = 0
+        while cur is not None:
+            nxt = next(walk, None)
+            if nxt is not None:   # launch the next slice's forwards and reduction before waiting for the copy of this one
+                ensemble_statistics(nxt[1], channels, quantiles, events, channel_offset, out=ring[(i + 1) % 2])
                 done[(i + 1) % 2].record(main)
             copy.wait_event(done[i % 2])
             with torch.cuda.stream(copy):
                 for h, d in zip(host[i % 2], ring[i % 2]):
                     h.copy_(d, non_blocking=True)
                 copied.record(copy)
-            copied.synchronize()
-            yield (n,) + host[i % 2]
+            copied.synchronize()   # also orders the next reduction into ring[i % 2] (launched at i + 1) after this copy
+            yield (cur[0],) + host[i % 2]
+            cur, i = nxt, i + 1
+
+    def iter_scores(self, n_steps: int, truth_at, clim=None, channels=None, row_weights=None, channel_offset: int = 0):
+        """Steps ``n_steps`` times and scores this rank's members at every lead n = 0 .. n_steps against
+        ``truth_at(n)`` (host fp32 (n_sel, H, W) of the selected channels), with the static climatology ``clim`` (host
+        fp32 (n_sel, H, W) or None) and the regions of ``row_weights`` (fp64 (n_regions, H)): ``engine.forecast_scores``.
+        Per lead the forwards are launched first and the truth is fetched on the host while they run, then uploaded on a
+        copy stream into a ring of two device buffers (events order each upload after the scoring that last read its
+        buffer, and the scoring after the upload).  Every lead's sums stay in one device tensor that crosses to the host
+        once, at the end.  Returns (leads, fp64 host tensor (n_leads, n_regions, n_sel, 9))."""
+        import torch
+        from .engine import forecast_scores
+        dev = self.x.device
+        main = torch.cuda.current_stream(dev)
+        copy = torch.cuda.Stream(dev)
+        H, W = self.x.shape[-2:]
+        n_sel = self.x.shape[1] - channel_offset if channels is None else len(channels)
+        rw = torch.as_tensor(np.asarray(row_weights, dtype=np.float64), device=dev).contiguous()
+        kd = None if clim is None else torch.from_numpy(np.ascontiguousarray(clim, dtype=np.float32)).to(dev)
+        sums = torch.empty((n_steps + 1, rw.shape[0], n_sel, 9), dtype=torch.float64, device=dev)
+        dbuf = [torch.empty((n_sel, H, W), dtype=torch.float32, device=dev) for _ in range(2)]
+        hbuf = [torch.empty((n_sel, H, W), dtype=torch.float32).pin_memory() for _ in range(2)]
+        uploaded = [torch.cuda.Event() for _ in range(2)]   # truth i % 2 is on the device
+        scored = [torch.cuda.Event() for _ in range(2)]     # the scoring that read dbuf[i % 2] is done
+        leads = []
+        for i, (n, members) in enumerate(self._walk(n_steps, every_slice=True)):
+            y = truth_at(n)                                 # the host fetch runs under the forwards just launched
+            uploaded[i % 2].synchronize()                   # lead i - 2's upload has left hbuf[i % 2]
+            np.copyto(hbuf[i % 2].numpy(), y)
+            copy.wait_event(scored[i % 2])                  # lead i - 2's scoring has read dbuf[i % 2]
+            with torch.cuda.stream(copy):
+                dbuf[i % 2].copy_(hbuf[i % 2], non_blocking=True)
+                uploaded[i % 2].record(copy)
+            main.wait_event(uploaded[i % 2])
+            forecast_scores(members, dbuf[i % 2], rw, channels, kd, channel_offset, out=sums[i])
+            scored[i % 2].record(main)
+            leads.append(n)
+        return leads, sums.cpu()
+
+
+class HierarchicalEnsembleRunner(EnsembleRunner):
+    """``EnsembleRunner`` on Pangu's hierarchical schedule (schedule.py): ``engine`` is the 6-h handle, ``engine_24`` the
+    24-h one on its workspace, both batched over the M members, whose anchor states sit beside their chain states in the
+    plan's four buffers.  Without ``every_slice``, ``iter_stats`` yields only steps n_steps - 1 and n_steps, reached with
+    the fewest forwards; ``iter_scores`` always scores every slice.  The members are perturbed exactly as
+    ``EnsembleRunner`` perturbs them."""
+
+    def __init__(self, engine, *args, engine_24, every_slice: bool = True, **kw):
+        super().__init__(engine, *args, **kw)
+        self.engine_24, self.every_slice = engine_24, every_slice
+
+    def step(self, n: int = 1):
+        raise NotImplementedError("a hierarchical ensemble steps through iter_stats / iter_scores, which follow the "
+                                  "schedule")
+
+    def _walk(self, n_steps: int, every_slice: bool | None = None):
+        """the plan's forward walk: yields (n, buffer of slice n) once the forwards completing slice n are launched"""
+        import torch
+        from . import schedule
+        p = schedule.plan("hierarchical", n_steps, self.every_slice if every_slice is None else every_slice)
+        bufs = [self.x, self.y] + [torch.empty_like(self.x) for _ in range(schedule.N_BUFFERS - 2)]
+        engines = {"6h": self.engine, "24h": self.engine_24}
+        issued = 0
+        for n, buf, after in p.slices:   # none for slice 0; a last-slices plan may need many before its first slice
+            for op, src, dst in p.forwards[issued:after]:
+                engines[op].step(bufs[src], bufs[dst])
+            issued = after
+            yield n, bufs[buf]
         last = p.slices[-1][1]
         self.x, self.y = bufs[last], bufs[schedule.A1 if last == schedule.A0 else schedule.A0]
         self.steps += n_steps

@@ -5,10 +5,13 @@ defaults; same `run_forecast` signature and return value) on top of the H100 eng
     python -m skyrim_b200.forecast -m pangu -l 24 --members 8 --quantiles 0.1,0.5,0.9 --exceed t2m:273.15 -o outputs
     python -m skyrim_b200.forecast --models pangu,fourcastnet_v2,graphcast -l 24 --members 4 -o outputs
     python -m skyrim_b200.forecast -m pangu -l 168 --pangu_schedule hierarchical -o outputs
+    python -m skyrim_b200.forecast -m pangu -l 72 --score --truth era5.nc --climatology clim.nc -o outputs
 
 The second form runs a perturbed-initial-condition ensemble and saves its per-step statistics (mean, spread, quantiles)
 and exceedance probabilities instead of the members.  The third runs several models side by side on one GPU
 (``GlobalEnsemble``): with ``--members 1`` it saves every model's steps and their mean, above 1 the pooled statistics.
+The fifth verifies the forecast (``--members`` members) against analyses and saves one scorecard of latitude-weighted
+scores per lead time (``GlobalModel.score``).
 
 Differences, all forced by the scope of this build (SURVEY.md section 2): `--initial_conditions` accepts `synthetic`
 (the default here: the network IC providers cds / ifs / gfs are the reference's `libs/ic`, out of scope, and raise a clear
@@ -60,6 +63,23 @@ def run_ensemble_forecast(model_name: str, date: str, time: str, lead_time: int,
     return paths
 
 
+def run_score(model_name: str, date: str, time: str, lead_time: int, initial_conditions: str, output_dir: str,
+              filter_vars: str, members: int, perturbation: str, amp: float, seed: int, truth: str = "",
+              climatology: str = "", **model_kw):
+    """``--score``: ``Skyrim.score(save=True)`` against the netCDF analyses ``truth`` (time, channel, lat, lon; default: the
+    initial-condition source) and climatology (channel, lat, lon); returns the scorecard's path"""
+    from . import xr_shim as xr
+    from .core import Skyrim
+    model = Skyrim(model_name, ic_source=initial_conditions, **model_kw)
+    _, paths = model.score(
+        date=date, time=time, lead_time=lead_time, members=members, perturbation=perturbation if members > 1 else None,
+        amp=amp, seed=seed, truth=xr.open_dataarray(truth) if truth else None,
+        climatology=xr.open_dataarray(climatology) if climatology else None, save=True,
+        save_config={"output_dir": output_dir or str(Path.cwd() / "outputs"),
+                     "filter_vars": [v.strip() for v in filter_vars.split(",") if v.strip()]})
+    return paths
+
+
 def parse_quantiles(text: str):
     """"0.1,0.5,0.9" -> [0.1, 0.5, 0.9]"""
     return [float(v) for v in text.split(",") if v.strip()]
@@ -104,8 +124,12 @@ def parse_exceed(text: str):
 @click.option("--pangu_schedule", type=click.Choice(SCHEDULES), default=None,
               help="Pangu alone: '6h' (default) chains the 6-h model; 'hierarchical' interleaves the 6-h and 24-h models "
                    "as earth2mip's PanguInference does")
+@click.option("--score", is_flag=True, help="Verify the forecast (--members members) against analyses and save a scorecard")
+@click.option("--truth", type=str, default="", help="--score: netCDF analyses (time, channel, lat, lon) on the model grid "
+              "(default: the initial-condition source)")
+@click.option("--climatology", type=str, default="", help="--score: netCDF climatology (channel, lat, lon) for the ACC")
 def main(model_name, date, time, lead_time, list_models, initial_conditions, output_dir, filter_vars, modal, weight_seed, device, grid,
-         members, perturbation, amp, seed, quantiles, exceed, models, pangu_schedule):
+         members, perturbation, amp, seed, quantiles, exceed, models, pangu_schedule, score, truth, climatology):
     if modal:
         raise click.UsageError("--modal: remote execution through Modal is outside this build (SURVEY.md section 2); run locally")
     if not 1 <= members <= 64:
@@ -137,7 +161,14 @@ def main(model_name, date, time, lead_time, list_models, initial_conditions, out
             kw["cfg"] = small(model_name)
     if names:
         model_name = names
-    if members > 1 and not list_models:
+    if (truth or climatology) and not score:
+        raise click.UsageError("--truth and --climatology belong to --score")
+    if score and (names or q or events or list_models):
+        raise click.UsageError("--score verifies one model (-m), without --models, --quantiles, --exceed or --list_models")
+    if score:
+        paths = run_score(model_name, date, time, lead_time, initial_conditions, output_dir, filter_vars, members,
+                          perturbation, amp, seed, truth, climatology, **kw)
+    elif members > 1 and not list_models:
         paths = run_ensemble_forecast(model_name, date, time, lead_time, initial_conditions, output_dir, filter_vars, members,
                                       perturbation, amp, seed, q, events, **kw)
     else:

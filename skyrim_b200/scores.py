@@ -1,0 +1,161 @@
+"""Forecast verification: latitude-weighted scores per channel, region and lead time against supplied analyses, as
+earth2mip's ``score_deterministic`` / ``score_ensemble`` report them.  The device writes weighted fp64 sums
+(``engine.forecast_scores``, include/skyrim_b200.h sky_forecast_scores); this module holds the definitions, forms the
+metrics from the sums, and adapts truth and climatology sources to the model's grid and channels.
+
+Notation: channel c, region r, lead n; members x_1..x_M; ensemble mean x_bar, summed in member order in fp64 (the
+unrounded mean of ``k_ens_stats``); truth y; optional climatology k.  A region is a latitude band [lat_min, lat_max], both
+ends included (at most 4; default ``{"global": (-90, 90)}``).  The weight of point p in region r is
+w_p = cos(phi_p) / sum_{q in r} cos(phi_q), phi the latitude, with the pole rows weighted exactly 0 (earth2mip's cos-latitude
+convention; cell-area weights are not offered).  With all sums over the points of the region:
+
+    bias       sum w (x_bar - y)                                             M = 1: the forecast bias
+    rmse       sqrt(sum w (x_bar - y)^2)                                     M = 1: the deterministic RMSE
+    acc        sum w f'o' / sqrt(sum w f'^2 sum w o'^2), f' = x_bar - k, o' = y - k (uncentred, earth2mip's
+               ``weighted_acc``)                                              NaN without a climatology
+    spread     sqrt(sum w s^2), s^2 = sum_m (x_m - x_bar)^2 / (M - 1)          M = 1: NaN
+    ssr        sqrt((M + 1) / M) spread / rmse (Fortin et al. 2014)           M = 1: NaN
+    crps       sum w [(1/M) sum_m |x_m - y| - 1/(2 M^2) sum_{m,k} |x_m - x_k|] (the empirical-CDF CRPS, as properscoring
+               computes it)                                                   M = 1: the MAE
+    crps_fair  the same with 1/(2 M (M - 1)) in the second term              M = 1: NaN
+
+A NaN member, truth or climatology value at a point with w > 0 in a region makes that channel's scores for that region NaN;
+points with w = 0 are not read into that region's sums; scores never depend on which other channels or regions were
+requested.
+"""
+from __future__ import annotations
+
+import datetime
+
+import numpy as np
+
+METRICS = ("bias", "rmse", "acc", "spread", "ssr", "crps", "crps_fair")
+# the nine sums the device writes per (region, channel), in order (G = sum_{m<k} |x_m - x_k|)
+SUMS = ("w", "w_e", "w_e2", "w_var", "w_mae", "w_g", "w_fo", "w_ff", "w_oo")
+MAX_REGIONS = 4
+DEFAULT_REGIONS = {"global": (-90.0, 90.0)}
+_LAT_EPS = 1e-9   # degrees: a band end equal to a grid latitude up to rounding includes that row
+
+
+def region_weights(lat, regions=None):
+    """(names, fp64 (n_regions, nlat) row weights): for region r, row i gets cos(lat_i) if lat_i lies in the band (both
+    ends included), else 0; the pole rows get exactly 0; each region's row weights sum to 1 (the weight of a point is its
+    row's weight over nlon)."""
+    regions = dict(DEFAULT_REGIONS if regions is None else regions)
+    if not 1 <= len(regions) <= MAX_REGIONS:
+        raise ValueError(f"{len(regions)} regions: 1 to {MAX_REGIONS} latitude bands")
+    lat = np.asarray(lat, dtype=np.float64)
+    cos = np.cos(np.deg2rad(lat))
+    cos[np.abs(np.abs(lat) - 90.0) <= _LAT_EPS] = 0.0
+    cos = np.maximum(cos, 0.0)
+    names, rows = [], []
+    for name, band in regions.items():
+        lo, hi = (float(v) for v in band)
+        if not -90.0 <= lo <= hi <= 90.0:
+            raise ValueError(f"region {name!r}: band ({lo}, {hi}) must satisfy -90 <= lat_min <= lat_max <= 90")
+        w = np.where((lat >= lo - _LAT_EPS) & (lat <= hi + _LAT_EPS), cos, 0.0)
+        if not w.sum() > 0.0:
+            raise ValueError(f"region {name!r}: band ({lo}, {hi}) holds no grid row of positive weight")
+        names.append(str(name))
+        rows.append(w / w.sum())
+    return names, np.stack(rows)
+
+
+def metrics_from_sums(sums, members: int):
+    """fp64 (..., 7) metrics (``METRICS`` order) from fp64 (..., 9) sums of ``members`` members (``SUMS`` order)."""
+    s = np.asarray(sums, dtype=np.float64)
+    M = int(members)
+    if M < 1:
+        raise ValueError(f"members = {M} must be at least 1")
+    w, e, e2, var, mae, g, fo, ff, oo = (s[..., i] for i in range(9))
+    nan = np.full(w.shape, np.nan)
+    with np.errstate(divide="ignore", invalid="ignore"):
+        bias = e / w
+        rmse = np.sqrt(e2 / w)
+        acc = fo / np.sqrt(ff * oo)
+        if M > 1:
+            spread = np.sqrt(var / (M - 1) / w)
+            ssr = np.sqrt((M + 1) / M) * spread / rmse
+            crps_fair = (mae - g / (M * (M - 1))) / w
+        else:
+            spread = ssr = crps_fair = nan
+        crps = (mae - g / (M * M)) / w
+    return np.stack([bias, rmse, acc, spread, ssr, crps, crps_fair], axis=-1)
+
+
+# ---- truth and climatology ------------------------------------------------------------------------------------------------
+def _check_grid(da, lat, lon, what):
+    for name, want in (("lat", lat), ("lon", lon)):
+        have = np.asarray(da.coords[name], dtype=np.float64) if name in da.coords else None
+        if have is None or have.shape != np.shape(want) or not np.allclose(have, want, rtol=0.0, atol=1e-6):
+            n = "none" if have is None else len(have)
+            raise ValueError(f"{what}'s {name} ({n} values) differs from the model's grid ({len(want)} values); "
+                             "regrid it onto the model grid first")
+
+
+def _select(da, channels, what):
+    have = [str(c) for c in np.asarray(da.coords["channel"])] if "channel" in da.coords else []
+    missing = [c for c in channels if c not in have]
+    if missing:
+        raise ValueError(f"{what} lacks channel(s) {missing}")
+    vals = np.asarray(da.values, dtype=np.float32)
+    ax = list(da.dims).index("channel")
+    return np.ascontiguousarray(np.take(vals, [have.index(c) for c in channels], axis=ax))
+
+
+def truth_fetcher(truth, channels, lat, lon, times=()):
+    """``time -> fp32 (n_sel, nlat, nlon)`` from ``truth``: a data source (``source[time] -> DataArray(channel, lat,
+    lon)``, the ``ic_source`` protocol) or a DataArray with dims (time, channel, lat, lon).  Refuses a grid that differs
+    from the model's, a missing channel and a missing time, each by name; a DataArray is checked for every one of
+    ``times`` at once, a data source when each time is fetched."""
+    if hasattr(truth, "dims") and "time" in tuple(truth.dims):
+        if tuple(truth.dims) != ("time", "channel", "lat", "lon"):
+            raise ValueError(f"truth dims {tuple(truth.dims)}: (time, channel, lat, lon) needed")
+        _check_grid(truth, lat, lon, "truth")
+        have = np.asarray(truth.coords["time"]).astype("datetime64[s]")
+        vals = _select(truth, channels, "truth")
+
+        def at(t):
+            hit = np.nonzero(have == np.datetime64(t, "s"))[0]
+            if hit.size == 0:
+                raise ValueError(f"truth has no analysis at {np.datetime64(t, 's')}")
+            return vals[hit[0]]
+        for t in times:
+            at(t)
+        return at
+    if not hasattr(truth, "__getitem__") or isinstance(truth, str):
+        raise TypeError("truth must be a data source (source[time] -> DataArray) or a DataArray with a time dimension")
+
+    def at(t):
+        try:
+            da = truth[t]
+        except KeyError as e:
+            raise ValueError(f"truth has no analysis at {np.datetime64(t, 's')}") from e
+        if tuple(da.dims)[-2:] != ("lat", "lon") or "channel" not in da.dims:
+            raise ValueError(f"truth[{t}] has dims {tuple(da.dims)}: (channel, lat, lon) needed")
+        _check_grid(da, lat, lon, "truth")
+        v = _select(da, channels, "truth")
+        return v[-1] if v.ndim == 4 else v
+    return at
+
+
+def climatology_fields(clim, channels, lat, lon):
+    """fp32 (n_sel, nlat, nlon) of a static climatology DataArray (channel, lat, lon), or None"""
+    if clim is None:
+        return None
+    if tuple(clim.dims) != ("channel", "lat", "lon"):
+        raise ValueError(f"climatology dims {tuple(clim.dims)}: (channel, lat, lon) needed")
+    _check_grid(clim, lat, lon, "climatology")
+    return _select(clim, channels, "climatology")
+
+
+def scorecard(sums, members: int, leads_hours, regions, channels, model: str, start_time: datetime.datetime):
+    """DataArray (lead_time, metric, region, channel) of fp64 metrics from fp64 sums (lead, region, channel, 9); lead_time in
+    hours (0: the initial condition); the model, members and start time in attrs."""
+    from . import xr_shim as xr
+    m = metrics_from_sums(sums, members)                     # (lead, region, channel, metric)
+    return xr.DataArray(np.ascontiguousarray(np.moveaxis(m, -1, 1)), dims=["lead_time", "metric", "region", "channel"],
+                        coords=dict(lead_time=np.asarray(leads_hours, dtype=np.float64), metric=np.array(METRICS),
+                                    region=np.array(list(regions)), channel=np.array(list(channels))),
+                        attrs=dict(model=str(model), members=int(members),
+                                   start_time=str(np.datetime64(start_time, "s"))))

@@ -147,8 +147,11 @@ class DataArray:
                 else:
                     v = f.createVariable(d, "d", (d,))
                     v[:] = c.astype(np.float64)
-            var = f.createVariable(self.name or "__xarray_dataarray_variable__", "f", self.dims)
-            var[:] = self.values.astype(np.float32)
+            wide = self.values.dtype == np.float64   # fp64 arrays (scorecards) keep their precision; the rest is fp32
+            var = f.createVariable(self.name or "__xarray_dataarray_variable__", "d" if wide else "f", self.dims)
+            var[:] = self.values.astype(np.float64 if wide else np.float32)
+            for k, v in self.attrs.items():   # scalar attributes become global attributes, as xarray writes them
+                setattr(f, k, v)
 
     def to_zarr(self, store, mode="w", append_dim=None, consolidated=True):
         """zarr v2 directory store, uncompressed, one chunk per leading index."""
@@ -253,7 +256,9 @@ def open_dataarray(path, engine=None):
                     coords[d] = np.asarray(v[:]).astype("int64").astype("datetime64[s]")
                 else:
                     coords[d] = np.array(v[:])
-        return DataArray(np.array(var[:]), dims, coords)
+        attrs = {k: v.decode() if isinstance(v, bytes) else v.item() if np.ndim(v) == 0 or np.size(v) == 1 else v
+                 for k, v in f._attributes.items()}
+        return DataArray(np.array(var[:]), dims, coords, attrs=attrs)
 
 
 if HAVE_XARRAY:  # pragma: no cover
