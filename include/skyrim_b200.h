@@ -260,6 +260,45 @@ SKY_API int sky_forecast_scores(const float* x, int32_t members, int64_t member_
                                 const float* clim, const double* row_weights, int32_t n_regions, double* partial,
                                 uint64_t partial_bytes, double* sums, void* stream);
 
+/* Rank histogram (Talagrand diagram) of the truth among `members` states on one device, per latitude-band region and
+ * selected channel, into caller-owned device buffers.  x, members, member_stride, nlat, nlon, channel_count, channels,
+ * n_sel, truth and row_weights as for sky_forecast_scores;
+ *   seed, date_index, lead_index  the Philox key (seed < 2^32, date_index) and the lead word of the tie-breaking draws;
+ *   counts       device int32 workspace of at least counts_bytes = 4 * n_sel * nlat * (members + 2) bytes;
+ *   hist         device fp64 [n_regions][n_sel][members + 1].
+ * At each point, with L = #{x_m < y} and E = #{x_m = y}, the truth's rank is L + floor(u (E + 1)), u = w / 2^32 and w the
+ * first output word of Philox4x32-10 at key (seed, date_index), counter (point index in the plane, "RNK1" = 0x524E4B31,
+ * channels[s], lead_index): ties are broken at random (Hamill 2001), so a 1-member forecast equal to its truth spreads
+ * over both bins instead of filling bin 0.  A point's rank depends on nothing else: not on the channel selection, the
+ * regions, the batch or the launch geometry.  hist[r][s][k] = sum over the points with w > 0 of (w / nlon) 1{rank = k},
+ * which sums to 1 over k for the normalised weights of skyrim_b200.scores.region_weights.  A NaN member or truth value at
+ * a point with w > 0 in a region makes that region's whole histogram of that channel NaN.  Two launches, no atomics on
+ * floating-point values: per (row, channel) integer counts per rank, then a sum over the rows in row order, so the
+ * histogram is bitwise reproducible and independent of the SM count.  Refused with SKY_ERR_ARG before any CUDA call:
+ * the arguments sky_forecast_scores refuses, a seed of 2^32 or more, a negative date_index or lead_index, counts_bytes
+ * out of range, null pointers; and before any launch: x, truth, row_weights, counts or hist not device memory on one
+ * device.  Asynchronous and stream-ordered; launches on the device that owns x. */
+SKY_API int sky_forecast_rank_histogram(const float* x, int32_t members, int64_t member_stride, int32_t nlat, int32_t nlon,
+                                        int32_t channel_count, const int32_t* channels, int32_t n_sel, const float* truth,
+                                        const double* row_weights, int32_t n_regions, uint64_t seed, int32_t date_index,
+                                        int32_t lead_index, int32_t* counts, uint64_t counts_bytes, double* hist,
+                                        void* stream);
+
+/* Per-point score-map accumulators of `members` states on one device against an analysis, added in place.
+ * x, members, member_stride, nlat, nlon, channel_count, channels, n_sel and truth as for sky_forecast_scores;
+ *   maps         device fp64 [n_sel][5][plane], accumulated in place: maps[s][t][p] += term t at point p.
+ * The five terms are sky_forecast_scores' sums 1..5 per point instead of summed: e = x_bar - y, e^2,
+ * sum_m (x_m - x_bar)^2, (1/M) sum_m |x_m - y| and G = sum_{m<k} |x_m - x_k|, with the same fp64 arithmetic (one shared
+ * device function), so bias, RMSE, spread and CRPS maps follow from them as skyrim_b200.scores.metrics_from_sums forms
+ * the scalars.  One thread per (channel, point); each call adds once per point, so accumulators summed over calls are
+ * bitwise reproducible in call order.  A NaN member or truth value makes only that point's five accumulators NaN.
+ * Refused with SKY_ERR_ARG before any CUDA call: the member, grid, channel and truth arguments sky_forecast_scores
+ * refuses, a null maps; and before any launch: x, truth or maps not device memory on one device.  Asynchronous and
+ * stream-ordered; launches on the device that owns x. */
+SKY_API int sky_forecast_score_maps(const float* x, int32_t members, int64_t member_stride, int32_t nlat, int32_t nlon,
+                                    int32_t channel_count, const int32_t* channels, int32_t n_sel, const float* truth,
+                                    double* maps, void* stream);
+
 /* Per-kernel-family device timing (CUDA events recorded on the launching stream around the
  * launches whose family bit is set in tag_mask).  profile_end synchronises on the recorded
  * events and returns the summed milliseconds and launch counts per family.  Used by bench.py

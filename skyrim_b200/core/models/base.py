@@ -243,13 +243,36 @@ class GlobalModel:
         default to the forecast channels (forcings excluded), ``regions`` to ``{"global": (-90, 90)}`` (at most 4 latitude
         bands).  The scores are formed on the device and the sums of all leads cross to the host once.  ``save`` writes
         the scorecard as one netCDF file, model "<model>-score<M>", under the forecast id."""
+        from ... import scores as S
+        if n_steps < 0:
+            raise ValueError(f"n_steps = {n_steps} must not be negative")
+        times = [start_time + n * self.time_step for n in range(n_steps + 1)]
+        perturbation, sel, region_names, row_weights, truth_at, clim = self._score_setup(
+            members, perturbation, channels, regions, truth, climatology, times, save, save_config)
+        names = list(self.out_channel_names)
+        runner, offset = self._score_runner(start_time, members, perturbation, amp, seed, grf)
+        leads, sums = runner.iter_scores(n_steps, lambda n: truth_at(times[n]), clim,
+                                         [names.index(c) for c in sel], row_weights, offset)
+        hours = [n * self.time_step.total_seconds() / 3600 for n in leads]
+        card = S.scorecard(np.asarray(sums), members, hours, region_names, sel, self.model_name, start_time)
+        logger.success(f"Scored {len(leads)} leads of {members} member(s) on {len(sel)} channels")
+        paths = []
+        if save:
+            save_config = {k: v for k, v in save_config.items() if k != "filter_vars"}   # selected on the device already
+            save_config.setdefault("forecast_id", generate_forecast_id())
+            source = self.ic_source if isinstance(self.ic_source, str) else "file"
+            paths.append(save_forecast(card, f"{self.model_name}-score{members}", start_time,
+                                       start_time + n_steps * self.time_step, source, config=save_config))
+        return card, paths
+
+    def _score_setup(self, members, perturbation, channels, regions, truth, climatology, times, save, save_config):
+        """the checks and host inputs shared by ``score`` and ``score_period``, before any engine call: (perturbation,
+        scored channel names, region names, row weights, truth fetcher, climatology fields)"""
         from ... import engine as E
         from ... import scores as S
         names = list(self.out_channel_names)
         if not 1 <= members <= E.ENS_MAX_MEMBERS:
             raise ValueError(f"members = {members} must lie in [1, {E.ENS_MAX_MEMBERS}]")
-        if n_steps < 0:
-            raise ValueError(f"n_steps = {n_steps} must not be negative")
         if perturbation is None:
             perturbation = "none" if members == 1 else "spherical_grf"
         if perturbation not in ("none", "gaussian", "spherical_grf"):
@@ -274,32 +297,106 @@ class GlobalModel:
             if truth is None:
                 raise ValueError(f"{self.model_name} has no data source to verify against (synthetic initial conditions): "
                                  "pass truth=")
-        times = [start_time + n * self.time_step for n in range(n_steps + 1)]
         truth_at = S.truth_fetcher(truth, sel, lat, lon, times)
         clim = S.climatology_fields(climatology, sel, lat, lon)
+        return perturbation, sel, region_names, row_weights, truth_at, clim
+
+    def _score_runner(self, start_time, members, perturbation, amp, seed, grf):
+        """(member runner of the forecast from ``start_time``, offset of the scored channels in its state)"""
         from ...ensemble import EnsembleRunner, HierarchicalEnsembleRunner
         if perturbation == "spherical_grf" and grf is None:
-            grf = dict(lmax=min(180, (len(lat) - 1) // 2))
+            grf = dict(lmax=min(180, (len(self.model.grid.lat) - 1) // 2))
         base, sigma, offset = self._ensemble_initial_state(start_time)
         make = EnsembleRunner
         if hasattr(self.model, "engine_24"):   # Pangu's hierarchical schedule: every slice is scored
             make = functools.partial(HierarchicalEnsembleRunner, engine_24=self.model.engine_24, every_slice=True)
         runner = make(self.model.engine, base, sigma, members_per_gpu=members, rank=0, amp=amp, seed=seed,
                       perturbation=perturbation, grf=grf)
-        leads, sums = runner.iter_scores(n_steps, lambda n: truth_at(times[n]), clim,
-                                         [names.index(c) for c in sel], row_weights, offset)
-        hours = [n * self.time_step.total_seconds() / 3600 for n in leads]
-        card = S.scorecard(np.asarray(sums), members, hours, region_names, sel, self.model_name, start_time)
-        logger.success(f"Scored {len(leads)} leads of {members} member(s) on {len(sel)} channels")
+        return runner, offset
+
+    def score_period(self, start_times, n_steps: int, truth=None, climatology=None, members: int = 1,
+                     perturbation: str | None = None, amp: float = 0.05, seed: int = 0, grf: dict | None = None,
+                     channels: List[str] = [], regions: dict | None = None, map_leads=(), map_channels=(),
+                     save: bool = False, save_config: dict = {}):
+        """Verifies the forecasts from every one of ``start_times`` (distinct, increasing) at leads 0, 6, .., 6 ``n_steps`` h
+        and returns (``scores.PeriodScores``, paths).  Date d is the forecast ``score(start_times[d], seed=seed + d)``
+        verifies, with the same arguments; its scorecard is ``.cards[d]`` bit for bit.  ``.card`` holds the period's
+        metrics (``scores.period_metrics``), ``.rank_histogram`` the rank histogram (lead_time, region, channel, rank)
+        averaged over the dates, with ties broken by Philox draws keyed by (``seed``, d).  With ``map_leads`` (hours,
+        multiples of the time step in [0, lead]) and ``map_channels`` (scored forecast channels), ``.maps`` holds per-point
+        bias, rmse, spread and crps over the period, fp32 (lead_time, metric, channel, lat, lon).  Everything is checked
+        before the first engine call, a truth DataArray for every valid time of every date.  One member runner serves all
+        dates, restarted in place, and the truth buffers, the sums, histograms and map accumulators are allocated once;
+        only the results cross to the host, at the end.  ``save`` writes the period card, the per-date cards, the rank
+        histogram and the maps as netCDF files, models "<model>-period<M>[-cards|-rank|-maps]", under one forecast id."""
+        import torch
+        from ... import engine as E
+        from ... import scores as S
+        names = list(self.out_channel_names)
+        starts = list(start_times)
+        if not starts:
+            raise ValueError("score_period needs at least one start time")
+        if any(b <= a for a, b in zip(starts, starts[1:])):
+            raise ValueError(f"start times must be distinct and sorted: {[str(np.datetime64(t, 's')) for t in starts]}")
+        if n_steps < 0:
+            raise ValueError(f"n_steps = {n_steps} must not be negative")
+        if not 0 <= seed < 2 ** 32:
+            raise ValueError(f"seed = {seed} must lie in [0, 2^32)")
+        step_h = self.time_step.total_seconds() / 3600
+        bad = [h for h in map_leads if not (0 <= h <= n_steps * step_h and float(h) / step_h == int(float(h) / step_h))]
+        if bad:
+            raise ValueError(f"map lead(s) {list(bad)} h: multiples of the {step_h:g}-h time step in [0, {n_steps * step_h:g}] "
+                             "needed")
+        if bool(len(map_leads)) != bool(len(map_channels)):
+            raise ValueError("map_leads and map_channels go together: give both or neither")
+        times = sorted({t + n * self.time_step for t in starts for n in range(n_steps + 1)})
+        perturbation, sel, region_names, row_weights, truth_at, clim = self._score_setup(
+            members, perturbation, channels, regions, truth, climatology, times, save, save_config)
+        mch = list(dict.fromkeys(map_channels))
+        unknown = [c for c in mch if c not in names]
+        if unknown:
+            raise ValueError(f"unknown map channel(s) {unknown} for {self.model_name}")
+        forcing = [c for c in mch if c in self.forcing_channels]
+        if forcing:
+            raise ValueError(f"map channel(s) {forcing} are forcings, not forecasts, and are not scored")
+        unscored = [c for c in mch if c not in sel]
+        if unscored:
+            raise ValueError(f"map channel(s) {unscored} are not among the scored channels {sel}")
+        mch = [c for c in sel if c in mch]
+        slots = {int(round(h / step_h)): i for i, h in enumerate(sorted({float(h) for h in map_leads}))}
+        D, L, R, Sn, M = len(starts), n_steps + 1, len(region_names), len(sel), members
+        runner = None
+        for d, t0 in enumerate(starts):
+            if runner is None:
+                runner, offset = self._score_runner(t0, members, perturbation, amp, seed, grf)
+                dev = runner.x.device
+                H, W = runner.x.shape[-2:]
+                sums = torch.empty((D, L, R, Sn, len(S.SUMS)), dtype=torch.float64, device=dev)
+                hist = torch.empty((D, L, R, Sn, M + 1), dtype=torch.float64, device=dev)
+                maps = torch.zeros((len(slots), len(mch), E.MAP_TERMS, H, W), dtype=torch.float64, device=dev)
+                ring = runner.truth_ring(Sn)
+            else:
+                runner.restart(self._ensemble_initial_state(t0)[0], seed + d)
+            valid = [t0 + n * self.time_step for n in range(L)]
+            runner.iter_scores(n_steps, lambda n: truth_at(valid[n]), clim, [names.index(c) for c in sel], row_weights,
+                               offset, hist=hist[d], seed=seed, date_index=d, maps=maps, map_slot=slots,
+                               map_channels=[sel.index(c) for c in mch], sums=sums[d], ring=ring)
+            logger.success(f"Scored start date {d + 1}/{D}: {np.datetime64(t0, 's')}")
+        sums, hist = sums.cpu().numpy(), hist.cpu().numpy()
+        hours = [n * step_h for n in range(L)]
+        res = S.PeriodScores.build(sums, hist, maps.cpu().numpy() if mch else None, members, starts, hours,
+                                   sorted(slots, key=slots.get), step_h, region_names, sel, mch, self.model_name,
+                                   np.array(self.model.grid.lat), np.array(self.model.grid.lon))
         paths = []
         if save:
             save_config = {k: v for k, v in save_config.items() if k != "filter_vars"}   # selected on the device already
             save_config.setdefault("forecast_id", generate_forecast_id())
             source = self.ic_source if isinstance(self.ic_source, str) else "file"
-            paths.append(save_forecast(card, f"{self.model_name}-score{members}", start_time,
-                                       start_time + n_steps * self.time_step, source, config=save_config))
-        return card, paths
-
+            label, t_end = f"{self.model_name}-period{members}", starts[-1] + n_steps * self.time_step
+            for suffix, da in (("", res.card), ("-cards", res.cards), ("-rank", res.rank_histogram), ("-maps", res.maps)):
+                if da is not None:
+                    paths.append(save_forecast(da, label + suffix, starts[0], t_end, source, config=save_config))
+        return res, paths
 
 class GlobalPrediction:
     filepath: Path | None = None

@@ -194,6 +194,10 @@ class GlobalEnsemble:
         raise NotImplementedError("forecast scores are computed per model: score each model with Skyrim(name).score; "
                                   "multi-model scoring is not built")
 
+    def score_period(self, *args, **kw):
+        raise NotImplementedError("forecast scores are computed per model: verify a period for each model with "
+                                  "Skyrim(name).score_period; multi-model scoring is not built")
+
     # -- device states ---------------------------------------------------------------------------------------------------
     def _layout(self, m):
         """(state channels, offset of the output slice in the state): a GraphCast state holds two time slices"""

@@ -69,3 +69,27 @@ class Skyrim:
         n_steps = self.model.time_steps(lead_time)
         logger.debug(f"Scoring {n_steps} steps")
         return self.model.score(start_time=start_time, n_steps=n_steps, **kw)
+
+    def score_period(self, start: str, end: str, time: str = "0000", every: int = 24, lead_time: int = 6, **kw):
+        """Verification over a period (``GlobalModel.score_period``): start dates from ``start`` (YYYYMMDD) at ``time``
+        (HHMM) every ``every`` hours (a multiple of 6) through the date ``end``, inclusive; the lead time is read as
+        ``predict`` reads it; ``kw`` goes to ``GlobalModel.score_period`` (truth, climatology, members, perturbation, amp,
+        seed, grf, channels, regions, map_leads, map_channels, save, save_config).  Returns (PeriodScores, paths)."""
+        return self.model.score_period(start_times=period_start_times(start, end, time, every),
+                                       n_steps=self.model.time_steps(lead_time), **kw)
+
+
+def period_start_times(start: str, end: str, time: str = "0000", every: int = 24):
+    """start times from ``start`` + ``time`` every ``every`` hours (a positive multiple of 6) while their date is at most
+    ``end``"""
+    if every <= 0 or every % 6:
+        raise ValueError(f"every = {every} h: a positive multiple of 6 h needed")
+    t = datetime.datetime(int(start[:4]), int(start[4:6]), int(start[6:8]), int(time[:2]), int(time[2:4]))
+    stop = datetime.datetime(int(end[:4]), int(end[4:6]), int(end[6:8])) + datetime.timedelta(days=1)
+    if t >= stop:
+        raise ValueError(f"end date {end} lies before the first start time {t}")
+    out = []
+    while t < stop:
+        out.append(t)
+        t += datetime.timedelta(hours=every)
+    return out

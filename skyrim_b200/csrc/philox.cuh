@@ -1,7 +1,11 @@
-// Philox4x32-10 (Salmon et al., SC'11; the Random123 constants), shared by the two initial-condition perturbations:
-// K11's per-grid-point Gaussian noise (sky_abi.cu) and the spherical Gaussian random field (perturb_grf.cu).  The
-// counter layouts of the two never meet: K11's second counter word is the high half of a grid index, which is 0 for
-// every grid this project runs, and the field's second word is the constant "GRF1".
+// Philox4x32-10 (Salmon et al., SC'11; the Random123 constants), shared by the two initial-condition perturbations,
+// K11's per-grid-point Gaussian noise (sky_abi.cu) and the spherical Gaussian random field (perturb_grf.cu), and by the
+// rank histogram's tie-breaking draws (score_points.cu).  The counter layouts never meet, whatever the keys:
+//   K11          key seed,                 counter (quad index, its high half = 0 on every grid this project runs, channel,
+//                                                   member)
+//   GRF          key seed,                 counter (l | m << 16, "GRF1", channel, member)
+//   rank ties    key (seed, date index),   counter (point, "RNK1", channel, lead index)
+// The second counter word tells them apart: 0, "GRF1" (0x47524631) or "RNK1" (0x524E4B31).
 #pragma once
 #include <stdint.h>
 

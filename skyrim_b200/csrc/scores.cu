@@ -11,18 +11,18 @@
 // is 0 (a point with weight 0 in every region is not loaded at all).
 //
 // One thread owns one (channel, point) at a time (U of them per pass, loaded together) and holds its M values in
-// registers, padded to MP (8, 16, 32, 64) with +inf, as k_ens_stats does; G takes the bitonic network of sort_net.cuh (the
-// M = 1 instantiation does no sort).  No atomics.  Launch 1: a fixed grid of kBlocks x n_sel blocks; block b takes rows
-// b, b + kBlocks, ... in order, thread j sums the terms of points j, j + kThreads, ... of a row, then adds the row's sums,
-// weighted per region, to its running sums; the block adds its threads' sums in thread order and writes one partial per
-// (region, channel, term, block).  Launch 2 sums the kBlocks partials of each (region, channel, term) in block order.  The
+// registers, padded to MP (8, 16, 32, 64) with +inf, as k_ens_stats does; the mean, var, mae and G come from
+// ens_point_terms (point_terms.cuh), which the per-point score maps share.  No atomics.  Launch 1: a fixed grid of
+// kBlocks x n_sel blocks; block b takes rows b, b + kBlocks, ... in order, thread j sums the terms of points j,
+// j + kThreads, ... of a row, then adds the row's sums, weighted per region, to its running sums; the block adds its
+// threads' sums in thread order and writes one partial per (region, channel, term, block).  Launch 2 sums the kBlocks partials of each (region, channel, term) in block order.  The
 // partial layout does not depend on the SM count, so the sums are bitwise reproducible and a channel's or a region's sums
 // do not depend on the rest of the request.
 #include <cmath>
 
 #include "engine.h"
+#include "point_terms.cuh"
 #include "sky_common.cuh"
-#include "sort_net.cuh"
 
 namespace sky {
 namespace {
@@ -82,33 +82,16 @@ __global__ void __launch_bounds__(kThreads) k_scores_partial(const __grid_consta
       for (int u = 0; u < U; ++u) {
         if (j0 + u * kThreads >= P.nlon) break;
         const double y = yf[u];
-        bool nan = yf[u] != yf[u] || kf[u] != kf[u];
-        double sum = 0.0;
-#pragma unroll
-        for (int m = 0; m < MP; ++m)
-          if (m < M) { sum = __dadd_rn(sum, (double)v[u][m]); nan |= v[u][m] != v[u][m]; }
-        const double xb = __ddiv_rn(sum, (double)M);
-        // the remaining terms do not depend on the member order: take them from the sorted values
-        if constexpr (MP > 1) bitonic_sort(v[u]);
-        const double lo = v[u][0];
-        double var = 0.0, mae = 0.0, g = 0.0, c = 1.0 - M;
-#pragma unroll
-        for (int m = 0; m < MP; ++m)
-          if (m < M) {
-            const double xm = v[u][m], d = xm - xb;
-            var += d * d;
-            mae += fabs(xm - y);
-            g += c * (xm - lo);   // G = sum_i (2i - M + 1) x_(i), shifted by x_(0): no cancellation
-            c += 2.0;
-          }
-        const double e = xb - y;
+        const EnsPointTerms q = ens_point_terms(v[u], M, y, yf[u] != yf[u] || kf[u] != kf[u]);
+        const bool nan = q.nan;
+        const double xb = q.xb, e = xb - y;
         double term[kTerms];
         term[0] = 1.0;
         term[1] = e;
         term[2] = e * e;
-        term[3] = var;
-        term[4] = mae * invM;
-        term[5] = g;
+        term[3] = q.var;
+        term[4] = q.mae * invM;
+        term[5] = q.g;
         if (ks) {
           const double k = kf[u], f = xb - k, o = y - k;
           term[6] = f * o;

@@ -1,6 +1,6 @@
 // Ascending in-register sort of MP floats (MP a power of two): a fully unrolled bitonic network, min / max on registers
 // only, so v[] stays in registers.  +inf padding sorts behind every finite value.  Shared by the ensemble statistics'
-// quantiles (ens_stats.cu) and the CRPS spread term of the forecast scores (scores.cu).
+// quantiles (ens_stats.cu) and the CRPS spread term of the forecast scores and score maps (point_terms.cuh).
 #pragma once
 
 namespace sky {

@@ -417,16 +417,13 @@ def multi_model_statistics(sources, channels_per_source, quantiles=(), events=()
 
 
 SCORES_MAX_REGIONS, SCORES_TERMS, SCORES_BLOCKS = 4, 9, 128
+MAP_TERMS = 5
 
 
-def forecast_scores(x, truth, row_weights, channels=None, clim=None, channel_offset: int = 0, out=None):
-    """Verification sums of the members of a CUDA fp32 (M, C, H, W) tensor, or a view of one whose members each hold
-    contiguous (C, H, W) planes, against ``truth`` (CUDA fp32 (n_sel, H, W)) and optionally ``clim`` (same shape), per
-    region of ``row_weights`` (CUDA fp64 (n_regions, H), ``scores.region_weights``) (include/skyrim_b200.h
-    sky_forecast_scores).  Channels are counted from ``channel_offset`` (a GraphCast state scores its new time slice with
-    offset 83); ``channels`` lists the scored ones (default: all), in the order of the truth's planes.  Returns the CUDA
-    fp64 sums (n_regions, n_sel, 9) (``scores.SUMS`` names them; ``scores.metrics_from_sums`` forms the metrics), into
-    ``out`` when given.  Asynchronous on the current stream."""
+def _verified_members(x, channels, channel_offset, row_weights=None, **fields):
+    """the member, channel and truth checks of the verification entries: (M, H, W, plane, count, member_stride, sel) of x,
+    with every named field (truth, clim) None or a contiguous CUDA fp32 (n_sel, H, W) tensor, and ``row_weights`` None or
+    a contiguous CUDA fp64 (n_regions, H) tensor"""
     import torch
     if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4):
         raise ValueError("x must be a CUDA fp32 (members, channels, nlat, nlon) tensor")
@@ -439,13 +436,28 @@ def forecast_scores(x, truth, row_weights, channels=None, clim=None, channel_off
     count = Cn - channel_offset
     member_stride = x.stride(0) if M > 1 else max(x.stride(0), Cn * plane)
     sel = list(range(count)) if channels is None else [int(c) for c in channels]
-    for name, t in (("truth", truth), ("clim", clim)):
+    for name, t in fields.items():
         if t is not None and (not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous()
                               or tuple(t.shape) != (len(sel), H, W)):
             raise ValueError(f"{name} must be a contiguous CUDA fp32 {(len(sel), H, W)} tensor (got {tuple(t.shape)})")
-    if not (row_weights.is_cuda and row_weights.dtype == torch.float64 and row_weights.is_contiguous()
-            and row_weights.dim() == 2 and row_weights.shape[1] == H):
+    if row_weights is not None and not (row_weights.is_cuda and row_weights.dtype == torch.float64
+                                        and row_weights.is_contiguous() and row_weights.dim() == 2
+                                        and row_weights.shape[1] == H):
         raise ValueError(f"row_weights must be a contiguous CUDA fp64 (n_regions, {H}) tensor")
+    return M, H, W, plane, count, member_stride, sel
+
+
+def forecast_scores(x, truth, row_weights, channels=None, clim=None, channel_offset: int = 0, out=None):
+    """Verification sums of the members of a CUDA fp32 (M, C, H, W) tensor, or a view of one whose members each hold
+    contiguous (C, H, W) planes, against ``truth`` (CUDA fp32 (n_sel, H, W)) and optionally ``clim`` (same shape), per
+    region of ``row_weights`` (CUDA fp64 (n_regions, H), ``scores.region_weights``) (include/skyrim_b200.h
+    sky_forecast_scores).  Channels are counted from ``channel_offset`` (a GraphCast state scores its new time slice with
+    offset 83); ``channels`` lists the scored ones (default: all), in the order of the truth's planes.  Returns the CUDA
+    fp64 sums (n_regions, n_sel, 9) (``scores.SUMS`` names them; ``scores.metrics_from_sums`` forms the metrics), into
+    ``out`` when given.  Asynchronous on the current stream."""
+    import torch
+    M, H, W, plane, count, member_stride, sel = _verified_members(x, channels, channel_offset, row_weights,
+                                                                  truth=truth, clim=clim)
     R = row_weights.shape[0]
     shape = (R, len(sel), SCORES_TERMS)
     if out is None:
@@ -460,6 +472,53 @@ def forecast_scores(x, truth, row_weights, channels=None, clim=None, channel_off
                                      None if clim is None else clim.data_ptr(), row_weights.data_ptr(), R, ws.data_ptr(),
                                      8 * ws.numel(), out.data_ptr(), st), "sky_forecast_scores", L)
     return out
+
+
+def forecast_rank_histogram(x, truth, row_weights, seed: int, date_index: int, lead_index: int, channels=None,
+                            channel_offset: int = 0, out=None):
+    """Rank histogram of ``truth`` (CUDA fp32 (n_sel, H, W)) among the members of x (as for ``forecast_scores``), per
+    region of ``row_weights`` (include/skyrim_b200.h sky_forecast_rank_histogram): ties between the truth and members are
+    broken by Philox draws keyed by (``seed``, ``date_index``) and counted by (point, channel index in x from
+    ``channel_offset``, ``lead_index``).  Returns the CUDA fp64 (n_regions, n_sel, M + 1) histogram, each summing to 1,
+    into ``out`` when given.  Asynchronous on the current stream."""
+    import torch
+    M, H, W, plane, count, member_stride, sel = _verified_members(x, channels, channel_offset, row_weights, truth=truth)
+    if not 0 <= int(seed) < 2 ** 32 or int(date_index) < 0 or int(lead_index) < 0:
+        raise ValueError(f"seed = {seed} must lie in [0, 2^32), date_index = {date_index} and lead_index = {lead_index} "
+                         "must not be negative")
+    R = row_weights.shape[0]
+    shape = (R, len(sel), M + 1)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float64, device=x.device)
+    if tuple(out.shape) != shape or out.dtype != torch.float64 or not out.is_contiguous():
+        raise ValueError(f"output of shape {tuple(out.shape)} {out.dtype}: contiguous fp64 {shape} needed")
+    ws = torch.empty(max(len(sel) * H * (M + 2), 1), dtype=torch.int32, device=x.device)
+    L = _ffi.lib()
+    st = torch.cuda.current_stream(x.device).cuda_stream
+    _ffi.check(L.sky_forecast_rank_histogram(x.data_ptr() + 4 * channel_offset * plane, M, member_stride, H, W, count,
+                                             (C.c_int32 * max(len(sel), 1))(*sel), len(sel), truth.data_ptr(),
+                                             row_weights.data_ptr(), R, int(seed), int(date_index), int(lead_index),
+                                             ws.data_ptr(), 4 * ws.numel(), out.data_ptr(), st),
+               "sky_forecast_rank_histogram", L)
+    return out
+
+
+def score_maps_accumulate(x, truth, maps, channels=None, channel_offset: int = 0):
+    """Adds the per-point terms e, e^2, sum_m (x_m - x_bar)^2, mae and G of the members of x against ``truth`` (both as
+    for ``forecast_scores``) to ``maps``, a CUDA fp64 (n_sel, 5, H, W) tensor of accumulators (include/skyrim_b200.h
+    sky_forecast_score_maps; ``scores.map_metrics`` forms the maps).  Returns ``maps``.  Asynchronous on the current
+    stream."""
+    import torch
+    M, H, W, plane, count, member_stride, sel = _verified_members(x, channels, channel_offset, truth=truth)
+    shape = (len(sel), MAP_TERMS, H, W)
+    if tuple(maps.shape) != shape or maps.dtype != torch.float64 or not maps.is_contiguous() or not maps.is_cuda:
+        raise ValueError(f"maps of shape {tuple(maps.shape)} {maps.dtype}: contiguous CUDA fp64 {shape} needed")
+    L = _ffi.lib()
+    st = torch.cuda.current_stream(x.device).cuda_stream
+    _ffi.check(L.sky_forecast_score_maps(x.data_ptr() + 4 * channel_offset * plane, M, member_stride, H, W, count,
+                                         (C.c_int32 * max(len(sel), 1))(*sel), len(sel), truth.data_ptr(),
+                                         maps.data_ptr(), st), "sky_forecast_score_maps", L)
+    return maps
 
 
 def unix_seconds(when) -> float:

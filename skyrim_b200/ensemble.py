@@ -44,21 +44,36 @@ class EnsembleRunner:
         ``grf`` = keyword arguments of ``engine.perturb_ic_grf`` (alpha, tau, lmax); "none" leaves every member equal to
         ``base_state`` (one member is then the model's own unperturbed trajectory)."""
         import torch
-        from .engine import perturb_ic, perturb_ic_grf
         if perturbation not in ("gaussian", "spherical_grf", "none"):
             raise ValueError(f"unknown perturbation {perturbation!r} (gaussian, spherical_grf, none)")
         if grf and perturbation != "spherical_grf":
             raise ValueError("grf options need perturbation='spherical_grf'")
         self.engine, self.M, self.rank = engine, members_per_gpu, rank
+        self.amp, self.perturbation, self.grf = amp, perturbation, grf
         dev = torch.device("cuda", engine.device)
         x = torch.as_tensor(base_state, dtype=torch.float32)[None].repeat(self.M, 1, 1, 1).to(dev).contiguous()
         self.sigma = torch.as_tensor(sigma_c, dtype=torch.float32, device=dev)
-        # Philox keyed by the GLOBAL member id
-        if perturbation == "gaussian":
-            perturb_ic(x, self.sigma, amp, seed=seed, member0=rank * self.M)
-        elif perturbation == "spherical_grf":
-            perturb_ic_grf(x, self.sigma, amp, seed=seed, member0=rank * self.M, **(grf or {}))
+        self._perturb(x, seed)
         self.x, self.y = x, torch.empty_like(x)
+        self.steps = 0
+
+    def _perturb(self, x, seed: int):
+        from .engine import perturb_ic, perturb_ic_grf
+        # Philox keyed by the GLOBAL member id
+        if self.perturbation == "gaussian":
+            perturb_ic(x, self.sigma, self.amp, seed=seed, member0=self.rank * self.M)
+        elif self.perturbation == "spherical_grf":
+            perturb_ic_grf(x, self.sigma, self.amp, seed=seed, member0=self.rank * self.M, **(self.grf or {}))
+
+    def restart(self, base_state, seed: int):
+        """Starts a new forecast in the existing member tensors: every member becomes ``base_state`` perturbed with
+        ``seed`` (the perturbation, amplitude and options of the constructor), bit for bit the members a new runner
+        built with ``seed`` would hold.  A verification campaign restarts one runner for each start date."""
+        import torch
+        self.x[0].copy_(torch.as_tensor(base_state, dtype=torch.float32))
+        if self.M > 1:
+            self.x[1:].copy_(self.x[:1].expand(self.M - 1, *self.x.shape[1:]))
+        self._perturb(self.x, seed)
         self.steps = 0
 
     def step(self, n: int = 1):
@@ -114,28 +129,49 @@ class EnsembleRunner:
             yield (cur[0],) + host[i % 2]
             cur, i = nxt, i + 1
 
-    def iter_scores(self, n_steps: int, truth_at, clim=None, channels=None, row_weights=None, channel_offset: int = 0):
+    def truth_ring(self, n_sel: int):
+        """the truth buffers of ``iter_scores`` for ``n_sel`` channels: a copy stream and two device and two pinned host
+        (n_sel, H, W) fp32 buffers with their events.  Pinning dominates the set-up of a scoring call, so a campaign over
+        many start dates makes one ring and passes it to every call."""
+        import torch
+        dev = self.x.device
+        H, W = self.x.shape[-2:]
+        return dict(copy=torch.cuda.Stream(dev),
+                    dbuf=[torch.empty((n_sel, H, W), dtype=torch.float32, device=dev) for _ in range(2)],
+                    hbuf=[torch.empty((n_sel, H, W), dtype=torch.float32).pin_memory() for _ in range(2)],
+                    uploaded=[torch.cuda.Event() for _ in range(2)],   # truth i % 2 is on the device
+                    scored=[torch.cuda.Event() for _ in range(2)])     # the work that read dbuf[i % 2] is done
+
+    def iter_scores(self, n_steps: int, truth_at, clim=None, channels=None, row_weights=None, channel_offset: int = 0,
+                    hist=None, seed: int = 0, date_index: int = 0, maps=None, map_slot=None, map_channels=(), sums=None,
+                    ring=None):
         """Steps ``n_steps`` times and scores this rank's members at every lead n = 0 .. n_steps against
         ``truth_at(n)`` (host fp32 (n_sel, H, W) of the selected channels), with the static climatology ``clim`` (host
         fp32 (n_sel, H, W) or None) and the regions of ``row_weights`` (fp64 (n_regions, H)): ``engine.forecast_scores``.
         Per lead the forwards are launched first and the truth is fetched on the host while they run, then uploaded on a
         copy stream into a ring of two device buffers (events order each upload after the scoring that last read its
         buffer, and the scoring after the upload).  Every lead's sums stay in one device tensor that crosses to the host
-        once, at the end.  Returns (leads, fp64 host tensor (n_leads, n_regions, n_sel, 9))."""
+        once, at the end.  Returns (leads, fp64 host tensor (n_leads, n_regions, n_sel, 9)).
+
+        Off the same uploaded truth, optionally: ``hist`` (CUDA fp64 (n_leads, n_regions, n_sel, M + 1)) receives each
+        lead's ``engine.forecast_rank_histogram`` with key (``seed``, ``date_index``) and lead index n; ``maps`` (CUDA fp64
+        (n_slots, len(map_channels), 5, H, W)) accumulates ``engine.score_maps_accumulate`` of the channels at positions
+        ``map_channels`` of ``channels`` at each lead n in ``map_slot`` (dict lead -> slot).  ``sums`` (CUDA fp64
+        (n_leads, n_regions, n_sel, 9)) receives the sums, and is returned on the device instead of a host copy; ``ring``
+        (``truth_ring``) replaces the truth buffers this call would allocate."""
         import torch
-        from .engine import forecast_scores
+        from .engine import forecast_rank_histogram, forecast_scores, score_maps_accumulate
         dev = self.x.device
         main = torch.cuda.current_stream(dev)
-        copy = torch.cuda.Stream(dev)
-        H, W = self.x.shape[-2:]
         n_sel = self.x.shape[1] - channel_offset if channels is None else len(channels)
+        sel = list(range(n_sel)) if channels is None else list(channels)
         rw = torch.as_tensor(np.asarray(row_weights, dtype=np.float64), device=dev).contiguous()
         kd = None if clim is None else torch.from_numpy(np.ascontiguousarray(clim, dtype=np.float32)).to(dev)
-        sums = torch.empty((n_steps + 1, rw.shape[0], n_sel, 9), dtype=torch.float64, device=dev)
-        dbuf = [torch.empty((n_sel, H, W), dtype=torch.float32, device=dev) for _ in range(2)]
-        hbuf = [torch.empty((n_sel, H, W), dtype=torch.float32).pin_memory() for _ in range(2)]
-        uploaded = [torch.cuda.Event() for _ in range(2)]   # truth i % 2 is on the device
-        scored = [torch.cuda.Event() for _ in range(2)]     # the scoring that read dbuf[i % 2] is done
+        out = sums if sums is not None else torch.empty((n_steps + 1, rw.shape[0], n_sel, 9), dtype=torch.float64,
+                                                        device=dev)
+        ring = ring or self.truth_ring(n_sel)
+        copy, dbuf, hbuf, uploaded, scored = (ring[k] for k in ("copy", "dbuf", "hbuf", "uploaded", "scored"))
+        map_slot = map_slot or {}
         leads = []
         for i, (n, members) in enumerate(self._walk(n_steps, every_slice=True)):
             y = truth_at(n)                                 # the host fetch runs under the forwards just launched
@@ -146,10 +182,17 @@ class EnsembleRunner:
                 dbuf[i % 2].copy_(hbuf[i % 2], non_blocking=True)
                 uploaded[i % 2].record(copy)
             main.wait_event(uploaded[i % 2])
-            forecast_scores(members, dbuf[i % 2], rw, channels, kd, channel_offset, out=sums[i])
+            forecast_scores(members, dbuf[i % 2], rw, channels, kd, channel_offset, out=out[i])
+            if hist is not None:
+                forecast_rank_histogram(members, dbuf[i % 2], rw, seed, date_index, n, channels, channel_offset,
+                                        out=hist[i])
+            if n in map_slot:
+                for j, k in enumerate(map_channels):       # one plane of the truth per map channel
+                    score_maps_accumulate(members, dbuf[i % 2][k:k + 1], maps[map_slot[n], j:j + 1], [sel[k]],
+                                          channel_offset)
             scored[i % 2].record(main)
             leads.append(n)
-        return leads, sums.cpu()
+        return leads, (out if sums is not None else out.cpu())
 
 
 class HierarchicalEnsembleRunner(EnsembleRunner):
@@ -172,7 +215,9 @@ class HierarchicalEnsembleRunner(EnsembleRunner):
         import torch
         from . import schedule
         p = schedule.plan("hierarchical", n_steps, self.every_slice if every_slice is None else every_slice)
-        bufs = [self.x, self.y] + [torch.empty_like(self.x) for _ in range(schedule.N_BUFFERS - 2)]
+        if getattr(self, "_spare", None) is None:   # the plan's other buffers, kept for the next walk
+            self._spare = [torch.empty_like(self.x) for _ in range(schedule.N_BUFFERS - 2)]
+        bufs = [self.x, self.y] + self._spare
         engines = {"6h": self.engine, "24h": self.engine_24}
         issued = 0
         for n, buf, after in p.slices:   # none for slice 0; a last-slices plan may need many before its first slice
@@ -182,6 +227,7 @@ class HierarchicalEnsembleRunner(EnsembleRunner):
             yield n, bufs[buf]
         last = p.slices[-1][1]
         self.x, self.y = bufs[last], bufs[schedule.A1 if last == schedule.A0 else schedule.A0]
+        self._spare = [b for b in bufs if b is not self.x and b is not self.y]
         self.steps += n_steps
 
 

@@ -6,12 +6,16 @@ defaults; same `run_forecast` signature and return value) on top of the H100 eng
     python -m skyrim_b200.forecast --models pangu,fourcastnet_v2,graphcast -l 24 --members 4 -o outputs
     python -m skyrim_b200.forecast -m pangu -l 168 --pangu_schedule hierarchical -o outputs
     python -m skyrim_b200.forecast -m pangu -l 72 --score --truth era5.nc --climatology clim.nc -o outputs
+    python -m skyrim_b200.forecast -m pangu -d 20240501 -l 72 --score --until 20240531 --map_channels z500,t850 \
+        --map_leads 24,72 --truth era5.nc -o outputs
 
 The second form runs a perturbed-initial-condition ensemble and saves its per-step statistics (mean, spread, quantiles)
 and exceedance probabilities instead of the members.  The third runs several models side by side on one GPU
 (``GlobalEnsemble``): with ``--members 1`` it saves every model's steps and their mean, above 1 the pooled statistics.
 The fifth verifies the forecast (``--members`` members) against analyses and saves one scorecard of latitude-weighted
-scores per lead time (``GlobalModel.score``).
+scores per lead time (``GlobalModel.score``).  With ``--until`` (or ``--every`` / ``--map_channels`` / ``--map_leads``) it
+verifies every start date through the last one (``GlobalModel.score_period``) and saves the period's scorecard, the
+per-date scorecards, the rank histogram and, for ``--map_channels`` at ``--map_leads``, per-point score maps.
 
 Differences, all forced by the scope of this build (SURVEY.md section 2): `--initial_conditions` accepts `synthetic`
 (the default here: the network IC providers cds / ifs / gfs are the reference's `libs/ic`, out of scope, and raise a clear
@@ -80,6 +84,25 @@ def run_score(model_name: str, date: str, time: str, lead_time: int, initial_con
     return paths
 
 
+def run_score_period(model_name: str, date: str, time: str, lead_time: int, until: str, every: int, map_channels,
+                     map_leads, initial_conditions: str, output_dir: str, filter_vars: str, members: int,
+                     perturbation: str, amp: float, seed: int, truth: str = "", climatology: str = "", **model_kw):
+    """``--score --until``: ``Skyrim.score_period(save=True)`` over the start dates ``date`` .. ``until``; returns the
+    paths of the period card, the per-date cards, the rank histogram and the maps"""
+    from . import xr_shim as xr
+    from .core import Skyrim
+    model = Skyrim(model_name, ic_source=initial_conditions, **model_kw)
+    _, paths = model.score_period(
+        start=date, end=until, time=time, every=every, lead_time=lead_time, members=members,
+        perturbation=perturbation if members > 1 else None, amp=amp, seed=seed,
+        truth=xr.open_dataarray(truth) if truth else None,
+        climatology=xr.open_dataarray(climatology) if climatology else None, map_leads=map_leads,
+        map_channels=map_channels, save=True,
+        save_config={"output_dir": output_dir or str(Path.cwd() / "outputs"),
+                     "filter_vars": [v.strip() for v in filter_vars.split(",") if v.strip()]})
+    return paths
+
+
 def parse_quantiles(text: str):
     """"0.1,0.5,0.9" -> [0.1, 0.5, 0.9]"""
     return [float(v) for v in text.split(",") if v.strip()]
@@ -128,8 +151,16 @@ def parse_exceed(text: str):
 @click.option("--truth", type=str, default="", help="--score: netCDF analyses (time, channel, lat, lon) on the model grid "
               "(default: the initial-condition source)")
 @click.option("--climatology", type=str, default="", help="--score: netCDF climatology (channel, lat, lon) for the ACC")
+@click.option("--until", type=str, default="", help="--score: the last start date YYYYMMDD; verifies every start date from "
+              "--date through it and saves period scores and a rank histogram")
+@click.option("--every", type=int, default=None, help="--score --until: hours between start dates (a multiple of 6; "
+              "default 24)")
+@click.option("--map_channels", type=str, default="", help="--score --until: channels of per-point score maps such as "
+              "z500,t850")
+@click.option("--map_leads", type=str, default="", help="--score --until: lead times in hours of the maps such as 24,72")
 def main(model_name, date, time, lead_time, list_models, initial_conditions, output_dir, filter_vars, modal, weight_seed, device, grid,
-         members, perturbation, amp, seed, quantiles, exceed, models, pangu_schedule, score, truth, climatology):
+         members, perturbation, amp, seed, quantiles, exceed, models, pangu_schedule, score, truth, climatology, until, every,
+         map_channels, map_leads):
     if modal:
         raise click.UsageError("--modal: remote execution through Modal is outside this build (SURVEY.md section 2); run locally")
     if not 1 <= members <= 64:
@@ -165,7 +196,19 @@ def main(model_name, date, time, lead_time, list_models, initial_conditions, out
         raise click.UsageError("--truth and --climatology belong to --score")
     if score and (names or q or events or list_models):
         raise click.UsageError("--score verifies one model (-m), without --models, --quantiles, --exceed or --list_models")
-    if score:
+    period = bool(until or every is not None or map_channels or map_leads)
+    if period and not score:
+        raise click.UsageError("--until, --every, --map_channels and --map_leads belong to --score")
+    if period:
+        try:
+            m_leads = [float(v) for v in map_leads.split(",") if v.strip()]
+        except ValueError:
+            raise click.UsageError(f"--map_leads {map_leads}: lead times in hours such as 24,72")
+        m_chans = [v.strip() for v in map_channels.split(",") if v.strip()]
+        paths = run_score_period(model_name, date, time, lead_time, until or date, 24 if every is None else every, m_chans,
+                                 m_leads, initial_conditions, output_dir, filter_vars, members, perturbation, amp, seed,
+                                 truth, climatology, **kw)
+    elif score:
         paths = run_score(model_name, date, time, lead_time, initial_conditions, output_dir, filter_vars, members,
                           perturbation, amp, seed, truth, climatology, **kw)
     elif members > 1 and not list_models:

@@ -83,6 +83,38 @@ def metrics_from_sums(sums, members: int):
     return np.stack([bias, rmse, acc, spread, ssr, crps, crps_fair], axis=-1)
 
 
+def period_metrics(sums_per_date, members: int):
+    """fp64 (..., 7) metrics of a verification period from fp64 (n_dates, ..., 9) per-date sums.  acc is the mean over the
+    dates of each date's acc (WeatherBench2 averages ACC per initial time); every other metric is formed from the sums
+    added over the dates: rmse = sqrt(mean MSE), bias = mean bias, spread = sqrt(mean variance), crps = mean crps, and
+    ssr from the period's spread and rmse.  One date gives ``metrics_from_sums`` of its sums exactly."""
+    s = np.asarray(sums_per_date, dtype=np.float64)
+    if s.ndim < 2 or s.shape[0] < 1 or s.shape[-1] != len(SUMS):
+        raise ValueError(f"sums of shape {s.shape}: (n_dates >= 1, ..., {len(SUMS)}) needed")
+    m = metrics_from_sums(s.sum(axis=0), members)
+    m[..., METRICS.index("acc")] = metrics_from_sums(s, members)[..., METRICS.index("acc")].mean(axis=0)
+    return m
+
+
+MAP_METRICS = ("bias", "rmse", "spread", "crps")
+MAP_TERMS = ("e", "e2", "var", "mae", "g")    # the five per-point accumulators of sky_forecast_score_maps, in order
+
+
+def map_metrics(acc, n_dates: int, members: int):
+    """fp32 (..., 4, H, W) maps (``MAP_METRICS`` order) from fp64 (..., 5, H, W) per-point accumulators summed over
+    ``n_dates`` start dates, formed point by point as ``metrics_from_sums`` forms the scalars (each point with weight 1
+    per date)."""
+    a = np.asarray(acc, dtype=np.float64)
+    lead = a.shape[:-3]
+    out = np.empty(lead + (len(MAP_METRICS),) + a.shape[-2:], dtype=np.float32)
+    pick = [METRICS.index(k) for k in MAP_METRICS]
+    for idx in np.ndindex(*lead):            # one (5, H, W) block at a time: the (H, W, 9) sums stay small
+        t = np.moveaxis(a[idx], 0, -1)
+        s9 = np.concatenate([np.full(t.shape[:-1] + (1,), float(n_dates)), t, np.full(t.shape[:-1] + (3,), np.nan)], -1)
+        out[idx] = np.moveaxis(metrics_from_sums(s9, members)[..., pick], -1, 0)
+    return out
+
+
 # ---- truth and climatology ------------------------------------------------------------------------------------------------
 def _check_grid(da, lat, lon, what):
     for name, want in (("lat", lat), ("lon", lon)):
@@ -159,3 +191,45 @@ def scorecard(sums, members: int, leads_hours, regions, channels, model: str, st
                                     region=np.array(list(regions)), channel=np.array(list(channels))),
                         attrs=dict(model=str(model), members=int(members),
                                    start_time=str(np.datetime64(start_time, "s"))))
+
+
+class PeriodScores:
+    """What ``GlobalModel.score_period`` returns: DataArrays of a verification period over several start dates.
+        card            fp64 (lead_time, metric, region, channel): the period's metrics (``period_metrics``)
+        cards           fp64 (start_time, lead_time, metric, region, channel): each date's scorecard
+        rank_histogram  fp64 (lead_time, region, channel, rank): the rank histograms averaged over the dates
+        maps            fp32 (lead_time, metric, channel, lat, lon) of ``MAP_METRICS`` over the period, or None"""
+
+    def __init__(self, card, cards, rank_histogram, maps=None):
+        self.card, self.cards, self.rank_histogram, self.maps = card, cards, rank_histogram, maps
+
+    @classmethod
+    def build(cls, sums, hist, maps, members: int, start_times, leads_hours, map_leads, step_hours: float, regions,
+              channels, map_channels, model: str, lat, lon):
+        """from host fp64 sums (date, lead, region, channel, 9), histograms (date, lead, region, channel, M + 1) and map
+        accumulators (map lead, map channel, 5, lat, lon) summed over the dates, or None; ``map_leads`` lists the steps of
+        the map slots in slot order"""
+        from . import xr_shim as xr
+        starts = np.array([str(np.datetime64(t, "s")) for t in start_times])
+        attrs = dict(model=str(model), members=int(members), first_start=str(starts[0]), last_start=str(starts[-1]),
+                     n_dates=len(starts))
+        common = dict(lead_time=np.asarray(leads_hours, dtype=np.float64), region=np.array(list(regions)),
+                      channel=np.array(list(channels)))
+        card = xr.DataArray(np.ascontiguousarray(np.moveaxis(period_metrics(sums, members), -1, 1)),
+                            dims=["lead_time", "metric", "region", "channel"],
+                            coords=dict(common, metric=np.array(METRICS)), attrs=dict(attrs))
+        cards = xr.DataArray(np.ascontiguousarray(np.moveaxis(metrics_from_sums(sums, members), -1, 2)),
+                             dims=["start_time", "lead_time", "metric", "region", "channel"],
+                             coords=dict(common, start_time=starts, metric=np.array(METRICS)), attrs=dict(attrs))
+        rank = xr.DataArray(np.ascontiguousarray(np.asarray(hist, dtype=np.float64).mean(axis=0)),
+                            dims=["lead_time", "region", "channel", "rank"],
+                            coords=dict(common, rank=np.arange(members + 1, dtype=np.float64)), attrs=dict(attrs))
+        mp = None
+        if maps is not None:
+            mp = xr.DataArray(np.ascontiguousarray(np.swapaxes(map_metrics(maps, len(starts), members), 1, 2)),
+                              dims=["lead_time", "metric", "channel", "lat", "lon"],
+                              coords=dict(lead_time=np.array([n * step_hours for n in map_leads], dtype=np.float64),
+                                          metric=np.array(MAP_METRICS), channel=np.array(list(map_channels)),
+                                          lat=np.asarray(lat, dtype=np.float64), lon=np.asarray(lon, dtype=np.float64)),
+                              attrs=dict(attrs))
+        return cls(card, cards, rank, mp)
