@@ -16,6 +16,8 @@ namespace sky {
 extern std::atomic<uint64_t> g_launches;
 inline void count_launch(int n = 1) { g_launches.fetch_add((uint64_t)n, std::memory_order_relaxed); }
 void set_error(const char* fmt, ...);
+// 0 when p is device memory (on device *dev, or on the device of the first pointer checked); else SKY_ERR_ARG / CUDA
+int device_of(const void* p, const char* what, int* dev);
 
 // kernel families, used for per-kernel CUDA-event timing (bench.py roofline) and launch counting
 enum KTag { KT_EMBED = 0, KT_QKV, KT_ATTN, KT_PROJ, KT_FC1, KT_FC2, KT_MLP, KT_DOWN, KT_UP, KT_RECOVER, KT_COPY,

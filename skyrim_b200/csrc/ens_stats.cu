@@ -19,13 +19,14 @@
 #include <cmath>
 
 #include "engine.h"
+#include "member_fields.h"
 #include "sky_common.cuh"
 #include "sort_net.cuh"
 
 namespace sky {
 namespace {
 
-constexpr int kMaxMembers = 64, kMaxSel = 128, kMaxQ = 8, kMaxEvents = 64, kThreads = 128;
+constexpr int kMaxQ = 8, kMaxEvents = 64, kThreads = 128;
 
 // travels by value (kernel parameter space): the host validates everything before any CUDA call
 struct EnsStatsParams {
@@ -161,6 +162,13 @@ void launch(const MultiStatsParams& P, dim3 grid, cudaStream_t st) {
 template <class Params>
 int set_quantiles_events(Params& P, int members, int n_sel, const double* quantiles, int n_q, const int32_t* event_sel,
                          const float* event_thr, int n_events) {
+  if (n_q < 0 || n_q > kMaxQ || (n_q && !quantiles)) { set_error("n_q = %d quantiles must lie in [0, %d]", n_q, kMaxQ); return SKY_ERR_ARG; }
+  if (n_events < 0 || n_events > kMaxEvents || (n_events && (!event_sel || !event_thr))) {
+    set_error("n_events = %d events must lie in [0, %d]", n_events, kMaxEvents);
+    return SKY_ERR_ARG;
+  }
+  P.n_q = n_q;
+  P.n_events = n_events;
   for (int q = 0; q < n_q; ++q) {
     const double v = quantiles[q];
     if (!(v >= 0.0 && v <= 1.0)) { set_error("quantile %g is outside [0, 1]", v); return SKY_ERR_ARG; }
@@ -179,15 +187,6 @@ int set_quantiles_events(Params& P, int members, int n_sel, const double* quanti
   return 0;
 }
 
-int device_ptr(const void* p, const char* what, int* dev) {
-  cudaPointerAttributes attr;
-  SKY_CUDA_OK(cudaPointerGetAttributes(&attr, p));
-  if (attr.type != cudaMemoryTypeDevice) { set_error("%s must be device memory", what); return SKY_ERR_ARG; }
-  if (*dev >= 0 && attr.device != *dev) { set_error("%s is on device %d, x on device %d", what, attr.device, *dev); return SKY_ERR_ARG; }
-  *dev = attr.device;
-  return 0;
-}
-
 }  // namespace
 }  // namespace sky
 
@@ -199,46 +198,27 @@ int sky_ensemble_stats(const float* x, int32_t members, int64_t member_stride, i
                        const int32_t* channels, int32_t n_sel, const double* quantiles, int32_t n_q,
                        const int32_t* event_sel, const float* event_thr, int32_t n_events, float* stats, float* prob,
                        void* stream) {
-  if (members < 1 || members > kMaxMembers) { set_error("members = %d must lie in [1, %d]", members, kMaxMembers); return SKY_ERR_ARG; }
-  if (plane < 1 || channel_count < 1) { set_error("plane (%lld) and channel_count (%d) must be positive", (long long)plane, channel_count); return SKY_ERR_ARG; }
-  if (member_stride < (int64_t)channel_count * plane) {
-    set_error("member_stride = %lld is below channel_count x plane = %lld", (long long)member_stride, (long long)channel_count * plane);
-    return SKY_ERR_ARG;
-  }
-  if (n_sel < 1 || n_sel > kMaxSel || !channels) { set_error("n_sel = %d channels must lie in [1, %d]", n_sel, kMaxSel); return SKY_ERR_ARG; }
-  if (n_q < 0 || n_q > kMaxQ || (n_q && !quantiles)) { set_error("n_q = %d quantiles must lie in [0, %d]", n_q, kMaxQ); return SKY_ERR_ARG; }
-  if (n_events < 0 || n_events > kMaxEvents || (n_events && (!event_sel || !event_thr))) {
-    set_error("n_events = %d events must lie in [0, %d]", n_events, kMaxEvents);
-    return SKY_ERR_ARG;
-  }
   EnsStatsParams P{};
-  P.member_stride = member_stride;
-  P.plane = plane;
-  P.members = members;
-  P.n_sel = n_sel;
-  P.n_q = n_q;
-  P.n_events = n_events;
-  for (int s = 0; s < n_sel; ++s) {
-    if (channels[s] < 0 || channels[s] >= channel_count) { set_error("channel %d is outside [0, %d)", channels[s], channel_count); return SKY_ERR_ARG; }
-    P.chan[s] = channels[s];
-  }
   int rc;
-  if ((rc = set_quantiles_events(P, members, n_sel, quantiles, n_q, event_sel, event_thr, n_events))) return rc;
+  if ((rc = check_members(members, member_stride, plane, channel_count, channels, n_sel, P.chan)) ||
+      (rc = set_quantiles_events(P, members, n_sel, quantiles, n_q, event_sel, event_thr, n_events)))
+    return rc;
   if (!x || !stats || (n_events && !prob)) { set_error("x, stats and (with events) prob must not be null"); return SKY_ERR_ARG; }
   int dev = -1;
-  if ((rc = device_ptr(x, "x", &dev)) || (rc = device_ptr(stats, "stats", &dev)) ||
-      (n_events && (rc = device_ptr(prob, "prob", &dev))))
+  if ((rc = device_of(x, "x", &dev)) || (rc = device_of(stats, "stats", &dev)) ||
+      (n_events && (rc = device_of(prob, "prob", &dev))))
     return rc;
   P.x = x;
   P.stats = stats;
   P.prob = prob;
+  P.member_stride = member_stride;
+  P.plane = plane;
+  P.members = members;
+  P.n_sel = n_sel;
   DeviceGuard guard(dev);   // launch on the device that owns the members, whatever the caller's current device is
   const dim3 grid((unsigned)((plane + kThreads - 1) / kThreads), (unsigned)n_sel);
   cudaStream_t st = (cudaStream_t)stream;
-  if (members <= 8) launch<8>(P, grid, st);
-  else if (members <= 16) launch<16>(P, grid, st);
-  else if (members <= 32) launch<32>(P, grid, st);
-  else launch<64>(P, grid, st);
+  dispatch_padding<8>(members, [&](auto mp) { launch<mp>(P, grid, st); });
   count_launch();
   SKY_CUDA_OK(cudaGetLastError());
   return SKY_OK;
@@ -266,17 +246,10 @@ int sky_ensemble_stats_multi(int32_t n_sources, const float* const* x, const int
   }
   if (total > kMaxMembers) { set_error("total members = %d exceed %d", total, kMaxMembers); return SKY_ERR_ARG; }
   if (n_sel < 1 || n_sel > kMaxSel || !channels) { set_error("n_sel = %d channels must lie in [1, %d]", n_sel, kMaxSel); return SKY_ERR_ARG; }
-  if (n_q < 0 || n_q > kMaxQ || (n_q && !quantiles)) { set_error("n_q = %d quantiles must lie in [0, %d]", n_q, kMaxQ); return SKY_ERR_ARG; }
-  if (n_events < 0 || n_events > kMaxEvents || (n_events && (!event_sel || !event_thr))) {
-    set_error("n_events = %d events must lie in [0, %d]", n_events, kMaxEvents);
-    return SKY_ERR_ARG;
-  }
   MultiStatsParams P{};
   P.plane = plane;
   P.members = total;
   P.n_sel = n_sel;
-  P.n_q = n_q;
-  P.n_events = n_events;
   P.n_src = n_sources;
   for (int k = 0; k < n_sources; ++k) {
     P.src_members[k] = members[k];
@@ -293,9 +266,9 @@ int sky_ensemble_stats_multi(int32_t n_sources, const float* const* x, const int
   if (!stats || (n_events && !prob)) { set_error("stats and (with events) prob must not be null"); return SKY_ERR_ARG; }
   int dev = -1;
   for (int k = 0; k < n_sources; ++k)
-    if ((rc = device_ptr(x[k], "x[k]", &dev))) return rc;
-  if ((rc = device_ptr(stats, "stats", &dev)) || (n_events && (rc = device_ptr(prob, "prob", &dev))) ||
-      (means && (rc = device_ptr(means, "means", &dev))))
+    if ((rc = device_of(x[k], "x[k]", &dev))) return rc;
+  if ((rc = device_of(stats, "stats", &dev)) || (n_events && (rc = device_of(prob, "prob", &dev))) ||
+      (means && (rc = device_of(means, "means", &dev))))
     return rc;
   for (int k = 0, m = 0; k < n_sources; ++k)
     for (int j = 0; j < members[k]; ++j, ++m) {
@@ -308,10 +281,7 @@ int sky_ensemble_stats_multi(int32_t n_sources, const float* const* x, const int
   DeviceGuard guard(dev);
   const dim3 grid((unsigned)((plane + kThreads - 1) / kThreads), (unsigned)n_sel);
   cudaStream_t st = (cudaStream_t)stream;
-  if (total <= 8) launch<8>(P, grid, st);
-  else if (total <= 16) launch<16>(P, grid, st);
-  else if (total <= 32) launch<32>(P, grid, st);
-  else launch<64>(P, grid, st);
+  dispatch_padding<8>(total, [&](auto mp) { launch<mp>(P, grid, st); });
   count_launch();
   SKY_CUDA_OK(cudaGetLastError());
   return SKY_OK;

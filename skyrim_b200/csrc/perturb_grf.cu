@@ -231,17 +231,6 @@ bool grf_shape_ok(int members, int channels, int nlat, int nlon, int lmax) {
   return true;
 }
 
-// 0 when p is device memory (on device *dev, or on the device of the first pointer checked); else SKY_ERR_ARG / CUDA
-int device_of(const void* p, const char* what, int* dev) {
-  if (!p) { set_error("%s is null", what); return SKY_ERR_ARG; }
-  cudaPointerAttributes attr;
-  SKY_CUDA_OK(cudaPointerGetAttributes(&attr, p));
-  if (attr.type != cudaMemoryTypeDevice) { set_error("%s must be device memory", what); return SKY_ERR_ARG; }
-  if (*dev >= 0 && attr.device != *dev) { set_error("%s is on device %d, x on device %d", what, attr.device, *dev); return SKY_ERR_ARG; }
-  *dev = attr.device;
-  return 0;
-}
-
 int launch_draw(float2* a, const float* spec_std, uint64_t seed, int member0, int channels, long long f0, long long n,
                 int lmax, cudaStream_t st) {
   k_grf_draw<<<dim3((unsigned)n, lmax + 1), 64, 0, st>>>(a, spec_std, seed, member0, channels, (int)f0, lmax);

@@ -17,6 +17,7 @@
 #include <cmath>
 
 #include "engine.h"
+#include "member_fields.h"
 #include "philox.cuh"
 #include "point_terms.cuh"
 #include "sky_common.cuh"
@@ -24,7 +25,7 @@
 namespace sky {
 namespace {
 
-constexpr int kMaxMembers = 64, kMaxSel = 128, kMaxRegions = 4, kMapTerms = 5, kRankThreads = 256, kMapThreads = 128;
+constexpr int kMapTerms = 5, kRankThreads = 256, kMapThreads = 128;
 constexpr uint32_t kRankTag = 0x524E4B31u;   // "RNK1": second Philox counter word (K11 uses 0 there, the GRF "GRF1")
 
 struct PointParams {
@@ -114,51 +115,6 @@ __global__ void __launch_bounds__(kMapThreads) k_score_maps(const __grid_constan
   for (int t = 0; t < kMapTerms; ++t) o[t * (long long)P.plane] += nan ? __longlong_as_double(0x7ff8000000000000ll) : term[t];
 }
 
-int device_ptr(const void* p, const char* what, int* dev) {
-  cudaPointerAttributes attr;
-  SKY_CUDA_OK(cudaPointerGetAttributes(&attr, p));
-  if (attr.type != cudaMemoryTypeDevice) { set_error("%s must be device memory", what); return SKY_ERR_ARG; }
-  if (*dev >= 0 && attr.device != *dev) { set_error("%s is on device %d, x on device %d", what, attr.device, *dev); return SKY_ERR_ARG; }
-  *dev = attr.device;
-  return 0;
-}
-
-// the member / channel / truth arguments both entries share with sky_forecast_scores; no CUDA call
-int check_fields(PointParams& P, const float* x, int32_t members, int64_t member_stride, int32_t nlat, int32_t nlon,
-                 int32_t channel_count, const int32_t* channels, int32_t n_sel, const float* truth) {
-  if (members < 1 || members > kMaxMembers) { set_error("members = %d must lie in [1, %d]", members, kMaxMembers); return SKY_ERR_ARG; }
-  if (nlat < 1 || nlon < 1 || (int64_t)nlat * nlon > INT32_MAX) {
-    set_error("nlat = %d and nlon = %d must be positive with nlat x nlon < 2^31", nlat, nlon);
-    return SKY_ERR_ARG;
-  }
-  const int64_t plane = (int64_t)nlat * nlon;
-  if (channel_count < 1) { set_error("channel_count = %d must be positive", channel_count); return SKY_ERR_ARG; }
-  if (member_stride < (int64_t)channel_count * plane) {
-    set_error("member_stride = %lld is below channel_count x plane = %lld", (long long)member_stride, (long long)channel_count * plane);
-    return SKY_ERR_ARG;
-  }
-  if (n_sel < 1 || n_sel > kMaxSel || !channels) { set_error("n_sel = %d channels must lie in [1, %d]", n_sel, kMaxSel); return SKY_ERR_ARG; }
-  for (int s = 0; s < n_sel; ++s) {
-    if (channels[s] < 0 || channels[s] >= channel_count) { set_error("channel %d is outside [0, %d)", channels[s], channel_count); return SKY_ERR_ARG; }
-    P.chan[s] = channels[s];
-  }
-  if (!x || !truth) { set_error("x and truth must not be null"); return SKY_ERR_ARG; }
-  P.x = x;
-  P.truth = truth;
-  P.member_stride = member_stride;
-  P.plane = (int)plane;
-  P.nlat = nlat;
-  P.nlon = nlon;
-  P.members = members;
-  P.n_sel = n_sel;
-  return 0;
-}
-
-template <int MP>
-void launch_maps(const PointParams& P, cudaStream_t st) {
-  k_score_maps<MP><<<dim3((P.plane + kMapThreads - 1) / kMapThreads, P.n_sel), kMapThreads, 0, st>>>(P);
-}
-
 }  // namespace
 }  // namespace sky
 
@@ -172,7 +128,9 @@ int sky_forecast_rank_histogram(const float* x, int32_t members, int64_t member_
                                 int32_t lead_index, int32_t* counts, uint64_t counts_bytes, double* hist, void* stream) {
   PointParams P{};
   int rc;
-  if ((rc = check_fields(P, x, members, member_stride, nlat, nlon, channel_count, channels, n_sel, truth))) return rc;
+  if ((rc = check_grid(nlat, nlon)) ||
+      (rc = check_members(members, member_stride, (int64_t)nlat * nlon, channel_count, channels, n_sel, P.chan)))
+    return rc;
   if (n_regions < 1 || n_regions > kMaxRegions) { set_error("n_regions = %d must lie in [1, %d]", n_regions, kMaxRegions); return SKY_ERR_ARG; }
   if (seed > UINT32_MAX) { set_error("seed = %llu must lie in [0, 2^32)", (unsigned long long)seed); return SKY_ERR_ARG; }
   if (date_index < 0 || lead_index < 0) {
@@ -185,12 +143,23 @@ int sky_forecast_rank_histogram(const float* x, int32_t members, int64_t member_
               (unsigned long long)need);
     return SKY_ERR_ARG;
   }
-  if (!row_weights || !counts || !hist) { set_error("row_weights, counts and hist must not be null"); return SKY_ERR_ARG; }
+  if (!x || !truth || !row_weights || !counts || !hist) {
+    set_error("x, truth, row_weights, counts and hist must not be null");
+    return SKY_ERR_ARG;
+  }
   int dev = -1;
-  if ((rc = device_ptr(x, "x", &dev)) || (rc = device_ptr(truth, "truth", &dev)) ||
-      (rc = device_ptr(row_weights, "row_weights", &dev)) || (rc = device_ptr(counts, "counts", &dev)) ||
-      (rc = device_ptr(hist, "hist", &dev)))
+  if ((rc = device_of(x, "x", &dev)) || (rc = device_of(truth, "truth", &dev)) ||
+      (rc = device_of(row_weights, "row_weights", &dev)) || (rc = device_of(counts, "counts", &dev)) ||
+      (rc = device_of(hist, "hist", &dev)))
     return rc;
+  P.x = x;
+  P.truth = truth;
+  P.member_stride = member_stride;
+  P.plane = nlat * nlon;
+  P.nlat = nlat;
+  P.nlon = nlon;
+  P.members = members;
+  P.n_sel = n_sel;
   P.roww = row_weights;
   P.counts = counts;
   P.out = hist;
@@ -215,19 +184,24 @@ int sky_forecast_score_maps(const float* x, int32_t members, int64_t member_stri
                             void* stream) {
   PointParams P{};
   int rc;
-  if ((rc = check_fields(P, x, members, member_stride, nlat, nlon, channel_count, channels, n_sel, truth))) return rc;
-  if (!maps) { set_error("maps must not be null"); return SKY_ERR_ARG; }
-  int dev = -1;
-  if ((rc = device_ptr(x, "x", &dev)) || (rc = device_ptr(truth, "truth", &dev)) || (rc = device_ptr(maps, "maps", &dev)))
+  if ((rc = check_grid(nlat, nlon)) ||
+      (rc = check_members(members, member_stride, (int64_t)nlat * nlon, channel_count, channels, n_sel, P.chan)))
     return rc;
+  if (!x || !truth || !maps) { set_error("x, truth and maps must not be null"); return SKY_ERR_ARG; }
+  int dev = -1;
+  if ((rc = device_of(x, "x", &dev)) || (rc = device_of(truth, "truth", &dev)) || (rc = device_of(maps, "maps", &dev)))
+    return rc;
+  P.x = x;
+  P.truth = truth;
   P.out = maps;
+  P.member_stride = member_stride;
+  P.plane = nlat * nlon;
+  P.members = members;
+  P.n_sel = n_sel;
   DeviceGuard guard(dev);
   cudaStream_t st = (cudaStream_t)stream;
-  if (members == 1) launch_maps<1>(P, st);
-  else if (members <= 8) launch_maps<8>(P, st);
-  else if (members <= 16) launch_maps<16>(P, st);
-  else if (members <= 32) launch_maps<32>(P, st);
-  else launch_maps<64>(P, st);
+  const dim3 grid((unsigned)((P.plane + kMapThreads - 1) / kMapThreads), (unsigned)n_sel);
+  dispatch_padding<1>(members, [&](auto mp) { k_score_maps<mp><<<grid, kMapThreads, 0, st>>>(P); });
   count_launch();
   SKY_CUDA_OK(cudaGetLastError());
   return SKY_OK;

@@ -21,13 +21,14 @@
 #include <cmath>
 
 #include "engine.h"
+#include "member_fields.h"
 #include "point_terms.cuh"
 #include "sky_common.cuh"
 
 namespace sky {
 namespace {
 
-constexpr int kMaxMembers = 64, kMaxSel = 128, kMaxRegions = 4, kTerms = 9, kThreads = 128, kBlocks = SKY_SCORES_BLOCKS;
+constexpr int kTerms = 9, kThreads = 128, kBlocks = SKY_SCORES_BLOCKS;
 
 struct ScoresParams {
   const float* x;              // member m, selected channel s at x + m member_stride + chan[s] plane
@@ -137,15 +138,6 @@ void launch(const ScoresParams& P, cudaStream_t st) {
   k_scores_partial<MP, U><<<dim3(kBlocks, P.n_sel), kThreads, 0, st>>>(P);
 }
 
-int device_ptr(const void* p, const char* what, int* dev) {
-  cudaPointerAttributes attr;
-  SKY_CUDA_OK(cudaPointerGetAttributes(&attr, p));
-  if (attr.type != cudaMemoryTypeDevice) { set_error("%s must be device memory", what); return SKY_ERR_ARG; }
-  if (*dev >= 0 && attr.device != *dev) { set_error("%s is on device %d, x on device %d", what, attr.device, *dev); return SKY_ERR_ARG; }
-  *dev = attr.device;
-  return 0;
-}
-
 }  // namespace
 }  // namespace sky
 
@@ -157,24 +149,12 @@ int sky_forecast_scores(const float* x, int32_t members, int64_t member_stride, 
                         int32_t channel_count, const int32_t* channels, int32_t n_sel, const float* truth, const float* clim,
                         const double* row_weights, int32_t n_regions, double* partial, uint64_t partial_bytes, double* sums,
                         void* stream) {
-  if (members < 1 || members > kMaxMembers) { set_error("members = %d must lie in [1, %d]", members, kMaxMembers); return SKY_ERR_ARG; }
-  if (nlat < 1 || nlon < 1 || (int64_t)nlat * nlon > INT32_MAX) {
-    set_error("nlat = %d and nlon = %d must be positive with nlat x nlon < 2^31", nlat, nlon);
-    return SKY_ERR_ARG;
-  }
-  const int64_t plane = (int64_t)nlat * nlon;
-  if (channel_count < 1) { set_error("channel_count = %d must be positive", channel_count); return SKY_ERR_ARG; }
-  if (member_stride < (int64_t)channel_count * plane) {
-    set_error("member_stride = %lld is below channel_count x plane = %lld", (long long)member_stride, (long long)channel_count * plane);
-    return SKY_ERR_ARG;
-  }
-  if (n_sel < 1 || n_sel > kMaxSel || !channels) { set_error("n_sel = %d channels must lie in [1, %d]", n_sel, kMaxSel); return SKY_ERR_ARG; }
-  if (n_regions < 1 || n_regions > kMaxRegions) { set_error("n_regions = %d must lie in [1, %d]", n_regions, kMaxRegions); return SKY_ERR_ARG; }
   ScoresParams P{};
-  for (int s = 0; s < n_sel; ++s) {
-    if (channels[s] < 0 || channels[s] >= channel_count) { set_error("channel %d is outside [0, %d)", channels[s], channel_count); return SKY_ERR_ARG; }
-    P.chan[s] = channels[s];
-  }
+  int rc;
+  if ((rc = check_grid(nlat, nlon)) ||
+      (rc = check_members(members, member_stride, (int64_t)nlat * nlon, channel_count, channels, n_sel, P.chan)))
+    return rc;
+  if (n_regions < 1 || n_regions > kMaxRegions) { set_error("n_regions = %d must lie in [1, %d]", n_regions, kMaxRegions); return SKY_ERR_ARG; }
   const uint64_t need = (uint64_t)n_regions * n_sel * kTerms * kBlocks * sizeof(double);
   if (partial_bytes < need) {
     set_error("partial_bytes = %llu is below %llu (n_regions x n_sel x 9 x %d doubles)", (unsigned long long)partial_bytes,
@@ -185,10 +165,10 @@ int sky_forecast_scores(const float* x, int32_t members, int64_t member_stride, 
     set_error("x, truth, row_weights, partial and sums must not be null");
     return SKY_ERR_ARG;
   }
-  int dev = -1, rc;
-  if ((rc = device_ptr(x, "x", &dev)) || (rc = device_ptr(truth, "truth", &dev)) || (clim && (rc = device_ptr(clim, "clim", &dev))) ||
-      (rc = device_ptr(row_weights, "row_weights", &dev)) || (rc = device_ptr(partial, "partial", &dev)) ||
-      (rc = device_ptr(sums, "sums", &dev)))
+  int dev = -1;
+  if ((rc = device_of(x, "x", &dev)) || (rc = device_of(truth, "truth", &dev)) || (clim && (rc = device_of(clim, "clim", &dev))) ||
+      (rc = device_of(row_weights, "row_weights", &dev)) || (rc = device_of(partial, "partial", &dev)) ||
+      (rc = device_of(sums, "sums", &dev)))
     return rc;
   P.x = x;
   P.truth = truth;
@@ -197,7 +177,7 @@ int sky_forecast_scores(const float* x, int32_t members, int64_t member_stride, 
   P.partial = partial;
   P.sums = sums;
   P.member_stride = member_stride;
-  P.plane = (int)plane;
+  P.plane = nlat * nlon;
   P.nlat = nlat;
   P.nlon = nlon;
   P.members = members;
@@ -205,11 +185,7 @@ int sky_forecast_scores(const float* x, int32_t members, int64_t member_stride, 
   P.n_reg = n_regions;
   DeviceGuard guard(dev);   // launch on the device that owns the members, whatever the caller's current device is
   cudaStream_t st = (cudaStream_t)stream;
-  if (members == 1) launch<1>(P, st);
-  else if (members <= 8) launch<8>(P, st);
-  else if (members <= 16) launch<16>(P, st);
-  else if (members <= 32) launch<32>(P, st);
-  else launch<64>(P, st);
+  dispatch_padding<1>(members, [&](auto mp) { launch<mp>(P, st); });
   count_launch();
   SKY_CUDA_OK(cudaGetLastError());
   k_scores_final<<<(n_regions * n_sel * kTerms + kThreads - 1) / kThreads, kThreads, 0, st>>>(P);

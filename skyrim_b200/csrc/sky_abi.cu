@@ -20,6 +20,16 @@ void set_error(const char* fmt, ...) {
   va_end(ap);
 }
 
+int device_of(const void* p, const char* what, int* dev) {
+  if (!p) { set_error("%s is null", what); return SKY_ERR_ARG; }
+  cudaPointerAttributes attr;
+  SKY_CUDA_OK(cudaPointerGetAttributes(&attr, p));
+  if (attr.type != cudaMemoryTypeDevice) { set_error("%s must be device memory", what); return SKY_ERR_ARG; }
+  if (*dev >= 0 && attr.device != *dev) { set_error("%s is on device %d, x on device %d", what, attr.device, *dev); return SKY_ERR_ARG; }
+  *dev = attr.device;
+  return 0;
+}
+
 void Engine::drop_graphs() {
   for (auto& g : graphs) if (g.exec) cudaGraphExecDestroy(g.exec);
   graphs.clear();
@@ -306,10 +316,9 @@ int sky_model_set_clock(sky_model_t* m, double unix_seconds, void* stream) {
 
 int sky_toa_radiation(float* out, int32_t nlat, int32_t nlon, double unix_seconds, void* stream) {
   if (!out || nlat < 2 || nlon < 1) { set_error("bad argument"); return SKY_ERR_ARG; }
-  cudaPointerAttributes attr;
-  SKY_CUDA_OK(cudaPointerGetAttributes(&attr, out));
-  if (attr.type != cudaMemoryTypeDevice) { set_error("out must be device memory"); return SKY_ERR_ARG; }
-  DeviceGuard guard(attr.device);
+  int dev = -1, rc;
+  if ((rc = device_of(out, "out", &dev))) return rc;
+  DeviceGuard guard(dev);
   return toa_radiation_launch(out, nlat, nlon, unix_seconds, (cudaStream_t)stream);
 }
 
@@ -328,10 +337,9 @@ int sky_model_debug_set(sky_model_t* m, const char* key, int64_t value) {
 int sky_perturb_ic(float* x, const float* sigma_c, float amp, uint64_t seed, int32_t member0, int32_t members,
                    int32_t channels, int64_t plane, void* stream) {
   if (!x || !sigma_c || members <= 0 || channels <= 0 || plane <= 0) { set_error("bad argument"); return SKY_ERR_ARG; }
-  cudaPointerAttributes attr;
-  SKY_CUDA_OK(cudaPointerGetAttributes(&attr, x));
-  if (attr.type != cudaMemoryTypeDevice) { set_error("x must be device memory"); return SKY_ERR_ARG; }
-  DeviceGuard guard(attr.device);   // launch on the device that owns the state, whatever the caller's current device is
+  int dev = -1, rc;
+  if ((rc = device_of(x, "x", &dev))) return rc;
+  DeviceGuard guard(dev);   // launch on the device that owns the state, whatever the caller's current device is
   long long qpp = (plane + 3) / 4;
   long long total = qpp * channels * members;
   k_perturb_ic<<<(unsigned)((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, sigma_c, amp, seed, member0,

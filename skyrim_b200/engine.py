@@ -328,6 +328,52 @@ ENS_MAX_MEMBERS, ENS_MAX_CHANNELS, ENS_MAX_QUANTILES, ENS_MAX_EVENTS = 64, 128, 
 ENS_MAX_SOURCES = 4
 
 
+def _c_array(ctype, values):
+    """a ctypes array of ``values`` (one element even when empty, so the pointer is never null)"""
+    return (ctype * max(len(values), 1))(*values)
+
+
+def _check_out(t, shape, dtype, name):
+    if tuple(t.shape) != shape or t.dtype != dtype or not t.is_contiguous() or not t.is_cuda:
+        raise ValueError(f"{name} of shape {tuple(t.shape)} {t.dtype} on {t.device}: contiguous CUDA {dtype} {shape} "
+                         "needed")
+
+
+def _member_view(x, channel_offset: int = 0, name: str = "x"):
+    """(M, H, W, count, member_stride, base) of ``x``, a CUDA fp32 (M, C, H, W) tensor or a view of one whose members each
+    hold contiguous (C, H, W) planes, as the statistics and verification entries read it: the count = C - channel_offset
+    channels from ``channel_offset`` on, member m's at the address base + 4 m member_stride"""
+    import torch
+    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4):
+        raise ValueError(f"{name} must be a CUDA fp32 (members, channels, nlat, nlon) tensor")
+    M, Cn, H, W = x.shape
+    plane = H * W
+    if x.stride(3) != 1 or x.stride(2) != W or x.stride(1) != plane:
+        raise ValueError(f"each member of {name} must hold contiguous (C, H, W) planes (strides {x.stride()})")
+    if not 0 <= channel_offset < Cn:
+        raise ValueError(f"channel_offset = {channel_offset} is outside [0, {Cn})")
+    member_stride = x.stride(0) if M > 1 else max(x.stride(0), Cn * plane)
+    return M, H, W, Cn - channel_offset, member_stride, x.data_ptr() + 4 * channel_offset * plane
+
+
+def _verified_members(x, channels, channel_offset, row_weights=None, **fields):
+    """``_member_view(x, channel_offset)`` and the selected channels sel (default: all), with every named field (truth,
+    clim) None or a contiguous CUDA fp32 (n_sel, H, W) tensor, and ``row_weights`` None or a contiguous CUDA fp64
+    (n_regions, H) tensor: (M, H, W, count, member_stride, base, sel)"""
+    import torch
+    M, H, W, count, member_stride, base = _member_view(x, channel_offset)
+    sel = list(range(count)) if channels is None else [int(c) for c in channels]
+    for name, t in fields.items():
+        if t is not None and (not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous()
+                              or tuple(t.shape) != (len(sel), H, W)):
+            raise ValueError(f"{name} must be a contiguous CUDA fp32 {(len(sel), H, W)} tensor (got {tuple(t.shape)})")
+    if row_weights is not None and not (row_weights.is_cuda and row_weights.dtype == torch.float64
+                                        and row_weights.is_contiguous() and row_weights.dim() == 2
+                                        and row_weights.shape[1] == H):
+        raise ValueError(f"row_weights must be a contiguous CUDA fp64 (n_regions, {H}) tensor")
+    return M, H, W, count, member_stride, base, sel
+
+
 def ensemble_statistics(x, channels=None, quantiles=(), events=(), channel_offset: int = 0, out=None):
     """Per-point statistics over the members of a CUDA fp32 (M, C, H, W) tensor, or a view of one whose members each hold
     contiguous (C, H, W) planes (include/skyrim_b200.h sky_ensemble_stats).  Channels are counted from ``channel_offset``
@@ -336,32 +382,20 @@ def ensemble_statistics(x, channels=None, quantiles=(), events=(), channel_offse
     with i nondecreasing.  Returns (stats (2 + n_q, n_sel, H, W): mean, spread, quantiles; prob (n_events, H, W)), into
     ``out`` = (stats, prob) when given.  Asynchronous on the current stream."""
     import torch
-    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4):
-        raise ValueError("x must be a CUDA fp32 (members, channels, nlat, nlon) tensor")
-    M, Cn, H, W = x.shape
-    plane = H * W
-    if x.stride(3) != 1 or x.stride(2) != W or x.stride(1) != plane:
-        raise ValueError(f"each member of x must hold contiguous (C, H, W) planes (strides {x.stride()})")
-    if not 0 <= channel_offset < Cn:
-        raise ValueError(f"channel_offset = {channel_offset} is outside [0, {Cn})")
-    count = Cn - channel_offset
-    member_stride = x.stride(0) if M > 1 else max(x.stride(0), Cn * plane)
-    sel = list(range(count)) if channels is None else [int(c) for c in channels]
+    M, H, W, count, member_stride, base, sel = _verified_members(x, channels, channel_offset)
     q = [float(v) for v in quantiles]
     ev_sel, ev_thr = [int(i) for i, _ in events], [float(t) for _, t in events]
     shapes = ((2 + len(q), len(sel), H, W), (len(ev_sel), H, W))
     if out is None:
         out = tuple(torch.empty(s, dtype=torch.float32, device=x.device) for s in shapes)
     stats, prob = out
-    for t, s in zip(out, shapes):
-        if tuple(t.shape) != s or t.dtype != torch.float32 or not t.is_contiguous():
-            raise ValueError(f"output of shape {tuple(t.shape)} {t.dtype}: contiguous fp32 {s} needed")
-    arr = lambda ct, v: (ct * max(len(v), 1))(*v)  # noqa: E731
+    for t, s, name in zip(out, shapes, ("stats", "prob")):
+        _check_out(t, s, torch.float32, name)
     L = _ffi.lib()
     st = torch.cuda.current_stream(x.device).cuda_stream
-    _ffi.check(L.sky_ensemble_stats(x.data_ptr() + 4 * channel_offset * plane, M, member_stride, plane, count,
-                                    arr(C.c_int32, sel), len(sel), arr(C.c_double, q), len(q), arr(C.c_int32, ev_sel),
-                                    arr(C.c_float, ev_thr), len(ev_sel), stats.data_ptr(),
+    _ffi.check(L.sky_ensemble_stats(base, M, member_stride, H * W, count, _c_array(C.c_int32, sel), len(sel),
+                                    _c_array(C.c_double, q), len(q), _c_array(C.c_int32, ev_sel),
+                                    _c_array(C.c_float, ev_thr), len(ev_sel), stats.data_ptr(),
                                     prob.data_ptr() if prob.numel() else None, st), "sky_ensemble_stats", L)
     return stats, prob
 
@@ -379,13 +413,11 @@ def multi_model_statistics(sources, channels_per_source, quantiles=(), events=()
     if not 1 <= K <= ENS_MAX_SOURCES or len(channels_per_source) != K:
         raise ValueError(f"{K} sources with {len(channels_per_source)} channel lists: 1 to {ENS_MAX_SOURCES} sources, one "
                          "list each")
-    H, W = sources[0].shape[2:]
-    plane = H * W
-    for x in sources:
-        if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4 and tuple(x.shape[2:]) == (H, W)):
-            raise ValueError("each source must be a CUDA fp32 (members, channels, nlat, nlon) tensor on one grid")
-        if x.stride(3) != 1 or x.stride(2) != W or x.stride(1) != plane:
-            raise ValueError(f"each member of a source must hold contiguous (C, H, W) planes (strides {x.stride()})")
+    views = [_member_view(x, name=f"source {k}") for k, x in enumerate(sources)]
+    members, nlat, nlon, counts, strides, bases = zip(*views)
+    if len(set(zip(nlat, nlon))) != 1:
+        raise ValueError(f"every source must lie on one grid ({list(zip(nlat, nlon))})")
+    H, W = nlat[0], nlon[0]
     sel = [[int(c) for c in chans] for chans in channels_per_source]
     n_sel = len(sel[0])
     if any(len(c) != n_sel for c in sel):
@@ -398,19 +430,17 @@ def multi_model_statistics(sources, channels_per_source, quantiles=(), events=()
         if not source_means:
             out = out[:2] + (None,)
     stats, prob, means = out
-    for t, s in zip(out, shapes):
-        if t is not None and (tuple(t.shape) != s or t.dtype != torch.float32 or not t.is_contiguous()):
-            raise ValueError(f"output of shape {tuple(t.shape)} {t.dtype}: contiguous fp32 {s} needed")
-    arr = lambda ct, v: (ct * max(len(v), 1))(*v)  # noqa: E731
-    members = [x.shape[0] for x in sources]
-    strides = [x.stride(0) if x.shape[0] > 1 else max(x.stride(0), x.shape[1] * plane) for x in sources]
+    for t, s, name in zip(out, shapes, ("stats", "prob", "means")):
+        if t is not None:
+            _check_out(t, s, torch.float32, name)
     L = _ffi.lib()
     st = torch.cuda.current_stream(sources[0].device).cuda_stream
-    _ffi.check(L.sky_ensemble_stats_multi(K, arr(C.c_void_p, [x.data_ptr() for x in sources]), arr(C.c_int32, members),
-                                          arr(C.c_int64, strides), arr(C.c_int32, [x.shape[1] for x in sources]),
-                                          arr(C.c_int32, [c for chans in sel for c in chans]), n_sel, plane,
-                                          arr(C.c_double, q), len(q), arr(C.c_int32, ev_sel), arr(C.c_float, ev_thr),
-                                          len(ev_sel), stats.data_ptr(), prob.data_ptr() if prob.numel() else None,
+    _ffi.check(L.sky_ensemble_stats_multi(K, _c_array(C.c_void_p, bases), _c_array(C.c_int32, members),
+                                          _c_array(C.c_int64, strides), _c_array(C.c_int32, counts),
+                                          _c_array(C.c_int32, [c for chans in sel for c in chans]), n_sel, H * W,
+                                          _c_array(C.c_double, q), len(q), _c_array(C.c_int32, ev_sel),
+                                          _c_array(C.c_float, ev_thr), len(ev_sel), stats.data_ptr(),
+                                          prob.data_ptr() if prob.numel() else None,
                                           means.data_ptr() if means is not None else None, st),
                "sky_ensemble_stats_multi", L)
     return stats, prob, means
@@ -418,33 +448,6 @@ def multi_model_statistics(sources, channels_per_source, quantiles=(), events=()
 
 SCORES_MAX_REGIONS, SCORES_TERMS, SCORES_BLOCKS = 4, 9, 128
 MAP_TERMS = 5
-
-
-def _verified_members(x, channels, channel_offset, row_weights=None, **fields):
-    """the member, channel and truth checks of the verification entries: (M, H, W, plane, count, member_stride, sel) of x,
-    with every named field (truth, clim) None or a contiguous CUDA fp32 (n_sel, H, W) tensor, and ``row_weights`` None or
-    a contiguous CUDA fp64 (n_regions, H) tensor"""
-    import torch
-    if not (x.is_cuda and x.dtype == torch.float32 and x.dim() == 4):
-        raise ValueError("x must be a CUDA fp32 (members, channels, nlat, nlon) tensor")
-    M, Cn, H, W = x.shape
-    plane = H * W
-    if x.stride(3) != 1 or x.stride(2) != W or x.stride(1) != plane:
-        raise ValueError(f"each member of x must hold contiguous (C, H, W) planes (strides {x.stride()})")
-    if not 0 <= channel_offset < Cn:
-        raise ValueError(f"channel_offset = {channel_offset} is outside [0, {Cn})")
-    count = Cn - channel_offset
-    member_stride = x.stride(0) if M > 1 else max(x.stride(0), Cn * plane)
-    sel = list(range(count)) if channels is None else [int(c) for c in channels]
-    for name, t in fields.items():
-        if t is not None and (not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous()
-                              or tuple(t.shape) != (len(sel), H, W)):
-            raise ValueError(f"{name} must be a contiguous CUDA fp32 {(len(sel), H, W)} tensor (got {tuple(t.shape)})")
-    if row_weights is not None and not (row_weights.is_cuda and row_weights.dtype == torch.float64
-                                        and row_weights.is_contiguous() and row_weights.dim() == 2
-                                        and row_weights.shape[1] == H):
-        raise ValueError(f"row_weights must be a contiguous CUDA fp64 (n_regions, {H}) tensor")
-    return M, H, W, plane, count, member_stride, sel
 
 
 def forecast_scores(x, truth, row_weights, channels=None, clim=None, channel_offset: int = 0, out=None):
@@ -456,21 +459,19 @@ def forecast_scores(x, truth, row_weights, channels=None, clim=None, channel_off
     fp64 sums (n_regions, n_sel, 9) (``scores.SUMS`` names them; ``scores.metrics_from_sums`` forms the metrics), into
     ``out`` when given.  Asynchronous on the current stream."""
     import torch
-    M, H, W, plane, count, member_stride, sel = _verified_members(x, channels, channel_offset, row_weights,
-                                                                  truth=truth, clim=clim)
+    M, H, W, count, member_stride, base, sel = _verified_members(x, channels, channel_offset, row_weights,
+                                                                 truth=truth, clim=clim)
     R = row_weights.shape[0]
     shape = (R, len(sel), SCORES_TERMS)
     if out is None:
         out = torch.empty(shape, dtype=torch.float64, device=x.device)
-    if tuple(out.shape) != shape or out.dtype != torch.float64 or not out.is_contiguous():
-        raise ValueError(f"output of shape {tuple(out.shape)} {out.dtype}: contiguous fp64 {shape} needed")
+    _check_out(out, shape, torch.float64, "out")
     ws = torch.empty(max(R * len(sel) * SCORES_TERMS * SCORES_BLOCKS, 1), dtype=torch.float64, device=x.device)
     L = _ffi.lib()
     st = torch.cuda.current_stream(x.device).cuda_stream
-    _ffi.check(L.sky_forecast_scores(x.data_ptr() + 4 * channel_offset * plane, M, member_stride, H, W, count,
-                                     (C.c_int32 * max(len(sel), 1))(*sel), len(sel), truth.data_ptr(),
-                                     None if clim is None else clim.data_ptr(), row_weights.data_ptr(), R, ws.data_ptr(),
-                                     8 * ws.numel(), out.data_ptr(), st), "sky_forecast_scores", L)
+    _ffi.check(L.sky_forecast_scores(base, M, member_stride, H, W, count, _c_array(C.c_int32, sel), len(sel),
+                                     truth.data_ptr(), None if clim is None else clim.data_ptr(), row_weights.data_ptr(),
+                                     R, ws.data_ptr(), 8 * ws.numel(), out.data_ptr(), st), "sky_forecast_scores", L)
     return out
 
 
@@ -482,7 +483,7 @@ def forecast_rank_histogram(x, truth, row_weights, seed: int, date_index: int, l
     ``channel_offset``, ``lead_index``).  Returns the CUDA fp64 (n_regions, n_sel, M + 1) histogram, each summing to 1,
     into ``out`` when given.  Asynchronous on the current stream."""
     import torch
-    M, H, W, plane, count, member_stride, sel = _verified_members(x, channels, channel_offset, row_weights, truth=truth)
+    M, H, W, count, member_stride, base, sel = _verified_members(x, channels, channel_offset, row_weights, truth=truth)
     if not 0 <= int(seed) < 2 ** 32 or int(date_index) < 0 or int(lead_index) < 0:
         raise ValueError(f"seed = {seed} must lie in [0, 2^32), date_index = {date_index} and lead_index = {lead_index} "
                          "must not be negative")
@@ -490,15 +491,13 @@ def forecast_rank_histogram(x, truth, row_weights, seed: int, date_index: int, l
     shape = (R, len(sel), M + 1)
     if out is None:
         out = torch.empty(shape, dtype=torch.float64, device=x.device)
-    if tuple(out.shape) != shape or out.dtype != torch.float64 or not out.is_contiguous():
-        raise ValueError(f"output of shape {tuple(out.shape)} {out.dtype}: contiguous fp64 {shape} needed")
+    _check_out(out, shape, torch.float64, "out")
     ws = torch.empty(max(len(sel) * H * (M + 2), 1), dtype=torch.int32, device=x.device)
     L = _ffi.lib()
     st = torch.cuda.current_stream(x.device).cuda_stream
-    _ffi.check(L.sky_forecast_rank_histogram(x.data_ptr() + 4 * channel_offset * plane, M, member_stride, H, W, count,
-                                             (C.c_int32 * max(len(sel), 1))(*sel), len(sel), truth.data_ptr(),
-                                             row_weights.data_ptr(), R, int(seed), int(date_index), int(lead_index),
-                                             ws.data_ptr(), 4 * ws.numel(), out.data_ptr(), st),
+    _ffi.check(L.sky_forecast_rank_histogram(base, M, member_stride, H, W, count, _c_array(C.c_int32, sel), len(sel),
+                                             truth.data_ptr(), row_weights.data_ptr(), R, int(seed), int(date_index),
+                                             int(lead_index), ws.data_ptr(), 4 * ws.numel(), out.data_ptr(), st),
                "sky_forecast_rank_histogram", L)
     return out
 
@@ -509,15 +508,12 @@ def score_maps_accumulate(x, truth, maps, channels=None, channel_offset: int = 0
     sky_forecast_score_maps; ``scores.map_metrics`` forms the maps).  Returns ``maps``.  Asynchronous on the current
     stream."""
     import torch
-    M, H, W, plane, count, member_stride, sel = _verified_members(x, channels, channel_offset, truth=truth)
-    shape = (len(sel), MAP_TERMS, H, W)
-    if tuple(maps.shape) != shape or maps.dtype != torch.float64 or not maps.is_contiguous() or not maps.is_cuda:
-        raise ValueError(f"maps of shape {tuple(maps.shape)} {maps.dtype}: contiguous CUDA fp64 {shape} needed")
+    M, H, W, count, member_stride, base, sel = _verified_members(x, channels, channel_offset, truth=truth)
+    _check_out(maps, (len(sel), MAP_TERMS, H, W), torch.float64, "maps")
     L = _ffi.lib()
     st = torch.cuda.current_stream(x.device).cuda_stream
-    _ffi.check(L.sky_forecast_score_maps(x.data_ptr() + 4 * channel_offset * plane, M, member_stride, H, W, count,
-                                         (C.c_int32 * max(len(sel), 1))(*sel), len(sel), truth.data_ptr(),
-                                         maps.data_ptr(), st), "sky_forecast_score_maps", L)
+    _ffi.check(L.sky_forecast_score_maps(base, M, member_stride, H, W, count, _c_array(C.c_int32, sel), len(sel),
+                                         truth.data_ptr(), maps.data_ptr(), st), "sky_forecast_score_maps", L)
     return maps
 
 

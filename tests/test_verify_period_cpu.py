@@ -186,6 +186,41 @@ def test_score_maps_refuse_bad_arguments_before_any_cuda_call(kw, what):
     assert rc == -1 and what in msg, msg
 
 
+# Every statistics and verification entry reads one field of members: here 5 channels of 8 x 12 points per member, with
+# every other argument valid and bogus pointers that are never inspected.
+def _field_entry(name, members=4, stride=5 * 96, channels=(0, 4)):
+    from skyrim_b200 import _ffi
+    L = _ffi.lib()
+    bogus, plane, big = C.c_void_p(0x1000), 96, 1 << 40
+    sel, n_sel = (C.c_int32 * max(len(channels), 1))(*channels), len(channels)
+    if name == "sky_ensemble_stats":
+        rc = L.sky_ensemble_stats(bogus, members, stride, plane, 5, sel, n_sel, None, 0, None, None, 0, bogus, None, None)
+    elif name == "sky_ensemble_stats_multi":
+        one = lambda ct, v: (ct * 1)(v)  # noqa: E731
+        rc = L.sky_ensemble_stats_multi(1, one(C.c_void_p, 0x1000), one(C.c_int32, members), one(C.c_int64, stride),
+                                        one(C.c_int32, 5), sel, n_sel, plane, None, 0, None, None, 0, bogus, None, None, None)
+    elif name == "sky_forecast_scores":
+        rc = L.sky_forecast_scores(bogus, members, stride, 8, 12, 5, sel, n_sel, bogus, None, bogus, 1, bogus, big, bogus,
+                                   None)
+    elif name == "sky_forecast_rank_histogram":
+        rc = L.sky_forecast_rank_histogram(bogus, members, stride, 8, 12, 5, sel, n_sel, bogus, bogus, 1, 0, 0, 0, bogus, big,
+                                           bogus, None)
+    else:
+        rc = L.sky_forecast_score_maps(bogus, members, stride, 8, 12, 5, sel, n_sel, bogus, bogus, None)
+    return rc, L.sky_last_error().decode()
+
+
+@pytest.mark.parametrize("entry", ["sky_ensemble_stats", "sky_ensemble_stats_multi", "sky_forecast_scores",
+                                   "sky_forecast_rank_histogram", "sky_forecast_score_maps"])
+@pytest.mark.parametrize("kw, what", [
+    (dict(members=0), "members"), (dict(members=65), "members"), (dict(stride=5 * 96 - 1), "member_stride"),
+    (dict(channels=(0, 5)), "channel 5"), (dict(channels=()), "n_sel"), (dict(channels=(0,) * 129), "n_sel"),
+])
+def test_every_entry_refuses_a_bad_member_field_before_any_cuda_call(entry, kw, what):
+    rc, msg = _field_entry(entry, **kw)
+    assert rc == -1 and what in msg, msg
+
+
 # ---- score_period() host logic on a CPU fake of EnsembleRunner --------------------------------------------------------------
 class TimeSource:
     """seeded truth that changes with time: source[t] -> DataArray(channel, lat, lon)"""
