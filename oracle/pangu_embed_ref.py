@@ -14,6 +14,7 @@ from __future__ import annotations
 import numpy as np
 
 from oracle import gemm_ref as gr
+from oracle import pangu_resample_ref as pr
 
 
 def a_operands(cfg, w, x: np.ndarray) -> tuple[np.ndarray, np.ndarray]:
@@ -54,9 +55,6 @@ def embed_reference(cfg, w, x: np.ndarray) -> tuple[np.ndarray, np.ndarray]:
 
 
 def skip_image_offset(cfg, B: int) -> int:
-    """byte offset of the skip image in the engine's workspace for B members (PanguEngine::carve)"""
-    def take(n):
-        return -(-n // 1024) * 1024
-    C = cfg.dim
-    R1, R2 = B * cfg.Z * cfg.H * cfg.W, B * cfg.Z * cfg.H2 * cfg.W2
-    return take(R1 * C * 4) + take(R2 * 2 * C * 4) + take(-(-R1 // 128) * (C // 64) * 128 * 128)   # x1, x2, x1h
+    """byte offset of the skip image in the engine's workspace for B members (pr.workspace_layout, the mirror of
+    PanguEngine::carve)"""
+    return pr.workspace_layout(cfg, B)["skiph"]

@@ -11,6 +11,7 @@ import pytest
 
 from oracle import gemm_ref as gr
 from oracle import pangu_embed_ref as pe
+from oracle import pangu_resample_ref as pr
 
 torch = pytest.importorskip("torch")
 pytestmark = pytest.mark.gpu
@@ -61,6 +62,7 @@ def test_embedding_per_element(engine, B, stream):
         assert not bad.any(), (name, int(bad.sum()), np.argwhere(bad)[:4].tolist())
 
     tiles = -(-R1 // 128)
+    assert eng._L.sky_model_workspace_bytes(eng._h, B) == pr.workspace_layout(cfg, B)["total"]
     off = pe.skip_image_offset(cfg, B)
     img = raw[off: off + tiles * (C // 64) * 128 * 128].reshape(tiles, C // 64, 128, 128)
     assert (img[-1, :, R1 - (tiles - 1) * 128:] == 0xFF).all(), "skip image rows past the last token written"
