@@ -16,6 +16,7 @@
 #include <vector>
 
 #include "gemm_tb.cuh"
+#include "mlp_fused.cuh"
 #define SKY_GC_EPILOGUES_ONLY   // graphcast_ops.cuh: the epilogues, not the engine's kernels (defined in graphcast_engine.o)
 #include "graphcast_ops.cuh"
 #include "attention_tc.cuh"   // EpiQkvWin (the attention kernels are defined in pangu_engine.o)
@@ -23,7 +24,10 @@
 
 extern "C" {
 
-enum { SKY_PROBE_W = 0, SKY_PROBE_W_TRI = 1, SKY_PROBE_TB = 2, SKY_PROBE_PAIR = 3 };
+// SKY_PROBE_MLP: Pangu's fused MLP (mlp_fused.cuh) at C = n = 192 (k_mlp_fused) or 384 (k_mlp_fused_pair), in place on the
+// stream image `hi` (img_nkb = C / 64 k-blocks).  W1 at BLOCK_N 64 is `w`, W2 at BLOCK_N 192 is `b_hi` (b_bytes), the fc1 bias
+// is `add` (add_bytes) and fc2's bias, gamma, beta and eps are the LayerNorm's; `epi` is ignored.
+enum { SKY_PROBE_W = 0, SKY_PROBE_W_TRI = 1, SKY_PROBE_TB = 2, SKY_PROBE_PAIR = 3, SKY_PROBE_MLP = 4 };
 enum {
   SKY_PROBE_EPI_F32 = 0,          // EpiF32Batched<false>
   SKY_PROBE_EPI_F32_ACC = 1,      // EpiF32Batched<true>
@@ -390,6 +394,34 @@ template <> FragEpi<EpiQkvWin> make_epi(const Case& c) {
   return {EpiQkvWin{(uint8_t*)c.hi, c.part_stride, c.bias, probe_geo(c.geo), c.roll, c.geo.C, c.pairs}};
 }
 
+// ---- the fused MLP (SKY_PROBE_MLP) ----
+int check_mlp(const Case& c) {
+  const int C = c.n;
+  PROBE_REQUIRE((C == 192 || C == 384) && c.m >= 1 && c.grid_sms >= 0, "fused MLP: N=%d (must be 192 or 384), M=%lld, grid_sms %d", C,
+                (long long)c.m, c.grid_sms);
+  PROBE_REQUIRE(C == 192 || c.grid_sms != 1, "fused MLP: grid_sms 1 (CTA pairs at N=384)");
+  PROBE_REQUIRE(c.img_nkb == C / 64 && c.hi && aligned16(c.hi) && cdiv(c.m, G2_BLOCK_M) * (C / 64) * TILE <= c.img_bytes,
+                "fused MLP: stream image too small or not %d k-blocks", C / 64);
+  const long long wbytes = 4LL * C * C * 2;
+  PROBE_REQUIRE(c.w && aligned16(c.w) && c.w_bytes >= wbytes && c.b_hi && aligned16(c.b_hi) && c.b_bytes >= wbytes,
+                "fused MLP: weight images of %lld bytes", wbytes);
+  PROBE_REQUIRE(c.add && aligned16(c.add) && c.add_bytes >= 4LL * C * 4, "fused MLP: fc1 bias of %d floats", 4 * C);
+  int rc;
+  if ((rc = check_vec(c, c.bias, C, "bias")) || (rc = check_vec(c, c.gamma, C, "gamma")) || (rc = check_vec(c, c.beta, C, "beta")))
+    return rc;
+  return 0;
+}
+int run_mlp(const Case& c, cudaStream_t st) {
+  int sms = c.grid_sms;
+  if (sms == 0) {
+    int dev = 0;
+    SKY_CUDA_OK(cudaGetDevice(&dev));
+    SKY_CUDA_OK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  }
+  const MlpArgs a{(uint8_t*)c.hi, (const uint8_t*)c.w, (const uint8_t*)c.b_hi, c.add, {make_ln<2>(c)}, c.m};
+  return c.n == 192 ? launch_mlp_fused<3>(a, sms, st) : launch_mlp_fused_pair(a, sms, st);
+}
+
 template <int... BNs> struct BnList {};
 
 // launch epilogue e with the case's BLOCK_N if it is in the list, else refuse
@@ -485,8 +517,9 @@ int dispatch(const Case& c, cudaStream_t st) {
 extern "C" SKY_API int sky_probe_gemm(const sky_probe_case_t* c, void* stream) {
   using namespace sky;
   if (!c) { set_error("gemm probe: null case"); return SKY_ERR_ARG; }
-  if (c->kernel < SKY_PROBE_W || c->kernel > SKY_PROBE_PAIR) { set_error("gemm probe: unknown kernel %d", c->kernel); return SKY_ERR_ARG; }
+  if (c->kernel < SKY_PROBE_W || c->kernel > SKY_PROBE_MLP) { set_error("gemm probe: unknown kernel %d", c->kernel); return SKY_ERR_ARG; }
   int rc;
+  if (c->kernel == SKY_PROBE_MLP) return (rc = check_mlp(*c)) ? rc : run_mlp(*c, (cudaStream_t)stream);
   if ((rc = check_operands(*c)) || (rc = check_epilogue(*c))) return rc;
   return dispatch(*c, (cudaStream_t)stream);
 }

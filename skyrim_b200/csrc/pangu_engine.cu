@@ -15,6 +15,7 @@
 #include "attention_tc.cuh"
 #include "engine.h"
 #include "gemm2.cuh"
+#include "mlp_fused.cuh"
 #include "pangu_ops.cuh"
 
 namespace sky {
@@ -391,6 +392,7 @@ struct GemmW {
 };
 struct BlockW {
   GemmW qkv, proj, fc1, fc2;   // all at BLOCK_N 192: at C = 384 projection and fc2 are the two halves of a CTA pair
+  GemmW fc1c;                   // C = 192: fc1 again at BLOCK_N 64, W1's 64-row slices of the fused MLP (mlp_fused.cuh)
   const float *qkv_b, *proj_b, *fc1_b, *fc2_b, *ln1_g, *ln1_b, *ln2_g, *ln2_b;
   __half* bias_tab;  // (n_type, heads, 3312), fp16, pre-scaled by log2 e
 };
@@ -494,6 +496,7 @@ struct PanguEngine : Engine {
         if ((rc = pack(b.proj, N("proj.w"), c, c, 192, false, st))) return rc;
         if ((rc = pack(b.fc1, N("fc1.w"), 4 * c, c, 192, false, st))) return rc;
         if ((rc = pack(b.fc2, N("fc2.w"), c, 4 * c, 192, false, st))) return rc;
+        if (c == 192 && (rc = pack(b.fc1c, N("fc1.w"), 4 * c, c, 64, false, st))) return rc;
         P(b.qkv_b, N("qkv.b"), 3 * c); P(b.proj_b, N("proj.b"), c);
         P(b.fc1_b, N("fc1.b"), 4 * c); P(b.fc2_b, N("fc2.b"), c);
         P(b.ln1_g, N("ln1.g"), c); P(b.ln1_b, N("ln1.b"), c);
@@ -609,7 +612,16 @@ struct PanguEngine : Engine {
       rc = C == 192 ? gemm2<192>(KT_PROJ, A, e, b.proj, R, st) : gemm2<192, true>(KT_PROJ, A, e, b.proj, R, st);
       if (rc) return rc;
     }
-    {  // MLP: fc1 + GELU into the fp16 hidden image, then fc2 + LayerNorm + residual
+    if (IMG && C == 192) {   // MLP in one kernel: the hidden activation stays on the SM (mlp_fused.cuh).  At C = 384 the
+                             // fused CTA-pair kernel measured 2.4x slower than fc1 + fc2 (DESIGN.md section 4)
+      const MlpArgs m{xh, b.fc1c.img, b.fc2.img, b.fc1_b,
+                      {Epi2F32Img<true, 2>{xh, nullptr, C, xh, nkb, nullptr, b.fc2_b, b.ln2_g, b.ln2_b, cfg.ln_eps}}, R};
+      prof_begin(KT_MLP, st);
+      count_launch();
+      rc = launch_mlp_fused<3>(m, num_sms, st);
+      prof_end(KT_MLP, st);
+      if (rc) return rc;
+    } else {  // MLP: fc1 + GELU into the fp16 hidden image, then fc2 + LayerNorm + residual
       AOperand A(xh, nkb);
       FragEpi<Epi2F16<true, true>> e{reinterpret_cast<__half*>(ws.hidh), 0, 4 * nkb, b.fc1_b};
       if ((rc = gemm2<192>(KT_FC1, A, e, b.fc1, R, st))) return rc;

@@ -40,8 +40,9 @@ def pangu_bytes(cfg: PanguConfig) -> dict:
       attn   read q|k|v 6 B, write the projection's operand image 2 B
       proj   read operand image 2 B, residual read from xh 2 B, xh written in place 2 B
       mlp    read xh 2 B (operand; the epilogue re-reads the same image as the residual: an L2 hit), xh written in place 2 B
-             (the 4C hidden activation is not mandatory traffic: the H100 engine moves it through HBM as fc1's fp16 image,
-             8 B written and 8 B read per token and feature, which these figures do not count)
+             (the 4C hidden activation is not mandatory traffic: at C = 192 the fused MLP kernel keeps it in shared memory;
+             at C = 384, and with the fp32 token stream, fc1 writes it as an fp16 image that fc2 reads back, 8 B written and
+             8 B read per token and feature, which these figures do not count)
     (with the fp32 token stream, "fp32_stream", proj and mlp move 12 B)"""
     C = cfg.dim
     HW = cfg.H * cfg.W

@@ -13,6 +13,11 @@ CUDA events around --iters back-to-back launches after five warm-up launches.  T
 turn, --rounds times (a power-limited card's clocks drift over a run), and the median counts.  Per GEMM and path it
 prints us per launch, TFLOP/s (2 M N K over the time), the tile count and us per tile per SM (time x SMs / tiles).
 
+It also times Pangu's fused MLP (mlp_fused.cuh: fc1, GELU and fc2 per row tile, the hidden activation in shared memory; CTA
+pairs at C = 384) against fc1 + fc2 of the fragment path launched back to back on the same operands, alternated --rounds
+times:
+  mlp    fused against fc1_fc2, us per launch (pair) and TFLOP/s of the 4 M C^2 x 2 FLOPs of both GEMMs.
+
 --kscan times fc1's tile grid (N = 4C) at K = C, 2C and 4C on the staged path: the same tiles with more k-blocks.  The
 least-squares line through (k-blocks per tile, us per tile) splits a tile's time into the main loop's cost per k-block
 (slope) and a fixed cost per tile (intercept).
@@ -33,6 +38,7 @@ TILE = 16384
 BN = 192
 # sky_probe_gemm epilogue ids of the fragment path (gemm_probe.cu): EPI_F16_GELU_IMG / EPI_LN_IMG wrapped in FragEpi
 EPI_F16_GELU_IMG_FRAG, EPI_LN_IMG_FRAG = 18, 19
+MLP = 4   # sky_probe_gemm kernel id of the fused MLP (gemm_probe.cu SKY_PROBE_MLP)
 
 
 def main():
@@ -75,15 +81,18 @@ def main():
     def nbytes(t):
         return t.numel() * t.element_size()
 
-    def time_case(case):
+    def time_case(*cases):
+        """us per launch of `cases` one after the other"""
         for _ in range(5):
-            rc, msg = gp.launch(case)
-            assert rc == 0, msg
+            for case in cases:
+                rc, msg = gp.launch(case)
+                assert rc == 0, msg
         torch.cuda.synchronize()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
         for _ in range(args.iters):
-            gp.launch(case)
+            for case in cases:
+                gp.launch(case)
         e1.record()
         torch.cuda.synchronize()
         return e0.elapsed_time(e1) * 1e3 / args.iters
@@ -138,6 +147,22 @@ def main():
                         times[path].append(time_case(cases[path]))
                 for path in args.paths:
                     res["gemms"].append(report(name, path, C, B, M, N, K, float(np.median(times[path])), mt * N // BN))
+            # the fused MLP against fc1 + fc2 on the fragment path: W1 packed at BLOCK_N 64 for the fused kernel (the
+            # weights are random, so a different packing of the same values is not needed for the timing)
+            fc1 = gemm_case(gp.W, EPI_F16_GELU_IMG_FRAG, 4 * C, M, x, nkb, w_fc1, hi=hid.data_ptr(), img_bytes=nbytes(hid),
+                            img_nkb=4 * nkb, bias=b4.data_ptr(), vec_floats=4 * C)
+            fc2 = gemm_case(ln_kernel, EPI_LN_IMG_FRAG, C, M, hid, 4 * nkb, w_fc2, **ln)
+            fused = gp.make_case(kernel=MLP, block_n=BN, n=C, n_valid=C, batches=1, grid_sms=0, m=M, w=w_fc1.data_ptr(),
+                                 w_bytes=nbytes(w_fc1), b_hi=w_fc2.data_ptr(), b_bytes=nbytes(w_fc2), add=b4.data_ptr(),
+                                 add_bytes=nbytes(b4), **ln)
+            times = {"fc1_fc2": [], "fused": []}
+            for _ in range(args.rounds):
+                times["fc1_fc2"].append(time_case(fc1, fc2))
+                times["fused"].append(time_case(fused))
+            for path, t in times.items():
+                rec = report("mlp", path, C, B, M, 4 * C, 2 * C, float(np.median(t)), mt)
+                rec["share_of_989_tflops"] = round(rec["tflops"] / 989.0, 3)
+                res["gemms"].append(rec)
             del x, hid, att
             torch.cuda.empty_cache()
         if args.kscan:
