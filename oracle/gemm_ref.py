@@ -187,19 +187,65 @@ def col_stats(f_ref, f_bound, rows_per_sum: int = 32):
     return s, q, bs, bq
 
 
-def layer_norm(R, S, bias, gamma, beta, res, eps, tau=TAU):
-    """Epi2F32Img<true, kRes> (Pangu's and GraphCast's LayerNorm epilogue): out = LN(acc + bias) * gamma + beta + res over
-    whole rows, with its bound; res = 0 for kRes 0"""
+def ln_depth(chain: int, merges: int) -> int:
+    """fp32 roundings a LayerNorm row mean passes through in a kernel (first order, a value's error is u |value| per
+    addition its partial sum passes through): `chain`, the most additions any one value meets in a thread's sum, two per
+    merge of partial statistics (ln_merge: weighted means and their sum), one for the division and one for the product
+    mean * rstd that the normalisation adds.  The paths of gemm2.cuh, BN columns per CTA:
+      FragEpi<Epi2F32Img>   chain BN / 16 + 2 (pairs of columns onto two running sums), merges 2 (lane quad) + 1 in a pair
+      Epi2F32Img::run       chain BN / 8 + 2 (four-column trees onto a running sum, every other 32-column group),
+                            merges 1 (the two warps of a lane quarter) + 1 in a pair
+      Epi2UpShuffle         chain BN (one lane adds its row in sequence), no merge"""
+    return chain + 2 * merges + 2
+
+
+def ln_shift(bn: int) -> tuple[int, int]:
+    """Epi2F32Img::run's one pass (the `shift` of layer_norm): each lane sums its BN / 2 columns about the mean of its
+    first 32"""
+    return 32, bn // 2
+
+
+def layer_norm(R, S, bias, gamma, beta, res, eps, tau=TAU, depth=None, shift=None):
+    """Epi2F32Img<true, kRes> (Pangu's and GraphCast's LayerNorm epilogue) and Epi2UpShuffle: out = LN(acc + bias) * gamma
+    + beta + res over whole rows, with its bound; res = 0 for kRes 0.
+
+    The kernels take the statistics of a thread's m columns about their mean, as (mean, m2 = sum of squared deviations),
+    and merge partials of disjoint columns with Chan's formula (gemm2.cuh ln_merge).  A thread either makes two passes
+    (shift None: the mean, then the squared deviations from it) or one pass about k, the mean of its first q columns
+    (shift = (q, m), ln_shift: mean = k + s / m, m2 = ss - s^2 / m with s, ss the sums of y - k and its square).
+    First order in u = 2^-24, with e the error of each y = acc + bias (tau S and its fp32 roundings), n the row width,
+    sd its standard deviation, and `depth` the roundings of a thread's sum (ln_depth; default n + 2, more than any path):
+      mean  the propagated e.mean() and the summation error dsum.  Two passes: depth u mean|y|, linear in the row's
+            |mean|.  One pass: (k - mean_t)^2 <= m2_t / q for the thread's columns (their first q deviate by k - mean_t
+            on average) and m2_t <= m2, so mean|y - k| <= (1 + sqrt(m / q)) sqrt(n / m) sd, and dsum = depth u (1 +
+            sqrt(m / q)) sqrt(n / m) sd + 10 u |mean| (k + s / m, two per merge, the product mean * rstd);
+      var   sum (y_i - mu')^2 = n var + n (mu - mu')^2 exactly, so the mean's error enters a thread's m2 only to second
+            order (dsum^2); a merge's d^2 na nb / n term carries the local means' summation error to first order, at
+            most 2 sqrt(m2 n / 4) dsum <= n sd dsum per level of the merge tree, 4 levels at most (quad, lane quarter,
+            pair); the propagated 2 |y - mu| e; the roundings of the positive sum of squares and its division, depth + 4
+            of them (two passes), or 3 depth + 3 of the sum about k, which is at most 1 + m / q times m2 (one pass);
+      rstd  rsqrtf within 2 ulp: 2^-21 on top of half the variance's relative error.
+    """
     y = R + bias
     e = tau * S + 2 * U32 * np.abs(y)
+    n = y.shape[1]
+    depth = n + 2 if depth is None else depth
     mu = y.mean(1, keepdims=True)
     var = y.var(1, keepdims=True)
+    sd = np.sqrt(var)
     rstd = 1.0 / np.sqrt(var + eps)
     yn = (y - mu) * rstd
     out = yn * gamma + beta + res
-    # fp32 single-pass variance (E[y^2] - mean^2) and rsqrtf: relative error of the variance
-    rel_var = (2 * (np.abs(y - mu) * e).mean(1, keepdims=True) + 2.0 ** -20 * (y * y).mean(1, keepdims=True)) / (var + eps)
-    bound = (np.abs(gamma) * rstd * (e + e.mean(1, keepdims=True)) + np.abs(gamma * yn) * (0.5 * rel_var + 2.0 ** -21)
+    if shift is None:
+        dsum = depth * U32 * np.abs(y).mean(1, keepdims=True)
+        rounding = depth + 4
+    else:
+        q, m = shift
+        dsum = U32 * (10 * np.abs(mu) + depth * (1 + np.sqrt(m / q)) * np.sqrt(n / m) * sd)
+        rounding = (3 * depth + 3) * (1 + m / q)
+    e_mu = e.mean(1, keepdims=True) + dsum
+    rel_var = (2 * (np.abs(y - mu) * e).mean(1, keepdims=True) + 4 * dsum * sd + dsum * dsum + rounding * U32 * var) / (var + eps)
+    bound = (np.abs(gamma) * rstd * (e + e_mu) + np.abs(gamma * yn) * (0.5 * rel_var + 2.0 ** -21)
              + 4 * U32 * (np.abs(gamma * yn) + np.abs(beta) + np.abs(res)))
     return out, bound
 

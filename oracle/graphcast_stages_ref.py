@@ -164,7 +164,9 @@ def ref_ln(hid, w, name, res, eps, extra=None):
     if extra is not None:
         S = S + extra / gr.TAU
     f64 = lambda k: np.asarray(w[f"{name}.{k}"], np.float64)
-    y, yb = gr.layer_norm(R, S, f64("b2")[None], f64("ln.g")[None], f64("ln.b")[None], 0.0, eps)
+    # every GraphCast LayerNorm runs Epi2F32Img::run on the CTA pairs at 2 x 256 columns
+    y, yb = gr.layer_norm(R, S, f64("b2")[None], f64("ln.g")[None], f64("ln.b")[None], 0.0, eps, depth=gr.ln_depth(256 // 8 + 2, 2),
+                          shift=gr.ln_shift(256))
     if res is None:
         return y, y, yb
     return y, y + res, yb + 4 * gr.U32 * np.abs(res)

@@ -8,7 +8,7 @@ workspace layout (PanguEngine::carve) that the engine-level tests read raw regio
                 zero rows where 2 h2 + hs >= H, two-pass fp32 LayerNorm over all 4C (the zeros included), fp16 image;
                 then the down GEMM (Epi2F32Img<false, 0>: the plain product, fp16 image and, with the fp32 token stream,
                 fp32 rows)
-  up-sample     linear1 on Epi2UpShuffle: n-tile `sub` = (hs, ws) of the 4C outputs, single-pass LayerNorm over its C
+  up-sample     linear1 on Epi2UpShuffle: n-tile `sub` = (hs, ws) of the 4C outputs, two-pass LayerNorm over its C
                 columns, stored at the fine token (z, 2 h2 + hs, 2 w2 + ws) when 2 h2 + hs < H; then linear2
                 (Epi2F32Img<false, 0>)
   recovery      Epi2Recover on k_gemm2 at BLOCK_N 224: A = [skip | x1] along K, weight columns ((v 2 + dz) 4 + dh) 4 + dw
@@ -33,8 +33,9 @@ Bound of k_down_merge_ln (two-pass statistics; u = 2^-24, n = 4C = 768, 24 value
   out    fl(fl(fl(d_i r') g) + b) = g r (v_i - mu) + g r (mu - mu') + g r (v_i - mu') theta + rounding of the sum, with
          |theta| <= rho + 3u: |out' - out| <= |g| r dmu + |g yn| (rho + 4u) + u |b| (yn = (v_i - mu) r), then the fp16
          store (half an fp16 ulp).
-The single-pass LayerNorm of Epi2UpShuffle (E[y^2] - mean^2 in fp32) is gemm_ref.layer_norm's model with bias 0 and
-residual 0.
+The LayerNorm of Epi2UpShuffle is gemm_ref.layer_norm's model with bias 0 and residual 0: one lane adds its row's C
+values in sequence (the mean, ln_depth(C, 0) roundings), then their squared deviations from that mean; the variance is
+taken about the mean, so the bound stays linear in |mean| / std, as for k_down_merge_ln.
 """
 from __future__ import annotations
 

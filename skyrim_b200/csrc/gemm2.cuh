@@ -121,10 +121,25 @@ template <class E> struct is_fragment_epi<E, std::void_t<decltype(E::kFragment)>
 template <class E, class = void> struct is_scatter_epi : std::false_type {};
 template <class E> struct is_scatter_epi<E, std::void_t<decltype(E::kScatter)>> : std::true_type {};
 
+// LayerNorm statistics of a row, or of a part of its columns: the mean and m2, the sum of squared deviations from that
+// mean.  Every LayerNorm epilogue takes the statistics of the values a thread holds about their mean (two passes, or the
+// staged path's one pass about a nearby shift) and merges the partials of disjoint column sets with Chan's formula; one
+// pass over (sum, sum of squares) loses the variance to cancellation once |mean| / std reaches ~100 (ss / n - mean^2 in
+// fp32 keeps 2^-24 mean^2 / var of it).
+struct LnStat {
+  float mean, m2;
+};
+// merge of the partials a (na columns) and b (nb columns): bit for bit symmetric in (a, na) and (b, nb), so the lanes of a
+// quad, the warps of a lane quarter and the two CTAs of a pair that merge the same partials agree exactly
+__device__ __forceinline__ LnStat ln_merge(LnStat a, float na, LnStat b, float nb) {
+  const float n = na + nb, d = b.mean - a.mean;
+  return {(na / n) * a.mean + (nb / n) * b.mean, (a.m2 + b.m2) + d * d * (na * nb / n)};
+}
+
 // LayerNorm row statistics of a column-split CTA pair (k_gemm2_pair): the two CTAs hold the two column halves of the same
-// 128 rows.  For each tile and 32-row group, a CTA posts its rows' (sum, sum of squares) into the peer's slot and reads
-// the peer's from its own.  Slots [tile parity][32-row group][row % 32][sum, sum of squares] and one barrier per (tile
-// parity, group) follow the barrier block (gemm2_body).  own_bar == nullptr outside a pair.
+// 128 rows.  For each tile and 32-row group, a CTA posts its rows' LnStat (mean, m2 of its half) into the peer's slot and
+// reads the peer's from its own.  Slots [tile parity][32-row group][row % 32][mean, m2] and one barrier per (tile parity,
+// group) follow the barrier block (gemm2_body).  own_bar == nullptr outside a pair.
 struct PairStats {
   uint64_t* own_bar = nullptr;            // completes when the peer's 32 rows of this group have landed
   uint32_t own_stat = 0;                  // shared-space address of this CTA's slot
@@ -143,22 +158,23 @@ struct PairStats {
   }
   // one lane per group and tile: announces the bytes of the peer's 32 posts
   __device__ __forceinline__ void expect() const { mbar_arrive_expect_tx(own_bar, 32 * 8); }
-  // tile row r's sums into the peer's slot.  st.async itself completes the peer's barrier transaction: no fence, no release
-  // arrive.
-  __device__ __forceinline__ void post(int r, float s, float ss) const {
+  // tile row r's statistics into the peer's slot.  st.async itself completes the peer's barrier transaction: no fence, no
+  // release arrive.
+  __device__ __forceinline__ void post(int r, LnStat v) const {
     asm volatile("st.async.weak.shared::cluster.mbarrier::complete_tx::bytes.v2.f32 [%0], {%1, %2}, [%3];" ::"r"(
                      peer_stat + (uint32_t)(r & 31) * 8u),
-                 "f"(s), "f"(ss), "r"(peer_bar)
+                 "f"(v.mean), "f"(v.m2), "r"(peer_bar)
                  : "memory");
   }
-  // CTA-scope acquire: the peer's sums arrive in THIS CTA's shared memory through st.async, whose completion the barrier
-  // phase carries (as for bulk copies); a cluster-scope wait added an L1 invalidate (CCTL.IVALL) per tile
+  // CTA-scope acquire: the peer's statistics arrive in THIS CTA's shared memory through st.async, whose completion the
+  // barrier phase carries (as for bulk copies); a cluster-scope wait added an L1 invalidate (CCTL.IVALL) per tile
   __device__ __forceinline__ void wait() const { mbar_wait(own_bar, parity); }
-  // after wait(): adds the peer's sums of tile row r
-  __device__ __forceinline__ void add_peer(int r, float& s, float& ss) const {
-    float ps, pss;
-    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ps), "=f"(pss) : "r"(own_stat + (uint32_t)(r & 31) * 8u));
-    s += ps; ss += pss;
+  // after wait(): merges the peer's statistics of tile row r (its half: n columns, as many as this CTA's) into v.  Both
+  // CTAs of the pair end with the same statistics (ln_merge is symmetric).
+  __device__ __forceinline__ void merge_peer(int r, LnStat& v, float n) const {
+    LnStat p;
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(p.mean), "=f"(p.m2) : "r"(own_stat + (uint32_t)(r & 31) * 8u));
+    v = ln_merge(v, n, p, n);
   }
 };
 
@@ -894,29 +910,47 @@ struct Epi2F32Img {
 #pragma unroll
     for (int it = 0; it < 8; ++it) { rs[it] = 1.f; ns[it] = 0.f; }
     if (kLn) {
-      float s = 0.f, ss = 0.f;
+      // columns of the row this warp's lane holds: the column groups part, part + nparts, ...
+      const auto cols = [&](int p) { return (float)(32 * ((NG - p + e.nparts - 1) / e.nparts)); };
+      // One pass over the staged tile (a second pass that re-read it cost a GraphCast step 1.5 %, H100 80GB HBM3 at
+      // 700 W): sums about k, the mean of the lane's first 32-column group, which is in registers.  (k - mean)^2 <= m2 / 32,
+      // so the sum of squares about k is at most (1 + cols / 32) m2 whatever |mean| / std is.
+      float k = 0.f, s = 0.f, ss = 0.f;
       for (int g = e.part; g < NG; g += e.nparts) {
         float v[32];
         acc.load32(g * 32, v);
 #pragma unroll
         for (int j = 0; j < 32; j += 4) {
           const float4 b = lds_f32x4_ro(e.svec_s + (g * 32 + j) * 4);
-          const float y0 = v[j] + b.x, y1 = v[j + 1] + b.y, y2 = v[j + 2] + b.z, y3 = v[j + 3] + b.w;
+          v[j] += b.x; v[j + 1] += b.y; v[j + 2] += b.z; v[j + 3] += b.w;
+        }
+        if (g == e.part) {
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) k += (v[j] + v[j + 1]) + (v[j + 2] + v[j + 3]);
+          k *= 1.f / 32.f;
+        }
+#pragma unroll
+        for (int j = 0; j < 32; j += 4) {
+          const float y0 = v[j] - k, y1 = v[j + 1] - k, y2 = v[j + 2] - k, y3 = v[j + 3] - k;
           s += (y0 + y1) + (y2 + y3);
           ss += (y0 * y0 + y1 * y1) + (y2 * y2 + y3 * y3);
         }
       }
+      const float d = s / cols(e.part);
+      LnStat st{k + d, fmaxf(ss - s * d, 0.f)};
       if (e.nparts > 1) {
-        // the warps of a lane quarter are 4 warps apart, and so are their patches
+        // the warps of a lane quarter are 4 warps apart, and so are their patches.  Every warp merges all parts in the
+        // same order, so all hold the same statistics.
         const uint32_t slot = e.patch_s + e.lane * 8;
-        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(slot), "f"(s), "f"(ss) : "memory");
+        asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(slot), "f"(st.mean), "f"(st.m2) : "memory");
         const int q = (int)((e.row0 >> 5) & 3);
         asm volatile("bar.sync %0, %1;" ::"r"(8 + q), "r"(32 * e.nparts) : "memory");
+        float n = 0.f;
         for (int p = 0; p < e.nparts; ++p) {
-          if (p == e.part) continue;
-          float ps, pss;
-          asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(ps), "=f"(pss) : "r"(slot + (p - e.part) * 4 * (G2_PATCH_FLOATS * 4)));
-          s += ps; ss += pss;
+          LnStat o;
+          asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(o.mean), "=f"(o.m2) : "r"(slot + (p - e.part) * 4 * (G2_PATCH_FLOATS * 4)));
+          st = p ? ln_merge(st, n, o, cols(p)) : o;
+          n += cols(p);
         }
         asm volatile("bar.sync %0, %1;" ::"r"(8 + q), "r"(32 * e.nparts) : "memory");   // the patches are reused below
       }
@@ -925,14 +959,14 @@ struct Epi2F32Img {
         if (e.part == 0) {
           if (e.lane == 0) e.pair.expect();
           __syncwarp();
-          e.pair.post(e.lane, s, ss);
+          e.pair.post(e.lane, st);
         }
         e.pair.wait();
-        e.pair.add_peer(e.lane, s, ss);
+        e.pair.merge_peer(e.lane, st, (float)BN);
         width = (float)(2 * BN);
       }
-      const float mean = s / width;
-      const float rstd = rsqrtf(fmaxf(ss / width - mean * mean, 0.f) + eps);
+      const float mean = st.mean;
+      const float rstd = rsqrtf(st.m2 / width + eps);
       const float nmr = -mean * rstd;
 #pragma unroll
       for (int it = 0; it < 8; ++it) {
@@ -1008,22 +1042,41 @@ struct Epi2F32Img {
   template <int BN, class Acc>
   __device__ void frag(Acc& acc, const FragCtx& x) const {
     static_assert(kLn && kRes == 2, "fragment path: LayerNorm with the fp16 image's in-place residual");
-    float s[2] = {0.f, 0.f}, ss[2] = {0.f, 0.f};   // rows x.row, x.row + 8
+    constexpr float kCols = (float)(BN / 4);        // columns of a row in one thread
+    // rows x.row, x.row + 8; each pass adds the even and the odd 8-column groups in two independent chains, which halves
+    // the latency the second pass puts in front of the next tile's main loop
+    LnStat st[2];
+    float a[2][2] = {{0.f, 0.f}, {0.f, 0.f}};
 #pragma unroll
     for (int i = 0; i < BN / 8; ++i) {
       float2 b;
       asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(b.x), "=f"(b.y) : "r"(x.svec_s + (uint32_t)(8 * i + x.c2) * 4u));
       float* d = acc.d + 4 * i;
       d[0] += b.x; d[1] += b.y; d[2] += b.x; d[3] += b.y;
-      s[0] += d[0] + d[1]; ss[0] += d[0] * d[0] + d[1] * d[1];
-      s[1] += d[2] + d[3]; ss[1] += d[2] * d[2] + d[3] * d[3];
+      a[0][i & 1] += d[0] + d[1];
+      a[1][i & 1] += d[2] + d[3];
     }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      st[h].mean = (a[h][0] + a[h][1]) * (1.f / kCols);
+      a[h][0] = a[h][1] = 0.f;
+    }
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i)   // second pass, about the thread's mean
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float y0 = acc.d[4 * i + 2 * h] - st[h].mean, y1 = acc.d[4 * i + 2 * h + 1] - st[h].mean;
+        a[h][i & 1] += y0 * y0 + y1 * y1;
+      }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) st[h].m2 = a[h][0] + a[h][1];
+    // the lane quad holds the whole row: two merges of equal halves
 #pragma unroll
     for (int h = 0; h < 2; ++h)
 #pragma unroll
       for (int o = 1; o < 4; o <<= 1) {
-        s[h] += __shfl_xor_sync(0xffffffffu, s[h], o);
-        ss[h] += __shfl_xor_sync(0xffffffffu, ss[h], o);
+        const LnStat p{__shfl_xor_sync(0xffffffffu, st[h].mean, o), __shfl_xor_sync(0xffffffffu, st[h].m2, o)};
+        st[h] = ln_merge(st[h], kCols * o, p, kCols * o);
       }
     float width = (float)BN;
     if (x.pair.own_bar) {
@@ -1032,18 +1085,17 @@ struct Epi2F32Img {
       const int lane = threadIdx.x & 31, h = lane & 3;
       if (x.post_bar && lane == 0) x.pair.expect();
       __syncwarp();
-      if (h < 2) x.pair.post(x.row + 8 * h, h ? s[1] : s[0], h ? ss[1] : ss[0]);
+      if (h < 2) x.pair.post(x.row + 8 * h, h ? st[1] : st[0]);
       x.pair.wait();
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh) x.pair.add_peer(x.row + 8 * hh, s[hh], ss[hh]);
+      for (int hh = 0; hh < 2; ++hh) x.pair.merge_peer(x.row + 8 * hh, st[hh], (float)BN);
       width = (float)(2 * BN);
     }
     float rs[2], ns[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const float mean = s[h] / width;
-      rs[h] = rsqrtf(fmaxf(ss[h] / width - mean * mean, 0.f) + eps);
-      ns[h] = -mean * rs[h];
+      rs[h] = rsqrtf(st[h].m2 / width + eps);
+      ns[h] = -st[h].mean * rs[h];
     }
     mbar_wait(x.out_ready, x.ready_parity);
 #pragma unroll
@@ -1075,14 +1127,22 @@ struct Epi2UpShuffle {
   int H, W, H2, W2;
   template <int BN, class Acc>
   __device__ void run(Acc& acc, const EpiCtx& e) const {
-    float s = 0.f, ss = 0.f;
+    // the lane holds its whole row: two passes, the mean, then m2 about it (LnStat)
+    float mean = 0.f, m2 = 0.f;
     for (int c = 0; c < BN; c += 32) {
       float v[32];
       acc.load32(c, v);
 #pragma unroll
-      for (int j = 0; j < 32; ++j) { s += v[j]; ss += v[j] * v[j]; }
+      for (int j = 0; j < 32; ++j) mean += v[j];
     }
-    const float mean = s / BN, rstd = rsqrtf(fmaxf(ss / BN - mean * mean, 0.f) + eps);
+    mean /= BN;
+    for (int c = 0; c < BN; c += 32) {
+      float v[32];
+      acc.load32(c, v);
+#pragma unroll
+      for (int j = 0; j < 32; ++j) { const float t = v[j] - mean; m2 += t * t; }
+    }
+    const float rstd = rsqrtf(m2 / BN + eps);
     const int sub = e.n0 / C, hs = sub >> 1, ws = sub & 1;
     long long dst = -1;
     {

@@ -163,9 +163,9 @@ def _emulate_shuffle(cfg, w, x2, wu1, B):
     coarse, sub = pr.shuffle_sources(cfg, B)
     acc = _emulate_gemm(x2, wu1).reshape(-1, 4, C)[coarse, sub]            # [R1, C] fp32
     s = np.cumsum(acc, 1, dtype=F32)[:, -1:]                              # sequential fp32 sums, as one thread adds them
-    ss = np.cumsum((acc * acc).astype(F32), 1, dtype=F32)[:, -1:]
     mean = (s / F32(C)).astype(F32)
-    var = np.maximum((ss / F32(C) - mean * mean).astype(F32), F32(0))
+    d = (acc - mean).astype(F32)                                           # second pass, about the mean
+    var = (np.cumsum((d * d).astype(F32), 1, dtype=F32)[:, -1:] / F32(C)).astype(F32)
     rstd = (1.0 / np.sqrt((var + F32(cfg.ln_eps)).astype(np.float64))).astype(F32)
     yn = ((acc - mean).astype(F32) * rstd).astype(F32)
     return ((yn * np.asarray(w["up.ln.g"], F32)).astype(F32) + np.asarray(w["up.ln.b"], F32)).astype(np.float16)
