@@ -299,6 +299,43 @@ SKY_API int sky_forecast_score_maps(const float* x, int32_t members, int64_t mem
                                     int32_t channel_count, const int32_t* channels, int32_t n_sel, const float* truth,
                                     double* maps, void* stream);
 
+/* The three verification entries above over members pooled from several sources (the members of several models on one
+ * device, each model with its own channel layout).  In place of (x, members, member_stride, channel_count, channels) they
+ * take the source arguments of sky_ensemble_stats_multi:
+ *   n_sources      1..4;  host arrays of n_sources entries:
+ *   x[k]           device pointer of source k: its member j, channel c is the plane x[k] + j * member_stride[k] + c * plane;
+ *   members[k]     >= 1, sum over k (M) at most 64;  member_stride[k] >= channel_count[k] * plane;
+ *   channels       host int32 [n_sources][n_sel]: the plane index, in source k, of selected channel s.
+ * Everything else (truth, clim, row_weights, n_regions, the workspaces and their sizes, seed / date_index / lead_index and
+ * the outputs) is as for the single-source entry, with M the pooled member count: hist is [n_regions][n_sel][M + 1] and
+ * counts_bytes at least 4 * n_sel * nlat * (M + 2).
+ * Members are pooled in source-then-member order.  Each entry returns, bit for bit, what its single-source entry returns on
+ * one contiguous tensor holding the pooled members in that order, laid out in source 0's channel order (x' with member
+ * m = the pooled member m, channels' = channels[0]).  That includes the rank histogram's tie-breaking draws: their Philox
+ * channel word is channels[0][s], source 0's plane index of the selected channel.  So one source gives the single-source
+ * entry's results exactly.  The kernels are the single-source kernels; each block forms the base pointers of its channel's
+ * M members once, so the bytes read are the same.  Parameter blocks: 2712 bytes (scores) and 2720 bytes (histogram, maps),
+ * inside the 4 KB launch-parameter limit.  Refused with SKY_ERR_ARG before any CUDA call: the source arguments
+ * sky_ensemble_stats_multi refuses (a count out of range, a source with no members, more than 64 members in all, a stride
+ * below channel_count[k] * plane, a channel outside its source's range, null pointers) and the single-source entry's own
+ * grid, region, key and workspace arguments; and before any launch: pointers that are not device memory on one device.
+ * Asynchronous and stream-ordered; launches on the device that owns the sources. */
+SKY_API int sky_forecast_scores_multi(int32_t n_sources, const float* const* x, const int32_t* members,
+                                      const int64_t* member_stride, const int32_t* channel_count, const int32_t* channels,
+                                      int32_t n_sel, int32_t nlat, int32_t nlon, const float* truth, const float* clim,
+                                      const double* row_weights, int32_t n_regions, double* partial, uint64_t partial_bytes,
+                                      double* sums, void* stream);
+SKY_API int sky_forecast_rank_histogram_multi(int32_t n_sources, const float* const* x, const int32_t* members,
+                                              const int64_t* member_stride, const int32_t* channel_count,
+                                              const int32_t* channels, int32_t n_sel, int32_t nlat, int32_t nlon,
+                                              const float* truth, const double* row_weights, int32_t n_regions,
+                                              uint64_t seed, int32_t date_index, int32_t lead_index, int32_t* counts,
+                                              uint64_t counts_bytes, double* hist, void* stream);
+SKY_API int sky_forecast_score_maps_multi(int32_t n_sources, const float* const* x, const int32_t* members,
+                                          const int64_t* member_stride, const int32_t* channel_count,
+                                          const int32_t* channels, int32_t n_sel, int32_t nlat, int32_t nlon,
+                                          const float* truth, double* maps, void* stream);
+
 /* Per-kernel-family device timing (CUDA events recorded on the launching stream around the
  * launches whose family bit is set in tag_mask).  profile_end synchronises on the recorded
  * events and returns the summed milliseconds and launch counts per family.  Used by bench.py

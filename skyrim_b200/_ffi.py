@@ -81,6 +81,18 @@ EXPORTS = {
                                               C.c_void_p]),
     "sky_forecast_score_maps": (C.c_int, [C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.c_int32, C.c_int32,
                                           C.POINTER(C.c_int32), C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sky_forecast_scores_multi": (C.c_int, [C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_int32), C.POINTER(C.c_int64),
+                                            C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32, C.c_int32, C.c_int32,
+                                            C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_uint64,
+                                            C.c_void_p, C.c_void_p]),
+    "sky_forecast_rank_histogram_multi": (C.c_int, [C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_int32),
+                                                    C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                                    C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_int32,
+                                                    C.c_uint64, C.c_int32, C.c_int32, C.c_void_p, C.c_uint64, C.c_void_p,
+                                                    C.c_void_p]),
+    "sky_forecast_score_maps_multi": (C.c_int, [C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_int32),
+                                                C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
+                                                C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "sky_model_profile_begin": (C.c_int, [C.c_void_p, C.c_uint64]),
     "sky_model_profile_end": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int32]),
     "sky_profile_tag_count": (C.c_int, []),

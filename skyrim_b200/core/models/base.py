@@ -343,27 +343,12 @@ class GlobalModel:
         if not 0 <= seed < 2 ** 32:
             raise ValueError(f"seed = {seed} must lie in [0, 2^32)")
         step_h = self.time_step.total_seconds() / 3600
-        bad = [h for h in map_leads if not (0 <= h <= n_steps * step_h and float(h) / step_h == int(float(h) / step_h))]
-        if bad:
-            raise ValueError(f"map lead(s) {list(bad)} h: multiples of the {step_h:g}-h time step in [0, {n_steps * step_h:g}] "
-                             "needed")
-        if bool(len(map_leads)) != bool(len(map_channels)):
-            raise ValueError("map_leads and map_channels go together: give both or neither")
+        check_map_leads(map_leads, map_channels, n_steps, step_h)
         times = sorted({t + n * self.time_step for t in starts for n in range(n_steps + 1)})
         perturbation, sel, region_names, row_weights, truth_at, clim = self._score_setup(
             members, perturbation, channels, regions, truth, climatology, times, save, save_config)
-        mch = list(dict.fromkeys(map_channels))
-        unknown = [c for c in mch if c not in names]
-        if unknown:
-            raise ValueError(f"unknown map channel(s) {unknown} for {self.model_name}")
-        forcing = [c for c in mch if c in self.forcing_channels]
-        if forcing:
-            raise ValueError(f"map channel(s) {forcing} are forcings, not forecasts, and are not scored")
-        unscored = [c for c in mch if c not in sel]
-        if unscored:
-            raise ValueError(f"map channel(s) {unscored} are not among the scored channels {sel}")
-        mch = [c for c in sel if c in mch]
-        slots = {int(round(h / step_h)): i for i, h in enumerate(sorted({float(h) for h in map_leads}))}
+        mch, slots = map_plan(map_leads, map_channels, sel, names, self.forcing_channels, step_h,
+                              f"unknown map channel(s) {{}} for {self.model_name}")
         D, L, R, Sn, M = len(starts), n_steps + 1, len(region_names), len(sel), members
         runner = None
         for d, t0 in enumerate(starts):
@@ -397,6 +382,34 @@ class GlobalModel:
                 if da is not None:
                     paths.append(save_forecast(da, label + suffix, starts[0], t_end, source, config=save_config))
         return res, paths
+
+def check_map_leads(map_leads, map_channels, n_steps: int, step_h: float):
+    """refuses map leads (hours) that are not multiples of the time step in [0, n_steps steps], and map leads without map
+    channels or the reverse"""
+    bad = [h for h in map_leads if not (0 <= h <= n_steps * step_h and float(h) / step_h == int(float(h) / step_h))]
+    if bad:
+        raise ValueError(f"map lead(s) {list(bad)} h: multiples of the {step_h:g}-h time step in [0, {n_steps * step_h:g}] "
+                         "needed")
+    if bool(len(map_leads)) != bool(len(map_channels)):
+        raise ValueError("map_leads and map_channels go together: give both or neither")
+
+
+def map_plan(map_leads, map_channels, sel, names, forcing_channels, step_h: float, unknown_msg: str):
+    """(map channels in the order of the scored channels ``sel``, {step: slot} of the map leads in increasing order),
+    refusing a map channel not in ``names`` (``unknown_msg`` formatted with the list), a forcing or one not scored"""
+    mch = list(dict.fromkeys(map_channels))
+    unknown = [c for c in mch if c not in names]
+    if unknown:
+        raise ValueError(unknown_msg.format(unknown))
+    forcing = [c for c in mch if c in forcing_channels]
+    if forcing:
+        raise ValueError(f"map channel(s) {forcing} are forcings, not forecasts, and are not scored")
+    unscored = [c for c in mch if c not in sel]
+    if unscored:
+        raise ValueError(f"map channel(s) {unscored} are not among the scored channels {sel}")
+    mch = [c for c in sel if c in mch]
+    return mch, {int(round(h / step_h)): i for i, h in enumerate(sorted({float(h) for h in map_leads}))}
+
 
 class GlobalPrediction:
     filepath: Path | None = None

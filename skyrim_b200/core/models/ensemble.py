@@ -12,7 +12,7 @@ from loguru import logger
 from ... import xr_shim as xr
 from ...common import generate_forecast_id, save_forecast
 from ...engine import ENS_MAX_MEMBERS, ENS_MAX_SOURCES
-from .base import GlobalPrediction, SyntheticDataSource
+from .base import GlobalPrediction, SyntheticDataSource, check_map_leads, map_plan
 from .graphcast import GraphcastModel
 
 
@@ -191,12 +191,13 @@ class GlobalEnsemble:
         raise NotImplementedError("a multi-model ensemble steps through rollout / forecast (as the reference's)")
 
     def score(self, *args, **kw):
-        raise NotImplementedError("forecast scores are computed per model: score each model with Skyrim(name).score; "
-                                  "multi-model scoring is not built")
+        raise NotImplementedError("forecast scores are computed per model: score each model with Skyrim(name).score, or "
+                                  "compare the models with compare(); multi-model scoring through score is not built")
 
     def score_period(self, *args, **kw):
         raise NotImplementedError("forecast scores are computed per model: verify a period for each model with "
-                                  "Skyrim(name).score_period; multi-model scoring is not built")
+                                  "Skyrim(name).score_period, or compare the models with compare(); multi-model scoring "
+                                  "through score_period is not built")
 
     # -- device states ---------------------------------------------------------------------------------------------------
     def _layout(self, m):
@@ -321,6 +322,156 @@ class GlobalEnsemble:
         return xr.DataArray(np.stack(means), dims=["time", "channel", "lat", "lon"],
                             coords=dict(time=np.array([np.datetime64(t, "s") for t in times]), channel=np.array(sel),
                                         lat=np.array(g.lat), lon=np.array(g.lon)))
+
+    # -- verification: the models head to head ------------------------------------------------------------------------
+    def compare(self, start_times, n_steps: int, truth=None, climatology=None, members: int = 1,
+                perturbation: str | None = None, amp: float = 0.05, seed: int = 0, grf: dict | None = None,
+                channels: List[str] = [], regions: dict | None = None, map_leads=(), map_channels=(), save: bool = False,
+                save_config: dict = {}):
+        """Verifies every model and their pooled ensemble over the same start dates against one truth, and returns
+        (``scores.ModelComparison``, paths).
+
+        The models (2 to 4, K x ``members`` at most 64) step in lockstep from each of ``start_times`` (distinct,
+        increasing and equally spaced: the paired significance assumes it) through leads 0 .. ``n_steps``.  ``members = 1``
+        starts each model from exactly the state its own ``score_period`` starts from (perturbation "none"); above 1,
+        ``perturbation`` defaults to "spherical_grf" and date d's members are ``ensemble_members(t, members, ..., seed +
+        d)``, the same perturbation of the same variable for every model.  The scored channels are the shared channels
+        that are no model's forcing (``channels`` must name shared channels); ``truth`` defaults to the ensemble's data
+        source.  Per lead every model's forwards are launched, the truth is fetched on the host under them and uploaded
+        once (``ensemble.upload_truth``); each model is scored with the single-source entries (its own channel indices and
+        state slice, so its per-date cards, rank histograms and maps are bitwise its own ``score_period``'s), and the K x
+        ``members`` pooled members with the ``*_multi`` entries, off the same buffer.  Only the sums, histograms and maps
+        reach the host, at the end.  Everything ``score_period`` checks is checked before the first engine call.
+
+        ``.scores[entry]`` is that entry's ``PeriodScores``, ``.card`` the period cards stacked (model, lead_time, metric,
+        region, channel), ``.differences`` the paired differences of every pair (``scores.paired_differences``).  ``save``
+        writes netCDF files under one forecast id, label "<sorted names joined by _>-compare<M>": "" the card, "-cards",
+        "-rank-<entry>", "-maps" (with map leads) and "-diff"."""
+        import torch
+        from ... import engine as E
+        from ... import scores as S
+        from ...ensemble import truth_ring, upload_truth
+        K, names = len(self.models), self.shared_channels
+        if not 2 <= K <= ENS_MAX_SOURCES:
+            raise ValueError(f"{K} model(s): a comparison holds 2 to {ENS_MAX_SOURCES} models")
+        if not 1 <= members or K * members > ENS_MAX_MEMBERS:
+            raise ValueError(f"members = {members} per model: {K} models x members must lie in [1, {ENS_MAX_MEMBERS}]")
+        starts = list(start_times)
+        if not starts:
+            raise ValueError("compare needs at least one start time")
+        if any(b <= a for a, b in zip(starts, starts[1:])):
+            raise ValueError(f"start times must be distinct and sorted: {[str(np.datetime64(t, 's')) for t in starts]}")
+        gaps = [b - a for a, b in zip(starts, starts[1:])]
+        uneven = [(a, b) for a, b, g in zip(starts, starts[1:], gaps) if g != gaps[0]]
+        if uneven:
+            a, b = uneven[0]
+            raise ValueError(f"start times must be equally spaced (the paired significance assumes it): the gap "
+                             f"{np.datetime64(a, 's')} -> {np.datetime64(b, 's')} is {b - a}, not {gaps[0]}")
+        if n_steps < 0:
+            raise ValueError(f"n_steps = {n_steps} must not be negative")
+        if not 0 <= seed < 2 ** 32:
+            raise ValueError(f"seed = {seed} must lie in [0, 2^32)")
+        if perturbation is None:
+            perturbation = "none" if members == 1 else "spherical_grf"
+        if perturbation not in ("none", "gaussian", "spherical_grf"):
+            raise ValueError(f"unknown perturbation {perturbation!r} (none, gaussian, spherical_grf)")
+        if grf and perturbation != "spherical_grf":
+            raise ValueError("grf options need perturbation='spherical_grf'")
+        if save and save_config.get("file_type", "netcdf") == "zarr":
+            raise ValueError("a comparison is written as netCDF only: the zarr writer appends along time")
+        step_h = self.time_step.total_seconds() / 3600
+        check_map_leads(map_leads, map_channels, n_steps, step_h)
+        forcings = {c for m in self.models for c in m.forcing_channels}
+        wanted = list(channels) or list(save_config.get("filter_vars", ()))
+        unknown = [c for c in wanted if c not in names]
+        if unknown:
+            raise ValueError(f"channel(s) {unknown} are not shared by {self.model_names}")
+        forcing = [c for c in wanted if c in forcings]
+        if forcing:
+            raise ValueError(f"{forcing} are forcings, not forecasts, and are not scored")
+        sel = [c for c in names if (c in wanted if wanted else c not in forcings)]
+        if len(sel) > E.ENS_MAX_CHANNELS:
+            raise ValueError(f"{len(sel)} channels: at most {E.ENS_MAX_CHANNELS}")
+        mch, slots = map_plan(map_leads, map_channels, sel, names, forcings, step_h,
+                              f"map channel(s) {{}} are not shared by {self.model_names}")
+        g = self.models[0].model.grid
+        lat, lon = np.array(g.lat), np.array(g.lon)
+        region_names, row_weights = S.region_weights(lat, regions)
+        times = sorted({t + n * self.time_step for t in starts for n in range(n_steps + 1)})
+        truth_at = S.truth_fetcher(self.data_source if truth is None else truth, sel, lat, lon, times)
+        clim = S.climatology_fields(climatology, sel, lat, lon)
+        if perturbation == "spherical_grf" and grf is None:
+            grf = dict(lmax=min(180, (len(g.lat) - 1) // 2))
+
+        entries = list(self.model_names) + ["pooled"]
+        chans = [[m.out_channel_names.index(c) for c in sel] for m in self.models]
+        offsets = [self._layout(m)[1] for m in self.models]
+        mpos = [sel.index(c) for c in mch]
+        D, L, R, Sn = len(starts), n_steps + 1, len(region_names), len(sel)
+        init, states = None, None
+        for d, t0 in enumerate(starts):
+            if perturbation == "none":
+                fresh = [torch.as_tensor(m._ensemble_initial_state(t0)[0], dtype=torch.float32, device=m.model.device)
+                         [None].expand(members, -1, -1, -1) for m in self.models]
+            else:
+                fresh = self.ensemble_members(t0, members, perturbation, amp, seed + d, grf)
+            if init is None:   # the member states, the results and the truth ring: allocated once for the campaign
+                init = [f.contiguous() for f in fresh]
+                dev = init[0].device
+                H, W = init[0].shape[-2:]
+                main = torch.cuda.current_stream(dev)
+                sums = torch.empty((K + 1, D, L, R, Sn, len(S.SUMS)), dtype=torch.float64, device=dev)
+                hist = [torch.empty((D, L, R, Sn, (K if e == K else 1) * members + 1), dtype=torch.float64, device=dev)
+                        for e in range(K + 1)]
+                maps = torch.zeros((K + 1, len(slots), len(mch), E.MAP_TERMS, H, W), dtype=torch.float64, device=dev)
+                rw = torch.as_tensor(row_weights, dtype=torch.float64, device=dev).contiguous()
+                kd = None if clim is None else torch.from_numpy(np.ascontiguousarray(clim, dtype=np.float32)).to(dev)
+                ring = truth_ring(dev, Sn, H, W)
+            else:
+                for x, f in zip(init, fresh):
+                    x.copy_(f)
+            states = list(init)
+            valid = [t0 + n * self.time_step for n in range(L)]
+            for n in range(L):
+                if n > 0:
+                    self._step_all(states, first=n == 1)
+                y = upload_truth(ring, n, truth_at(valid[n]), main)   # the host fetch runs under the forwards
+                for k in range(K):
+                    E.forecast_scores(states[k], y, rw, chans[k], kd, offsets[k], out=sums[k, d, n])
+                    E.forecast_rank_histogram(states[k], y, rw, seed, d, n, chans[k], offsets[k], out=hist[k][d, n])
+                    if n in slots:
+                        for j, c in enumerate(mpos):
+                            E.score_maps_accumulate(states[k], y[c:c + 1], maps[k, slots[n], j:j + 1], [chans[k][c]],
+                                                    offsets[k])
+                outs = self._outputs(states)
+                E.forecast_scores_multi(outs, chans, y, rw, kd, out=sums[K, d, n])
+                E.forecast_rank_histogram_multi(outs, chans, y, rw, seed, d, n, out=hist[K][d, n])
+                if n in slots:
+                    for j, c in enumerate(mpos):
+                        E.score_maps_accumulate_multi(outs, [[ch[c]] for ch in chans], y[c:c + 1], maps[K, slots[n], j:j + 1])
+                ring["scored"][n % 2].record(main)
+            logger.success(f"Compared start date {d + 1}/{D}: {np.datetime64(t0, 's')}")
+        sums, maps = sums.cpu().numpy(), maps.cpu().numpy()
+        hours = [n * step_h for n in range(L)]
+        scores = {e: S.PeriodScores.build(sums[i], hist[i].cpu().numpy(), maps[i] if mch else None,
+                                          members * (K if i == K else 1), starts, hours, sorted(slots, key=slots.get),
+                                          step_h, region_names, sel, mch, e, lat, lon)
+                  for i, e in enumerate(entries)}
+        res = S.ModelComparison.build(scores)
+        paths = []
+        if save:
+            save_config = {k: v for k, v in save_config.items() if k != "filter_vars"}   # selected on the device already
+            save_config.setdefault("forecast_id", generate_forecast_id())
+            source = self.ic_source if isinstance(self.ic_source, str) else "file"
+            label, t_end = f"{self.label}-compare{members}", starts[-1] + n_steps * self.time_step
+            files = [("", res.card), ("-cards", _stack(res, "cards", "model"))]
+            files += [(f"-rank-{e}", res.scores[e].rank_histogram) for e in entries]
+            if mch:
+                files.append(("-maps", _stack(res, "maps", "model")))
+            files.append(("-diff", res.differences))
+            for suffix, da in files:
+                paths.append(save_forecast(da, label + suffix, starts[0], t_end, source, config=save_config))
+        return res, paths
 
     # -- perturbed members ------------------------------------------------------------------------------------------------
     def predict_ensemble(self, start_time: datetime.datetime, n_steps: int, members: int, perturbation: str = "spherical_grf",
@@ -460,3 +611,12 @@ class GlobalEnsemble:
                 m.model.engine.set_clock(start_time)
             states.append(xm.reshape(members, -1, *xm.shape[-2:]).contiguous())
         return states
+
+
+def _stack(res, field: str, dim: str):
+    """the entries' ``field`` DataArrays of a ModelComparison stacked along a new first dimension ``dim``"""
+    das = [getattr(res.scores[e], field) for e in res.entries]
+    first = das[0]
+    return xr.DataArray(np.stack([da.values for da in das]), dims=[dim] + list(first.dims),
+                        coords=dict({d: np.asarray(first.coords[d]) for d in first.dims}, **{dim: np.array(res.entries)}),
+                        attrs=dict(res.card.attrs))

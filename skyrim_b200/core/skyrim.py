@@ -78,6 +78,17 @@ class Skyrim:
         return self.model.score_period(start_times=period_start_times(start, end, time, every),
                                        n_steps=self.model.time_steps(lead_time), **kw)
 
+    def compare(self, start: str, end: str | None = None, time: str = "0000", every: int = 24, lead_time: int = 6, **kw):
+        """Head-to-head verification of several models and their pooled ensemble (``GlobalEnsemble.compare``): start
+        dates as ``score_period`` reads them, ``end = None`` meaning the single date ``start``; ``kw`` goes to
+        ``GlobalEnsemble.compare`` (truth, climatology, members, perturbation, amp, seed, grf, channels, regions,
+        map_leads, map_channels, save, save_config).  Returns (ModelComparison, paths)."""
+        if not isinstance(self.model, GlobalEnsemble):
+            raise ValueError(f"compare needs two to four models, e.g. Skyrim('pangu', 'graphcast'); this Skyrim runs "
+                             f"{self.model_names[0]} alone")
+        return self.model.compare(start_times=period_start_times(start, start if end is None else end, time, every),
+                                  n_steps=self.model.time_steps(lead_time), **kw)
+
 
 def period_start_times(start: str, end: str, time: str = "0000", every: int = 24):
     """start times from ``start`` + ``time`` every ``every`` hours (a positive multiple of 6) while their date is at most

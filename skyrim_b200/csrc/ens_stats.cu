@@ -42,19 +42,15 @@ struct EnsStatsParams {
   float ev_thr[kMaxEvents];
 };
 
-constexpr int kMaxSources = 4;
-
-// sky_ensemble_stats_multi's block: the fields reduce_point reads carry EnsStatsParams' names
+// sky_ensemble_stats_multi's block: the source table (member_fields.h), then the fields reduce_point reads, with
+// EnsStatsParams' names
 struct MultiStatsParams {
-  const float* member[kMaxMembers];      // member m's (source base + j member_stride), source-then-member order
+  PooledSources src;
   float* stats;
   float* prob;
   float* means;                          // [n_src][n_sel][plane], or null
   long long plane;
-  int members, n_sel, n_q, n_events, n_src;
-  int src_members[kMaxSources];
-  unsigned char member_src[kMaxMembers];
-  int chan[kMaxSources][kMaxSel];
+  int members, n_sel, n_q, n_events;
   int q_lo[kMaxQ], q_hi[kMaxQ];
   double q_g[kMaxQ];
   int ev_sel[kMaxEvents];
@@ -119,8 +115,8 @@ __global__ void __launch_bounds__(kThreads) k_ens_stats(const __grid_constant__ 
   reduce_point<MP, QUANT>(v, P, s, p);
 }
 
-// Several sources (models) pooled: member m (source-then-member order) starts at member[m], a pointer of the host's table,
-// and its selected channel s is the plane chan[member_src[m]][s] of its own source.  v[] is indexed by unrolled constants
+// Several sources (models) pooled: member m (source-then-member order) starts at src.member[m], a pointer of the host's
+// table, and its selected channel s is the plane src.chan[src.member_src[m]][s] of its own source.  v[] is indexed by unrolled constants
 // only, so it stays in registers.  With means set, the mean of each source's own members, summed in member order (the
 // arithmetic of k_ens_stats over that source alone), goes to means[k][s][p]; it is taken before reduce_point sorts v.
 template <int MP, bool QUANT>
@@ -131,16 +127,16 @@ __global__ void __launch_bounds__(kThreads) k_ens_stats_multi(const __grid_const
   float v[MP];
 #pragma unroll
   for (int m = 0; m < MP; ++m)
-    v[m] = m < M ? P.member[m][(long long)P.chan[P.member_src[m]][s] * P.plane + p] : __int_as_float(0x7f800000);
+    v[m] = m < M ? P.src.member[m][(long long)P.src.chan[P.src.member_src[m]][s] * P.plane + p] : __int_as_float(0x7f800000);
   if (P.means) {
 #pragma unroll
     for (int k = 0; k < kMaxSources; ++k) {
-      if (k >= P.n_src) break;
+      if (k >= P.src.n_src) break;
       double sum = 0.0;
 #pragma unroll
       for (int m = 0; m < MP; ++m)
-        if (m < M && P.member_src[m] == k) sum = __dadd_rn(sum, (double)v[m]);
-      P.means[((long long)k * P.n_sel + s) * P.plane + p] = (float)__ddiv_rn(sum, (double)P.src_members[k]);
+        if (m < M && P.src.member_src[m] == k) sum = __dadd_rn(sum, (double)v[m]);
+      P.means[((long long)k * P.n_sel + s) * P.plane + p] = (float)__ddiv_rn(sum, (double)P.src.src_members[k]);
     }
   }
   reduce_point<MP, QUANT>(v, P, s, p);
@@ -228,53 +224,19 @@ int sky_ensemble_stats_multi(int32_t n_sources, const float* const* x, const int
                              const int32_t* channel_count, const int32_t* channels, int32_t n_sel, int64_t plane,
                              const double* quantiles, int32_t n_q, const int32_t* event_sel, const float* event_thr,
                              int32_t n_events, float* stats, float* prob, float* means, void* stream) {
-  if (n_sources < 1 || n_sources > kMaxSources || !x || !members || !member_stride || !channel_count) {
-    set_error("n_sources = %d must lie in [1, %d], with x, members, member_stride and channel_count given", n_sources, kMaxSources);
-    return SKY_ERR_ARG;
-  }
-  if (plane < 1) { set_error("plane = %lld must be positive", (long long)plane); return SKY_ERR_ARG; }
-  int total = 0;
-  for (int k = 0; k < n_sources; ++k) {
-    if (members[k] < 1 || members[k] > kMaxMembers) { set_error("members[%d] = %d must lie in [1, %d]", k, members[k], kMaxMembers); return SKY_ERR_ARG; }
-    total += members[k];
-    if (channel_count[k] < 1) { set_error("channel_count[%d] = %d must be positive", k, channel_count[k]); return SKY_ERR_ARG; }
-    if (member_stride[k] < (int64_t)channel_count[k] * plane) {
-      set_error("member_stride[%d] = %lld is below channel_count x plane = %lld", k, (long long)member_stride[k],
-                (long long)channel_count[k] * plane);
-      return SKY_ERR_ARG;
-    }
-  }
-  if (total > kMaxMembers) { set_error("total members = %d exceed %d", total, kMaxMembers); return SKY_ERR_ARG; }
-  if (n_sel < 1 || n_sel > kMaxSel || !channels) { set_error("n_sel = %d channels must lie in [1, %d]", n_sel, kMaxSel); return SKY_ERR_ARG; }
   MultiStatsParams P{};
+  int total = 0, rc;
+  if ((rc = check_sources(n_sources, x, members, member_stride, channel_count, channels, n_sel, plane, P.src, &total)) ||
+      (rc = set_quantiles_events(P, total, n_sel, quantiles, n_q, event_sel, event_thr, n_events)))
+    return rc;
   P.plane = plane;
   P.members = total;
   P.n_sel = n_sel;
-  P.n_src = n_sources;
-  for (int k = 0; k < n_sources; ++k) {
-    P.src_members[k] = members[k];
-    for (int s = 0; s < n_sel; ++s) {
-      const int c = channels[k * n_sel + s];
-      if (c < 0 || c >= channel_count[k]) { set_error("channel %d of source %d is outside [0, %d)", c, k, channel_count[k]); return SKY_ERR_ARG; }
-      P.chan[k][s] = c;
-    }
-  }
-  int rc;
-  if ((rc = set_quantiles_events(P, total, n_sel, quantiles, n_q, event_sel, event_thr, n_events))) return rc;
-  for (int k = 0; k < n_sources; ++k)
-    if (!x[k]) { set_error("x[%d] must not be null", k); return SKY_ERR_ARG; }
   if (!stats || (n_events && !prob)) { set_error("stats and (with events) prob must not be null"); return SKY_ERR_ARG; }
   int dev = -1;
-  for (int k = 0; k < n_sources; ++k)
-    if ((rc = device_of(x[k], "x[k]", &dev))) return rc;
-  if ((rc = device_of(stats, "stats", &dev)) || (n_events && (rc = device_of(prob, "prob", &dev))) ||
+  if ((rc = sources_device(n_sources, x, &dev)) || (rc = device_of(stats, "stats", &dev)) || (n_events && (rc = device_of(prob, "prob", &dev))) ||
       (means && (rc = device_of(means, "means", &dev))))
     return rc;
-  for (int k = 0, m = 0; k < n_sources; ++k)
-    for (int j = 0; j < members[k]; ++j, ++m) {
-      P.member[m] = x[k] + j * member_stride[k];
-      P.member_src[m] = (unsigned char)k;
-    }
   P.stats = stats;
   P.prob = prob;
   P.means = means;

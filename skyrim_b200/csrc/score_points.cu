@@ -14,10 +14,14 @@
 // Score maps.  One thread per (channel, point) holds the members in registers, takes ens_point_terms (point_terms.cuh,
 // shared with k_scores_partial) and adds e = xb - y, e^2, var, mae / M and G to the point's five fp64 accumulators, once
 // per call: each accumulator sees its terms in call order, so the maps are bitwise reproducible.
+//
+// The *_multi entries run the same kernels over members pooled from several sources (member_reader.cuh); the Philox
+// channel word of a pooled histogram is source 0's plane index of the selected channel.
 #include <cmath>
 
 #include "engine.h"
 #include "member_fields.h"
+#include "member_reader.cuh"
 #include "philox.cuh"
 #include "point_terms.cuh"
 #include "sky_common.cuh"
@@ -38,18 +42,37 @@ struct PointParams {
   int plane, nlat, nlon, members, n_sel, n_reg;
   uint32_t seed, date, lead;
   int chan[kMaxSel];
+  static constexpr bool kPooled = false;
+  __device__ uint32_t philox_chan(int s) const { return (uint32_t)chan[s]; }
 };
 
-__global__ void __launch_bounds__(kRankThreads) k_rank_counts(const __grid_constant__ PointParams P) {
+// the block of the *_multi entries: the source table, then PointParams' other fields
+struct PooledPointParams {
+  PooledSources src;
+  const float* truth;
+  const double* roww;
+  int* counts;
+  double* out;
+  int plane, nlat, nlon, members, n_sel, n_reg;   // members: all sources' together
+  uint32_t seed, date, lead;
+  static constexpr bool kPooled = true;
+  __device__ uint32_t philox_chan(int s) const { return (uint32_t)src.chan[0][s]; }
+};
+// 2720 bytes: inside the 4 KB every sm_90 launch accepts without the large-parameter path
+static_assert(sizeof(PooledPointParams) == 2720, "keep the header comments of the *_multi entries in step");
+
+template <class Params>
+__global__ void __launch_bounds__(kRankThreads) k_rank_counts(const __grid_constant__ Params P) {
   const int row = blockIdx.x, s = blockIdx.y, M = P.members, tid = threadIdx.x;
   bool any = false;
   for (int r = 0; r < P.n_reg; ++r) any |= P.roww[r * P.nlat + row] > 0.0;
   if (!any) return;   // the same for the whole block: a row outside every region is not read
   __shared__ int cnt[kMaxMembers + 2];
+  __shared__ const float* base[Params::kPooled ? kMaxMembers : 1];
   for (int i = tid; i < M + 2; i += kRankThreads) cnt[i] = 0;
+  const auto xs = members_of(P, s, base);   // synchronises the block when pooled
   __syncthreads();
   const long long p0 = (long long)row * P.nlon;
-  const float* xs = P.x + (long long)P.chan[s] * P.plane + p0;
   const float* ys = P.truth + (long long)s * P.plane + p0;
   for (int j = tid; j < P.nlon; j += kRankThreads) {
     const float y = ys[j];
@@ -57,7 +80,7 @@ __global__ void __launch_bounds__(kRankThreads) k_rank_counts(const __grid_const
     bool nan = y != y;
 #pragma unroll 16
     for (int m = 0; m < M; ++m) {
-      const float xm = xs[m * P.member_stride + j];
+      const float xm = xs(m, p0 + j);
       lt += xm < y;
       eq += xm == y;
       nan |= xm != xm;
@@ -66,7 +89,7 @@ __global__ void __launch_bounds__(kRankThreads) k_rank_counts(const __grid_const
     if (!nan) {
       bin = lt;
       if (eq > 0) {
-        uint32_t c[4] = {(uint32_t)(p0 + j), kRankTag, (uint32_t)P.chan[s], P.lead};
+        uint32_t c[4] = {(uint32_t)(p0 + j), kRankTag, P.philox_chan(s), P.lead};
         philox4x32_10(c, P.seed, P.date);
         bin += (int)(((uint64_t)c[0] * (uint32_t)(eq + 1)) >> 32);   // floor(u (E + 1)), u = c0 / 2^32
       }
@@ -78,7 +101,8 @@ __global__ void __launch_bounds__(kRankThreads) k_rank_counts(const __grid_const
   for (int i = tid; i < M + 2; i += kRankThreads) dst[i] = cnt[i];
 }
 
-__global__ void __launch_bounds__(kRankThreads) k_rank_final(const __grid_constant__ PointParams P) {
+template <class Params>
+__global__ void __launch_bounds__(kRankThreads) k_rank_final(const __grid_constant__ Params P) {
   const int bins = P.members + 1, i = blockIdx.x * kRankThreads + threadIdx.x;
   if (i >= P.n_reg * P.n_sel * bins) return;
   const int r = i / (P.n_sel * bins), s = i / bins % P.n_sel, k = i % bins;
@@ -95,15 +119,16 @@ __global__ void __launch_bounds__(kRankThreads) k_rank_final(const __grid_consta
   P.out[i] = nan ? __longlong_as_double(0x7ff8000000000000ll) : a / P.nlon;
 }
 
-template <int MP>
-__global__ void __launch_bounds__(kMapThreads) k_score_maps(const __grid_constant__ PointParams P) {
+template <class Params, int MP>
+__global__ void __launch_bounds__(kMapThreads) k_score_maps(const __grid_constant__ Params P) {
   const int s = blockIdx.y, M = P.members;
   const long long p = (long long)blockIdx.x * kMapThreads + threadIdx.x;
+  __shared__ const float* base[Params::kPooled ? kMaxMembers : 1];
+  const auto xs = members_of(P, s, base);   // every thread, before any returns
   if (p >= P.plane) return;
-  const float* xs = P.x + (long long)P.chan[s] * P.plane + p;
   float v[MP];
 #pragma unroll
-  for (int m = 0; m < MP; ++m) v[m] = m < M ? xs[m * P.member_stride] : __int_as_float(0x7f800000);
+  for (int m = 0; m < MP; ++m) v[m] = m < M ? xs(m, p) : __int_as_float(0x7f800000);
   const float yf = P.truth[(long long)s * P.plane + p];
   const double y = yf;
   const EnsPointTerms q = ens_point_terms(v, M, y, yf != yf);
@@ -115,22 +140,13 @@ __global__ void __launch_bounds__(kMapThreads) k_score_maps(const __grid_constan
   for (int t = 0; t < kMapTerms; ++t) o[t * (long long)P.plane] += nan ? __longlong_as_double(0x7ff8000000000000ll) : term[t];
 }
 
-}  // namespace
-}  // namespace sky
-
-using namespace sky;
-
-extern "C" {
-
-int sky_forecast_rank_histogram(const float* x, int32_t members, int64_t member_stride, int32_t nlat, int32_t nlon,
-                                int32_t channel_count, const int32_t* channels, int32_t n_sel, const float* truth,
-                                const double* row_weights, int32_t n_regions, uint64_t seed, int32_t date_index,
-                                int32_t lead_index, int32_t* counts, uint64_t counts_bytes, double* hist, void* stream) {
-  PointParams P{};
-  int rc;
-  if ((rc = check_grid(nlat, nlon)) ||
-      (rc = check_members(members, member_stride, (int64_t)nlat * nlon, channel_count, channels, n_sel, P.chan)))
-    return rc;
+// The histogram of both entries, once P's members are set and checked (x_given: their pointers are not null): the region,
+// key, workspace and null-pointer checks (no CUDA call), then member_device(&dev) and the other buffers' device checks.
+template <class Params, class MemberDevice>
+int run_rank_histogram(Params& P, int nlat, int nlon, int n_sel, const float* truth, const double* row_weights,
+                       int n_regions, uint64_t seed, int date_index, int lead_index, int32_t* counts, uint64_t counts_bytes,
+                       double* hist, bool x_given, MemberDevice&& member_device, void* stream) {
+  const int members = P.members;
   if (n_regions < 1 || n_regions > kMaxRegions) { set_error("n_regions = %d must lie in [1, %d]", n_regions, kMaxRegions); return SKY_ERR_ARG; }
   if (seed > UINT32_MAX) { set_error("seed = %llu must lie in [0, 2^32)", (unsigned long long)seed); return SKY_ERR_ARG; }
   if (date_index < 0 || lead_index < 0) {
@@ -143,22 +159,19 @@ int sky_forecast_rank_histogram(const float* x, int32_t members, int64_t member_
               (unsigned long long)need);
     return SKY_ERR_ARG;
   }
-  if (!x || !truth || !row_weights || !counts || !hist) {
+  if (!x_given || !truth || !row_weights || !counts || !hist) {
     set_error("x, truth, row_weights, counts and hist must not be null");
     return SKY_ERR_ARG;
   }
-  int dev = -1;
-  if ((rc = device_of(x, "x", &dev)) || (rc = device_of(truth, "truth", &dev)) ||
+  int dev = -1, rc;
+  if ((rc = member_device(&dev)) || (rc = device_of(truth, "truth", &dev)) ||
       (rc = device_of(row_weights, "row_weights", &dev)) || (rc = device_of(counts, "counts", &dev)) ||
       (rc = device_of(hist, "hist", &dev)))
     return rc;
-  P.x = x;
   P.truth = truth;
-  P.member_stride = member_stride;
   P.plane = nlat * nlon;
   P.nlat = nlat;
   P.nlon = nlon;
-  P.members = members;
   P.n_sel = n_sel;
   P.roww = row_weights;
   P.counts = counts;
@@ -179,6 +192,66 @@ int sky_forecast_rank_histogram(const float* x, int32_t members, int64_t member_
   return SKY_OK;
 }
 
+// The maps of both entries, as run_rank_histogram
+template <class Params, class MemberDevice>
+int run_score_maps(Params& P, int nlat, int nlon, int n_sel, const float* truth, double* maps, bool x_given,
+                   MemberDevice&& member_device, void* stream) {
+  if (!x_given || !truth || !maps) { set_error("x, truth and maps must not be null"); return SKY_ERR_ARG; }
+  int dev = -1, rc;
+  if ((rc = member_device(&dev)) || (rc = device_of(truth, "truth", &dev)) || (rc = device_of(maps, "maps", &dev)))
+    return rc;
+  P.truth = truth;
+  P.out = maps;
+  P.plane = nlat * nlon;
+  P.n_sel = n_sel;
+  DeviceGuard guard(dev);
+  cudaStream_t st = (cudaStream_t)stream;
+  const dim3 grid((unsigned)((P.plane + kMapThreads - 1) / kMapThreads), (unsigned)n_sel);
+  dispatch_padding<1>(P.members, [&](auto mp) { k_score_maps<Params, mp><<<grid, kMapThreads, 0, st>>>(P); });
+  count_launch();
+  SKY_CUDA_OK(cudaGetLastError());
+  return SKY_OK;
+}
+
+}  // namespace
+}  // namespace sky
+
+using namespace sky;
+
+extern "C" {
+
+int sky_forecast_rank_histogram(const float* x, int32_t members, int64_t member_stride, int32_t nlat, int32_t nlon,
+                                int32_t channel_count, const int32_t* channels, int32_t n_sel, const float* truth,
+                                const double* row_weights, int32_t n_regions, uint64_t seed, int32_t date_index,
+                                int32_t lead_index, int32_t* counts, uint64_t counts_bytes, double* hist, void* stream) {
+  PointParams P{};
+  int rc;
+  if ((rc = check_grid(nlat, nlon)) ||
+      (rc = check_members(members, member_stride, (int64_t)nlat * nlon, channel_count, channels, n_sel, P.chan)))
+    return rc;
+  P.x = x;
+  P.member_stride = member_stride;
+  P.members = members;
+  return run_rank_histogram(P, nlat, nlon, n_sel, truth, row_weights, n_regions, seed, date_index, lead_index, counts,
+                            counts_bytes, hist, x != nullptr, [&](int* dev) { return device_of(x, "x", dev); }, stream);
+}
+
+int sky_forecast_rank_histogram_multi(int32_t n_sources, const float* const* x, const int32_t* members,
+                                      const int64_t* member_stride, const int32_t* channel_count, const int32_t* channels,
+                                      int32_t n_sel, int32_t nlat, int32_t nlon, const float* truth,
+                                      const double* row_weights, int32_t n_regions, uint64_t seed, int32_t date_index,
+                                      int32_t lead_index, int32_t* counts, uint64_t counts_bytes, double* hist,
+                                      void* stream) {
+  PooledPointParams P{};
+  int rc;
+  if ((rc = check_grid(nlat, nlon)) ||
+      (rc = check_sources(n_sources, x, members, member_stride, channel_count, channels, n_sel, (int64_t)nlat * nlon, P.src,
+                          &P.members)))
+    return rc;
+  return run_rank_histogram(P, nlat, nlon, n_sel, truth, row_weights, n_regions, seed, date_index, lead_index, counts,
+                            counts_bytes, hist, true, [&](int* dev) { return sources_device(n_sources, x, dev); }, stream);
+}
+
 int sky_forecast_score_maps(const float* x, int32_t members, int64_t member_stride, int32_t nlat, int32_t nlon,
                             int32_t channel_count, const int32_t* channels, int32_t n_sel, const float* truth, double* maps,
                             void* stream) {
@@ -187,24 +260,24 @@ int sky_forecast_score_maps(const float* x, int32_t members, int64_t member_stri
   if ((rc = check_grid(nlat, nlon)) ||
       (rc = check_members(members, member_stride, (int64_t)nlat * nlon, channel_count, channels, n_sel, P.chan)))
     return rc;
-  if (!x || !truth || !maps) { set_error("x, truth and maps must not be null"); return SKY_ERR_ARG; }
-  int dev = -1;
-  if ((rc = device_of(x, "x", &dev)) || (rc = device_of(truth, "truth", &dev)) || (rc = device_of(maps, "maps", &dev)))
-    return rc;
   P.x = x;
-  P.truth = truth;
-  P.out = maps;
   P.member_stride = member_stride;
-  P.plane = nlat * nlon;
   P.members = members;
-  P.n_sel = n_sel;
-  DeviceGuard guard(dev);
-  cudaStream_t st = (cudaStream_t)stream;
-  const dim3 grid((unsigned)((P.plane + kMapThreads - 1) / kMapThreads), (unsigned)n_sel);
-  dispatch_padding<1>(members, [&](auto mp) { k_score_maps<mp><<<grid, kMapThreads, 0, st>>>(P); });
-  count_launch();
-  SKY_CUDA_OK(cudaGetLastError());
-  return SKY_OK;
+  return run_score_maps(P, nlat, nlon, n_sel, truth, maps, x != nullptr, [&](int* dev) { return device_of(x, "x", dev); },
+                        stream);
+}
+
+int sky_forecast_score_maps_multi(int32_t n_sources, const float* const* x, const int32_t* members,
+                                  const int64_t* member_stride, const int32_t* channel_count, const int32_t* channels,
+                                  int32_t n_sel, int32_t nlat, int32_t nlon, const float* truth, double* maps, void* stream) {
+  PooledPointParams P{};
+  int rc;
+  if ((rc = check_grid(nlat, nlon)) ||
+      (rc = check_sources(n_sources, x, members, member_stride, channel_count, channels, n_sel, (int64_t)nlat * nlon, P.src,
+                          &P.members)))
+    return rc;
+  return run_score_maps(P, nlat, nlon, n_sel, truth, maps, true, [&](int* dev) { return sources_device(n_sources, x, dev); },
+                        stream);
 }
 
 }  // extern "C"

@@ -17,11 +17,13 @@
 // j + kThreads, ... of a row, then adds the row's sums, weighted per region, to its running sums; the block adds its
 // threads' sums in thread order and writes one partial per (region, channel, term, block).  Launch 2 sums the kBlocks partials of each (region, channel, term) in block order.  The
 // partial layout does not depend on the SM count, so the sums are bitwise reproducible and a channel's or a region's sums
-// do not depend on the rest of the request.
+// do not depend on the rest of the request.  sky_forecast_scores_multi runs the same kernels over members pooled from
+// several sources (member_reader.cuh): only the loads of the members differ.
 #include <cmath>
 
 #include "engine.h"
 #include "member_fields.h"
+#include "member_reader.cuh"
 #include "point_terms.cuh"
 #include "sky_common.cuh"
 
@@ -40,13 +42,29 @@ struct ScoresParams {
   long long member_stride;
   int plane, nlat, nlon, members, n_sel, n_reg;
   int chan[kMaxSel];
+  static constexpr bool kPooled = false;
 };
 
-template <int MP, int U>
-__global__ void __launch_bounds__(kThreads) k_scores_partial(const __grid_constant__ ScoresParams P) {
+// sky_forecast_scores_multi's block: the source table, then ScoresParams' other fields
+struct PooledScoresParams {
+  PooledSources src;
+  const float* truth;
+  const float* clim;
+  const double* roww;
+  double* partial;
+  double* sums;
+  int plane, nlat, nlon, members, n_sel, n_reg;   // members: all sources' together
+  static constexpr bool kPooled = true;
+};
+// 2712 bytes: inside the 4 KB every sm_90 launch accepts without the large-parameter path
+static_assert(sizeof(PooledScoresParams) == 2712, "keep the header comment of sky_forecast_scores_multi in step");
+
+template <class Params, int MP, int U>
+__global__ void __launch_bounds__(kThreads) k_scores_partial(const __grid_constant__ Params P) {
   const int s = blockIdx.y, b = blockIdx.x, M = P.members, R = P.n_reg, tid = threadIdx.x;
   const double invM = 1.0 / M;
-  const float* xs = P.x + (long long)P.chan[s] * P.plane;
+  __shared__ const float* base[Params::kPooled ? kMaxMembers : 1];
+  const auto xs = members_of(P, s, base);
   const float* ys = P.truth + (long long)s * P.plane;
   const float* ks = P.clim ? P.clim + (long long)s * P.plane : nullptr;
   const double qnan = __longlong_as_double(0x7ff8000000000000ll);
@@ -75,7 +93,7 @@ __global__ void __launch_bounds__(kThreads) k_scores_partial(const __grid_consta
         const bool in = j < P.nlon;
         const long long p = (long long)row * P.nlon + (in ? j : 0);
 #pragma unroll
-        for (int m = 0; m < MP; ++m) v[u][m] = m < M && in ? xs[m * P.member_stride + p] : __int_as_float(0x7f800000);
+        for (int m = 0; m < MP; ++m) v[u][m] = m < M && in ? xs(m, p) : __int_as_float(0x7f800000);
         yf[u] = in ? ys[p] : 0.f;
         kf[u] = in && ks ? ks[p] : 0.f;
       }
@@ -122,7 +140,8 @@ __global__ void __launch_bounds__(kThreads) k_scores_partial(const __grid_consta
   }
 }
 
-__global__ void __launch_bounds__(kThreads) k_scores_final(const __grid_constant__ ScoresParams P) {
+template <class Params>
+__global__ void __launch_bounds__(kThreads) k_scores_final(const __grid_constant__ Params P) {
   const int i = blockIdx.x * kThreads + threadIdx.x;
   if (i >= P.n_reg * P.n_sel * kTerms) return;
   const double* src = P.partial + (long long)i * kBlocks;
@@ -132,10 +151,54 @@ __global__ void __launch_bounds__(kThreads) k_scores_final(const __grid_constant
 }
 
 // points per thread per pass: enough loads in flight at the occupancy each padding allows
-template <int MP>
-void launch(const ScoresParams& P, cudaStream_t st) {
+template <int MP, class Params>
+void launch(const Params& P, cudaStream_t st) {
   constexpr int U = MP <= 8 ? 4 : MP == 16 ? 2 : 1;
-  k_scores_partial<MP, U><<<dim3(kBlocks, P.n_sel), kThreads, 0, st>>>(P);
+  k_scores_partial<Params, MP, U><<<dim3(kBlocks, P.n_sel), kThreads, 0, st>>>(P);
+}
+
+// Both entries, once P's members are set and checked (x_given: the members' pointers are not null): the region, workspace
+// and null-pointer checks (no CUDA call), then member_device(&dev) and the device checks of the other buffers, then the
+// two launches on the members' device.
+template <class Params, class MemberDevice>
+int run_scores(Params& P, int nlat, int nlon, int n_sel, const float* truth, const float* clim, const double* row_weights,
+               int n_regions, double* partial, uint64_t partial_bytes, double* sums, bool x_given,
+               MemberDevice&& member_device, void* stream) {
+  if (n_regions < 1 || n_regions > kMaxRegions) { set_error("n_regions = %d must lie in [1, %d]", n_regions, kMaxRegions); return SKY_ERR_ARG; }
+  const uint64_t need = (uint64_t)n_regions * n_sel * kTerms * kBlocks * sizeof(double);
+  if (partial_bytes < need) {
+    set_error("partial_bytes = %llu is below %llu (n_regions x n_sel x 9 x %d doubles)", (unsigned long long)partial_bytes,
+              (unsigned long long)need, kBlocks);
+    return SKY_ERR_ARG;
+  }
+  if (!x_given || !truth || !row_weights || !partial || !sums) {
+    set_error("x, truth, row_weights, partial and sums must not be null");
+    return SKY_ERR_ARG;
+  }
+  int dev = -1, rc;
+  if ((rc = member_device(&dev)) || (rc = device_of(truth, "truth", &dev)) || (clim && (rc = device_of(clim, "clim", &dev))) ||
+      (rc = device_of(row_weights, "row_weights", &dev)) || (rc = device_of(partial, "partial", &dev)) ||
+      (rc = device_of(sums, "sums", &dev)))
+    return rc;
+  P.truth = truth;
+  P.clim = clim;
+  P.roww = row_weights;
+  P.partial = partial;
+  P.sums = sums;
+  P.plane = nlat * nlon;
+  P.nlat = nlat;
+  P.nlon = nlon;
+  P.n_sel = n_sel;
+  P.n_reg = n_regions;
+  DeviceGuard guard(dev);   // launch on the device that owns the members, whatever the caller's current device is
+  cudaStream_t st = (cudaStream_t)stream;
+  dispatch_padding<1>(P.members, [&](auto mp) { launch<mp>(P, st); });
+  count_launch();
+  SKY_CUDA_OK(cudaGetLastError());
+  k_scores_final<<<(n_regions * n_sel * kTerms + kThreads - 1) / kThreads, kThreads, 0, st>>>(P);
+  count_launch();
+  SKY_CUDA_OK(cudaGetLastError());
+  return SKY_OK;
 }
 
 }  // namespace
@@ -154,44 +217,25 @@ int sky_forecast_scores(const float* x, int32_t members, int64_t member_stride, 
   if ((rc = check_grid(nlat, nlon)) ||
       (rc = check_members(members, member_stride, (int64_t)nlat * nlon, channel_count, channels, n_sel, P.chan)))
     return rc;
-  if (n_regions < 1 || n_regions > kMaxRegions) { set_error("n_regions = %d must lie in [1, %d]", n_regions, kMaxRegions); return SKY_ERR_ARG; }
-  const uint64_t need = (uint64_t)n_regions * n_sel * kTerms * kBlocks * sizeof(double);
-  if (partial_bytes < need) {
-    set_error("partial_bytes = %llu is below %llu (n_regions x n_sel x 9 x %d doubles)", (unsigned long long)partial_bytes,
-              (unsigned long long)need, kBlocks);
-    return SKY_ERR_ARG;
-  }
-  if (!x || !truth || !row_weights || !partial || !sums) {
-    set_error("x, truth, row_weights, partial and sums must not be null");
-    return SKY_ERR_ARG;
-  }
-  int dev = -1;
-  if ((rc = device_of(x, "x", &dev)) || (rc = device_of(truth, "truth", &dev)) || (clim && (rc = device_of(clim, "clim", &dev))) ||
-      (rc = device_of(row_weights, "row_weights", &dev)) || (rc = device_of(partial, "partial", &dev)) ||
-      (rc = device_of(sums, "sums", &dev)))
-    return rc;
   P.x = x;
-  P.truth = truth;
-  P.clim = clim;
-  P.roww = row_weights;
-  P.partial = partial;
-  P.sums = sums;
   P.member_stride = member_stride;
-  P.plane = nlat * nlon;
-  P.nlat = nlat;
-  P.nlon = nlon;
   P.members = members;
-  P.n_sel = n_sel;
-  P.n_reg = n_regions;
-  DeviceGuard guard(dev);   // launch on the device that owns the members, whatever the caller's current device is
-  cudaStream_t st = (cudaStream_t)stream;
-  dispatch_padding<1>(members, [&](auto mp) { launch<mp>(P, st); });
-  count_launch();
-  SKY_CUDA_OK(cudaGetLastError());
-  k_scores_final<<<(n_regions * n_sel * kTerms + kThreads - 1) / kThreads, kThreads, 0, st>>>(P);
-  count_launch();
-  SKY_CUDA_OK(cudaGetLastError());
-  return SKY_OK;
+  return run_scores(P, nlat, nlon, n_sel, truth, clim, row_weights, n_regions, partial, partial_bytes, sums, x != nullptr,
+                    [&](int* dev) { return device_of(x, "x", dev); }, stream);
+}
+
+int sky_forecast_scores_multi(int32_t n_sources, const float* const* x, const int32_t* members, const int64_t* member_stride,
+                              const int32_t* channel_count, const int32_t* channels, int32_t n_sel, int32_t nlat,
+                              int32_t nlon, const float* truth, const float* clim, const double* row_weights,
+                              int32_t n_regions, double* partial, uint64_t partial_bytes, double* sums, void* stream) {
+  PooledScoresParams P{};
+  int rc;
+  if ((rc = check_grid(nlat, nlon)) ||
+      (rc = check_sources(n_sources, x, members, member_stride, channel_count, channels, n_sel, (int64_t)nlat * nlon, P.src,
+                          &P.members)))
+    return rc;
+  return run_scores(P, nlat, nlon, n_sel, truth, clim, row_weights, n_regions, partial, partial_bytes, sums, true,
+                    [&](int* dev) { return sources_device(n_sources, x, dev); }, stream);
 }
 
 }  // extern "C"

@@ -517,6 +517,107 @@ def score_maps_accumulate(x, truth, maps, channels=None, channel_offset: int = 0
     return maps
 
 
+def _pooled_sources(sources, channels_per_source, truth=None, clim=None, row_weights=None):
+    """the source arguments of the *_multi verification entries: (K, M, H, W, bases, members, strides, counts, flat
+    channels, n_sel), with sources and their channel lists checked as ``multi_model_statistics`` checks them and truth /
+    clim / row_weights as ``_verified_members`` checks them"""
+    import torch
+    K = len(sources)
+    if not 1 <= K <= ENS_MAX_SOURCES or len(channels_per_source) != K:
+        raise ValueError(f"{K} sources with {len(channels_per_source)} channel lists: 1 to {ENS_MAX_SOURCES} sources, one "
+                         "list each")
+    views = [_member_view(x, name=f"source {k}") for k, x in enumerate(sources)]
+    members, nlat, nlon, counts, strides, bases = zip(*views)
+    if len(set(zip(nlat, nlon))) != 1:
+        raise ValueError(f"every source must lie on one grid ({list(zip(nlat, nlon))})")
+    if len({x.device for x in sources}) != 1:
+        raise ValueError(f"every source must lie on one device ({[str(x.device) for x in sources]})")
+    H, W = nlat[0], nlon[0]
+    sel = [[int(c) for c in chans] for chans in channels_per_source]
+    n_sel = len(sel[0])
+    if any(len(c) != n_sel for c in sel):
+        raise ValueError("every source must list the same number of channels")
+    for name, t in dict(truth=truth, clim=clim).items():
+        if t is not None and (not t.is_cuda or t.dtype != torch.float32 or not t.is_contiguous()
+                              or tuple(t.shape) != (n_sel, H, W)):
+            raise ValueError(f"{name} must be a contiguous CUDA fp32 {(n_sel, H, W)} tensor (got {tuple(t.shape)})")
+    if row_weights is not None and not (row_weights.is_cuda and row_weights.dtype == torch.float64
+                                        and row_weights.is_contiguous() and row_weights.dim() == 2
+                                        and row_weights.shape[1] == H):
+        raise ValueError(f"row_weights must be a contiguous CUDA fp64 (n_regions, {H}) tensor")
+    flat = [c for chans in sel for c in chans]
+    return (K, sum(members), H, W, _c_array(C.c_void_p, bases), _c_array(C.c_int32, members),
+            _c_array(C.c_int64, strides), _c_array(C.c_int32, counts), _c_array(C.c_int32, flat), n_sel)
+
+
+def forecast_scores_multi(sources, channels_per_source, truth, row_weights, clim=None, out=None):
+    """``forecast_scores`` of the members of up to four sources pooled in source-then-member order
+    (include/skyrim_b200.h sky_forecast_scores_multi): ``sources`` and ``channels_per_source`` as for
+    ``multi_model_statistics`` (a GraphCast state's new slice is a view), ``truth`` / ``clim`` CUDA fp32 (n_sel, H, W) in
+    the order of the channel lists.  Bitwise the sums ``forecast_scores`` gives on the pooled members stacked into one
+    tensor in source 0's channel order.  Returns the CUDA fp64 sums (n_regions, n_sel, 9), into ``out`` when given.
+    Asynchronous on the current stream."""
+    import torch
+    K, M, H, W, bases, members, strides, counts, flat, n_sel = _pooled_sources(sources, channels_per_source, truth, clim,
+                                                                               row_weights)
+    dev = sources[0].device
+    R = row_weights.shape[0]
+    shape = (R, n_sel, SCORES_TERMS)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float64, device=dev)
+    _check_out(out, shape, torch.float64, "out")
+    ws = torch.empty(max(R * n_sel * SCORES_TERMS * SCORES_BLOCKS, 1), dtype=torch.float64, device=dev)
+    L = _ffi.lib()
+    st = torch.cuda.current_stream(dev).cuda_stream
+    _ffi.check(L.sky_forecast_scores_multi(K, bases, members, strides, counts, flat, n_sel, H, W, truth.data_ptr(),
+                                           None if clim is None else clim.data_ptr(), row_weights.data_ptr(), R,
+                                           ws.data_ptr(), 8 * ws.numel(), out.data_ptr(), st),
+               "sky_forecast_scores_multi", L)
+    return out
+
+
+def forecast_rank_histogram_multi(sources, channels_per_source, truth, row_weights, seed: int, date_index: int,
+                                  lead_index: int, out=None):
+    """``forecast_rank_histogram`` of the pooled members of ``sources`` (as for ``forecast_scores_multi``;
+    include/skyrim_b200.h sky_forecast_rank_histogram_multi): the tie-breaking draws are counted by source 0's channel
+    index.  Returns the CUDA fp64 (n_regions, n_sel, M + 1) histogram, M the pooled member count, into ``out`` when given.
+    Asynchronous on the current stream."""
+    import torch
+    K, M, H, W, bases, members, strides, counts, flat, n_sel = _pooled_sources(sources, channels_per_source, truth, None,
+                                                                               row_weights)
+    if not 0 <= int(seed) < 2 ** 32 or int(date_index) < 0 or int(lead_index) < 0:
+        raise ValueError(f"seed = {seed} must lie in [0, 2^32), date_index = {date_index} and lead_index = {lead_index} "
+                         "must not be negative")
+    dev = sources[0].device
+    R = row_weights.shape[0]
+    shape = (R, n_sel, M + 1)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float64, device=dev)
+    _check_out(out, shape, torch.float64, "out")
+    ws = torch.empty(max(n_sel * H * (M + 2), 1), dtype=torch.int32, device=dev)
+    L = _ffi.lib()
+    st = torch.cuda.current_stream(dev).cuda_stream
+    _ffi.check(L.sky_forecast_rank_histogram_multi(K, bases, members, strides, counts, flat, n_sel, H, W, truth.data_ptr(),
+                                                   row_weights.data_ptr(), R, int(seed), int(date_index), int(lead_index),
+                                                   ws.data_ptr(), 4 * ws.numel(), out.data_ptr(), st),
+               "sky_forecast_rank_histogram_multi", L)
+    return out
+
+
+def score_maps_accumulate_multi(sources, channels_per_source, truth, maps):
+    """``score_maps_accumulate`` of the pooled members of ``sources`` (as for ``forecast_scores_multi``;
+    include/skyrim_b200.h sky_forecast_score_maps_multi) into ``maps``, CUDA fp64 (n_sel, 5, H, W).  Returns ``maps``.
+    Asynchronous on the current stream."""
+    import torch
+    K, M, H, W, bases, members, strides, counts, flat, n_sel = _pooled_sources(sources, channels_per_source, truth)
+    _check_out(maps, (n_sel, MAP_TERMS, H, W), torch.float64, "maps")
+    L = _ffi.lib()
+    st = torch.cuda.current_stream(sources[0].device).cuda_stream
+    _ffi.check(L.sky_forecast_score_maps_multi(K, bases, members, strides, counts, flat, n_sel, H, W, truth.data_ptr(),
+                                               maps.data_ptr(), st), "sky_forecast_score_maps_multi", L)
+    return maps
+
+
 def unix_seconds(when) -> float:
     """datetime (naive = UTC) / numpy datetime64 / number -> unix seconds"""
     import datetime as _dt

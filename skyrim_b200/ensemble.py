@@ -130,17 +130,9 @@ class EnsembleRunner:
             cur, i = nxt, i + 1
 
     def truth_ring(self, n_sel: int):
-        """the truth buffers of ``iter_scores`` for ``n_sel`` channels: a copy stream and two device and two pinned host
-        (n_sel, H, W) fp32 buffers with their events.  Pinning dominates the set-up of a scoring call, so a campaign over
-        many start dates makes one ring and passes it to every call."""
-        import torch
-        dev = self.x.device
-        H, W = self.x.shape[-2:]
-        return dict(copy=torch.cuda.Stream(dev),
-                    dbuf=[torch.empty((n_sel, H, W), dtype=torch.float32, device=dev) for _ in range(2)],
-                    hbuf=[torch.empty((n_sel, H, W), dtype=torch.float32).pin_memory() for _ in range(2)],
-                    uploaded=[torch.cuda.Event() for _ in range(2)],   # truth i % 2 is on the device
-                    scored=[torch.cuda.Event() for _ in range(2)])     # the work that read dbuf[i % 2] is done
+        """``truth_ring`` for ``n_sel`` channels on this runner's device and grid.  Pinning dominates the set-up of a
+        scoring call, so a campaign over many start dates makes one ring and passes it to every call."""
+        return truth_ring(self.x.device, n_sel, *self.x.shape[-2:])
 
     def iter_scores(self, n_steps: int, truth_at, clim=None, channels=None, row_weights=None, channel_offset: int = 0,
                     hist=None, seed: int = 0, date_index: int = 0, maps=None, map_slot=None, map_channels=(), sums=None,
@@ -148,9 +140,8 @@ class EnsembleRunner:
         """Steps ``n_steps`` times and scores this rank's members at every lead n = 0 .. n_steps against
         ``truth_at(n)`` (host fp32 (n_sel, H, W) of the selected channels), with the static climatology ``clim`` (host
         fp32 (n_sel, H, W) or None) and the regions of ``row_weights`` (fp64 (n_regions, H)): ``engine.forecast_scores``.
-        Per lead the forwards are launched first and the truth is fetched on the host while they run, then uploaded on a
-        copy stream into a ring of two device buffers (events order each upload after the scoring that last read its
-        buffer, and the scoring after the upload).  Every lead's sums stay in one device tensor that crosses to the host
+        Per lead the forwards are launched first and the truth is fetched on the host while they run, then uploaded by
+        ``upload_truth``.  Every lead's sums stay in one device tensor that crosses to the host
         once, at the end.  Returns (leads, fp64 host tensor (n_leads, n_regions, n_sel, 9)).
 
         Off the same uploaded truth, optionally: ``hist`` (CUDA fp64 (n_leads, n_regions, n_sel, M + 1)) receives each
@@ -170,29 +161,48 @@ class EnsembleRunner:
         out = sums if sums is not None else torch.empty((n_steps + 1, rw.shape[0], n_sel, 9), dtype=torch.float64,
                                                         device=dev)
         ring = ring or self.truth_ring(n_sel)
-        copy, dbuf, hbuf, uploaded, scored = (ring[k] for k in ("copy", "dbuf", "hbuf", "uploaded", "scored"))
         map_slot = map_slot or {}
         leads = []
         for i, (n, members) in enumerate(self._walk(n_steps, every_slice=True)):
-            y = truth_at(n)                                 # the host fetch runs under the forwards just launched
-            uploaded[i % 2].synchronize()                   # lead i - 2's upload has left hbuf[i % 2]
-            np.copyto(hbuf[i % 2].numpy(), y)
-            copy.wait_event(scored[i % 2])                  # lead i - 2's scoring has read dbuf[i % 2]
-            with torch.cuda.stream(copy):
-                dbuf[i % 2].copy_(hbuf[i % 2], non_blocking=True)
-                uploaded[i % 2].record(copy)
-            main.wait_event(uploaded[i % 2])
-            forecast_scores(members, dbuf[i % 2], rw, channels, kd, channel_offset, out=out[i])
+            y = upload_truth(ring, i, truth_at(n), main)   # the host fetch runs under the forwards just launched
+            forecast_scores(members, y, rw, channels, kd, channel_offset, out=out[i])
             if hist is not None:
-                forecast_rank_histogram(members, dbuf[i % 2], rw, seed, date_index, n, channels, channel_offset,
-                                        out=hist[i])
+                forecast_rank_histogram(members, y, rw, seed, date_index, n, channels, channel_offset, out=hist[i])
             if n in map_slot:
                 for j, k in enumerate(map_channels):       # one plane of the truth per map channel
-                    score_maps_accumulate(members, dbuf[i % 2][k:k + 1], maps[map_slot[n], j:j + 1], [sel[k]],
-                                          channel_offset)
-            scored[i % 2].record(main)
+                    score_maps_accumulate(members, y[k:k + 1], maps[map_slot[n], j:j + 1], [sel[k]], channel_offset)
+            ring["scored"][i % 2].record(main)
             leads.append(n)
         return leads, (out if sums is not None else out.cpu())
+
+
+def truth_ring(device, n_sel: int, H: int, W: int):
+    """the truth buffers of a scoring loop for ``n_sel`` channels: a copy stream and two device and two pinned host
+    (n_sel, H, W) fp32 buffers with their events (``upload_truth``)"""
+    import torch
+    return dict(copy=torch.cuda.Stream(device),
+                dbuf=[torch.empty((n_sel, H, W), dtype=torch.float32, device=device) for _ in range(2)],
+                hbuf=[torch.empty((n_sel, H, W), dtype=torch.float32).pin_memory() for _ in range(2)],
+                uploaded=[torch.cuda.Event() for _ in range(2)],   # truth i % 2 is on the device
+                scored=[torch.cuda.Event() for _ in range(2)])     # the work that read dbuf[i % 2] is done
+
+
+def upload_truth(ring, i: int, y, main):
+    """Uploads lead i's host truth ``y`` (fp32 (n_sel, H, W)) into ``ring`` (``truth_ring``) and returns its device buffer,
+    which the work queued next on ``main`` may read.  The upload runs on the ring's copy stream through the pinned buffer
+    i % 2: it waits on the host until lead i - 2's upload has left that buffer and, on the copy stream, until the work that
+    read lead i - 2's device buffer is done; ``main`` waits for the upload.  The caller records ``ring["scored"][i % 2]``
+    on ``main`` after the last work that reads the buffer."""
+    import torch
+    copy, dbuf, hbuf, uploaded, scored = (ring[k] for k in ("copy", "dbuf", "hbuf", "uploaded", "scored"))
+    uploaded[i % 2].synchronize()                   # lead i - 2's upload has left hbuf[i % 2]
+    np.copyto(hbuf[i % 2].numpy(), y)
+    copy.wait_event(scored[i % 2])                  # lead i - 2's scoring has read dbuf[i % 2]
+    with torch.cuda.stream(copy):
+        dbuf[i % 2].copy_(hbuf[i % 2], non_blocking=True)
+        uploaded[i % 2].record(copy)
+    main.wait_event(uploaded[i % 2])
+    return dbuf[i % 2]
 
 
 class HierarchicalEnsembleRunner(EnsembleRunner):

@@ -8,6 +8,8 @@ defaults; same `run_forecast` signature and return value) on top of the H100 eng
     python -m skyrim_b200.forecast -m pangu -l 72 --score --truth era5.nc --climatology clim.nc -o outputs
     python -m skyrim_b200.forecast -m pangu -d 20240501 -l 72 --score --until 20240531 --map_channels z500,t850 \
         --map_leads 24,72 --truth era5.nc -o outputs
+    python -m skyrim_b200.forecast --models pangu,fourcastnet_v2,graphcast --compare -d 20240501 --until 20240531 -l 72 \
+        --truth era5.nc --climatology clim.nc --map_channels z500 --map_leads 24,72 -o outputs
 
 The second form runs a perturbed-initial-condition ensemble and saves its per-step statistics (mean, spread, quantiles)
 and exceedance probabilities instead of the members.  The third runs several models side by side on one GPU
@@ -15,7 +17,11 @@ and exceedance probabilities instead of the members.  The third runs several mod
 The fifth verifies the forecast (``--members`` members) against analyses and saves one scorecard of latitude-weighted
 scores per lead time (``GlobalModel.score``).  With ``--until`` (or ``--every`` / ``--map_channels`` / ``--map_leads``) it
 verifies every start date through the last one (``GlobalModel.score_period``) and saves the period's scorecard, the
-per-date scorecards, the rank histogram and, for ``--map_channels`` at ``--map_leads``, per-point score maps.
+per-date scorecards, the rank histogram and, for ``--map_channels`` at ``--map_leads``, per-point score maps.  The last
+compares the ``--models`` head to head (``GlobalEnsemble.compare``) over the start dates ``--date`` .. ``--until`` (one
+date without ``--until``): every model and their pooled ensemble are scored off one upload of each analysis, and the
+stacked period card, the per-date cards, each entry's rank histogram, the maps and the paired score differences of
+every pair of entries (mean, 95 % interval, p-value) are saved.
 
 Differences, all forced by the scope of this build (SURVEY.md section 2): `--initial_conditions` accepts `synthetic`
 (the default here: the network IC providers cds / ifs / gfs are the reference's `libs/ic`, out of scope, and raise a clear
@@ -103,6 +109,25 @@ def run_score_period(model_name: str, date: str, time: str, lead_time: int, unti
     return paths
 
 
+def run_compare(model_names, date: str, time: str, lead_time: int, until: str, every: int, map_channels, map_leads,
+                initial_conditions: str, output_dir: str, filter_vars: str, members: int, perturbation: str, amp: float,
+                seed: int, truth: str = "", climatology: str = "", **model_kw):
+    """``--compare``: ``Skyrim(*model_names).compare(save=True)`` over the start dates ``date`` .. ``until``; returns the
+    paths of the stacked card, the per-date cards, the rank histograms, the maps and the differences"""
+    from . import xr_shim as xr
+    from .core import Skyrim
+    model = Skyrim(*model_names, ic_source=initial_conditions, **model_kw)
+    _, paths = model.compare(
+        start=date, end=until, time=time, every=every, lead_time=lead_time, members=members,
+        perturbation=perturbation if members > 1 else None, amp=amp, seed=seed,
+        truth=xr.open_dataarray(truth) if truth else None,
+        climatology=xr.open_dataarray(climatology) if climatology else None, map_leads=map_leads,
+        map_channels=map_channels, save=True,
+        save_config={"output_dir": output_dir or str(Path.cwd() / "outputs"),
+                     "filter_vars": [v.strip() for v in filter_vars.split(",") if v.strip()]})
+    return paths
+
+
 def parse_quantiles(text: str):
     """"0.1,0.5,0.9" -> [0.1, 0.5, 0.9]"""
     return [float(v) for v in text.split(",") if v.strip()]
@@ -148,19 +173,23 @@ def parse_exceed(text: str):
               help="Pangu alone: '6h' (default) chains the 6-h model; 'hierarchical' interleaves the 6-h and 24-h models "
                    "as earth2mip's PanguInference does")
 @click.option("--score", is_flag=True, help="Verify the forecast (--members members) against analyses and save a scorecard")
-@click.option("--truth", type=str, default="", help="--score: netCDF analyses (time, channel, lat, lon) on the model grid "
+@click.option("--compare", is_flag=True, help="Verify the --models and their pooled ensemble head to head over the start "
+              "dates --date .. --until and save scores and paired differences")
+@click.option("--truth", type=str, default="", help="--score / --compare: netCDF analyses (time, channel, lat, lon) on the model grid "
               "(default: the initial-condition source)")
-@click.option("--climatology", type=str, default="", help="--score: netCDF climatology (channel, lat, lon) for the ACC")
-@click.option("--until", type=str, default="", help="--score: the last start date YYYYMMDD; verifies every start date from "
-              "--date through it and saves period scores and a rank histogram")
-@click.option("--every", type=int, default=None, help="--score --until: hours between start dates (a multiple of 6; "
-              "default 24)")
-@click.option("--map_channels", type=str, default="", help="--score --until: channels of per-point score maps such as "
-              "z500,t850")
-@click.option("--map_leads", type=str, default="", help="--score --until: lead times in hours of the maps such as 24,72")
+@click.option("--climatology", type=str, default="", help="--score / --compare: netCDF climatology (channel, lat, lon) for "
+              "the ACC")
+@click.option("--until", type=str, default="", help="--score / --compare: the last start date YYYYMMDD; verifies every start "
+              "date from --date through it and saves period scores and a rank histogram")
+@click.option("--every", type=int, default=None, help="--score --until / --compare: hours between start dates (a multiple "
+              "of 6; default 24)")
+@click.option("--map_channels", type=str, default="", help="--score --until / --compare: channels of per-point score maps "
+              "such as z500,t850")
+@click.option("--map_leads", type=str, default="", help="--score --until / --compare: lead times in hours of the maps such "
+              "as 24,72")
 def main(model_name, date, time, lead_time, list_models, initial_conditions, output_dir, filter_vars, modal, weight_seed, device, grid,
-         members, perturbation, amp, seed, quantiles, exceed, models, pangu_schedule, score, truth, climatology, until, every,
-         map_channels, map_leads):
+         members, perturbation, amp, seed, quantiles, exceed, models, pangu_schedule, score, compare, truth, climatology, until,
+         every, map_channels, map_leads):
     if modal:
         raise click.UsageError("--modal: remote execution through Modal is outside this build (SURVEY.md section 2); run locally")
     if not 1 <= members <= 64:
@@ -169,6 +198,9 @@ def main(model_name, date, time, lead_time, list_models, initial_conditions, out
         q, events = parse_quantiles(quantiles), parse_exceed(exceed)
     except ValueError as e:
         raise click.UsageError(str(e))
+    if compare and (not models.strip() or score or q or events or list_models):
+        raise click.UsageError("--compare verifies several models (--models), without -m alone, --score, --quantiles, "
+                               "--exceed or --list_models")
     if members == 1 and (q or events):
         raise click.UsageError("--quantiles and --exceed describe an ensemble: give --members > 1")
     kw = {"weight_seed": weight_seed, "device": device}
@@ -192,19 +224,24 @@ def main(model_name, date, time, lead_time, list_models, initial_conditions, out
             kw["cfg"] = small(model_name)
     if names:
         model_name = names
-    if (truth or climatology) and not score:
-        raise click.UsageError("--truth and --climatology belong to --score")
+    if (truth or climatology) and not (score or compare):
+        raise click.UsageError("--truth and --climatology belong to --score or --compare")
     if score and (names or q or events or list_models):
         raise click.UsageError("--score verifies one model (-m), without --models, --quantiles, --exceed or --list_models")
     period = bool(until or every is not None or map_channels or map_leads)
-    if period and not score:
-        raise click.UsageError("--until, --every, --map_channels and --map_leads belong to --score")
-    if period:
+    if period and not (score or compare):
+        raise click.UsageError("--until, --every, --map_channels and --map_leads belong to --score or --compare")
+    if period or compare:
         try:
             m_leads = [float(v) for v in map_leads.split(",") if v.strip()]
         except ValueError:
             raise click.UsageError(f"--map_leads {map_leads}: lead times in hours such as 24,72")
         m_chans = [v.strip() for v in map_channels.split(",") if v.strip()]
+    if compare:
+        paths = run_compare(model_name, date, time, lead_time, until or date, 24 if every is None else every, m_chans, m_leads,
+                            initial_conditions, output_dir, filter_vars, members, perturbation, amp, seed, truth,
+                            climatology, **kw)
+    elif period:
         paths = run_score_period(model_name, date, time, lead_time, until or date, 24 if every is None else every, m_chans,
                                  m_leads, initial_conditions, output_dir, filter_vars, members, perturbation, amp, seed,
                                  truth, climatology, **kw)

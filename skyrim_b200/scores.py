@@ -233,3 +233,93 @@ class PeriodScores:
                                           lat=np.asarray(lat, dtype=np.float64), lon=np.asarray(lon, dtype=np.float64)),
                               attrs=dict(attrs))
         return cls(card, cards, rank, mp)
+
+
+# ---- model comparison -------------------------------------------------------------------------------------------------------
+DIFF_METRICS = ("rmse", "crps", "acc")
+DIFF_STATS = ("mean", "ci_low", "ci_high", "p_value", "n_eff")
+
+
+def paired_difference_stats(d):
+    """fp64 (..., 5) statistics (``DIFF_STATS`` order) of per-date score differences d, fp64 (D, ...) along the first
+    axis, with dates equally spaced.  d̄ the mean, s the sample standard deviation (ddof 1), r1 = sum_{t<D-1} (d_t - d̄)
+    (d_{t+1} - d̄) / sum_t (d_t - d̄)^2 the lag-1 autocorrelation (0 when the denominator is 0), n_eff = D (1 - r1) /
+    (1 + r1) clipped to [2, D] (AR(1) variance inflation, Geer 2016), se = s / sqrt(n_eff); then p = 2 stdtr(n_eff - 1,
+    -|d̄ / se|) and the 95 % interval d̄ -/+ stdtrit(n_eff - 1, 0.975) se.  s = 0 gives the interval [d̄, d̄] with p = 1
+    when d̄ = 0 and 0 otherwise.  With D < 3 every statistic but the mean is NaN; a NaN d_t makes every statistic NaN."""
+    from scipy.special import stdtr, stdtrit
+    d = np.asarray(d, dtype=np.float64)
+    D = d.shape[0]
+    out = np.full(d.shape[1:] + (len(DIFF_STATS),), np.nan)
+    mean = d.sum(axis=0) / D
+    out[..., 0] = mean
+    if D < 3:
+        return out
+    dev = d - mean
+    den = (dev * dev).sum(axis=0)
+    num = (dev[:-1] * dev[1:]).sum(axis=0)
+    s = np.sqrt(den / (D - 1))
+    with np.errstate(divide="ignore", invalid="ignore"):
+        r1 = np.where(den > 0.0, num / den, 0.0)
+        n_eff = np.clip(D * (1.0 - r1) / (1.0 + r1), 2.0, float(D))
+        se = s / np.sqrt(n_eff)
+        q = stdtrit(n_eff - 1.0, 0.975)
+        p = 2.0 * stdtr(n_eff - 1.0, -np.abs(mean / se))
+    flat = s == 0.0
+    out[..., 1] = np.where(flat, mean, mean - q * se)
+    out[..., 2] = np.where(flat, mean, mean + q * se)
+    out[..., 3] = np.where(flat, np.where(mean == 0.0, 1.0, 0.0), p)
+    out[..., 4] = n_eff
+    out[np.isnan(d).any(axis=0)] = np.nan
+    return out
+
+
+def paired_differences(cards_a, cards_b):
+    """fp64 (metric, stat, lead_time, region, channel) statistics (``DIFF_METRICS`` x ``DIFF_STATS``) of the per-date
+    differences a - b of two entries' per-date cards, fp64 (start_time, lead_time, metric, region, channel) in ``METRICS``
+    order: negative means a is better for rmse and crps, positive for acc."""
+    a, b = np.asarray(cards_a, dtype=np.float64), np.asarray(cards_b, dtype=np.float64)
+    pick = [METRICS.index(m) for m in DIFF_METRICS]
+    st = paired_difference_stats(a[:, :, pick] - b[:, :, pick])      # (lead, metric, region, channel, stat)
+    return np.ascontiguousarray(np.moveaxis(np.moveaxis(st, -1, 0), 2, 0))
+
+
+class ModelComparison:
+    """What ``GlobalEnsemble.compare`` returns: several models and their pooled ensemble verified over the same start
+    dates against one truth.
+        entries      the model names, then "pooled"
+        scores       {entry: PeriodScores} (members: M per model, K M for the pooled entry)
+        card         fp64 (model, lead_time, metric, region, channel): the entries' period cards stacked
+        differences  fp64 (pair, metric, stat, lead_time, region, channel): ``paired_differences`` of the per-date cards
+                     of every pair "a-b" with a before b in ``entries``, over ``DIFF_METRICS`` and ``DIFF_STATS``"""
+
+    def __init__(self, entries, scores, card, differences):
+        self.entries, self.scores, self.card, self.differences = list(entries), dict(scores), card, differences
+
+    def __repr__(self) -> str:
+        return f"ModelComparison(entries={self.entries},dates={self.card.attrs.get('n_dates')})"
+
+    @property
+    def pairs(self):
+        return [str(p) for p in np.asarray(self.differences.coords["pair"])]
+
+    @classmethod
+    def build(cls, scores: dict):
+        """from {entry: PeriodScores} in entry order, all over the same dates, leads, regions and channels"""
+        from . import xr_shim as xr
+        entries = list(scores)
+        first = scores[entries[0]].card
+        attrs = {k: v for k, v in first.attrs.items() if k not in ("model", "members")}
+        attrs["members"] = [int(scores[e].card.attrs["members"]) for e in entries]
+        coords = {d: np.asarray(first.coords[d]) for d in first.dims}
+        card = xr.DataArray(np.stack([scores[e].card.values for e in entries]),
+                            dims=["model"] + list(first.dims), coords=dict(coords, model=np.array(entries)),
+                            attrs=dict(attrs))
+        pairs = [(a, b) for i, a in enumerate(entries) for b in entries[i + 1:]]
+        diff = np.stack([paired_differences(scores[a].cards.values, scores[b].cards.values) for a, b in pairs])
+        differences = xr.DataArray(diff, dims=["pair", "metric", "stat", "lead_time", "region", "channel"],
+                                   coords=dict(pair=np.array([f"{a}-{b}" for a, b in pairs]),
+                                               metric=np.array(DIFF_METRICS), stat=np.array(DIFF_STATS),
+                                               lead_time=coords["lead_time"], region=coords["region"],
+                                               channel=coords["channel"]), attrs=dict(attrs))
+        return cls(entries, scores, card, differences)
