@@ -165,9 +165,15 @@ class PanguRef:
         x = qs(x + F.layer_norm(y, (C,), w[p + "ln2.g"], w[p + "ln2.b"], cfg.ln_eps))
         return x
 
-    def layer(self, x, li):
+    def blocks(self, x, li):
+        """the token tensor after each block of layer li, in order"""
         for bi in range(self.cfg.depths[li]):
             x = self.block(x, f"layer{li}.block{bi}.", self.cfg.heads[li], roll=(bi % 2 == 1))
+            yield x
+
+    def layer(self, x, li):
+        for x in self.blocks(x, li):
+            pass
         return x
 
     def downsample(self, x):

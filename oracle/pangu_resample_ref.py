@@ -76,12 +76,16 @@ def workspace_layout(cfg, B: int) -> dict:
 # ---------------------------------------------------------------------------------------------------------------------
 # weights and index maps
 # ---------------------------------------------------------------------------------------------------------------------
+def packed(a, round16: bool = True) -> np.ndarray:
+    """a weight as k_pack_weight packs it (fp16 of the fp32 value), as float64; round16=False: the weight itself"""
+    return np.asarray(a, np.float32).astype(np.float16).astype(np.float64) if round16 else np.asarray(a, np.float64)
+
+
 def gemm_weights(cfg, w, round16: bool = True) -> dict:
     """the [N, K] weights of the down, up1, up2 and recovery GEMMs as the engine packs them (k_pack_weight: fp16 of the
     fp32 value; recovery: upper-air | surface columns of the transposed weights), as float64"""
     C = cfg.dim
-    f = (lambda a: np.asarray(a, np.float32).astype(np.float16).astype(np.float64)) if round16 else \
-        (lambda a: np.asarray(a, np.float64))
+    f = lambda a: packed(a, round16)   # noqa: E731
     rec = np.concatenate([np.asarray(w["recover.upper.w"]).reshape(2 * C, -1).T, np.asarray(w["recover.surf.w"]).reshape(2 * C, -1).T])
     assert rec.shape == (REC_N, 2 * C)
     return {"down": f(w["down.w"]), "up1": f(w["up.w1"]), "up2": f(w["up.w2"]), "rec": f(rec)}

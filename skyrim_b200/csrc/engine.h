@@ -40,7 +40,8 @@ struct Engine {
   std::vector<void*> kept;  // small persistent fp32 tensors (biases, norm vectors, masks): copies that outlive the arena
   bool loaded = false;
   int stop_after = 99;      // debug tap (sky_model_debug_set "stop_after"): return from step() after stage n
-  int stop_launch = -1;     // finer debug tap of the GraphCast engine ("stop_launch"): return after the n-th unit of a member
+  int stop_launch = -1;     // finer debug tap of the GraphCast and Pangu engines ("stop_launch"): return after the n-th unit
+                            // of a member's (GraphCast) or of the whole step (Pangu)
   // fp16-range guard (sky_model_debug_set "range_guard" 1): the step scans the fp16 operand images it produced and keeps
   // max |value| per class in range_dev[8] (read back with debug_copy "range").  The tensor cores take fp16 operands (5
   // exponent bits): with real checkpoints the caller runs the first step of a rollout guarded and refuses anything > 3e4.

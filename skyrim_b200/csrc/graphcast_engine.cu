@@ -184,10 +184,6 @@ struct GraphCastEngine : Engine {
   static constexpr int GC_STOPPED = 1 << 20;   // not an error code: step() swallows it
   int units_done = 0;
   int unit_done() { return stop_launch >= 0 && loaded && ++units_done >= stop_launch ? GC_STOPPED : 0; }
-  int debug_set(const char* key, long long value) override {
-    if (!strcmp(key, "stop_launch")) { stop_launch = (int)value; return 0; }
-    return Engine::debug_set(key, value);
-  }
   // fp16-range guard over the VALID rows of an M-row image: the whole tiles, then rows [0, M % 128) of each k-block of the
   // partial last tile (a row's 128 bytes stay inside the row under the swizzle; the rows past M hold whatever the workspace
   // held and are not scanned)

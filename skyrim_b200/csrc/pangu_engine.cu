@@ -571,8 +571,25 @@ struct PanguEngine : Engine {
   int run_block(float* x, uint8_t* xh, const Geo& g, const BlockW& b, int roll, int B, const Ws& ws, cudaStream_t st) {
     return img_stream ? run_block_t<true>(x, xh, g, b, roll, B, ws, st) : run_block_t<false>(x, xh, g, b, roll, B, ws, st);
   }
+  // ---- test tap: stop inside the step ---------------------------------------------------------------------------
+  // debug_set "stop_launch" n: the step returns after its n-th unit, counted in program order over the whole step: the
+  // embedding; per block QKV (GEMM + padding fill), attention, projection, then the fused MLP or fc1 and fc2; the
+  // down-sample, the up-sample and the recovery.  -1 (the default) never stops.  debug_copy then reads the buffers the
+  // unit wrote (the workspace is reused).  A stopped step is never captured (Engine::step_cached), and the counter is host
+  // state only: the launch sequence of an unstopped step is unchanged.
+  static constexpr int PG_STOPPED = 1 << 20;   // not an error code: step() swallows it
+  int units_done = 0;
+  const Geo* stop_geo = nullptr;   // grid level of the unit the step stopped after
+  bool stop_on_skip = false;       // the image-only token stream was the skip image there (embedding and layer 0)
+  int unit_done(const Geo& g, bool on_skip) {
+    if (stop_launch < 0 || !loaded || ++units_done < stop_launch) return 0;
+    stop_geo = &g; stop_on_skip = on_skip;
+    return PG_STOPPED;
+  }
+
   template <bool IMG>
   int run_block_t(float* x, uint8_t* xh, const Geo& g, const BlockW& b, int roll, int B, const Ws& ws, cudaStream_t st) {
+    const bool on_skip = xh == ws.skiph;
     // projection and fc2: the epilogue runs on the accumulator fragments on the fp16 stream (the fp32 rows stay staged).
     // Both update the stream in place: the residual is what the epilogue overwrites.
     using ELn = std::conditional_t<IMG, FragEpi<Epi2F32Img<true, 2>>, Epi2F32Img<true, 1>>;
@@ -595,6 +612,7 @@ struct PanguEngine : Engine {
         count_launch();
         if (rc) return rc;
       }
+      if ((rc = unit_done(g, on_skip))) return rc;
     }
     {
       AttnArgs a{ws.qkv, part_stride, ws.atth, nkb, b.bias_tab, g, roll, B, pairs,
@@ -603,14 +621,14 @@ struct PanguEngine : Engine {
       count_launch();
       rc = launch_window_attention_tc(a, num_sms, st);
       prof_end(KT_ATTN, st);
-      if (rc) return rc;
+      if (rc || (rc = unit_done(g, on_skip))) return rc;
     }
     {  // projection + LayerNorm + residual.  At C = 384 a 128 x 384 accumulator would take 192 registers per consumer thread:
        // the two CTAs of a cluster take 192 columns each of the same 128 rows, LayerNorm statistics cross through DSMEM
       AOperand A(ws.atth, nkb);
       ELn e{res, xout, C, xh, nkb, nullptr, b.proj_b, b.ln1_g, b.ln1_b, cfg.ln_eps};
       rc = C == 192 ? gemm2<192>(KT_PROJ, A, e, b.proj, R, st) : gemm2<192, true>(KT_PROJ, A, e, b.proj, R, st);
-      if (rc) return rc;
+      if (rc || (rc = unit_done(g, on_skip))) return rc;
     }
     if (IMG && C == 192) {   // MLP in one kernel: the hidden activation stays on the SM (mlp_fused.cuh).  At C = 384 the
                              // fused CTA-pair kernel measured 2.4x slower than fc1 + fc2 (DESIGN.md section 4)
@@ -620,15 +638,15 @@ struct PanguEngine : Engine {
       count_launch();
       rc = launch_mlp_fused<3>(m, num_sms, st);
       prof_end(KT_MLP, st);
-      if (rc) return rc;
+      if (rc || (rc = unit_done(g, on_skip))) return rc;
     } else {  // MLP: fc1 + GELU into the fp16 hidden image, then fc2 + LayerNorm + residual
       AOperand A(xh, nkb);
       FragEpi<Epi2F16<true, true>> e{reinterpret_cast<__half*>(ws.hidh), 0, 4 * nkb, b.fc1_b};
-      if ((rc = gemm2<192>(KT_FC1, A, e, b.fc1, R, st))) return rc;
+      if ((rc = gemm2<192>(KT_FC1, A, e, b.fc1, R, st)) || (rc = unit_done(g, on_skip))) return rc;
       AOperand A2(ws.hidh, 4 * nkb);
       ELn e2{res, xout, C, xh, nkb, nullptr, b.fc2_b, b.ln2_g, b.ln2_b, cfg.ln_eps};
       rc = C == 192 ? gemm2<192>(KT_FC2, A2, e2, b.fc2, R, st) : gemm2<192, true>(KT_FC2, A2, e2, b.fc2, R, st);
-      if (rc) return rc;
+      if (rc || (rc = unit_done(g, on_skip))) return rc;
     }
     if (range_guard) {   // fp16 operand images of this block (whole tiles only: the tail rows of the last tile are never written)
       const size_t full = (size_t)(R / 128) * nkb * G2_A_BYTES;
@@ -640,6 +658,12 @@ struct PanguEngine : Engine {
   }
 
   int step(const float* x_in, float* x_out, int B, void* wsp, size_t ws_bytes, cudaStream_t st) override {
+    units_done = 0;
+    stop_geo = nullptr;
+    const int rc = step_units(x_in, x_out, B, wsp, ws_bytes, st);
+    return rc == PG_STOPPED ? 0 : rc;
+  }
+  int step_units(const float* x_in, float* x_out, int B, void* wsp, size_t ws_bytes, cudaStream_t st) {
     if (!loaded) { set_error("weights not loaded"); return SKY_ERR_STATE; }
     Ws ws = carve(wsp, B);
     if (ws_bytes < ws.total) { set_error("workspace too small: %zu < %zu", ws_bytes, ws.total); return SKY_ERR_ARG; }
@@ -659,6 +683,7 @@ struct PanguEngine : Engine {
       ProdEmbedSurf ps{x_in, masks, mean, stdv, cfg.nlat, cfg.nlon, nch, nup, 4, 3, g1.H, g1.W, Ms};
       EpiStoreF32 es{img_stream ? nullptr : ws.x1, C, embed_s_b, g1.T, HW, 0, (long long)HW, ws.skiph, C / 64};
       if ((rc = gemm2<192>(KT_EMBED, SchedProd<ProdEmbedSurf>{ps, embed_s.img, embed_s.Kp / 64}, es, embed_s, Ms, st))) return rc;
+      if ((rc = unit_done(g1, true))) return rc;
     }
     if (stop == 0) return 0;
     for (size_t i = 0; i < blocks[0].size(); ++i)
@@ -678,6 +703,7 @@ struct PanguEngine : Engine {
       Epi2F32Img<false, 0> e{nullptr, img_stream ? nullptr : ws.x2, 2 * C, ws.x2h, 2 * C / 64, nullptr, nullptr, nullptr, nullptr, 0.f};
       if ((rc = gemm2<192>(KT_DOWN, A, e, down, R2, st))) return rc;
       if ((rc = range_scan(3, ws.x2h, (size_t)(R2 / 128) * (2 * C / 64) * G2_A_BYTES, st))) return rc;
+      if ((rc = unit_done(g2, false))) return rc;
     }
     if (stop == 2) return 0;
     for (int li = 1; li <= 2; ++li) {
@@ -692,7 +718,7 @@ struct PanguEngine : Engine {
       if ((rc = gemm2<192>(KT_UP, A, e, up1, R2, st))) return rc;
       AOperand A2(ws.hidh, C / 64);
       Epi2F32Img<false, 0> e2{nullptr, img_stream ? nullptr : ws.x1, C, ws.x1h, C / 64, nullptr, nullptr, nullptr, nullptr, 0.f};
-      if ((rc = gemm2<192>(KT_UP, A2, e2, up2, R1, st))) return rc;
+      if ((rc = gemm2<192>(KT_UP, A2, e2, up2, R1, st)) || (rc = unit_done(g1, false))) return rc;
     }
     if (stop == 5) return 0;
     for (size_t i = 0; i < blocks[3].size(); ++i)
@@ -704,7 +730,7 @@ struct PanguEngine : Engine {
       Epi2Recover e{x_out, rec_b, mean, stdv, cfg.nlat, cfg.nlon, nch, nup, cfg.n_levels, g1.H, g1.W, g1.T};
       if ((rc = gemm2<224>(KT_RECOVER, A, e, rec, R1, st))) return rc;
     }
-    return 0;
+    return unit_done(g1, false);
   }
 
   int debug_set(const char* key, long long value) override {
@@ -717,6 +743,24 @@ struct PanguEngine : Engine {
     const float* src = nullptr;
     uint64_t n = 0;
     const long long R1 = (long long)B * g1.T, R2 = (long long)B * g2.T;
+    if (!strcmp(what, "qkv") || !strcmp(what, "att_h") || !strcmp(what, "hid_h") || !strcmp(what, "stream_h")) {
+      // raw taps after a stop_launch stop: the buffer as it lies in memory at the stopped unit's grid level (decoded on the
+      // host), the whole of it: q | k | v window image (3 part_stride bytes), attention output, MLP hidden and token
+      // stream images (every 128-row tile, the rows past B T included)
+      if (!stop_geo) { set_error("debug buffer '%s' needs a step stopped by stop_launch", what); return SKY_ERR_STATE; }
+      const Geo& g = *stop_geo;
+      const long long R = (long long)B * g.T;
+      const size_t img = tiles(R) * (g.C / 64) * G2_A_BYTES;
+      const uint8_t* p = what[0] == 'q' ? ws.qkv : what[0] == 'a' ? ws.atth : what[0] == 'h' ? ws.hidh
+                       : &g == &g2 ? ws.x2h : stop_on_skip ? ws.skiph : ws.x1h;
+      const size_t bytes = what[0] == 'q' ? 3 * (size_t)B * g.nWin * (g.heads / 2) * AT_TILE_B : what[0] == 'h' ? 4 * img : img;
+      if (bytes != max_floats * sizeof(float)) {
+        set_error("debug buffer '%s' is %zu floats, destination %llu", what, bytes / sizeof(float), (unsigned long long)max_floats);
+        return SKY_ERR_ARG;
+      }
+      SKY_CUDA_OK(cudaMemcpyAsync(dst, p, bytes, cudaMemcpyDeviceToDevice, st));
+      return 0;
+    }
     const bool stream_tap = img_stream && (!strcmp(what, "tokens1") || !strcmp(what, "tokens2"));
     if (!stream_tap && !strcmp(what, "tokens1")) { src = ws.x1; n = (uint64_t)R1 * cfg.dim; }
     else if (!stream_tap && !strcmp(what, "tokens2")) { src = ws.x2; n = (uint64_t)R2 * 2 * cfg.dim; }
@@ -724,7 +768,8 @@ struct PanguEngine : Engine {
       // the fp16 operand image, expanded to fp32 rows.  With the image-only token stream "tokens1" is the skip image until the
       // down-sample (embedding and first layer work in place on it) and the x1 image from the up-sample on.
       const bool two = what[6] == '2';
-      const uint8_t* img = two ? ws.x2h : ((!strcmp(what, "skip_h") || (stream_tap && stop_after <= 1)) ? ws.skiph : ws.x1h);
+      const bool on_skip = stop_geo ? stop_on_skip : stop_after <= 1;
+      const uint8_t* img = two ? ws.x2h : ((!strcmp(what, "skip_h") || (stream_tap && on_skip)) ? ws.skiph : ws.x1h);
       const long long rows = two ? R2 : R1;
       const int cols = two ? 2 * cfg.dim : cfg.dim;
       if ((uint64_t)rows * cols > max_floats) { set_error("destination too small"); return SKY_ERR_ARG; }

@@ -184,6 +184,7 @@ const float* Engine::keep(const char* name, uint64_t expect, cudaStream_t st) {
 
 int Engine::debug_set(const char* key, long long value) {
   if (!strcmp(key, "stop_after")) { stop_after = (int)value; return 0; }
+  if (!strcmp(key, "stop_launch")) { stop_launch = (int)value; return 0; }
   if (!strcmp(key, "use_graphs")) { use_graphs = value != 0; return 0; }
   if (!strcmp(key, "range_guard")) {
     range_guard = value != 0;
