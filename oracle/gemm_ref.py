@@ -34,9 +34,11 @@ SUB16 = 2.0 ** -25        # half the smallest fp16 subnormal
 # ---------------------------------------------------------------------------------------------------------------------
 # layouts
 # ---------------------------------------------------------------------------------------------------------------------
-def _swz_index(tile_rows: int) -> np.ndarray:
-    """[T, 8]: stored chunk p of row r holds logical chunk p ^ (r & 7) (and vice versa: XOR is an involution)."""
-    return np.arange(8)[None, :] ^ (np.arange(tile_rows)[:, None] & 7)
+def _swz_index(rows) -> np.ndarray:
+    """[R, 8] for the row numbers ``rows`` (an int T: rows 0 .. T - 1): stored chunk p of row r holds logical chunk
+    p ^ (r & 7) (and vice versa: XOR is an involution)."""
+    r = np.arange(rows) if np.isscalar(rows) else np.asarray(rows)
+    return np.arange(8)[None, :] ^ (r[:, None] & 7)
 
 
 def pack_tiles(x: np.ndarray, tile_rows: int, nkb: int, row_fill=0.0, col_fill=0.0, rows_pad: int | None = None) -> np.ndarray:
@@ -62,6 +64,17 @@ def unpack_tiles(img: np.ndarray, tile_rows: int, nkb: int, rows: int, cols: int
     idx = np.broadcast_to(_swz_index(tile_rows)[None, None, :, :, None], v.shape)
     x = np.take_along_axis(v, idx, axis=3).transpose(0, 2, 1, 3, 4).reshape(nt * tile_rows, nkb * 64)
     return x[:rows, : (cols if cols is not None else nkb * 64)]
+
+
+def unpack_rows(pieces: np.ndarray, rows) -> np.ndarray:
+    """gathered rows of a tile image -> fp16 [n, nkb * 64].  pieces: [n, nkb, 128 B], piece kb of row r taken from byte
+    img_offset(r, 64 kb, nkb); the rows' own numbers undo the swizzle"""
+    pieces = np.ascontiguousarray(pieces)
+    if len(rows) == 0:
+        return np.zeros((0, pieces.shape[1] * 64), np.float16)
+    h = pieces.view(np.float16).reshape(len(rows), -1, 8, 8)
+    idx = np.broadcast_to(_swz_index(rows)[:, None, :, None], h.shape)
+    return np.take_along_axis(h, idx, axis=2).reshape(len(rows), -1)
 
 
 def img_offset(row: int, col: int, nkb: int, tile_rows: int = 128) -> int:

@@ -10,7 +10,10 @@ hidden GEMM, LayerNorm GEMM, per-node table, aggregation, the output head).  A b
   Recorder   lists the units (kind, name, outputs, rows): what a test has to read after which stop point;
   Checker    takes the ENGINE's decoded taps: every unit is recomputed in float64 from the engine's own inputs to it (the
              taps of the units before), compared per element, and the engine's output is handed on.  Errors do not
-             accumulate, and a wrong unit is named by the first check that fails;
+             accumulate, and a wrong unit is named by the first check that fails.  Given the checked rows of every unit,
+             it takes taps as Rows (row indices, values) and computes each reference for those rows only;
+  Planner    takes the rows checked in every unit and derives from the graph's index arrays which rows of which earlier
+             tap each check reads: the read plan of a sampled check (full_size_rows: the rules at 721 x 1440);
   Emulator   computes the taps itself in the engine's formulation (fp16 where the engine rounds, split first layers,
              per-node tables, chunked fp32 segment sums in the engine's order), optionally with one modelled mistake.
 
@@ -20,6 +23,8 @@ bounds come from oracle/gemm_ref.py: |D - R| <= TAU sum |a w| + epilogue roundin
 from __future__ import annotations
 
 import math
+import os
+from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
@@ -83,6 +88,47 @@ class Shapes:
         if rows is None:
             return x
         return x[:rows] if np.isscalar(rows) else x[rows]
+
+    def gather(self, name, raw, rows, kmajor=False, cols=None):
+        """rows of a raw tap (the float32 torch container debug_tensor returns, on any device) -> Rows of float64 values.
+        Only the rows' bytes leave the device: row r of a tile image is eight 128-byte pieces, piece kb at byte
+        ((r >> 7) nkb + kb) TILE + (r & 127) 128; a table row is a row-major slice.  ``rows``: logical (k-major images:
+        k n_grid + g)"""
+        import torch
+        rows = np.asarray(rows, np.int64)
+        phys = self.m2g_rows[rows] if kmajor else rows
+        if name in ("vm", "vm0"):
+            v = raw.view(-1, L)[torch.from_numpy(phys).to(raw.device)].cpu().numpy()
+        elif name in ("tg", "g2m_tr", "tm"):
+            v = raw.view(torch.float16).view(-1, cols or L)[torch.from_numpy(phys).to(raw.device)].cpu().numpy()
+        else:
+            nkb = FEAT_KP // 64 if name == "feat" else NKB
+            piece = ((phys >> 7)[:, None] * nkb + np.arange(nkb)[None]) * (TILE // 128) + (phys & 127)[:, None]
+            b = raw.view(torch.uint8).view(-1, 128)[torch.from_numpy(piece).to(raw.device)].cpu().numpy()
+            v = gr.unpack_rows(b, phys)
+        return Rows(rows, v.astype(np.float64))
+
+
+class Rows:
+    """rows ``idx`` (sorted, unique) of a tap and their values ``val``, indexed by row number like the whole tap:
+    ``t[rows]`` -> the values of those rows (each must be present), ``t[a:b]`` -> the rows in [a, b) numbered from a,
+    ``t[:, cols]`` -> the same rows, those columns"""
+
+    def __init__(self, idx, val):
+        self.idx, self.val = np.asarray(idx, np.int64), val
+
+    def __getitem__(self, key):
+        if isinstance(key, tuple):
+            rows, cols = key
+            assert rows == slice(None)
+            return Rows(self.idx, self.val[:, cols])
+        if isinstance(key, slice):
+            lo, hi = np.searchsorted(self.idx, [key.start, key.stop])
+            return Rows(self.idx[lo:hi] - key.start, self.val[lo:hi])
+        key = np.asarray(key, np.int64)
+        pos = np.searchsorted(self.idx, key)
+        assert (pos < len(self.idx)).all() and (self.idx[pos] == key).all(), "a row that was not read"
+        return self.val[pos]
 
 
 STATIC_TAPS = ("vm0", "vm0_img", "e_g2m_img", "e_m2g_img", "e_mesh_img", "g2m_tr")
@@ -180,17 +226,31 @@ def ref_table(a, wslices):
     return f, gr.f16_bound(f, fb)
 
 
-def ref_agg(y, ptr):
-    """fp64 segment sums of the update rows over the CSR pointer; fp32 accumulation bound deg 2^-24 sum |y| plus the fp16
-    store.  A segment without edges is exactly zero (bound 0)."""
+def seg_edges(ptr, nodes):
+    """the incoming edge rows of ``nodes`` over the CSR pointer, node after node"""
     ptr = np.asarray(ptr, np.int64)
-    z = np.zeros((1, y.shape[1]))
-    c = np.concatenate([z, np.cumsum(y, axis=0)])
-    ca = np.concatenate([z, np.cumsum(np.abs(y), axis=0)])
-    f, fa = c[ptr[1:]] - c[ptr[:-1]], ca[ptr[1:]] - ca[ptr[:-1]]
-    deg = (ptr[1:] - ptr[:-1])[:, None]
-    # the cumulative sums themselves carry 2^-53 of their running magnitude
-    bound = gr.f16_bound(f, deg * gr.U32 * fa + 2.0 ** -50 * ca[ptr[1:]])
+    nodes = np.asarray(nodes, np.int64)
+    deg = ptr[nodes + 1] - ptr[nodes]
+    return np.repeat(ptr[nodes] - (np.cumsum(deg) - deg), deg) + np.arange(int(deg.sum()))
+
+
+def ref_agg(y, ptr, nodes):
+    """fp64 sums of the update rows of each node's incoming edges (``y``: indexed by edge row), for ``nodes`` only; fp32
+    accumulation bound deg 2^-24 sum |y| plus the fp16 store.  A node without edges is exactly zero (bound 0)."""
+    ptr = np.asarray(ptr, np.int64)
+    nodes = np.asarray(nodes, np.int64)
+    deg = ptr[nodes + 1] - ptr[nodes]
+    v = np.asarray(y[seg_edges(ptr, nodes)], np.float64)
+    f = np.zeros((len(nodes), v.shape[1]))
+    fa = np.zeros_like(f)
+    has = deg > 0
+    if has.any():
+        start = (np.cumsum(deg) - deg)[has]
+        f[has] = np.add.reduceat(v, start, axis=0)
+        fa[has] = np.add.reduceat(np.abs(v), start, axis=0)
+    deg = deg[:, None]
+    # the fp64 sums themselves carry deg 2^-53 sum |y|
+    bound = gr.f16_bound(f, deg * (gr.U32 + 2.0 ** -53) * fa)
     return f, np.where(deg == 0, 0.0, bound)
 
 
@@ -325,107 +385,314 @@ def units(cfg, graph):
     return r.units
 
 
-class Checker:
-    """taps: {0: statics, n: {tap: decoded float64 values of the valid rows}} of one engine (or Emulator) step"""
+class _Src:
+    """what Planner hands on in place of a tap: the unit that wrote it, its name, and the first row of a slice"""
 
-    def __init__(self, cfg, graph, w, x, t_seconds, taps):
-        self.cfg, self.g, self.w, self.x, self.t, self.taps = cfg, graph, w, np.asarray(x, np.float32), t_seconds, taps
+    def __init__(self, n, tap, off=0):
+        self.n, self.tap, self.off = n, tap, off
+
+    def __getitem__(self, key):
+        if isinstance(key, slice):
+            return _Src(self.n, self.tap, self.off + key.start)
+        return self            # [:, columns]: a table's rows are read whole
+
+
+def every_row(kind, name, rows, kmajor):
+    return np.arange(rows)
+
+
+class Planner:
+    """``pick(kind, name, rows, kmajor) -> the rows checked`` in a unit (``name``: the static tap's for kind "static")
+    -> ``checked`` {n: rows, 0: {static tap: rows}} (Checker's ``rows``) and the read plan ``reads`` {n: {tap: [rows,
+    kmajor, table columns]}}: after stop n, read these rows of these taps (0: the load-time taps).  A unit reads the
+    checked rows of its A operands and residual, the sender and receiver rows of the tables it gathers, and every
+    incoming edge row of a checked aggregation node; rows are logical (k-major: k n_grid + g)."""
+
+    def __init__(self, cfg, graph, pick):
+        self.cfg, self.g, self.pick = cfg, graph, pick
         self.n = 0
-        self.checks = []     # (unit, kind, name, what, got, ref, bound)
+        self.checked, self.reads = {0: {}}, {0: {}}
 
-    def _chk(self, kind, name, what, got, ref, bound):
-        self.checks.append((self.n, kind, name, what, got, ref, bound))
+    def _read(self, src, rows):
+        r = self.reads[src.n][src.tap]
+        r[0] = np.union1d(r[0], src.off + np.asarray(rows, np.int64))
 
-    def _unit(self):
+    def _unit(self, kind, name, outs, rows, kmajor=False, cols=None):
         self.n += 1
-        return self.taps[self.n]
+        R = np.unique(np.asarray(self.pick(kind, name, rows, kmajor), np.int64))
+        self.checked[self.n] = R
+        self.reads[self.n] = {o: [R, kmajor, cols] for o in outs}
+        return R
+
+    def statics(self):
+        g, Nm = self.g, int(self.g["n_mesh"])
+        for tap, rows in (("vm0_img", Nm), ("e_g2m_img", len(g["g2m.senders"])), ("e_mesh_img", len(g["mesh.senders"])),
+                          ("e_m2g_img", 3 * self.cfg.n_grid), ("g2m_tr", Nm)):
+            R = np.unique(np.asarray(self.pick("static", tap, rows, tap == "e_m2g_img"), np.int64))
+            self.checked[0][tap] = R
+            self.reads[0][tap] = [R, tap == "e_m2g_img", L if tap == "g2m_tr" else None]
+        self.reads[0]["vm0"] = [self.checked[0]["vm0_img"], False, None]
+        self._read(_Src(0, "vm0_img"), self.checked[0]["g2m_tr"])
+        return {k: _Src(0, k) for k in STATIC_TAPS}
+
+    def features(self):
+        self._unit("features", "features", ["feat"], self.cfg.n_grid)
+        return _Src(self.n, "feat")
+
+    def hidden(self, name, parts, out, rows, gathers=(), kmajor=False):
+        R = self._unit("hidden", name, [out], rows, kmajor)
+        for a, _ in parts:
+            self._read(a, R)
+        for tb, i in gathers:
+            self._read(tb, np.asarray(i)[R])
+        return _Src(self.n, out)
+
+    def ln(self, name, hid, res, outs, rows, kmajor=False):
+        R = self._unit("ln", name, list(outs.values()), rows, kmajor)
+        self._read(hid, R)
+        if res is not None:
+            self._read(res, R)
+        return {k: _Src(self.n, tap) for k, tap in outs.items()}
+
+    def table(self, name, a, c0s, out, rows):
+        R = self._unit("table", name, [out], rows, cols=L * len(c0s))
+        self._read(a, R)
+        return _Src(self.n, out)
+
+    def agg(self, name, y, ptr):
+        R = self._unit("agg", name, ["agg_img"], len(ptr) - 1)
+        self._read(y, seg_edges(ptr, R))
+        return _Src(self.n, "agg_img")
+
+    def out(self, hid):
+        R = self._unit("out", "dec.out", ["x_out"], self.cfg.n_grid)
+        self._read(hid, R)
+
+
+def plan(cfg, graph, pick=every_row):
+    p = Planner(cfg, graph, pick)
+    run_program(cfg, graph, p)
+    return p
+
+
+def row_bytes(cfg, tap, cols=None):
+    """bytes of one row of a tap as the engine stores it"""
+    return {"feat": 2 * FEAT_KP, "vm": 4 * L, "vm0": 4 * L, "x_out": 8 * cfg.n_state}.get(tap, 2 * (cols or L))
+
+
+def full_size_rows(cfg, graph, seed=0, n_grid=4096, n_g2m_nodes=512, n_edges=16384, edge_layers=None):
+    """the rows the full-size check checks, as Planner's ``pick``:
+    mesh nodes   every row of every mesh-node unit (tables, node hidden and LayerNorm GEMMs, vm / vm_img, every
+                 aggregation but grid2mesh's), and vm0 / vm0_img / g2m_tr;
+    mesh edges   every row in layers ``edge_layers`` (default the first two and the last two), elsewhere the first and
+                 the last (partial) tile and ``n_edges`` seeded rows;
+    grid nodes   the first and the last (partial) tile, the first and the last latitude row, the grid points whose
+                 mesh2grid rows are the tiles on either side of byte 2^31 of the k-major edge images, ``n_grid`` seeded
+                 points; the mesh2grid units the three k-major rows k n_grid + g of each;
+    grid2mesh    the aggregation on every node whose segment is cut into chunks, every node without edges and
+                 ``n_g2m_nodes`` seeded others; the edge units on all their edges and the first and the last tile"""
+    rng = np.random.default_rng(seed)
+    Ng, nlon = cfg.n_grid, cfg.nlon
+    ends = lambda n: np.r_[0:min(128, n), n // 128 * 128 if n % 128 else n - 128:n]
+    sh = Shapes(cfg, graph)
+    r31 = 2 ** 31 // (NKB * TILE) * 128                     # the first image row at or past byte 2^31
+    phys = np.arange(r31 - 128, r31 + 128)
+    phys = phys[(phys < sh.E3) & (phys % sh.Ngp < Ng)]
+    grid = np.unique(np.concatenate([ends(Ng), np.arange(nlon), np.arange(Ng - nlon, Ng), phys % sh.Ngp,
+                                     rng.choice(Ng, min(n_grid, Ng), replace=False)]))
+    m2g = (np.arange(3)[:, None] * Ng + grid[None]).reshape(-1)
+    ptr = np.asarray(graph["g2m.ptr"], np.int64)
+    deg = np.diff(ptr)
+    special = np.flatnonzero((deg > SEG_CHUNK) | (deg == 0))
+    others = np.setdiff1d(np.arange(len(deg)), special)
+    g2m_nodes = np.union1d(special, rng.choice(others, min(n_g2m_nodes, len(others)), replace=False))
+    g2m_edges = np.union1d(seg_edges(ptr, g2m_nodes), ends(len(graph["g2m.senders"])))
+    Em, Nm = len(graph["mesh.senders"]), int(graph["n_mesh"])
+    full = {0, 1, cfg.layers - 2, cfg.layers - 1} if edge_layers is None else set(edge_layers)
+    edges = {i: np.arange(Em) if i in full else np.union1d(ends(Em), rng.choice(Em, min(n_edges, Em), replace=False))
+             for i in range(cfg.layers)}
+
+    def pick(kind, name, rows, kmajor):
+        if kind == "static":
+            return {"e_g2m_img": g2m_edges, "e_m2g_img": m2g, "e_mesh_img": edges[0]}.get(name, np.arange(Nm))
+        if kmajor:
+            return m2g
+        if name == "g2m":
+            return g2m_nodes
+        if name.startswith("mesh"):
+            return np.arange(Nm)
+        if name == "enc.g2m_edge" and kind != "table":
+            return g2m_edges
+        if name.startswith("proc") and name.endswith(".edge") and kind != "table":
+            return edges[int(name[4:-5])]
+        return np.arange(Nm) if rows == Nm else grid
+    return pick
+
+
+class Checker:
+    """taps: {0: statics, n: {tap: decoded float64 values}} of one engine (or Emulator) step.  ``rows``: {n: the rows
+    checked in unit n (its own row space; k-major units: k n_grid + g), 0: {static tap: rows}} — the taps are then Rows
+    holding at least what Planner lists; a unit without an entry is checked on every row.  References are evaluated in
+    blocks of BLOCK rows on up to WORKERS threads (numpy and BLAS release the GIL); each block reduces its checks to
+    (n_outside, worst ratio), and the blocks merge in order."""
+
+    def __init__(self, cfg, graph, w, x, t_seconds, taps, rows=None):
+        self.cfg, self.g, self.w, self.x, self.t, self.taps = cfg, graph, w, np.asarray(x, np.float32), t_seconds, taps
+        self.rows = rows or {}
+        self.n = 0
+        self.checks = []     # (unit, kind, name, what, n_outside, worst ratio)
+        self._at = {}
+
+    def _run(self, blocks, fn):
+        """fn(R, chk) for every row block R; chk(kind, name, what, got, ref, bound) checks one quantity on the block"""
+        def one(R):
+            out = []
+            fn(R, lambda kind, name, what, got, ref, bound: out.append((kind, name, what) + _summary(got, ref, bound)))
+            return out
+        if len(blocks) == 1:
+            res = [one(blocks[0])]
+        else:
+            with ThreadPoolExecutor(min(WORKERS, len(blocks))) as ex:
+                res = list(ex.map(one, blocks))
+        for out in res:
+            for kind, name, what, bad, wr in out:
+                key = (self.n, kind, name, what)
+                if key in self._at:
+                    i = self._at[key]
+                    self.checks[i] = key + (bad + self.checks[i][4], max(wr, self.checks[i][5]))
+                else:
+                    self._at[key] = len(self.checks)
+                    self.checks.append(key + (bad, wr))
+
+    def _unit(self, nrows):
+        """-> (taps of the next unit, the rows it is checked on in blocks of BLOCK)"""
+        self.n += 1
+        R = self.rows.get(self.n)
+        return self.taps[self.n], _blocks(np.arange(nrows) if R is None else R)
 
     def statics(self):
         cfg, g, w, t = self.cfg, self.g, self.w, self.taps[0]
-        Ng = cfg.n_grid
+        r0 = self.rows.get(0, {})
         for tap, name, feat in (("vm0_img", "enc.mesh_embed", g["mesh.node_feat"]), ("e_g2m_img", "enc.g2m_edge_embed", g["g2m.edge_feat"]),
                                 ("e_mesh_img", "proc.edge_embed", g["mesh.edge_feat"]), ("e_m2g_img", "dec.m2g_edge_embed", g["m2g.edge_feat"])):
-            _, y, yb = ref_static(np.asarray(feat, np.float32).reshape(-1, np.asarray(feat).shape[-1]), w, name, cfg.ln_eps)
-            self._chk("static", name, tap, t[tap], y, gr.f16_bound(y, yb))
-            if tap == "vm0_img":
-                self._chk("static", name, "vm0", t["vm0"], y, yb)
-                self._chk("static", name, "vm0_img = fp16(vm0)", t["vm0_img"], q16(t["vm0"]), 0.0)
-        f, fb = ref_table(t["vm0_img"], [np.asarray(w["enc.g2m_edge.w1"])[:, 2 * L:3 * L]])
-        self._chk("static", "enc.g2m_edge", "g2m_tr", t["g2m_tr"], f, fb)
+            feat = np.asarray(feat, np.float32).reshape(-1, np.asarray(feat).shape[-1])
+
+            def block(R, chk, tap=tap, name=name, feat=feat):
+                _, y, yb = ref_static(feat[R], w, name, cfg.ln_eps)
+                chk("static", name, tap, t[tap][R], y, gr.f16_bound(y, yb))
+                if tap == "vm0_img":
+                    chk("static", name, "vm0", t["vm0"][R], y, yb)
+                    chk("static", name, "vm0_img = fp16(vm0)", t["vm0_img"][R], q16(t["vm0"][R]), 0.0)
+            self._run(_blocks(r0.get(tap, np.arange(len(feat)))), block)
+
+        def block(R, chk):
+            f, fb = ref_table(t["vm0_img"][R], [np.asarray(w["enc.g2m_edge.w1"])[:, 2 * L:3 * L]])
+            chk("static", "enc.g2m_edge", "g2m_tr", t["g2m_tr"][R], f, fb)
+        self._run(_blocks(r0.get("g2m_tr", np.arange(int(g["n_mesh"])))), block)
         return t
 
     def features(self):
-        t = self._unit()
+        t, blocks = self._unit(self.cfg.n_grid)
         ref, bound = ref_features(self.cfg, self.w, self.g, self.x, self.t)
         nf = self.cfg.n_features
-        self._chk("features", "features", "feat", t["feat"][:, :nf], ref[:, :nf], bound[:, :nf])
-        self._chk("features", "features", "feat padding", t["feat"][:, nf:], 0.0, 0.0)
+
+        def block(R, chk):
+            got = t["feat"][R]
+            chk("features", "features", "feat", got[:, :nf], ref[R, :nf], bound[R, :nf])
+            chk("features", "features", "feat padding", got[:, nf:], 0.0, 0.0)
+        self._run(blocks, block)
         return t["feat"]
 
     def hidden(self, name, parts, out, rows, gathers=(), kmajor=False):
-        t = self._unit()
+        t, blocks = self._unit(rows)
         w1 = np.asarray(self.w[name + ".w1"])
-        f, fb = ref_hidden([(a, w1[:, c0:c1]) for a, (c0, c1) in parts], self.w[name + ".b1"], gathers)
-        self._chk("hidden", name, out, t[out], f, fb)
+
+        def block(R, chk):
+            f, fb = ref_hidden([(a[R], w1[:, c0:c1]) for a, (c0, c1) in parts], self.w[name + ".b1"],
+                               [(tb, np.asarray(i)[R]) for tb, i in gathers])
+            chk("hidden", name, out, t[out][R], f, fb)
+        self._run(blocks, block)
         return t[out]
 
     def ln(self, name, hid, res, outs, rows, kmajor=False):
-        t = self._unit()
-        y, s, b = ref_ln(hid, self.w, name, res, self.cfg.ln_eps)
-        got = {}
-        for k, tap in outs.items():
-            r = y if k == "yimg" else s
-            self._chk("ln", name, tap, t[tap], r, b if k == "xout" else gr.f16_bound(r, b))
-            got[k] = t[tap]
-        if "xout" in outs and "img" in outs:
-            self._chk("ln", name, f"{outs['img']} = fp16({outs['xout']})", t[outs["img"]], q16(t[outs["xout"]]), 0.0)
-        return got
+        t, blocks = self._unit(rows)
+
+        def block(R, chk):
+            y, s, b = ref_ln(hid[R], self.w, name, None if res is None else res[R], self.cfg.ln_eps)
+            for k, tap in outs.items():
+                r = y if k == "yimg" else s
+                chk("ln", name, tap, t[tap][R], r, b if k == "xout" else gr.f16_bound(r, b))
+            if "xout" in outs and "img" in outs:
+                chk("ln", name, f"{outs['img']} = fp16({outs['xout']})", t[outs["img"]][R], q16(t[outs["xout"]][R]), 0.0)
+        self._run(blocks, block)
+        return {k: t[tap] for k, tap in outs.items()}
 
     def table(self, name, a, c0s, out, rows):
-        t = self._unit()
+        t, blocks = self._unit(rows)
         w1 = np.asarray(self.w[name + ".w1"])
-        f, fb = ref_table(a, [w1[:, c0:c0 + L] for c0 in c0s])
-        self._chk("table", name, out, t[out], f, fb)
+
+        def block(R, chk):
+            f, fb = ref_table(a[R], [w1[:, c0:c0 + L] for c0 in c0s])
+            chk("table", name, out, t[out][R], f, fb)
+        self._run(blocks, block)
         return t[out]
 
     def agg(self, name, y, ptr):
-        t = self._unit()
-        f, fb = ref_agg(y, ptr)
-        self._chk("agg", name, "agg_img", t["agg_img"], f, fb)
+        t, blocks = self._unit(len(ptr) - 1)
+
+        def block(R, chk):
+            f, fb = ref_agg(y, ptr, R)
+            chk("agg", name, "agg_img", t["agg_img"][R], f, fb)
+        self._run(blocks, block)
         return t["agg_img"]
 
     def out(self, hid):
-        t = self._unit()
         cfg = self.cfg
+        t, blocks = self._unit(cfg.n_grid)
+        R = np.concatenate(blocks)
         ns, npg = cfg.n_state, cfg.n_prog
-        x1 = self.x.reshape(2 * ns, -1)[ns:ns + npg].T.astype(np.float64)
-        ref, bound = ref_out(hid, self.w, x1, npg)
-        xo = np.asarray(t["x_out"], np.float64).reshape(2 * ns, -1)
-        self._chk("out", "dec.out", "x_out", xo[ns:ns + npg].T, ref, bound)
+        x = self.x.reshape(2 * ns, -1)[:, R].astype(np.float64)
+        ref, bound = ref_out(hid[R], self.w, x[ns:ns + npg].T, npg)
+        # x_out: the new state [2 n_state, nlat, nlon], or Rows of grid points [n, 2 n_state]
+        xo = t["x_out"][R].T if isinstance(t["x_out"], Rows) else np.asarray(t["x_out"], np.float64).reshape(2 * ns, -1)[:, R]
         # the planes the feature kernel writes: slice 0 = the old slice 1 bit for bit, the new forcing = toa(t + dt)
         from oracle.graphcast_ref import toa_radiation
         lat = np.linspace(90.0, -90.0, cfg.nlat); lon = np.arange(cfg.nlon) * (360.0 / cfg.nlon)
         toa = toa_radiation(self.t + 3600.0 * cfg.dt_hours, lat, lon).reshape(-1)
-        self._chk("features", "features", "x_out slice 0", xo[:ns], self.x.reshape(2 * ns, -1)[ns:].astype(np.float64), 0.0)
-        self._chk("features", "features", "x_out toa(t+dt)", xo[2 * ns - 1], toa, TOA_REL * toa.max())
+
+        def block(_, chk):
+            chk("out", "dec.out", "x_out", xo[ns:ns + npg].T, ref, bound)
+            chk("features", "features", "x_out slice 0", xo[:ns], x[ns:], 0.0)
+            chk("features", "features", "x_out toa(t+dt)", xo[2 * ns - 1], toa[R], TOA_REL * toa.max())
+        self._run([R], block)
 
 
-def check_step(cfg, graph, w, x, t_seconds, taps):
-    """-> [(unit, kind, name, what, n_outside, worst ratio)]; NaN counts as outside"""
-    c = Checker(cfg, graph, w, x, t_seconds, taps)
+BLOCK = 8192           # rows per reference evaluation: bounds each thread's temporaries at full size
+WORKERS = min(8, os.cpu_count() or 1)
+
+
+def _blocks(R):
+    return [R[i:i + BLOCK] for i in range(0, len(R), BLOCK)] or [R]
+
+
+def _summary(got, ref, bound):
+    """-> (elements outside, worst |got - ref| / bound); NaN counts as outside, a bound of 0 asks for equality"""
+    got = np.asarray(got, np.float64)
+    ref = np.broadcast_to(np.asarray(ref, np.float64), got.shape)
+    bound = np.broadcast_to(np.asarray(bound, np.float64), got.shape)
+    bad = int(gr.exceed(got, ref, bound).sum())
+    exact = bound == 0
+    wr = gr.worst(got[~exact], ref[~exact], bound[~exact]) if (~exact).any() else 0.0
+    if exact.any() and not np.array_equal(got[exact], ref[exact]):
+        wr = math.inf
+    return bad, wr
+
+
+def check_step(cfg, graph, w, x, t_seconds, taps, rows=None):
+    """-> [(unit, kind, name, what, n_outside, worst ratio)]; NaN counts as outside.  ``rows``: Checker's"""
+    c = Checker(cfg, graph, w, x, t_seconds, taps, rows)
     run_program(cfg, graph, c)
-    out = []
-    for n, kind, name, what, got, ref, bound in c.checks:
-        got = np.asarray(got, np.float64)
-        ref = np.broadcast_to(np.asarray(ref, np.float64), got.shape)
-        bound = np.broadcast_to(np.asarray(bound, np.float64), got.shape)
-        bad = int(gr.exceed(got, ref, bound).sum())
-        exact = bound == 0
-        wr = gr.worst(got[~exact], ref[~exact], bound[~exact]) if (~exact).any() else 0.0
-        if exact.any() and not np.array_equal(got[exact], ref[exact]):
-            wr = math.inf
-        out.append((n, kind, name, what, bad, wr))
-    return out
+    return c.checks
 
 
 def by_stage(results):

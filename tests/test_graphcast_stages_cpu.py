@@ -158,3 +158,141 @@ def test_mutations_are_named_by_their_own_unit(mut):
           f"{ {k: round(v, 5) for k, v in errs.items()} } -> {'MISSED' if missed else 'caught'} by the 3e-3 norm"
           + (f"; clean emulation {max(base.values()):.2e}" if base else ""))
     assert missed == (mut in MISSED_BY_WHOLE_TENSOR_NORM), (mut, errs)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# the sampled check: a read plan (Planner) and the Checker on chosen rows
+# ---------------------------------------------------------------------------------------------------------------------
+@functools.lru_cache(maxsize=None)
+def _emulated(case, mut=None):
+    cfg, graph, w, x = _inputs(case)
+    return st.emulate(cfg, graph, w, x, T0, mut=mut).taps
+
+
+def _sampled(cfg, taps, p):
+    """what a device gather of the plan would return: the planned rows of every tap, as Rows"""
+    ns = cfg.n_state
+    rows = lambda tap, v, r: np.asarray(v, np.float64).reshape(2 * ns, -1)[:, r].T if tap == "x_out" else np.asarray(v)[r]
+    return {n: {tap: st.Rows(r, rows(tap, taps[n][tap], r)) for tap, (r, kmajor, cols) in p.reads[n].items()} for n in p.reads}
+
+
+@pytest.mark.parametrize("case", [c for c in CASES if c != "33x64-m1-L2"])
+def test_sampled_checker_on_every_row_is_check_step(case):
+    """the every-row plan read as Rows gives check_step's counts and worst ratios exactly, and lists every valid row"""
+    cfg, graph, w, x = _inputs(case)
+    taps = _emulated(case)
+    p = st.plan(cfg, graph)
+    for n, (kind, name, outs) in enumerate(st.units(cfg, graph), 1):
+        assert set(p.reads[n]) >= set(outs) and len(p.checked[n]) == (outs[next(iter(outs))][0] or cfg.n_grid)
+    assert st.check_step(cfg, graph, w, x, T0, _sampled(cfg, taps, p), rows=p.checked) == st.check_step(cfg, graph, w, x, T0, taps)
+
+
+SMALL = dict(n_grid=16, n_g2m_nodes=4, n_edges=16)       # the full-size rules with small seeded samples
+
+
+@pytest.mark.parametrize("mut", list(MUTATIONS))
+def test_full_size_rules_catch_every_mutation(mut):
+    """the full-size sampling rules (first and partial last tile, first and last latitude row, cut and degree-0 nodes, a
+    few seeded rows) applied to the small graphs name each modelled mistake in its own unit, as the every-row check does"""
+    case, where = MUTATIONS[mut]
+    cfg, graph, w, x = _inputs(case)
+    p = st.plan(cfg, graph, st.full_size_rows(cfg, graph, **SMALL))
+    assert any(len(r) < n for r, n in ((p.checked[1], cfg.n_grid), (p.checked[0]["e_g2m_img"], len(graph["g2m.senders"]))))
+    res = st.check_step(cfg, graph, w, x, T0, _sampled(cfg, _emulated(case, mut), p), rows=p.checked)
+    failing = [(n, kind, name, what, bad) for n, kind, name, what, bad, wr in res if bad]
+    at = [n for n, (kind, name, _) in enumerate(st.units(cfg, graph), 1) if (kind, name) == where][0]
+    assert failing and min(f[0] for f in failing) == at, (mut, failing)
+    assert {(kind, name) for n, kind, name, what, bad in failing if n == at} == {where}, failing
+    clean = st.check_step(cfg, graph, w, x, T0, _sampled(cfg, _emulated(case), p), rows=p.checked)
+    assert not [r for r in clean if r[4]], [r for r in clean if r[4]]
+
+
+def test_full_size_plan():
+    """721 x 1440 / refinement-6 multimesh / 16 layers (the graph is built on the host): every mesh-node unit on every
+    row; every mesh-edge row in layers 0, 1, 14 and 15; rows past byte 2^31 of the k-major mesh2grid images; every
+    partial tile; all 3,234 nodes whose grid2mesh segment is cut, with all their edges in every grid2mesh unit.  Prints
+    the most bytes a single stop reads."""
+    from skyrim_b200.config import graphcast_full
+    cfg = graphcast_full()
+    graph = icomesh.build_graph(cfg.nlat, cfg.nlon, cfg.mesh_levels, cfg.radius_frac)
+    sh = st.Shapes(cfg, graph)
+    p = st.plan(cfg, graph, st.full_size_rows(cfg, graph))
+    us = st.units(cfg, graph)
+    assert len(us) == 115
+    Ng, Nm, Em, Eg = cfg.n_grid, sh.Nm, sh.Em, sh.Eg
+    last = lambda n: np.arange(n // 128 * 128, n)
+    assert (Ng % 128, Nm % 128, Em % 128) == (32, 2, 108)
+    for n, (kind, name, outs) in enumerate(us, 1):
+        rows, kmajor, _ = next(iter(outs.values()))
+        R = p.checked[n]
+        if name == "g2m":
+            continue
+        if rows == Nm:
+            assert len(R) == Nm, (n, name)
+        elif kmajor:
+            assert all(np.isin(k * Ng + last(Ng), R).all() for k in range(3)), (n, name)
+        elif rows == Em:
+            layer = int(name[4:name.index(".")])
+            assert len(R) == Em if layer in (0, 1, 14, 15) else np.isin(last(Em), R).all() and R[0] == 0, (n, name)
+        elif rows == Eg:
+            assert np.isin(last(Eg), R).all() and R[0] == 0, (n, name)
+        else:
+            assert np.isin(last(Ng), R).all() and np.isin(np.arange(cfg.nlon), R).all(), (n, name)
+    assert all(len(p.checked[0][k]) == Nm for k in ("vm0_img", "g2m_tr"))
+    # the k-major mesh2grid images: tiles on either side of byte 2^31
+    m2g = [n for n, (kind, name, outs) in enumerate(us, 1) if name == "dec.m2g_edge" and kind != "table"]
+    for n in m2g:
+        for tap, (rows, kmajor, _) in p.reads[n].items():
+            byte = sh.m2g_rows[rows] // 128 * (st.NKB * st.TILE)
+            assert kmajor and (byte >= 2 ** 31).sum() >= 128 and (byte == 2 ** 31 - st.NKB * st.TILE).any(), (n, tap)
+    assert (sh.m2g_rows[p.checked[0]["e_m2g_img"]] >= 2 ** 31 // 1024).any()
+    # every node whose grid2mesh segment is cut, with all its edges
+    cut = np.array([node for node, p0, p1 in st.chunk_plan(graph["g2m.ptr"])[1]])
+    agg = [n for n, (kind, name, _) in enumerate(us, 1) if name == "g2m"][0]
+    assert len(cut) == 3234 and np.isin(cut, p.checked[agg]).all()
+    cut_edges = st.seg_edges(graph["g2m.ptr"], cut)
+    assert len(cut_edges) == 414552
+    for n, (kind, name, _) in enumerate(us, 1):
+        if name == "enc.g2m_edge" and kind != "table":
+            assert np.isin(cut_edges, p.checked[n]).all()
+    assert np.isin(cut_edges, p.checked[0]["e_g2m_img"]).all() and len(p.checked[0]["e_mesh_img"]) == Em
+    per_stop = {n: sum(len(r) * st.row_bytes(cfg, tap, cols) for tap, (r, kmajor, cols) in taps.items())
+                for n, taps in p.reads.items()}
+    n = max(per_stop, key=per_stop.get)
+    print(f"721x1440: most bytes read at one stop {per_stop[n] / 2 ** 20:.0f} MiB (stop {n}: {us[n - 1][:2] if n else 'load'}); "
+          f"in all {sum(per_stop.values()) / 2 ** 30:.2f} GiB over {len(per_stop)} stops")
+
+
+def test_device_gather_round_trips():
+    """Shapes.gather on a host torch tensor: rows of a full tile, of the partial last tile and of the last tile of a
+    k-major image, of a table and of an fp32 latent equal the whole decode"""
+    cfg, graph, w, x = _inputs("7x16-m1-L1")
+    sh = st.Shapes(cfg, graph)
+    rng = np.random.default_rng(1)
+    a = rng.standard_normal((sh.E3, st.L)).astype(np.float16)
+    raw = np.zeros(sh.tap_floats("hid") * 4, np.uint8)
+    img = st.gr.pack_tiles(a, 128, st.NKB)
+    raw[:img.size] = img
+    whole = sh.decode("hid", raw.view(np.float32), sh.m2g_rows)
+    Ng = cfg.n_grid
+    for rows in (np.arange(0, 128, 5), np.arange(Ng - 9, Ng), np.arange(2 * Ng, 3 * Ng)[[0, 7, -1]], np.array([Ng - 1, Ng, 2 * Ng + 3])):
+        got = sh.gather("hid", torch.from_numpy(raw.view(np.float32)), rows, kmajor=True)
+        assert np.array_equal(got.idx, rows) and np.array_equal(got.val, whole[rows]), rows
+    plain = sh.gather("hid", torch.from_numpy(raw.view(np.float32)), np.array([0, 127, 128, sh.E3 - 1]))
+    assert np.array_equal(plain.val, a[[0, 127, 128, sh.E3 - 1]].astype(np.float64))
+    t = rng.standard_normal((sh.Nmp, 2 * st.L)).astype(np.float16)
+    got = sh.gather("tm", torch.from_numpy(t.view(np.float32).reshape(-1)), [0, 5, sh.Nm - 1], cols=2 * st.L)
+    assert np.array_equal(got.val, t[[0, 5, sh.Nm - 1]].astype(np.float64))
+    v = rng.standard_normal((sh.Nm, st.L)).astype(np.float32)
+    got = sh.gather("vm", torch.from_numpy(v.reshape(-1)), [1, sh.Nm - 1])
+    assert np.array_equal(got.val, v[[1, sh.Nm - 1]].astype(np.float64))
+    r = st.Rows(got.idx, got.val)
+    assert np.array_equal(r[np.array([sh.Nm - 1])], got.val[1:]) and np.array_equal(r[1:sh.Nm].idx, [0, sh.Nm - 2])
+    with pytest.raises(AssertionError, match="not read"):
+        r[np.array([0])]
+    with pytest.raises(AssertionError, match="not read"):
+        r[np.array([sh.Nm])]
+    empty = sh.gather("hid", torch.from_numpy(raw.view(np.float32)), np.zeros(0, np.int64), kmajor=True)
+    assert empty.val.shape == (0, st.L) and empty[np.zeros(0, np.int64)].shape == (0, st.L)
+    with pytest.raises(AssertionError, match="not read"):
+        empty[np.array([0])]

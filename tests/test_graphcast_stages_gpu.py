@@ -9,10 +9,16 @@ and 4321 and whose mesh in-degrees are 0, 1, 64, 65 and 200.
 - stage-local: every unit from the engine's own inputs to it, per element, zero outside, rows of a partial tile included;
 - chained: every latent, update and aggregate against the fp64 oracle's taps, per row;
 - a workspace full of NaN bytes, a previous step's leftovers and a NaN member change no valid bit;
-- the feature-count limit, the range guard on partial tiles, the launch count of a step.
+- the feature-count limit, the range guard on partial tiles, the launch count of a step;
+- the full 721 x 1440 grid with the refinement-6 multimesh and 16 layers: every unit on the rows of
+  graphcast_stages_ref.full_size_rows (every mesh-node row, every mesh-edge row of the first and last two layers, the
+  tiles around byte 2^31 of the mesh2grid images, every partial tile, every cut grid2mesh segment with all its edges),
+  gathered on the device.
 """
 import dataclasses
 import functools
+import resource
+import time
 
 import numpy as np
 import pytest
@@ -33,21 +39,26 @@ def _need_gpu():
 
 def _inputs(case, seed=0, **cfg_kw):
     from oracle import graphcast_stages_ref as st
-    from oracle.graphcast_ref import toa_radiation
     from skyrim_b200 import icomesh
     from skyrim_b200.config import graphcast_small
-    from skyrim_b200.weights import make_graphcast_weights, synthetic_graphcast_state
+    from skyrim_b200.weights import make_graphcast_weights
     nlat, nlon, levels, layers, hand = CASES[case]
     cfg = dataclasses.replace(graphcast_small(nlat, nlon, levels, 512, layers), **cfg_kw)
     graph = icomesh.build_graph(cfg.nlat, cfg.nlon, cfg.mesh_levels, cfg.radius_frac)
     if hand:
         graph = st.hand_graph(graph)
-    w = make_graphcast_weights(cfg, 0)
+    return cfg, graph, make_graphcast_weights(cfg, 0), _state(cfg, seed)
+
+
+def _state(cfg, seed):
+    """the seeded state, its two toa forcing planes at T0 - 6 h and T0"""
+    from oracle.graphcast_ref import toa_radiation
+    from skyrim_b200.weights import synthetic_graphcast_state
     x = synthetic_graphcast_state(cfg, seed)
     lat = np.linspace(90.0, -90.0, cfg.nlat); lon = np.arange(cfg.nlon) * (360.0 / cfg.nlon)
     x[cfg.n_state - 1] = toa_radiation(T0 - 21600.0, lat, lon)
     x[2 * cfg.n_state - 1] = toa_radiation(T0, lat, lon)
-    return cfg, graph, w, x
+    return x
 
 
 def _engine(cfg, graph, w):
@@ -256,3 +267,117 @@ def test_launches_per_step(case):
         print(f"{case} B = {B}: launches per step {counts}")
         assert counts == [1 + B * expect] * 3, (counts, expect)
     eng.close()
+
+
+class _PlannedTaps:
+    """``[n]``: a step that stops after unit n (n = 0: no step, the load-time taps), then the planned rows of each of its
+    taps gathered on the device; a tap's raw device copy is freed before the next is read.  Units are read in order.
+    ``host[n]``: the seconds the checker spent on unit n's references, from its read to the next one (``done`` closes
+    the last)."""
+
+    def __init__(self, eng, cfg, sh, p, xs):
+        self.eng, self.cfg, self.sh, self.p, self.xs = eng, cfg, sh, p, xs
+        self.y, self.seconds, self.bytes, self.host, self.t_read = None, 0.0, {}, {}, None
+
+    def done(self):
+        self.host[max(self.bytes)] = time.perf_counter() - self.t_read
+
+    def __getitem__(self, n):
+        from oracle import graphcast_stages_ref as st
+        t0 = time.perf_counter()
+        if n:
+            self.host[n - 1] = t0 - self.t_read
+        if n:
+            self.eng.set_clock(T0)
+            self.eng.debug_set("stop_launch", n)
+            self.y = self.eng.step(self.xs)
+        out = {}
+        for tap, (rows, kmajor, cols) in self.p.reads[n].items():
+            if tap == "x_out":
+                idx = torch.from_numpy(rows).cuda()
+                out[tap] = st.Rows(rows, self.y[0].reshape(2 * self.cfg.n_state, -1)[:, idx].T.cpu().numpy().astype(np.float64))
+            else:
+                raw = self.eng.debug_tensor(tap, (self.sh.tap_floats(tap),))
+                out[tap] = self.sh.gather(tap, raw, rows, kmajor, cols)
+                del raw
+        self.bytes[n] = sum(len(r) * st.row_bytes(self.cfg, tap, cols) for tap, (r, _, cols) in self.p.reads[n].items())
+        self.t_read = time.perf_counter()
+        self.seconds += self.t_read - t0
+        print(f"721x1440 stop {n:3d} read {self.bytes[n] / 2 ** 20:7.1f} MiB, {self.seconds:6.1f} s in stops and gathers", flush=True)
+        return out
+
+
+def test_full_size_units():
+    """721 x 1440, refinement-6 multimesh, 16 layers, one member: each of the 115 units read after a step that stops
+    behind it, on the rows of graphcast_stages_ref.full_size_rows, from the engine's own inputs to it.  No checked element
+    outside its bound, no NaN; a step stopped behind its last unit is the whole step; a workspace of 0x00 and one of 0xFF
+    bytes give the same state; launches per step.  Prints one line per unit, the wall time split into
+    set-up, stops and gathers and host references per stage, and the memory used."""
+    _need_gpu()
+    from oracle import graphcast_stages_ref as st
+    from skyrim_b200 import icomesh
+    from skyrim_b200.config import graphcast_full
+    from skyrim_b200.engine import StepEngine, launch_count
+    from skyrim_b200.weights import make_graphcast_weights
+    t_start = time.perf_counter()
+    cfg = graphcast_full()
+    t_graph = time.perf_counter()
+    graph = icomesh.build_graph(cfg.nlat, cfg.nlon, cfg.mesh_levels, cfg.radius_frac)
+    t_graph = time.perf_counter() - t_graph
+    w = make_graphcast_weights(cfg, 0)
+    x = _state(cfg, 0)
+    sh = st.Shapes(cfg, graph)
+    p = st.plan(cfg, graph, st.full_size_rows(cfg, graph))
+    us = st.units(cfg, graph)
+    assert len(us) == 115
+    eng = StepEngine(cfg, 0, graph=graph)
+    eng.load_weights(w)
+    xs = torch.from_numpy(x)[None].cuda()
+    taps = _PlannedTaps(eng, cfg, sh, p, xs)
+    t_setup = time.perf_counter() - t_start
+    try:
+        res = st.check_step(cfg, graph, w, x, T0, taps, rows=p.checked)
+        taps.done()
+        stopped = taps.y.clone()
+    finally:
+        eng.debug_set("stop_launch", -1)
+    for n in range(len(us) + 1):
+        mine = [r for r in res if r[0] == n]
+        kind, name = us[n - 1][:2] if n else ("static", "load-time")
+        rows = sum(map(len, p.checked[0].values())) if n == 0 else len(p.checked[n])
+        print(f"721x1440 unit {n:3d} {kind:8s} {name:20s} rows {rows:8d}  worst |D-R|/bound "
+              f"{max(r[5] for r in mine):.3f}  outside {sum(r[4] for r in mine)}  host {taps.host[n]:5.1f} s")
+    per_kind = {}
+    for n, s in taps.host.items():
+        k = us[n - 1][0] if n else "static"
+        per_kind[k] = per_kind.get(k, 0.0) + s
+    print(f"721x1440 set-up {t_setup:.1f} s (graph {t_graph:.1f} s); host references {sum(per_kind.values()):.1f} s: "
+          + ", ".join(f"{k} {v:.1f}" for k, v in per_kind.items()) + f"; {st.WORKERS} threads")
+    print("721x1440 per stage: " + ", ".join(f"{k} {v:.3f}" for k, v in st.by_stage(res).items()))
+    m2g = sh.m2g_rows[p.reads[[n for n, u in enumerate(us, 1) if u[:2] == ("ln", "dec.m2g_edge")][0]]["yimg"][0]]
+    print(f"721x1440 mesh2grid rows past byte 2^31 checked: {int((m2g >= 2 ** 31 // 1024).sum())}; most bytes read at one "
+          f"stop {max(taps.bytes.values()) / 2 ** 20:.0f} MiB; stops and gathers {taps.seconds:.1f} s")
+    ws = eng._workspace(1)
+    whole = []
+    for fill in (0x00, 0xFF):
+        ws.fill_(fill)
+        eng.set_clock(T0)
+        whole.append(eng.step(xs))
+    split = lambda ptr: bool(st.chunk_plan(graph[ptr])[1])
+    expect = 1 + len(us) + split("g2m.ptr") + cfg.layers * split("mesh.ptr")
+    counts = []
+    for _ in range(3):            # eager, captured, replayed
+        l0 = launch_count()
+        eng.set_clock(T0)
+        eng.step(xs)
+        torch.cuda.synchronize()
+        counts.append(launch_count() - l0)
+    device_peak = torch.cuda.max_memory_allocated()
+    eng.close()
+    print(f"721x1440 launches per step {counts} (expected {expect}); wall time {time.perf_counter() - t_start:.0f} s, host "
+          f"peak RSS {resource.getrusage(resource.RUSAGE_SELF).ru_maxrss / 2 ** 20:.1f} GiB, device peak (torch) "
+          f"{device_peak / 2 ** 30:.1f} GiB")
+    assert not [r for r in res if r[4]], [r for r in res if r[4]]
+    assert torch.equal(stopped, whole[0]), "a step stopped behind its last unit is the whole step"
+    assert torch.isfinite(whole[0]).all() and torch.equal(whole[0], whole[1]), "0x00 and 0xFF workspaces"
+    assert counts == [expect] * 3, (counts, expect)
