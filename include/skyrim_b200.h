@@ -336,6 +336,61 @@ SKY_API int sky_forecast_score_maps_multi(int32_t n_sources, const float* const*
                                           const int32_t* channels, int32_t n_sel, int32_t nlat, int32_t nlon,
                                           const float* truth, double* maps, void* stream);
 
+/* Forecasts at sites.  A site table holds, for n_sites sites at (lat[i], lon[i]) in degrees, a 4-entry stencil of flat
+ * plane indices and fp64 weights on the equiangular (nlat, nlon) grid of skyrim_b200.timeloop.equiangular_grid (rows from
+ * 90 down to -90 degrees, dphi = 180 / (nlat - 1); columns from 0 degrees, dlam = 360 / nlon), computed on the host in
+ * fp64, one rounding per operation:
+ *   lam' = fmod(lon, 360), plus 360 if negative;  u = lam' / dlam;  j = floor(u);  b = u - j;  j0 = j mod nlon;
+ *   j1 = (j0 + 1) mod nlon;  t = (90 - lat) / dphi;
+ *   SKY_SITES_BILINEAR: i0 = min(floor(t), nlat - 2), a = t - i0; weights ((1-a)(1-b), (1-a) b, a (1-b), a b) on
+ *                       (i0, j0), (i0, j1), (i0 + 1, j0), (i0 + 1, j1);
+ *   SKY_SITES_NEAREST:  row floor(t + 0.5), column floor(u + 0.5) mod nlon (longitude distance around the circle, ties to
+ *                       the south and the east), weight 1 there and 0 on the three other entries.
+ * The table is validated and uploaded to `device` once by sky_sites_create; no index it holds lies outside the plane.
+ * Refused with SKY_ERR_ARG before any CUDA call: a lat outside [-90, 90], a non-finite lat or lon, n_sites outside
+ * [1, 2^20], nlat < 2, nlon < 1, nlat x nlon >= 2^31, an unknown method, null pointers.  sky_sites_destroy frees the table
+ * (NULL is accepted). */
+#define SKY_SITES_BILINEAR 0
+#define SKY_SITES_NEAREST 1
+typedef struct sky_sites sky_sites_t;
+SKY_API int sky_sites_create(sky_sites_t** out, const double* lat, const double* lon, int32_t n_sites, int32_t nlat,
+                             int32_t nlon, int32_t method, int device);
+SKY_API int sky_sites_destroy(sky_sites_t* s);
+
+/* Samples `members` states at the sites of table s, for the selected channels, into a caller-owned device buffer:
+ *   x, members, member_stride, channel_count, channels, n_sel as for sky_ensemble_stats, with plane = nlat x nlon of the
+ *              table (a GraphCast state's new slice is reached through x itself);
+ *   values     device fp32 [members][n_sel][n_sites].
+ * Each value is the fp64 sum of the stencil's terms w_k x_k, added in stencil order with no fused multiply-add, starting
+ * from 0; entries of weight exactly 0 are not read (a NaN beside a nearest-neighbour site does not reach it); the sum is
+ * rounded once to fp32.  A site on a grid point whose coordinates are exact in binary returns that grid value bit for bit
+ * under both methods.  sky_ensemble_stats(values, members, n_sel * n_sites, plane = n_sites, n_sel, ...) gives the site
+ * statistics.  One thread per (site, channel), sites along threads; any site order.  Refused with SKY_ERR_ARG before any
+ * CUDA call: a null table, the member and channel arguments sky_ensemble_stats refuses, a null x or values; and before any
+ * launch: x or values not device memory on the table's device.  Asynchronous and stream-ordered. */
+SKY_API int sky_sample_sites(const sky_sites_t* s, const float* x, int32_t members, int64_t member_stride,
+                             int32_t channel_count, const int32_t* channels, int32_t n_sel, float* values, void* stream);
+
+/* Site verification terms against observations with gaps, into caller-owned device buffers:
+ *   values   device fp32 [members][n_sel][n_sites] (sky_sample_sites), members 1..64, n_sel 1..128, n_sites 1..2^20;
+ *   obs      device fp32 [n_sel][n_sites]: the observation of each selected channel at each site, NaN where missing;
+ *   acc      device fp64 [n_sel][n_sites][6], accumulated in place;
+ *   partial  device fp64 workspace of at least partial_bytes = 8 * 6 * n_sel * ceil(n_sites / SKY_SITES_THREADS) bytes;
+ *   sums     device fp64 [n_sel][6].
+ * At a site with an observation y, with x_bar the members' mean summed in member order in fp64, the six terms are
+ *   1,  e = x_bar - y,  e^2,  sum_m (x_m - x_bar)^2,  (1/M) sum_m |x_m - y|,  G = sum_{m<k} |x_m - x_k|,
+ * the arithmetic of sky_forecast_score_maps (one shared device function).  acc[s][i][t] += term t once per call (call
+ * order, so accumulators summed over calls are bitwise reproducible); sums[s][t] is the sum of term t over the sites of
+ * channel s with an observation.  A missing observation adds nothing.  A NaN member at a site with an observation makes
+ * terms 1..5 of that site's accumulators and of that channel's sums NaN; term 0 counts the observations.  Two launches,
+ * no atomics: one partial per (channel, term, block of SKY_SITES_THREADS sites) summed in thread order, then the partials
+ * in block order, so the sums are bitwise reproducible and a channel's results do not depend on the other channels.
+ * Refused with SKY_ERR_ARG before any CUDA call: a count or partial_bytes out of range, null pointers; and before any
+ * launch: buffers not device memory on one device.  Asynchronous and stream-ordered; launches on the device of values. */
+#define SKY_SITES_THREADS 128
+SKY_API int sky_site_scores(const float* values, int32_t members, int32_t n_sel, int32_t n_sites, const float* obs,
+                            double* acc, double* partial, uint64_t partial_bytes, double* sums, void* stream);
+
 /* Per-kernel-family device timing (CUDA events recorded on the launching stream around the
  * launches whose family bit is set in tag_mask).  profile_end synchronises on the recorded
  * events and returns the summed milliseconds and launch counts per family.  Used by bench.py

@@ -93,6 +93,13 @@ EXPORTS = {
     "sky_forecast_score_maps_multi": (C.c_int, [C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_int32),
                                                 C.POINTER(C.c_int64), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32,
                                                 C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "sky_sites_create": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(C.c_double), C.POINTER(C.c_double), C.c_int32,
+                                   C.c_int32, C.c_int32, C.c_int32, C.c_int]),
+    "sky_sites_destroy": (C.c_int, [C.c_void_p]),
+    "sky_sample_sites": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_int32, C.POINTER(C.c_int32),
+                                   C.c_int32, C.c_void_p, C.c_void_p]),
+    "sky_site_scores": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_uint64, C.c_void_p, C.c_void_p]),
     "sky_model_profile_begin": (C.c_int, [C.c_void_p, C.c_uint64]),
     "sky_model_profile_end": (C.c_int, [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_uint64), C.c_int32]),
     "sky_profile_tag_count": (C.c_int, []),

@@ -383,6 +383,203 @@ class GlobalModel:
                     paths.append(save_forecast(da, label + suffix, starts[0], t_end, source, config=save_config))
         return res, paths
 
+    def _site_channels(self, channels, save_config, default):
+        """the checked channel names of a site request, in model order: ``channels``, else save_config's filter_vars,
+        else ``default``"""
+        from ... import engine as E
+        names = list(self.out_channel_names)
+        wanted = list(channels) or list(save_config.get("filter_vars", ())) or list(default)
+        unknown = [c for c in wanted if c not in names]
+        if unknown:
+            raise ValueError(f"unknown channel(s) {unknown} for {self.model_name}")
+        sel = [c for c in names if c in wanted]
+        if len(sel) > E.ENS_MAX_CHANNELS:
+            raise ValueError(f"{len(sel)} channels: at most {E.ENS_MAX_CHANNELS}")
+        return sel
+
+    def _site_checks(self, members, perturbation, method):
+        """the checks shared by ``predict_sites`` and ``score_sites``, before any engine call: the perturbation ("none"
+        for one member, else "spherical_grf", unless given)"""
+        from ... import engine as E
+        from ... import sites as St
+        if not 1 <= members <= E.ENS_MAX_MEMBERS:
+            raise ValueError(f"members = {members} must lie in [1, {E.ENS_MAX_MEMBERS}]")
+        if perturbation is None:
+            perturbation = "none" if members == 1 else "spherical_grf"
+        if perturbation not in ("none", "gaussian", "spherical_grf"):
+            raise ValueError(f"unknown perturbation {perturbation!r} (none, gaussian, spherical_grf)")
+        if method not in E.SITES_METHODS:
+            raise ValueError(f"unknown site method {method!r} ({', '.join(E.SITES_METHODS)})")
+        St.check_equiangular(self.model.grid.lat, self.model.grid.lon)
+        return perturbation
+
+    def predict_sites(self, start_time: datetime.datetime, n_steps: int, sites, members: int = 1,
+                      method: str = "bilinear", channels: List[str] = [], quantiles=(), events: dict = {},
+                      perturbation: str | None = None, amp: float = 0.05, seed: int = 0, grf: dict | None = None,
+                      save: bool = False, save_config: dict = {}):
+        """Forecast at ``sites`` (``sites.read_sites``: {name: (lat, lon)}, (names, lats, lons) or a CSV file) for leads 0,
+        6, .., 6 ``n_steps`` h: every member sampled on the device with the site stencil ``method`` ("bilinear" or
+        "nearest", include/skyrim_b200.h sky_sites_create).  ``members = 1`` (perturbation "none") samples the model's own
+        trajectory; above 1 the members are ``predict_ensemble``'s (perturbation, amp, seed, grf), and the site
+        statistics (mean, spread, ``quantiles``) and P(x > t) for ``events`` = {channel: threshold(s)} are reduced on the
+        device too.  Only the site arrays cross to the host, each step's copy under the next step's forwards.  Refused
+        before any engine call: unknown channels, a grid that is not equiangular, and returned arrays above 2^31 bytes.
+        ``save`` writes the values, statistics and probabilities as netCDF files, models "<model>-sites<M>[-stats|-prob]".
+        Returns (``sites.SiteForecast``, paths)."""
+        from ... import engine as E
+        from ... import sites as St
+        from .ensemble import event_name, quantile_name
+        perturbation = self._site_checks(members, perturbation, method)
+        if n_steps < 0:
+            raise ValueError(f"n_steps = {n_steps} must not be negative")
+        names, lat, lon = St.read_sites(sites)
+        ev = {c: [float(t) for t in np.atleast_1d(thr)] for c, thr in dict(events).items()}
+        q = [float(v) for v in quantiles]
+        if members == 1 and (q or ev):
+            raise ValueError("quantiles and events describe an ensemble: give members > 1")
+        if len(q) > E.ENS_MAX_QUANTILES or not all(0.0 <= v <= 1.0 for v in q):
+            raise ValueError(f"quantiles {q}: at most {E.ENS_MAX_QUANTILES}, each in [0, 1]")
+        if not all(np.isfinite(t) for ts in ev.values() for t in ts):
+            raise ValueError(f"event thresholds must be finite: {ev}")
+        if save and save_config.get("file_type", "netcdf") == "zarr":
+            raise ValueError("site forecasts are written as netCDF only: the zarr writer holds one variable per forecast id")
+        unknown = [c for c in ev if c not in self.out_channel_names]
+        if unknown:
+            raise ValueError(f"unknown channel(s) {unknown} for {self.model_name}")
+        wanted = set(self._site_channels(channels, save_config, self.out_channel_names)) | set(ev)
+        sel = [c for c in self.out_channel_names if c in wanted]
+        ev_list = [(i, t) for i, c in enumerate(sel) for t in ev.get(c, ())]
+        if len(sel) > E.ENS_MAX_CHANNELS or len(ev_list) > E.ENS_MAX_EVENTS:
+            raise ValueError(f"{len(sel)} channels and {len(ev_list)} events: at most {E.ENS_MAX_CHANNELS} and "
+                             f"{E.ENS_MAX_EVENTS}")
+        T, n, Sn = n_steps + 1, len(names), len(sel)
+        nbytes = 4 * T * n * (members * Sn + ((2 + len(q)) * Sn + len(ev_list) if members > 1 else 0))
+        if nbytes > St.RETURN_LIMIT:
+            raise ValueError(f"the site arrays of this request take {nbytes} bytes, above the 2^31 returned at most: "
+                             "ask for fewer steps, members, channels or sites")
+        runner, offset = self._score_runner(start_time, members, perturbation, amp, seed, grf)
+        table = E.SiteTable(lat, lon, len(self.model.grid.lat), len(self.model.grid.lon), method, runner.x.device.index)
+        values = np.empty((T, members, n, Sn), np.float32)
+        stats = np.empty((T, 2 + len(q), n, Sn), np.float32) if members > 1 else None
+        prob = np.empty((T, len(ev_list), n), np.float32) if ev_list else None
+        idx = [list(self.out_channel_names).index(c) for c in sel]
+        try:
+            for n_, v, *rest in runner.iter_sites(n_steps, table, idx, q, ev_list, offset):
+                values[n_] = v.numpy()[:, :, 0].transpose(0, 2, 1)
+                if stats is not None:
+                    stats[n_] = rest[0].numpy()[:, :, 0].transpose(0, 2, 1)
+                if prob is not None:
+                    prob[n_] = rest[1].numpy()[:, 0]
+        finally:
+            table.close()
+        times = np.array([np.datetime64(start_time + k * self.time_step, "s") for k in range(T)])
+        where = dict(site=np.array(names), lat=("site", lat), lon=("site", lon))
+        attrs = dict(model=self.model_name, members=int(members), method=method)
+        res = St.SiteForecast(
+            xr.DataArray(values, dims=["time", "member", "site", "channel"],
+                         coords=dict(where, time=times, member=np.arange(members, dtype=np.float64), channel=np.array(sel)),
+                         attrs=dict(attrs)),
+            None if stats is None else xr.DataArray(
+                stats, dims=["time", "statistic", "site", "channel"],
+                coords=dict(where, time=times, statistic=np.array(["mean", "spread"] + [quantile_name(v) for v in q]),
+                            channel=np.array(sel)), attrs=dict(attrs)),
+            None if prob is None else xr.DataArray(
+                prob, dims=["time", "event", "site"],
+                coords=dict(where, time=times, event=np.array([event_name(sel[i], t) for i, t in ev_list])),
+                attrs=dict(attrs)),
+            self.model_name, members)
+        logger.success(f"Sampled {members} member(s) at {n} site(s) for {T} leads")
+        paths = []
+        if save:
+            save_config = {k: v for k, v in save_config.items() if k != "filter_vars"}   # selected on the device already
+            save_config.setdefault("forecast_id", generate_forecast_id())
+            source = self.ic_source if isinstance(self.ic_source, str) else "file"
+            label, t_end = f"{self.model_name}-sites{members}", start_time + n_steps * self.time_step
+            for suffix, da in (("", res.values), ("-stats", res.stats), ("-prob", res.prob)):
+                if da is not None:
+                    paths.append(save_forecast(da, label + suffix, start_time, t_end, source, config=save_config))
+        return res, paths
+
+    def score_sites(self, start_times, n_steps: int, observations, members: int = 1, method: str = "bilinear",
+                    channels: List[str] = [], perturbation: str | None = None, amp: float = 0.05, seed: int = 0,
+                    grf: dict | None = None, save: bool = False, save_config: dict = {}):
+        """Verifies the forecasts from every one of ``start_times`` (distinct, increasing) at leads 0, 6, .., 6 ``n_steps``
+        h against station ``observations`` (``sites.read_observations``: a DataArray (time, site, channel) with lat / lon
+        along site, NaN where missing), sampling the members at the observation sites with ``method``.  Date d is the
+        forecast ``predict_sites`` makes with ``seed + d`` (one runner restarted per date); ``channels`` default to the
+        observations' channels.  A valid time absent from the observations counts as missing everywhere; the call is
+        refused, before any engine call, if no observation is usable at all, and for forcing channels.  The site terms
+        are accumulated on the device and cross to the host once, at the end.  ``save`` writes the card, the per-date
+        cards, the per-site scores and the counts as netCDF files, models "<model>-obs<M>[-cards|-sites|-count]".
+        Returns (``sites.SiteScores``, paths)."""
+        import torch
+        from ... import engine as E
+        from ... import sites as St
+        from ...ensemble import upload_truth, truth_ring
+        perturbation = self._site_checks(members, perturbation, method)
+        starts = list(start_times)
+        if not starts:
+            raise ValueError("score_sites needs at least one start time")
+        if any(b <= a for a, b in zip(starts, starts[1:])):
+            raise ValueError(f"start times must be distinct and sorted: {[str(np.datetime64(t, 's')) for t in starts]}")
+        if n_steps < 0:
+            raise ValueError(f"n_steps = {n_steps} must not be negative")
+        if not 0 <= seed < 2 ** 32:
+            raise ValueError(f"seed = {seed} must lie in [0, 2^32)")
+        if save and save_config.get("file_type", "netcdf") == "zarr":
+            raise ValueError("site scores are written as netCDF only: the zarr writer appends along time")
+        have = St.read_observations(observations)[4]
+        wanted = list(channels) or list(save_config.get("filter_vars", ()))
+        forcing = [c for c in wanted if c in self.forcing_channels]
+        if forcing:
+            raise ValueError(f"{forcing} are forcings, not forecasts, and are not scored")
+        sel = self._site_channels(channels, save_config, [c for c in have if c in self.out_channel_names
+                                                          and c not in self.forcing_channels])
+        if not sel:
+            raise ValueError(f"the observations hold none of {self.model_name}'s forecast channels ({have})")
+        names, lat, lon, times, sel, obs = St.read_observations(observations, sel)
+        D, L, Sn, n = len(starts), n_steps + 1, len(sel), len(names)
+        at = {t: i for i, t in enumerate(times.tolist())}
+        slot = [[at.get(np.datetime64(t0 + k * self.time_step, "s").tolist()) for k in range(L)] for t0 in starts]
+        if not any(i is not None and np.isfinite(obs[i]).any() for row in slot for i in row):
+            raise ValueError("the observations hold no value at any valid time of these forecasts: nothing to verify")
+        missing = np.full((Sn, n), np.nan, np.float32)
+        runner = None
+        for d, t0 in enumerate(starts):
+            if runner is None:
+                runner, offset = self._score_runner(t0, members, perturbation, amp, seed, grf)
+                dev = runner.x.device
+                table = E.SiteTable(lat, lon, len(self.model.grid.lat), len(self.model.grid.lon), method, dev.index)
+                sums = torch.empty((D, L, Sn, E.SITE_TERMS), dtype=torch.float64, device=dev)
+                acc = torch.zeros((L, Sn, n, E.SITE_TERMS), dtype=torch.float64, device=dev)
+                values = torch.empty((members, Sn, 1, n), dtype=torch.float32, device=dev)
+                ring = truth_ring(dev, Sn, 1, n)
+                main = torch.cuda.current_stream(dev)
+                idx = [list(self.out_channel_names).index(c) for c in sel]
+            else:
+                runner.restart(self._ensemble_initial_state(t0)[0], seed + d)
+            for i, (k, members_x) in enumerate(runner._walk(n_steps, every_slice=True)):
+                j = slot[d][k]
+                y = upload_truth(ring, i, (missing if j is None else obs[j].T)[:, None, :], main)
+                E.sample_sites(members_x, table, idx, offset, out=values)
+                E.site_scores(values, y.view(Sn, n), acc[k], out=sums[d, k])
+                ring["scored"][i % 2].record(main)
+            logger.success(f"Scored start date {d + 1}/{D} at {n} site(s): {np.datetime64(t0, 's')}")
+        table.close()
+        step_h = self.time_step.total_seconds() / 3600
+        res = St.SiteScores.build(sums.cpu().numpy(), acc.cpu().numpy(), members, starts, [k * step_h for k in range(L)],
+                                  names, lat, lon, sel, self.model_name)
+        paths = []
+        if save:
+            save_config = {k: v for k, v in save_config.items() if k != "filter_vars"}   # selected on the device already
+            save_config.setdefault("forecast_id", generate_forecast_id())
+            source = self.ic_source if isinstance(self.ic_source, str) else "file"
+            label, t_end = f"{self.model_name}-obs{members}", starts[-1] + n_steps * self.time_step
+            for suffix, da in (("", res.card), ("-cards", res.cards), ("-sites", res.sites), ("-count", res.count)):
+                paths.append(save_forecast(da, label + suffix, starts[0], t_end, source, config=save_config))
+        return res, paths
+
+
 def check_map_leads(map_leads, map_channels, n_steps: int, step_h: float):
     """refuses map leads (hours) that are not multiples of the time step in [0, n_steps steps], and map leads without map
     channels or the reverse"""
@@ -458,6 +655,9 @@ class GlobalPrediction:
         return data
 
     def point(self, lat: float, lon: float, channel: str, n_step: int | None = 1):
+        """The value of the grid point nearest to (lat, lon), as the reference reads it: longitudes are compared on
+        [0, 360) without wrapping, so near 360 degrees this can pick a different point than ``predict_sites(...,
+        method="nearest")``, which measures longitude distance around the circle, and it does not interpolate."""
         if lon < 0:
             lon = 360 + lon
         assert channel in self.channels, f"Variable {channel} not found in dataset."

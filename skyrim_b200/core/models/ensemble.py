@@ -199,6 +199,14 @@ class GlobalEnsemble:
                                   "Skyrim(name).score_period, or compare the models with compare(); multi-model scoring "
                                   "through score_period is not built")
 
+    def predict_sites(self, *args, **kw):
+        raise NotImplementedError("site forecasts are made per model: sample each model with Skyrim(name).predict_sites; "
+                                  "multi-model site forecasts are not built")
+
+    def score_sites(self, *args, **kw):
+        raise NotImplementedError("site scores are computed per model: verify each model with Skyrim(name).score_sites; "
+                                  "multi-model site verification is not built")
+
     # -- device states ---------------------------------------------------------------------------------------------------
     def _layout(self, m):
         """(state channels, offset of the output slice in the state): a GraphCast state holds two time slices"""

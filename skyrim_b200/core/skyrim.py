@@ -90,6 +90,23 @@ class Skyrim:
                                   n_steps=self.model.time_steps(lead_time), **kw)
 
 
+    def predict_sites(self, date: str, time: str, lead_time: int = 6, sites=None, **kw):
+        """Forecast at sites (``GlobalModel.predict_sites``): the date, time and lead time are read as ``predict`` reads
+        them, ``kw`` goes to ``GlobalModel.predict_sites`` (members, method, channels, quantiles, events, perturbation,
+        amp, seed, grf, save, save_config).  Returns (SiteForecast, paths)."""
+        start_time = datetime.datetime(int(date[:4]), int(date[4:6]), int(date[6:8]), int(time[:2]), int(time[2:4]))
+        return self.model.predict_sites(start_time=start_time, n_steps=self.model.time_steps(lead_time), sites=sites, **kw)
+
+    def score_sites(self, date: str, time: str, lead_time: int = 6, observations=None, until: str | None = None,
+                    every: int = 24, **kw):
+        """Verification against station observations (``GlobalModel.score_sites``) over the start dates from ``date`` at
+        ``time`` every ``every`` hours through ``until`` (default: ``date`` alone), as ``score_period`` reads them; ``kw``
+        goes to ``GlobalModel.score_sites`` (members, method, channels, perturbation, amp, seed, grf, save,
+        save_config).  Returns (SiteScores, paths)."""
+        return self.model.score_sites(start_times=period_start_times(date, until or date, time, every),
+                                      n_steps=self.model.time_steps(lead_time), observations=observations, **kw)
+
+
 def period_start_times(start: str, end: str, time: str = "0000", every: int = 24):
     """start times from ``start`` + ``time`` every ``every`` hours (a positive multiple of 6) while their date is at most
     ``end``"""

@@ -618,6 +618,87 @@ def score_maps_accumulate_multi(sources, channels_per_source, truth, maps):
     return maps
 
 
+SITES_METHODS = {"bilinear": 0, "nearest": 1}
+SITES_MAX, SITE_TERMS, SITES_THREADS = 1 << 20, 6, 128
+
+
+class SiteTable:
+    """A site table on one GPU (include/skyrim_b200.h sky_sites_create): the 4-point stencil of every site at (``lat``,
+    ``lon``) degrees on the equiangular (nlat, nlon) grid, "bilinear" or "nearest", validated on the host and uploaded
+    once.  ``sample_sites`` reads it; ``close`` (or garbage collection) frees it."""
+
+    def __init__(self, lat, lon, nlat: int, nlon: int, method: str = "bilinear", device: int = 0):
+        if method not in SITES_METHODS:
+            raise ValueError(f"unknown site method {method!r} ({', '.join(SITES_METHODS)})")
+        lat = np.ascontiguousarray(lat, dtype=np.float64).reshape(-1)
+        lon = np.ascontiguousarray(lon, dtype=np.float64).reshape(-1)
+        if lat.shape != lon.shape:
+            raise ValueError(f"{lat.size} latitudes and {lon.size} longitudes: one of each per site")
+        L = self._L = _ffi.lib()
+        h = C.c_void_p()
+        _ffi.check(L.sky_sites_create(C.byref(h), lat.ctypes.data_as(C.POINTER(C.c_double)),
+                                      lon.ctypes.data_as(C.POINTER(C.c_double)), lat.size, int(nlat), int(nlon),
+                                      SITES_METHODS[method], int(device)), "sky_sites_create", L)
+        self._h = h
+        self.n_sites, self.nlat, self.nlon, self.method, self.device = lat.size, int(nlat), int(nlon), method, int(device)
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._L.sky_sites_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def sample_sites(x, table: SiteTable, channels=None, channel_offset: int = 0, out=None):
+    """The members of a CUDA fp32 (M, C, H, W) tensor, or a view of one whose members each hold contiguous (C, H, W)
+    planes, sampled at the sites of ``table`` (include/skyrim_b200.h sky_sample_sites).  Channels are counted from
+    ``channel_offset`` (a GraphCast state samples its new time slice with offset 83); ``channels`` lists the sampled ones
+    (default: all).  Returns CUDA fp32 (M, n_sel, 1, n_sites), into ``out`` when given: ``ensemble_statistics`` of it gives
+    the site statistics.  Asynchronous on the current stream."""
+    import torch
+    M, H, W, count, member_stride, base, sel = _verified_members(x, channels, channel_offset)
+    if (H, W) != (table.nlat, table.nlon):
+        raise ValueError(f"x's grid {H} x {W} is not the site table's {table.nlat} x {table.nlon}")
+    shape = (M, len(sel), 1, table.n_sites)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=x.device)
+    _check_out(out, shape, torch.float32, "out")
+    L = _ffi.lib()
+    st = torch.cuda.current_stream(x.device).cuda_stream
+    _ffi.check(L.sky_sample_sites(table._h, base, M, member_stride, count, _c_array(C.c_int32, sel), len(sel),
+                                  out.data_ptr(), st), "sky_sample_sites", L)
+    return out
+
+
+def site_scores(values, obs, acc, out=None):
+    """Adds the site terms 1, e, e^2, sum_m (x_m - x_bar)^2, mae and G of ``values`` (CUDA fp32 (M, n_sel, 1, n_sites), from
+    ``sample_sites``) against ``obs`` (CUDA fp32 (n_sel, n_sites), NaN where missing) to ``acc`` (CUDA fp64 (n_sel,
+    n_sites, 6)), and returns the sums of the terms over the sites with an observation, CUDA fp64 (n_sel, 6), into ``out``
+    when given (include/skyrim_b200.h sky_site_scores).  Asynchronous on the current stream."""
+    import torch
+    if not (values.is_cuda and values.dtype == torch.float32 and values.is_contiguous() and values.dim() == 4
+            and values.shape[2] == 1):
+        raise ValueError("values must be a contiguous CUDA fp32 (members, n_sel, 1, n_sites) tensor")
+    M, n_sel, _, n = values.shape
+    _check_out(obs, (n_sel, n), torch.float32, "obs")
+    _check_out(acc, (n_sel, n, SITE_TERMS), torch.float64, "acc")
+    if out is None:
+        out = torch.empty((n_sel, SITE_TERMS), dtype=torch.float64, device=values.device)
+    _check_out(out, (n_sel, SITE_TERMS), torch.float64, "out")
+    ws = torch.empty(n_sel * SITE_TERMS * ((n + SITES_THREADS - 1) // SITES_THREADS), dtype=torch.float64,
+                     device=values.device)
+    L = _ffi.lib()
+    st = torch.cuda.current_stream(values.device).cuda_stream
+    _ffi.check(L.sky_site_scores(values.data_ptr(), M, n_sel, n, obs.data_ptr(), acc.data_ptr(), ws.data_ptr(),
+                                 8 * ws.numel(), out.data_ptr(), st), "sky_site_scores", L)
+    return out
+
+
 def unix_seconds(when) -> float:
     """datetime (naive = UTC) / numpy datetime64 / number -> unix seconds"""
     import datetime as _dt

@@ -101,24 +101,44 @@ class EnsembleRunner:
         device, and the device->host copy of step n runs on a copy stream while step n + 1 computes (the event pattern of
         ``timeloop._EngineTimeLoop.iter_host``, with rings of two statistics buffers on the device and on the host).  A
         yielded pair is valid until the second next() after it."""
-        import torch
         from .engine import ensemble_statistics
+        return self._iter_on_host(self._walk(n_steps), lambda members, out=None: ensemble_statistics(
+            members, channels, quantiles, events, channel_offset, out=out))
+
+    def iter_sites(self, n_steps: int, table, channels=None, quantiles=(), events=(), channel_offset: int = 0):
+        """``iter_stats`` at the sites of ``table`` (``engine.SiteTable``): yields (n, values) with one member, (n, values,
+        stats, prob) with more, as pinned host tensors: ``engine.sample_sites`` of this rank's members, (M, n_sel, 1,
+        n_sites), and ``engine.ensemble_statistics`` of those values, events (i, threshold) about ``channels[i]``.  Every
+        slice of the walk is sampled; each slice's copy runs under the next slice's forwards."""
+        from .engine import ensemble_statistics, sample_sites
+
+        def reduce(members, out=None):
+            v = sample_sites(members, table, channels, channel_offset, out=None if out is None else out[0])
+            if members.shape[0] == 1:
+                return (v,)
+            return (v,) + ensemble_statistics(v, None, quantiles, events, out=None if out is None else out[1:])
+        return self._iter_on_host(self._walk(n_steps, every_slice=True), reduce)
+
+    def _iter_on_host(self, walk, reduce):
+        """Yields (n,) + the host copies of ``reduce(members)`` (a tuple of CUDA tensors) for every (n, members) of
+        ``walk``, each slice's device->host copy on a copy stream under the next slice's forwards and reduction
+        (``reduce(members, out=)`` writes into a ring of two device tuples; the pinned host tuples are a ring of two)."""
+        import torch
         dev = self.x.device
         main = torch.cuda.current_stream(dev)
         copy = torch.cuda.Stream(dev)
-        walk = self._walk(n_steps)
         cur = next(walk)
-        ring = [ensemble_statistics(cur[1], channels, quantiles, events, channel_offset)]
+        ring = [reduce(cur[1])]
         ring.append(tuple(torch.empty_like(t) for t in ring[0]))
         host = [tuple(torch.empty(t.shape, dtype=t.dtype).pin_memory() for t in ring[0]) for _ in range(2)]
-        done = [torch.cuda.Event() for _ in range(2)]    # statistics i % 2 are complete on the main stream
+        done = [torch.cuda.Event() for _ in range(2)]    # reduction i % 2 is complete on the main stream
         copied = torch.cuda.Event()
         done[0].record(main)
         i = 0
         while cur is not None:
             nxt = next(walk, None)
             if nxt is not None:   # launch the next slice's forwards and reduction before waiting for the copy of this one
-                ensemble_statistics(nxt[1], channels, quantiles, events, channel_offset, out=ring[(i + 1) % 2])
+                reduce(nxt[1], out=ring[(i + 1) % 2])
                 done[(i + 1) % 2].record(main)
             copy.wait_event(done[i % 2])
             with torch.cuda.stream(copy):

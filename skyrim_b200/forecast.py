@@ -10,6 +10,9 @@ defaults; same `run_forecast` signature and return value) on top of the H100 eng
         --map_leads 24,72 --truth era5.nc -o outputs
     python -m skyrim_b200.forecast --models pangu,fourcastnet_v2,graphcast --compare -d 20240501 --until 20240531 -l 72 \
         --truth era5.nc --climatology clim.nc --map_channels z500 --map_leads 24,72 -o outputs
+    python -m skyrim_b200.forecast -m pangu -l 72 --members 16 --sites cities.csv --quantiles 0.1,0.9 -o outputs
+    python -m skyrim_b200.forecast -m pangu -d 20240501 --until 20240531 -l 72 --sites stations.csv \
+        --observations synop.nc -o outputs
 
 The second form runs a perturbed-initial-condition ensemble and saves its per-step statistics (mean, spread, quantiles)
 and exceedance probabilities instead of the members.  The third runs several models side by side on one GPU
@@ -21,7 +24,10 @@ per-date scorecards, the rank histogram and, for ``--map_channels`` at ``--map_l
 compares the ``--models`` head to head (``GlobalEnsemble.compare``) over the start dates ``--date`` .. ``--until`` (one
 date without ``--until``): every model and their pooled ensemble are scored off one upload of each analysis, and the
 stacked period card, the per-date cards, each entry's rank histogram, the maps and the paired score differences of
-every pair of entries (mean, 95 % interval, p-value) are saved.
+every pair of entries (mean, 95 % interval, p-value) are saved.  ``--sites`` saves the forecast of every member at the
+sites of a CSV file (``GlobalModel.predict_sites``, bilinear or ``--site_method nearest``), with the site statistics above
+one member; with ``--observations`` it verifies the forecast against station observations at those sites
+(``GlobalModel.score_sites``) over the start dates ``--date`` .. ``--until``.
 
 Differences, all forced by the scope of this build (SURVEY.md section 2): `--initial_conditions` accepts `synthetic`
 (the default here: the network IC providers cds / ifs / gfs are the reference's `libs/ic`, out of scope, and raise a clear
@@ -33,6 +39,7 @@ from datetime import datetime, timedelta
 from pathlib import Path
 
 import click
+import numpy as np
 from loguru import logger
 
 from .common import AVAILABLE_MODELS
@@ -128,6 +135,45 @@ def run_compare(model_names, date: str, time: str, lead_time: int, until: str, e
     return paths
 
 
+def run_sites(model_name: str, date: str, time: str, lead_time: int, sites: str, method: str, initial_conditions: str,
+              output_dir: str, filter_vars: str, members: int, perturbation: str, amp: float, seed: int, quantiles=(),
+              events: dict = {}, **model_kw):
+    """``--sites``: ``Skyrim.predict_sites(save=True)`` at the sites of the CSV file ``sites`` (name,lat,lon); returns the
+    paths of the site values, statistics and probabilities"""
+    from .core import Skyrim
+    model = Skyrim(model_name, ic_source=initial_conditions, **model_kw)
+    _, paths = model.predict_sites(
+        date=date, time=time, lead_time=lead_time, sites=sites, members=members, method=method,
+        perturbation=perturbation if members > 1 else None, amp=amp, seed=seed, quantiles=quantiles, events=events,
+        save=True, save_config={"output_dir": output_dir or str(Path.cwd() / "outputs"),
+                                "filter_vars": [v.strip() for v in filter_vars.split(",") if v.strip()]})
+    return paths
+
+
+def run_score_sites(model_name: str, date: str, time: str, lead_time: int, until: str, every: int, sites: str, method: str,
+                    observations: str, initial_conditions: str, output_dir: str, filter_vars: str, members: int,
+                    perturbation: str, amp: float, seed: int, **model_kw):
+    """``--sites --observations``: ``Skyrim.score_sites(save=True)`` against the netCDF observations (time, site, channel)
+    at the sites of the CSV file ``sites``, chosen by name; returns the paths of the card, the per-date cards, the
+    per-site scores and the counts"""
+    from . import sites as St
+    from . import xr_shim as xr
+    from .core import Skyrim
+    names = St.read_sites(sites)[0]
+    obs = xr.open_dataarray(observations)
+    have = [str(n) for n in np.asarray(obs.coords["site"])] if "site" in obs.coords else []
+    unknown = [n for n in names if n not in have]
+    if unknown:
+        raise click.UsageError(f"--observations {observations} holds no site named {unknown}")
+    model = Skyrim(model_name, ic_source=initial_conditions, **model_kw)
+    _, paths = model.score_sites(
+        date=date, time=time, lead_time=lead_time, observations=obs.sel(site=names), until=until, every=every,
+        members=members, method=method, perturbation=perturbation if members > 1 else None, amp=amp, seed=seed,
+        save=True, save_config={"output_dir": output_dir or str(Path.cwd() / "outputs"),
+                                "filter_vars": [v.strip() for v in filter_vars.split(",") if v.strip()]})
+    return paths
+
+
 def parse_quantiles(text: str):
     """"0.1,0.5,0.9" -> [0.1, 0.5, 0.9]"""
     return [float(v) for v in text.split(",") if v.strip()]
@@ -187,9 +233,15 @@ def parse_exceed(text: str):
               "such as z500,t850")
 @click.option("--map_leads", type=str, default="", help="--score --until / --compare: lead times in hours of the maps such "
               "as 24,72")
+@click.option("--sites", type=str, default="", help="CSV file of sites name,lat,lon: save every member (and with --members > 1 "
+              "the statistics) at those sites instead of the grid")
+@click.option("--site_method", type=click.Choice(["bilinear", "nearest"]), default=None,
+              help="--sites: interpolation to the sites (default bilinear)")
+@click.option("--observations", type=str, default="", help="--sites: netCDF station observations (time, site, channel) with "
+              "lat / lon along site; verifies the forecast at the --sites named there, from --date through --until")
 def main(model_name, date, time, lead_time, list_models, initial_conditions, output_dir, filter_vars, modal, weight_seed, device, grid,
          members, perturbation, amp, seed, quantiles, exceed, models, pangu_schedule, score, compare, truth, climatology, until,
-         every, map_channels, map_leads):
+         every, map_channels, map_leads, sites="", site_method=None, observations=""):
     if modal:
         raise click.UsageError("--modal: remote execution through Modal is outside this build (SURVEY.md section 2); run locally")
     if not 1 <= members <= 64:
@@ -224,6 +276,34 @@ def main(model_name, date, time, lead_time, list_models, initial_conditions, out
             kw["cfg"] = small(model_name)
     if names:
         model_name = names
+    if site_method is not None and not sites:
+        raise click.UsageError("--site_method belongs to --sites")
+    if observations and not sites:
+        raise click.UsageError("--observations verifies at sites: give --sites too")
+    if observations and (truth or climatology or compare or map_channels or map_leads):
+        raise click.UsageError("--observations verifies against station observations, without --truth, --climatology, "
+                               "--compare, --map_channels or --map_leads")
+    if sites and (names or score or compare or list_models):
+        raise click.UsageError("--sites forecasts one model (-m) at sites, without --models, --score, --compare or "
+                               "--list_models")
+    if observations and (q or events):
+        raise click.UsageError("--observations verifies the forecast: --quantiles and --exceed belong to --sites alone")
+    if sites and not observations and (until or every is not None or truth or climatology or map_channels or map_leads):
+        raise click.UsageError("--sites alone forecasts: --until and --every need --observations, and --truth, "
+                               "--climatology, --map_channels and --map_leads belong to --score or --compare")
+    if observations:
+        paths = run_score_sites(model_name, date, time, lead_time, until or date, 24 if every is None else every, sites,
+                                site_method or "bilinear", observations, initial_conditions, output_dir, filter_vars,
+                                members, perturbation, amp, seed, **kw)
+        for p in paths:
+            print(p)
+        return paths
+    if sites:
+        paths = run_sites(model_name, date, time, lead_time, sites, site_method or "bilinear", initial_conditions,
+                          output_dir, filter_vars, members, perturbation, amp, seed, q, events, **kw)
+        for p in paths:
+            print(p)
+        return paths
     if (truth or climatology) and not (score or compare):
         raise click.UsageError("--truth and --climatology belong to --score or --compare")
     if score and (names or q or events or list_models):

@@ -44,15 +44,21 @@ def _as_index(values, key, method=None):
 
 
 class DataArray:
-    """Minimal stand-in for xarray.DataArray (values + named dims + 1-D coords)."""
+    """Minimal stand-in for xarray.DataArray (values + named dims + 1-D coords).  A coordinate that is not a dimension may
+    lie along one, given as ``(dim, values)`` as xarray takes it (a site's lat / lon along "site"); ``coords[name]`` is
+    then its values, and selecting along the dimension selects them too."""
 
     def __init__(self, data, dims, coords=None, name=None, attrs=None):
         self.values = np.asarray(data)
         self.dims = tuple(dims)
         assert self.values.ndim == len(self.dims), (self.values.shape, dims)
         self.coords = {}
+        self.coord_dims = {}   # non-dimension coordinate -> the dimension it lies along
         for k, v in (coords or {}).items():
-            if k in self.dims:
+            if isinstance(v, tuple) and len(v) == 2 and v[0] in self.dims and k not in self.dims:
+                self.coord_dims[k], v = v[0], np.asarray(v[1])
+                assert v.shape == (self.values.shape[self.dims.index(self.coord_dims[k])],), (k, v.shape, self.values.shape)
+            elif k in self.dims:
                 v = np.asarray(v)
                 assert v.shape[0] == self.values.shape[self.dims.index(k)], (k, v.shape, self.values.shape)
             self.coords[k] = v
@@ -92,12 +98,15 @@ class DataArray:
         vals = np.take(self.values, idx, axis=ax) if not isinstance(idx, slice) else self.values[(slice(None),) * ax + (idx,)]
         coords = dict(self.coords)
         dims = list(self.dims)
+        along = self.__dict__.get("coord_dims", {})
+        for k in [dim] + [k for k, d in along.items() if d == dim]:
+            if k in coords:
+                coords[k] = np.asarray(coords[k])[idx]
         if isinstance(idx, (int, np.integer)):
             dims.pop(ax)
-            if dim in coords:
-                coords[dim] = np.asarray(coords[dim])[idx]
-        elif dim in coords:
-            coords[dim] = np.asarray(coords[dim])[idx]
+        else:   # the non-dimension coordinates keep their dimension
+            coords.update({k: (d, coords[k]) for k, d in along.items() if d == dim})
+        coords.update({k: (d, coords[k]) for k, d in along.items() if d != dim})
         return DataArray(vals, dims, coords, self.name, self.attrs)
 
     def isel(self, **kw):
@@ -150,6 +159,12 @@ class DataArray:
             wide = self.values.dtype == np.float64   # fp64 arrays (scorecards) keep their precision; the rest is fp32
             var = f.createVariable(self.name or "__xarray_dataarray_variable__", "d" if wide else "f", self.dims)
             var[:] = self.values.astype(np.float64 if wide else np.float32)
+            along = self.__dict__.get("coord_dims", {})
+            if along:   # after the data variable, named by its CF "coordinates" attribute, as xarray writes them
+                var.coordinates = " ".join(along).encode()
+                for k, d in along.items():
+                    v = f.createVariable(k, "d", (d,))
+                    v[:] = np.asarray(self.coords[k]).astype(np.float64)
             for k, v in self.attrs.items():   # scalar attributes become global attributes, as xarray writes them
                 setattr(f, k, v)
 
@@ -218,6 +233,11 @@ def _write_array(path: Path, arr, chunks, dims, attrs=None):
             _write_chunk(path, (i,) + (0,) * (arr.ndim - 1), arr[i:i + 1])
 
 
+def _attr(var, key):
+    v = getattr(var, key, b"")
+    return v.decode() if isinstance(v, bytes) else str(v)
+
+
 def open_dataarray(path, engine=None):
     """netCDF3 file or zarr v2 directory written by the methods above."""
     p = Path(path)
@@ -243,10 +263,13 @@ def open_dataarray(path, engine=None):
         return DataArray(data, dims, coords)
     from scipy.io import netcdf_file
     with netcdf_file(os.fspath(p), "r", mmap=False) as f:
-        name = [k for k in f.variables if k not in f.dimensions][0]
+        names = [k for k in f.variables if k not in f.dimensions]
+        aux = list(dict.fromkeys(c for k in names for c in _attr(f.variables[k], "coordinates").split()))
+        name = [k for k in names if k not in aux][0]
         var = f.variables[name]
         dims = list(var.dimensions)
-        coords = {}
+        coords = {c: (f.variables[c].dimensions[0], np.array(f.variables[c][:], dtype=np.float64)) for c in aux
+                  if c in f.variables}
         for d in dims:
             if d in f.variables:
                 v = f.variables[d]
